@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200-native plonky2 prover hot path.
+"""bench.py -- headline benchmark of the plonky2 prover hot path on an H100 (sm_90a CUDA).
 
 A "step" = one pass of the hot path over one batch of synthetic input: PolynomialBatch::from_values
 (plonky2/src/fri/oracle.rs:57-112) = iNTT of every column -> rate-2^-r coset LDE -> Poseidon Merkle
@@ -7,12 +7,14 @@ commitment of the LDE rows.  Workload at N=1 = BASELINE.json configs[1]: 234 col
 rate_bits 3, cap_height 4 (2^23 leaves of 234 elements).  Metric = Goldilocks field-elements/s
 (LDE output elements committed per second = B*N / t), whole job.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 N > 1: the SAME commitment is row-block sharded over the ranks (strong scaling): rank g builds leaf rows
 [g*N/G, (g+1)*N/G) on its own coset and the ranks all-gather their Merkle-cap entries over NCCL.
-Prints ONE JSON line on rank 0 (see DESIGN.md "Measurement").
+Prints ONE JSON line on rank 0 (see DESIGN.md "Measurement"). --dump-outputs DIR also writes what the last timed step
+computed (the cap, and fixed seeded samples of the coefficients and leaf rows) as DIR/<name>.npy, so that two builds
+can be compared output for output on identical inputs.
 """
 import argparse
 import ctypes as C
@@ -41,7 +43,7 @@ def load_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 PRESETS = {  # --config name: (columns, log_n, rate_bits, cap_height, generator seed, BASELINE.json configs index)
@@ -102,7 +104,7 @@ def workload_config(args, world):
         "workload": name,
         "columns": args.cols, "log_n": args.log_n, "rate_bits": args.rate_bits, "cap_height": args.cap_height,
         "lde_elements": args.cols * N,
-        "l2": "inputs %.2f GB + leaves %.2f GB per step, far larger than the 126 MB L2 (no flush needed)" % (
+        "l2": "inputs %.2f GB + leaves %.2f GB per step, far larger than the H100's 50 MB L2 (no flush needed)" % (
             args.cols * n * 8 / 1e9, args.cols * N * 8 / 1e9),
         "parallelism": ("column-sharded iNTT storing into every rank's coefficient matrix over NVLink (64-column "
                         "chunks), then row-block (coset) sharded LDE + Merkle x%d + NCCL all-gather of cap "
@@ -266,6 +268,68 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path returned in its last step
+# ------------------------------------------------------------------------------------------------
+DUMP_SEED = 0x5EED
+DUMP_COEFFS = 1 << 20  # coefficient entries sampled (at most): 16 MB as float64 pairs, 8 MB of indices
+DUMP_LEAVES = 256      # leaf rows sampled (at most)
+
+
+def u64_as_f64_pairs(a):
+    """uint64 words as float64 (low 32 bits, high 32 bits) pairs on a new last axis: exact, each half is below 2^53."""
+    a = np.ascontiguousarray(a, dtype=np.uint64)
+    return np.stack([(a & np.uint64(0xFFFFFFFF)).astype(np.float64), (a >> np.uint64(32)).astype(np.float64)], axis=-1)
+
+
+class _DeviceWords:
+    """Zero-copy view (for torch.as_tensor) of `n` int64 words in device memory owned by a commitment."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i8", "data": (ptr, False), "version": 2}
+
+
+def collect_outputs(N, L, ctx, hnd, cap, fri, dev):
+    """The arrays a caller of the commitment receives: the Merkle cap, a fixed seeded sample of the coefficient matrix
+    (PolynomialBatch.polynomials) and of the leaf rows (MerkleTree.leaves), and the FRI round caps and final polynomial
+    when the step includes the FRI commit phase. Values are uint64 here; indices are int64."""
+    import torch
+
+    rng = np.random.default_rng(DUMP_SEED)
+    B, n = L.gl_commit_num_polys(hnd), 1 << L.gl_commit_degree_log(hnd)
+    ptr = L.gl_commit_dev_coeffs(hnd)  # the commitment's own B x n matrix, column b at b*n: read in place
+    if not ptr:
+        raise RuntimeError("commitment holds no device coefficients")
+    coeffs = torch.as_tensor(_DeviceWords(ptr, B * n), device=dev)
+    ci = np.unique(rng.integers(0, B * n, DUMP_COEFFS)) if B * n > DUMP_COEFFS else np.arange(B * n)
+    out = {"cap": cap,
+           "coeffs_sample": coeffs[torch.from_numpy(ci).to(dev)].cpu().numpy().view(np.uint64),
+           "coeffs_sample_index": ci}
+    del coeffs
+    W = L.gl_commit_leaf_width(hnd)
+    shards = C.c_uint32()
+    N.check(L.gl_commit_shard(hnd, None, C.byref(shards)), ctx.h)
+    rows = (n << L.gl_commit_rate_bits(hnd)) // shards.value  # this rank's leaf rows
+    li = np.unique(rng.integers(0, rows, DUMP_LEAVES)) if rows > DUMP_LEAVES else np.arange(rows)
+    leaves = np.empty((len(li), W), dtype=np.uint64)
+    for k, i in enumerate(li):
+        N.check(L.gl_commit_leaves(hnd, int(i), 1, N.np_ptr(leaves[k]), N.MEM_HOST), ctx.h)
+    out.update(leaves_sample=leaves, leaves_sample_index=li)
+    if fri is not None:
+        caps, final = fri
+        out.update(fri_round_caps=np.stack([np.asarray(c.hashes, dtype=np.uint64) for c in caps]),
+                   fri_final_poly=np.asarray(final, dtype=np.uint64))
+    return out
+
+
+def dump_outputs(path, arrays):
+    """DIR/<name>.npy: uint64 values as float64 (low, high) pairs, int64 indices as float64 (exact below 2^53)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(path, name + ".npy"), u64_as_f64_pairs(a) if a.dtype == np.uint64 else a.astype(np.float64))
+
+
+# ------------------------------------------------------------------------------------------------
 # GPU arm
 # ------------------------------------------------------------------------------------------------
 def gpu_arm(args, rank, local_rank, world):
@@ -375,7 +439,7 @@ def gpu_arm(args, rank, local_rank, world):
                 fri_out[0] = fri_ctx(hnd, cap_full.cpu().numpy())
                 fb.record(stream)
                 fri_spans.append((fa, fb))
-            L.gl_commit_destroy(hnd)
+            return hnd
 
         def sync_all():
             torch.cuda.synchronize(dev)
@@ -384,7 +448,7 @@ def gpu_arm(args, rank, local_rank, world):
                 torch.cuda.synchronize(dev)
 
         for _ in range(max(args.warmup, 3)):
-            step_device()
+            L.gl_commit_destroy(step_device())
         sync_all()
         ctx.reset_phases()
         del fri_spans[:]
@@ -396,8 +460,10 @@ def gpu_arm(args, rank, local_rank, world):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
         marks = []
-        for _ in range(args.steps):
-            step_device()
+        for k in range(args.steps):
+            hnd = step_device()
+            if k + 1 < args.steps:  # the last step's commitment stays alive for --dump-outputs
+                L.gl_commit_destroy(hnd)
             m = torch.cuda.Event(enable_timing=True)
             m.record(stream)
             marks.append(m)
@@ -420,6 +486,9 @@ def gpu_arm(args, rank, local_rank, world):
         if fixture is not None:  # golden cap of this exact workload from the CPU oracle (tests/golden/fullscale_*.json)
             cap_ok = bool(np.array_equal(cap_dev, np.array(fixture["cap"], dtype=np.uint64)))
             assert cap_ok, "rank %d: the gathered Merkle cap differs from the oracle fixture" % rank
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, collect_outputs(N, L, ctx, hnd, cap_dev, fri_out[0], dev))
+        L.gl_commit_destroy(hnd)
 
         # ---- end to end through the C ABI with HOST buffers (pinned): H2D of the columns + D2H of the cap
         host_vals = torch.empty((B, n), dtype=torch.int64, pin_memory=True)
@@ -494,35 +563,15 @@ def gpu_arm(args, rank, local_rank, world):
     leaf_avg = leaf_ms / max(1, leaf_cnt)
     leaf_bytes = 8.0 * N_loc * B + 32.0 * N_loc
     perms = N_loc * ((B + 7) // 8 if B > 4 else 0)
-    traffic, traffic_note = None, None
-    try:  # DRAM bytes per launch from the committed ncu --set full capture (scaled by the algorithmic bytes)
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["k_leaf_hash"]
-        traffic = tr["dram_bytes_per_algorithmic_byte"] * leaf_bytes
-        traffic_note = "ncu dram read+write per algorithmic byte x this launch's algorithmic bytes; " + tr["source"]
-    except Exception:
-        pass
     roof = {
         "kernel": "k_leaf_hash (Poseidon sponge over each LDE row)", "bound": "hbm",
         "achieved": leaf_bytes / (leaf_avg * 1e-3) / 1e9 if leaf_avg else None, "peak": peak, "unit": "GB/s",
         "frac": (leaf_bytes / (leaf_avg * 1e-3) / 1e9 / peak) if leaf_avg else None,
-        "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src, "avg_ms": leaf_avg, "launches": leaf_cnt,
+        "peak_source": peak_src, "avg_ms": leaf_avg, "launches": leaf_cnt,
         "algorithmic_bytes": leaf_bytes,
         "permutations_per_s": perms / (leaf_avg * 1e-3) if leaf_avg else None,
         "note": "instruction-issue bound (x^7 S-boxes on the integer pipes, MDS / partial rounds on the FP64 pipe), not HBM bound: see DESIGN.md",
     }
-    # integer-issue roofline (what actually bounds these kernels): thread-instructions/s vs 128 lanes/clk/SM
-    issue = None
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        sm_clk = (clocks or {}).get("sm_mhz") or 1965.0
-        peak_issue = 148 * 128 * sm_clk * 1e6
-        ipp = tr["k_leaf_hash"]["thread_instructions_per_permutation"]
-        ach = ipp * roof["permutations_per_s"]
-        issue = {"kernel": "k_leaf_hash", "bound": "instruction issue (4 warp-instructions/clk/SM)",
-                 "achieved": ach, "peak": peak_issue, "unit": "thread-instructions/s", "frac": ach / peak_issue,
-                 "thread_instructions_per_permutation": ipp, "source": tr["k_leaf_hash"]["instr_source"]}
-    except Exception:
-        pass
     lde_ms = (phases["intt"][0] + phases["lde"][0]) / steps
     lde_bytes = 8.0 * n * B * (2 + (1 << r) / world)
     line = {
@@ -537,7 +586,6 @@ def gpu_arm(args, rank, local_rank, world):
                         "device behind the handle (fetched on demand by gl_commit_leaves/_open)"},
         "gpu_launches": int(launches),
         "roofline": roof,
-        "roofline_issue": issue,
         "phases_ms_per_step": dict({k: v[0] / steps for k, v in phases.items()},
                                    **({"side_stream_nvlink_copy_and_barriers (under the main stream)": side[0] / max(1, side[1])}
                                       if side else {})),
@@ -575,7 +623,7 @@ def gpu_arm(args, rank, local_rank, world):
             line["prove_recursion_shape"] = recursion_shape(local_rank)
         except Exception as e:  # never lose the headline line to the secondary measurement
             line["prove_recursion_shape"] = {"error": repr(e)}
-        try:   # in a child process with a timeout: new code, not yet run on a GPU -- it must not be able to take the line down
+        try:   # in a child process with a timeout: a failure of the secondary measurement must not take the line down
             env = dict(os.environ, CUDA_VISIBLE_DEVICES=os.environ.get("CUDA_VISIBLE_DEVICES", str(local_rank)))
             out = subprocess.run([sys.executable, os.path.abspath(__file__), "--plonk-circuit-only"], capture_output=True,
                                  text=True, timeout=300, env=env)
@@ -723,8 +771,7 @@ def plonk_circuit_proof(ctx_device, reps=3):
             "cpu_port_ms_per_proof": cpu_ms, "cpu_cores": oracle_lib.nproc(), "proof_bytes": len(proof_bytes),
             "bit_exact_vs_cpu_port": bool(proof_bytes == want),
             "accepted_by_restated_verifier": PC.oracle_verify(oracle_lib, plonk, c, digest, fri, parts) is None,
-            "note": "host witness in, proof bytes out, Python host transcript in the loop; first measurement of this path "
-                    "(written after the round's GPU budget was spent)"}
+            "note": "host witness in, proof bytes out, Python host transcript in the loop"}
 
 
 def main():
@@ -754,8 +801,14 @@ def main():
     ap.add_argument("--ntt-group", type=int, default=0, help="columns per NTT group (0 = library default)")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the recursion-shaped prove() timing")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float64)")
     ap.add_argument("--plonk-circuit-only", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU path computed; the reference arm has no such output")
     if args.plonk_circuit_only:   # child mode of the secondary measurement `prove_plonk_circuit`
         try:
             print(json.dumps(plonk_circuit_proof(0)), flush=True)

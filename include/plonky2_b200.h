@@ -1,6 +1,6 @@
 /*
- * plonky2_b200.h -- C ABI of the B200-native plonky2 prover hot path
- * (Goldilocks NTT / coset-LDE / Poseidon Merkle commitment / FRI commit phase, sm_100a CUDA).
+ * plonky2_b200.h -- C ABI of the H100-native plonky2 prover hot path
+ * (Goldilocks NTT / coset-LDE / Poseidon Merkle commitment / FRI commit phase, sm_90a CUDA).
  *
  * The reference (0xPolygonZero/plonky2 @ 5d9da5a) is pure Rust with no FFI; the seam this ABI
  * replaces is the trait/struct surface listed in SURVEY.md section 8(b). Each entry point below
@@ -96,7 +96,7 @@ int gl_ntt_bcast(gl_ctx* ctx, const uint64_t* in, size_t in_stride, uint32_t log
 
 /* Device copy of `words` u64 (even, 16-byte aligned) from this GPU's memory to every destination with 128-byte
  * line stores: the transfer half of the coefficient all-gather when the destinations are peer mappings or a multicast
- * address (measured at link speed, unlike the 64-byte segments gl_ntt_bcast's transposing stores produce).
+ * address (full lines run at link speed, unlike the 64-byte segments gl_ntt_bcast's transposing stores produce).
  * max_ctas bounds the grid (0 = 2 per SM) so the copy can share the GPU with a compute stream. */
 int gl_bcast(gl_ctx* ctx, const uint64_t* src, size_t words, uint64_t* const* dests, uint32_t n_dests, uint32_t max_ctas);
 

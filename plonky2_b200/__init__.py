@@ -1,4 +1,4 @@
-"""plonky2_b200 -- B200-native (sm_100a CUDA) implementation of the plonky2 prover hot path:
+"""plonky2_b200 -- H100-native (sm_90a CUDA) implementation of the plonky2 prover hot path:
 Goldilocks NTT / coset-LDE, Poseidon Merkle commitment and the FRI commit phase, behind the C ABI in
 include/plonky2_b200.h. This package is the host-side mirror of the reference's interface for that
 path (same names, argument meaning and error behaviour); see DESIGN.md and INTEGRATION.md."""

@@ -1,4 +1,4 @@
-"""Build the in-tree CUDA library (sm_100a) with nvcc. No torch dependency: the product is a plain
+"""Build the in-tree CUDA library (sm_90a, H100) with nvcc. No torch dependency: the product is a plain
 C-ABI shared object (include/plonky2_b200.h)."""
 import os
 import shutil
@@ -9,8 +9,9 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libplonky2_b200.so")
 SOURCES = ["plonky2_b200.cu"]
 DEPS = ["plonky2_b200.cu", "gl_field.cuh", "gl_lazy.cuh", "gl_ntt.cuh", "gl_ntt_host.cuh", "gl_poseidon.cuh", "gl_poseidon_constants.h",
-        os.path.join("..", "..", "include", "plonky2_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+        "gl_vanishing.cuh", os.path.join("..", "..", "include", "plonky2_b200.h"),
+        os.path.abspath(__file__)]  # this file holds NVCC_FLAGS (the target architecture among them)
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

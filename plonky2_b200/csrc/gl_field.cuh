@@ -1,4 +1,4 @@
-// gl_field.cuh -- Goldilocks field arithmetic, p = 2^64 - 2^32 + 1, for sm_100a device code
+// gl_field.cuh -- Goldilocks field arithmetic, p = 2^64 - 2^32 + 1, for sm_90a device code
 // (and the host, for the transcript's single permutations).
 //
 // Semantics follow the reference's GoldilocksField (field/src/goldilocks_field.rs:23-25,198-320,
@@ -247,8 +247,8 @@ GL_HD void mul_wide(uint64_t a, uint64_t b, uint64_t& lo, uint64_t& hi) {
 GL_HD void sqr_wide(uint64_t a, uint64_t& lo, uint64_t& hi) {
 #if defined(__CUDA_ARCH__) && defined(GL_SQR_3WIDE)
     // Variant: a^2 = a0^2 + 2*a0*a1*2^32 + a1^2*2^64 with THREE IMAD.WIDE.U32 and the cross term added twice on
-    // the ALU pipe. Measured on B200 (tools/variants): 909 vs 953 M perm/s for the generic 4-IMAD.WIDE product --
-    // after the mul_wide fix both integer pipes run at ~65 % and the extra ALU work costs more than it saves.
+    // the ALU pipe. Off by default: with both integer pipes busy, the extra ALU work can cost more than the saved
+    // IMAD.WIDE (tools/variants ranks the two forms on the GPU at hand).
     uint32_t r0, r1, r2, r3;
     asm("{\n\t.reg .u64 z, c, w;\n\t.reg .u32 z1, c0, c1, w0, w1;\n\t"
         "mul.wide.u32 z, %4, %4;\n\t"

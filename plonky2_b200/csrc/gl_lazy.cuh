@@ -1,7 +1,7 @@
 // gl_lazy.cuh -- lazily reduced Goldilocks values for the NTT butterflies.
 //
 // The reference's butterflies (field/src/fft.rs:165-202) reduce after every add/sub (goldilocks_field.rs:245-290);
-// on the B200 integer pipes a fully reduced modular add costs 10-12 instructions and a sub 8. Here a value
+// on the integer pipes a fully reduced modular add costs about a dozen instructions and a sub 8. Here a value
 // travels through the add/sub levels of an in-register radix-2^M transform as THREE 32-bit words
 //        v = w0 + w1*2^32 + e*2^64        (e a small SIGNED word: the carries and borrows accumulated so far)
 // so that add and sub are 3 carry-chain instructions with no fix-up, and is only brought back to one u64 where a

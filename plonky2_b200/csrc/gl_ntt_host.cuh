@@ -5,10 +5,9 @@
 // mbarrier) that overlaps the global loads of the data; the exchange tile lives next to it.
 #pragma once
 
-// ASYNC_TW: fetch the post twiddles with cp.async under step 2 (below). Measured on B200 (profiles/r02): it removes the
-// long-scoreboard stalls (3.0 -> 0.5 per issue) and wins where a pass has the extra coset multiplies to hide them under
-// (LDE 34.3 -> 32.7 ms for cfg2), but costs 8 % more instructions and one more barrier, which loses on the plain
-// transform (bare 2^20 NTT 1.15 -> 1.20 ms): used for coset passes only.
+// ASYNC_TW: fetch the post twiddles with cp.async under step 2 (below). It hides the twiddle loads' long-scoreboard
+// stalls and pays off where a pass has the extra coset multiplies to hide them under, but costs more instructions and
+// one more barrier, which does not pay on the plain transform: used for coset passes only.
 template <int LOG, bool ASYNC_TW>
 __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_MIN_BLOCKS) k_ntt_col(ColPass cp) {
     using Cf = PassCfg<LOG>;
@@ -34,7 +33,7 @@ __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_M
     __syncthreads();                     // every thread holds its part of the tile: S is free
     // the E post twiddles of this thread (L2-resident table, 8 KiB row stride) go to thread-private shared-memory
     // slots by cp.async WHILE step 2 runs: as plain loads at their use they were the kernel's main stall
-    // (long-scoreboard 3.0 per issue, profiles/r02 ncu) because 128 registers leave no room to hoist them
+    // (long-scoreboard stalls) because 128 registers leave no room to hoist them
 #pragma unroll
     for (int i = 0; i < Cf::E; i++) {
         const u64* src = col_twiddle_src<LOG>(cp, blockIdx.x, threadIdx.x, i);
@@ -50,8 +49,7 @@ __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_M
 
 // Even LOG (E == TPT): both steps of the pass are "radix-E lazy DFT, normalise, multiply by a twiddle", so ONE copy of
 // that body serves both (a rolled 2-trip loop; only the I/O around it differs). The two-copy kernel above is ~90 KiB of
-// SASS and its largest non-ALU stall was instruction fetch (no_instruction 0.9 per issue, profiles/r02); this one is
-// about half that.
+// SASS, large enough for instruction fetch to stall it; this one is about half that.
 template <int LOG, bool ASYNC_TW>
 __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_MIN_BLOCKS) k_ntt_col_shared(ColPass cp) {
     using Cf = PassCfg<LOG>;

@@ -16,9 +16,9 @@
 //    round) is only used on the host and under -DGL_PARTIAL_FAST;
 //  * u32 <-> f64 conversions are I2F / F2I on the XU pipe.
 // The rounds are rolled loops (one copy of each round body) so the permutation fits the instruction cache.
-// History on B200 (leaf hash of 234-wide rows, M permutations/s): 818 (integer fast form) -> 950 (single
-// 128-bit product) -> 1110 (FP64-resident partial rounds) -> 1300 (two rounds per step) -> 1459 (split circulant
-// MDS); profiles/r01_*.
+// Each of these steps (single 128-bit product, FP64-resident partial rounds, two rounds per step, split circulant
+// MDS) was kept because it raised the leaf-hash permutation rate over the integer fast form; tools/variants/
+// re-ranks the alternatives on the GPU at hand.
 #pragma once
 #include "gl_field.cuh"
 #include "gl_poseidon_constants.h"
@@ -468,8 +468,7 @@ GL_HD void poseidon_partial_rounds_noconst(uint64_t s[12]) {
 // pair, all lanes after the last pair) can be negative, so their constants carry a bias (bl, bh) = 0 (mod p) of
 // 2^50 and f64_pair_to_u64 sees non-negative integers < 2^51 (tests/emu/poseidon_f64_emu.cpp tracks the bound).
 // Versus the "fast" integer form (23 64x64 products + 12 reductions per round, all on the integer pipes that
-// bound this kernel): no init matrix, ~90 integer instructions per round instead of ~520; measured 950 -> 1300 M
-// permutations/s, 1424 with the split circulant (profiles/r01_poseidon_variants.md).
+// bound this kernel): no init matrix, ~90 integer instructions per round instead of ~520.
 // In: s after full round 4's MDS + first partial constant layer (original constants). Out: s after the last
 // partial round's MDS + the 5th full round's constant layer.
 GL_HD void poseidon_partial_rounds_f64(uint64_t s[12]) {

@@ -1,4 +1,4 @@
-// plonky2_b200.cu -- sm_100a kernels + host orchestration + the C ABI of include/plonky2_b200.h.
+// plonky2_b200.cu -- sm_90a kernels + host orchestration + the C ABI of include/plonky2_b200.h.
 //
 // Hot path implemented here (reference -> this file):
 //   PolynomialBatch::from_values/from_coeffs  plonky2/src/fri/oracle.rs:57-139   -> commit_build()
@@ -1425,14 +1425,14 @@ int gl_ntt_bcast(gl_ctx* ctx, const uint64_t* in, size_t in_stride, uint32_t log
 
 // src (this GPU's memory) -> every destination, 16 bytes per thread per step: full 128-byte lines per warp instruction,
 // the granularity NVLink / NVSwitch multicast writes need to run at link speed (the 64-byte segments of the fused
-// natural-order stores reach ~120 GB/s; this copy is bound by the link).
+// natural-order stores fall well short of it; this copy is bound by the link).
 struct BcastDests {
     ulonglong2* p[8];
     int n;
 };
 __global__ void __launch_bounds__(256) k_bcast_copy(const ulonglong2* __restrict__ src, size_t n16, BcastDests d) {
     // 8 independent 16-byte loads per thread before the first store: with few CTAs (the copy shares the GPU with the
-    // transforms) the bytes in flight, not the link, bounded the first version at ~120-190 GB/s
+    // transforms) the bytes in flight, not the link, bounded a version with one load per store
     constexpr int U = 8;
     const size_t step = (size_t)gridDim.x * blockDim.x;
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -142,8 +142,8 @@ class PipelinedCommitter:
     The iNTT (the reference's rayon axis, oracle.rs:65-69) and the H2D are divided by G. Transports:
       "multimem" / "p2p"  as above (torch symmetric memory: CUDA IPC / fabric handles);
       "fused"             the iNTT's last pass stores straight to the multicast address (gl_ntt_bcast): no second
-                          kernel, but its transposing stores are 64-byte segments and NVLink runs them at ~120 GB/s
-                          (measured, profiles/r02) -- kept for comparison;
+                          kernel, but its transposing stores are 64-byte segments, which NVLink runs well below
+                          link speed -- kept for comparison;
       "nccl"              ncclAllGather per chunk on the main stream (fallback when peer mappings are unavailable).
     The commitment is bit-identical to the single-device one.
 

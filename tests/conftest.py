@@ -15,7 +15,7 @@ P = 0xFFFFFFFF00000001
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _splitmix64(x):

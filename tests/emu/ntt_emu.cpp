@@ -1,5 +1,5 @@
 // CPU emulation of the CUDA NTT pass code (threads as loops, phases as barriers) checked against the oracle.
-// The SAME source that the sm_100a kernels compile (gl_ntt.cuh phase functions, ntt_make_job) runs here with the
+// The SAME source that the sm_90a kernels compile (gl_ntt.cuh phase functions, ntt_make_job) runs here with the
 // host formulation of the lazy field type. Test infrastructure: built and run by tests/test_emu.py.
 #include <cstdio>
 #include <cstdlib>

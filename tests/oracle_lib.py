@@ -21,11 +21,8 @@ u32p = C.POINTER(C.c_uint32)
 
 def build_oracle():
     """Compile the oracle if the shared object is missing or stale."""
-    src = os.path.join(ORACLE_DIR, "gl_oracle.cpp")
-    hdr = os.path.join(ORACLE_DIR, "gl_oracle.h")
-    if os.path.exists(LIB_PATH) and all(
-        os.path.getmtime(LIB_PATH) >= os.path.getmtime(p) for p in (src, hdr) if os.path.exists(p)
-    ):
+    deps = [os.path.join(ORACLE_DIR, f) for f in ("gl_oracle.cpp", "gl_oracle.h", "gl_poseidon_constants.h", "Makefile")]
+    if os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(p) for p in deps):
         return LIB_PATH
     subprocess.check_call(["make", "-C", ORACLE_DIR, "libgl_oracle.so"], stdout=subprocess.DEVNULL)
     return LIB_PATH

@@ -18,7 +18,7 @@ def pb():
     if not torch.cuda.is_available():
         if os.environ.get("GL_REQUIRE_GPU") == "1":
             raise AssertionError("GPU tests need a CUDA device")
-        pytest.skip("no CUDA device (gpu-marked tests run on the B200 box)")
+        pytest.skip("no CUDA device (gpu-marked tests run on an H100)")
     import plonky2_b200 as p
 
     p.default_context()

@@ -2,7 +2,7 @@
 fixtures made by the CPU oracle (tools/make_fullscale_fixtures.py, committed under tests/golden/): the cap, 64 sampled
 leaf rows (by digest, 4 of them word for word) with their Merkle paths, and a checksum of the coefficient matrix.
 The input is the SURVEY 8(d) splitmix64 generator, regenerated here; nothing on this path needs the 100-s oracle run
-or /root/reference. Run with `-m gpu` on the B200 box."""
+or anything outside the repository. Run with `-m gpu` on an H100."""
 import json
 import os
 
@@ -29,7 +29,7 @@ def pb():
     if not torch.cuda.is_available():
         if os.environ.get("GL_REQUIRE_GPU") == "1":
             raise AssertionError("GPU tests need a CUDA device")
-        pytest.skip("no CUDA device (gpu-marked tests run on the B200 box)")
+        pytest.skip("no CUDA device (gpu-marked tests run on an H100)")
     import plonky2_b200 as p
 
     p.default_context()

@@ -1,4 +1,4 @@
-// SASS-count lab: in-register radix-32 DIF variants. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -cubin -o /tmp/dft_lab.cubin dft_lab.cu
+// SASS-count lab: in-register radix-32 DIF variants. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -cubin -o /tmp/dft_lab.cubin dft_lab.cu
 #include "../../plonky2_b200/csrc/gl_field.cuh"
 using namespace gl;
 typedef uint64_t u64;

@@ -1,6 +1,6 @@
-// Integer-pipe microbenchmarks for B200 (what bounds Goldilocks arithmetic): issue rates of
+// Integer-pipe microbenchmarks for H100 (what bounds Goldilocks arithmetic): issue rates of
 // IMAD.WIDE.U32, 32-bit IMAD, IADD3 / carry chains, and the library's own modmul / modadd / Poseidon.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o /tmp/microbench tools/microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/microbench tools/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../plonky2_b200/csrc/gl_poseidon.cuh"

@@ -1,8 +1,7 @@
-// Which B200 pipes share an issue port? Times pure and interleaved streams of DFMA (FP64), IMAD / IMAD.WIDE
-// (FMA-heavy), LOP3 (ALU) and I2F.F64 (XU), each with 8 independent chains per thread (IMAD.HI streams were added
-// after the round-1 run: profiles/r01_pipe_mix.txt does not have them yet). If two classes share a port the
+// Which H100 pipes share an issue port? Times pure and interleaved streams of DFMA (FP64), IMAD / IMAD.WIDE
+// (FMA-heavy), LOP3 (ALU), IMAD.HI and I2F.F64 (XU), each with 8 independent chains per thread. If two classes share a port the
 // mixed stream takes the SUM of the pure times, otherwise about the MAX. Output feeds the cost model in DESIGN.md.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/pipe_mix tools/pipe_mix.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/pipe_mix tools/pipe_mix.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

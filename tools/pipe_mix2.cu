@@ -2,7 +2,7 @@
 // (IMAD.HI, IMAD.WIDE without addend, funnel shifts, carry chains, PRMT, SHFL, LDS) alone and mixed.
 // Each stream has ILP independent chains per thread; 16 warps per SMSP hide latency, so the numbers are
 // issue/pipe throughput: cycles per warp-instruction per SMSP.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/pipe_mix2 tools/pipe_mix2.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/pipe_mix2 tools/pipe_mix2.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -3,8 +3,8 @@
 set -e
 cd "$(dirname "$0")"
 mkdir -p out
-NV="nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo"
-nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -o out/variant_bench variant_bench.cu -lcuda
+NV="nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo"
+nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -o out/variant_bench variant_bench.cu -lcuda
 v() { name=$1; shift; $NV -cubin -o out/$name.cubin leaf_kernel.cu "$@" & }
 v base
 v cvtmagic -DGL_CVT_MAGIC
