@@ -325,12 +325,12 @@ static int get_step(gl_ctx* ctx, int log, u64 scale, u64 base, const u64** out) 
     auto it = ctx->step_tabs.find(key);
     if (it == ctx->step_tabs.end()) {
         const size_t words = ((size_t)1 << log) < 2 ? 2 : ((size_t)1 << log);
-        u64* p;
-        TRY(dmalloc(ctx, &p, words));
-        k_fill_step<<<((1 << log) + 255) / 256, 256, 0, ctx->stream>>>(log, canon(scale), canon(base), p);
+        DevBuf p(ctx);
+        TRY(p.alloc(words));
+        k_fill_step<<<((1 << log) + 255) / 256, 256, 0, ctx->stream>>>(log, canon(scale), canon(base), p.get());
         CKL(ctx);
         ctx->table_bytes += words * 8;
-        it = ctx->step_tabs.emplace(key, p).first;
+        it = ctx->step_tabs.emplace(key, p.release()).first;
     }
     *out = it->second;
     return GL_OK;
@@ -340,12 +340,12 @@ static int get_post(gl_ctx* ctx, int a, int b, u64 base, const u64** out) {
     auto it = ctx->post_tabs.find(key);
     if (it == ctx->post_tabs.end()) {
         const size_t words = (size_t)1 << (a + b);
-        u64* p;
-        TRY(dmalloc(ctx, &p, words));
-        k_fill_post<<<(unsigned)((words + 255) / 256), 256, 0, ctx->stream>>>(a, b, canon(base), p);
+        DevBuf p(ctx);
+        TRY(p.alloc(words));
+        k_fill_post<<<(unsigned)((words + 255) / 256), 256, 0, ctx->stream>>>(a, b, canon(base), p.get());
         CKL(ctx);
         ctx->table_bytes += words * 8;
-        it = ctx->post_tabs.emplace(key, p).first;
+        it = ctx->post_tabs.emplace(key, p.release()).first;
     }
     *out = it->second;
     return GL_OK;
@@ -366,20 +366,16 @@ static uint32_t group_cols(const gl_ctx* ctx, int log_n, uint32_t ncols) {
 }
 
 // Upload `bases` (host) and build ntab tables of `count` powers each on the device.
-static int build_pow_tables(gl_ctx* ctx, const std::vector<u64>& bases, size_t count, u64** out) {
+static int build_pow_tables(gl_ctx* ctx, const std::vector<u64>& bases, size_t count, DevBuf& out) {
     const int ntab = (int)bases.size();
-    u64* dbases = nullptr;
-    TRY(dmalloc(ctx, &dbases, ntab));
-    int rc = h2d(ctx, dbases, bases.data(), ntab);  // pageable source: staged by the runtime before the call returns
-    if (rc == GL_OK) rc = dmalloc(ctx, out, count * ntab);
-    if (rc == GL_OK) {
-        size_t total = count * ntab;
-        k_fill_pows<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(dbases, ntab, count, *out);
-        ctx->launches++;
-        if (cudaGetLastError() != cudaSuccess) rc = set_err(ctx, GL_ERR_CUDA, "k_fill_pows launch failed");
-    }
-    dfree(ctx, dbases);
-    return rc;
+    DevBuf dbases(ctx);
+    TRY(dbases.alloc(ntab));
+    TRY(h2d(ctx, dbases.get(), bases.data(), ntab));  // pageable source: staged by the runtime before the call returns
+    TRY(out.alloc(count * ntab));
+    size_t total = count * ntab;
+    k_fill_pows<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(dbases.get(), ntab, count, out.get());
+    CKL(ctx);
+    return GL_OK;
 }
 
 // One forward transform of `ncols` device columns: in (natural order) -> out, either natural order (mode RM_NATURAL,
@@ -473,12 +469,11 @@ static int ntt_natural(gl_ctx* ctx, const u64* in, size_t in_stride, u64* out, s
         const size_t lo_cnt = (size_t)1 << lowbits, hi_cnt = (size_t)1 << (log_n - lowbits);
         const u64 sinv = gl::inv(shift);
         const size_t tcnt = lo_cnt > hi_cnt ? lo_cnt : hi_cnt;
-        u64* tabs;
-        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(sinv, lo_cnt), sinv}, tcnt, &tabs));
-        k_mul_pows<<<dim3((unsigned)((n + 255) / 256), ncols), 256, 0, ctx->stream>>>(out, out_stride, n, tabs,
-                                                                                     tabs + tcnt, lowbits);
-        ctx->launches++;
-        dfree(ctx, tabs);
+        DevBuf tabs(ctx);
+        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(sinv, lo_cnt), sinv}, tcnt, tabs));
+        k_mul_pows<<<dim3((unsigned)((n + 255) / 256), ncols), 256, 0, ctx->stream>>>(out, out_stride, n, tabs.get(),
+                                                                                     tabs.get() + tcnt, lowbits);
+        CKL(ctx);
     }
     return GL_OK;
 }

@@ -12,7 +12,9 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <map>
+#include <memory>
 #include <set>
 #include <string>
 #include <tuple>
@@ -123,6 +125,35 @@ static int dmalloc(gl_ctx* ctx, u64** p, size_t words) {
 static void dfree(gl_ctx* ctx, u64* p) {
     if (p) cudaFreeAsync(p, ctx->stream);
 }
+// A device buffer owned by the scope that declares it: freed on ctx->stream (stream-ordered, like the allocation) when
+// the scope exits on any path, unless release() has handed the pointer to a long-lived owner (a Tree, gl_commit, gl_fri
+// or one of the context's table caches).
+class DevBuf {
+  public:
+    explicit DevBuf(gl_ctx* ctx) : ctx_(ctx) {}
+    DevBuf(DevBuf&& o) noexcept : ctx_(o.ctx_), p_(o.release()) {}
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { reset(); }
+    int alloc(size_t words) {
+        reset();
+        return dmalloc(ctx_, &p_, words);
+    }
+    void reset() {
+        dfree(ctx_, p_);
+        p_ = nullptr;
+    }
+    u64* get() const { return p_; }
+    u64* release() {
+        u64* p = p_;
+        p_ = nullptr;
+        return p;
+    }
+
+  private:
+    gl_ctx* ctx_;
+    u64* p_ = nullptr;
+};
 static int ensure_scratch(gl_ctx* ctx, size_t words) {
     if (ctx->scratch_words >= words) return GL_OK;
     if (ctx->scratch) dfree(ctx, ctx->scratch);
@@ -170,6 +201,25 @@ static int copy_out(gl_ctx* ctx, u64* out, const u64* dev, size_t words, int mem
         return GL_OK;
     }
     return d2h(ctx, out, dev, words);
+}
+// Device view of a caller's `words`-word input: the caller's pointer itself unless mem == GL_MEM_HOST, else a copy in
+// `stage`. The view is writable only for the entry points whose buffer is in-out (gl_poseidon_permute_many).
+static int device_in(gl_ctx* ctx, const u64* in, size_t words, int mem, DevBuf& stage, u64** view) {
+    *view = const_cast<u64*>(in);
+    if (mem != GL_MEM_HOST) return GL_OK;
+    TRY(stage.alloc(words));
+    TRY(h2d(ctx, stage.get(), in, words));
+    *view = stage.get();
+    return GL_OK;
+}
+// Where a `words`-word result is written on the device: the caller's `out` unless mem == GL_MEM_HOST, else `stage`,
+// which the entry point copies to `out` at the end
+static int device_out(u64* out, size_t words, int mem, DevBuf& stage, u64** view) {
+    *view = out;
+    if (mem != GL_MEM_HOST) return GL_OK;
+    TRY(stage.alloc(words));
+    *view = stage.get();
+    return GL_OK;
 }
 
 // =====================================================================================
@@ -552,13 +602,12 @@ static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int
         // fewer than n points per shard: restrict the polynomials to the sub-coset first
         const uint32_t logM = c->degree_log + c->rate_bits - sl;
         const size_t M = (size_t)1 << logM;
-        u64* folded;
-        TRY(dmalloc(ctx, &folded, (size_t)gc * M));
-        k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), gc), 128, 0, ctx->stream>>>(cg, n, n, M, gl::pow(c->sg, M), folded);
+        DevBuf folded(ctx);
+        TRY(folded.alloc((size_t)gc * M));
+        k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), gc), 128, 0, ctx->stream>>>(cg, n, n, M, gl::pow(c->sg, M),
+                                                                                     folded.get());
         CKL(ctx);
-        const int rc2 = lde_columns(ctx, folded, M, gc, (int)logM, 0, c->sg, t.leaves + (size_t)g0 * Nloc, Nloc);
-        dfree(ctx, folded);
-        TRY(rc2);
+        TRY(lde_columns(ctx, folded.get(), M, gc, (int)logM, 0, c->sg, t.leaves + (size_t)g0 * Nloc, Nloc));
     }
     return GL_OK;
 }
@@ -568,18 +617,13 @@ static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem) {
     Tree& t = c->tree;
     const size_t Nloc = t.N;
     if (salt) {
-        u64* dsalt = nullptr;
-        const u64* sp = salt;
-        if (mem == GL_MEM_HOST) {
-            TRY(dmalloc(ctx, &dsalt, GL_SALT_SIZE * N));
-            TRY(h2d(ctx, dsalt, salt, GL_SALT_SIZE * N));
-            sp = dsalt;
-        }
+        DevBuf dsalt(ctx);
+        u64* sp;
+        TRY(device_in(ctx, salt, GL_SALT_SIZE * N, mem, dsalt, &sp));
         k_salt<<<(unsigned)((Nloc + 255) / 256), 256, 0, ctx->stream>>>(sp, N, c->degree_log + c->rate_bits,
                                                                        (size_t)c->shard_index * Nloc, Nloc, t.leaves,
                                                                        Nloc, c->B);
         CKL(ctx);
-        if (dsalt) dfree(ctx, dsalt);
     }
     TRY(tree_build(ctx, t));
     c->finished = true;
@@ -1258,18 +1302,91 @@ static int fri_finish_begin(gl_ctx* ctx, gl_fri* f) {
     // lde_final_poly / coset_fft (oracle.rs:215-220) on both F_{p^2} components, leaf-major W = 2
     const size_t n = (size_t)1 << f->log_n, N = n << f->rate_bits;
     TRY(dmalloc(ctx, &f->values, 2 * N));
-    u64* cols;
-    TRY(dmalloc(ctx, &cols, 2 * N));
-    int rc = lde_columns(ctx, f->coeff_cols, n, 2, (int)f->log_n, (int)f->rate_bits, MULTIPLICATIVE_GROUP_GENERATOR, cols, N);
-    if (rc == GL_OK) {  // (c0 column | c1 column) -> interleaved F_{p^2} values, the FRI leaves' layout
-        k_interleave<<<(unsigned)((N + 255) / 256), 256, 0, ctx->stream>>>(cols, N, N, f->values);
-        ctx->launches++;
-    }
-    dfree(ctx, cols);
-    TRY(rc);
+    DevBuf cols(ctx);
+    TRY(cols.alloc(2 * N));
+    TRY(lde_columns(ctx, f->coeff_cols, n, 2, (int)f->log_n, (int)f->rate_bits, MULTIPLICATIVE_GROUP_GENERATOR, cols.get(), N));
+    // (c0 column | c1 column) -> interleaved F_{p^2} values, the FRI leaves' layout
+    k_interleave<<<(unsigned)((N + 255) / 256), 256, 0, ctx->stream>>>(cols.get(), N, N, f->values);
+    CKL(ctx);
     f->log_cur = f->log_n + f->rate_bits;
     f->shift = MULTIPLICATIVE_GROUP_GENERATOR;
     return GL_OK;
+}
+
+// ---- set-up shared by the entry points below
+typedef std::unique_ptr<gl_commit, void (*)(gl_commit*)> CommitPtr;
+typedef std::unique_ptr<gl_fri, void (*)(gl_fri*)> FriPtr;
+// A handle that an entry point destroys on its error paths and releases to the caller on success
+static CommitPtr commit_new(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits, bool blinding,
+                            uint32_t shard_index, uint32_t shard_log) {
+    CommitPtr c(new gl_commit(), gl_commit_destroy);
+    c->ctx = ctx;
+    c->B = B;
+    c->W = B + (blinding ? GL_SALT_SIZE : 0);
+    c->degree_log = log_n;
+    c->rate_bits = rate_bits;
+    c->blinding = blinding;
+    c->shard_index = shard_index;
+    c->shard_log = shard_log;
+    return c;
+}
+static FriPtr fri_new(gl_ctx* ctx, uint32_t log_n, uint32_t rate_bits, uint32_t cap_height) {
+    FriPtr f(new gl_fri(), gl_fri_destroy);
+    f->ctx = ctx;
+    f->log_n = log_n;
+    f->rate_bits = rate_bits;
+    f->cap_height = cap_height;
+    return f;
+}
+
+// The powers w^i, i < size, as two tables of x_pow_table_len(size) entries: w^i = hi[i >> 12] * lo[i & 4095] with
+// hi = tabs, lo = tabs + x_pow_table_len(size)
+static size_t x_pow_table_len(size_t size) { return 4096 > (size >> 12) + 1 ? 4096 : (size >> 12) + 1; }
+static int x_pow_tables(gl_ctx* ctx, u64 w, size_t size, DevBuf& tabs) {
+    return build_pow_tables(ctx, std::vector<u64>{gl::pow(w, 4096), w}, x_pow_table_len(size), tabs);
+}
+
+// ZeroPolyOnCoset::new(degree_bits, qd_bits) (field/src/zero_poly_coset.rs:20-34): Z_H on the 2^qd_bits cosets and inverses
+static void zero_poly_coset(uint32_t degree_bits, uint32_t qd_bits, u64* zh, u64* zh_inv) {
+    u64 g_pow_n = MULTIPLICATIVE_GROUP_GENERATOR;
+    for (uint32_t k = 0; k < degree_bits; k++) g_pow_n = sqr(g_pow_n);
+    const u64 wq = root_of_unity(qd_bits);
+    u64 xq = 1;
+    for (uint32_t j = 0; j < (1u << qd_bits); j++, xq = mul(xq, wq)) {
+        zh[j] = canon(sub(mul(g_pow_n, xq), 1));
+        zh_inv[j] = canon(gl::inv(zh[j]));
+    }
+}
+
+// The error-flag word kernels atomicOr failure bits into: zeroed here, read back (synchronising) by flag_status
+static int flag_alloc(gl_ctx* ctx, DevBuf& flag) {
+    TRY(flag.alloc(1));
+    CK(ctx, cudaMemsetAsync(flag.get(), 0, 8, ctx->stream));
+    return GL_OK;
+}
+struct FlagError {
+    u64 bits;
+    int code;
+    const char* msg;
+};
+// GL_OK, or the status and message of the first entry whose bits the kernels set
+static int flag_status(gl_ctx* ctx, const DevBuf& flag, std::initializer_list<FlagError> errors) {
+    u64 v = 0;
+    TRY(d2h(ctx, &v, flag.get(), 1));
+    for (const FlagError& e : errors)
+        if (v & e.bits) return set_err(ctx, e.code, "%s", e.msg);
+    return GL_OK;
+}
+static const FlagError INVERT_ZERO = {1, GL_ERR_DIV_ZERO, "Tried to invert zero"};
+static const FlagError QUOTIENT_FAILED = {2, GL_ERR_BAD_ARG, "Quotient has failed, the vanishing polynomial is not divisible by Z_H"};
+
+// A constraint program (validated by the caller) and its constants on the device; no constants still get one word
+static int upload_program(gl_ctx* ctx, const void* prog, size_t prog_bytes, const u64* consts, uint32_t n_consts,
+                          DevBuf& dprog, DevBuf& dconst) {
+    TRY(dprog.alloc((prog_bytes + 7) / 8));
+    CK(ctx, cudaMemcpyAsync(dprog.get(), prog, prog_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    TRY(dconst.alloc(n_consts ? n_consts : 1));
+    return h2d(ctx, dconst.get(), consts, n_consts);
 }
 
 // =====================================================================================
@@ -1388,21 +1505,17 @@ int gl_ntt(gl_ctx* ctx, uint64_t* data, uint32_t log_n, uint32_t batch, size_t s
     if (batch > 1 && stride < n) return set_err(ctx, GL_ERR_BAD_SHAPE, "stride %zu < n %zu", stride, n);
     if (canon(coset_shift) == 0) return set_err(ctx, GL_ERR_BAD_ARG, "coset_shift must be non-zero");
     if (mem == GL_MEM_DEVICE) return ntt_natural(ctx, data, stride, data, stride, (int)log_n, batch, inverse != 0, coset_shift);
-    u64* d;
-    TRY(dmalloc(ctx, &d, (size_t)batch * n));
+    DevBuf d(ctx);
+    TRY(d.alloc((size_t)batch * n));
     const size_t pitch = (batch > 1 ? stride : n) * 8;  // one strided copy each way
-    int rc = GL_OK;
-    if (cudaMemcpy2DAsync(d, n * 8, data, pitch, n * 8, batch, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-        rc = set_err(ctx, GL_ERR_CUDA, "H2D: %s", cudaGetErrorString(cudaGetLastError()));
-    if (rc == GL_OK) rc = ntt_natural(ctx, d, n, d, n, (int)log_n, batch, inverse != 0, coset_shift);
-    if (rc == GL_OK) {
-        cudaError_t e = cudaMemcpy2DAsync(data, pitch, d, n * 8, n * 8, batch, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e != cudaSuccess) rc = set_err(ctx, GL_ERR_CUDA, "D2H: %s", cudaGetErrorString(e));
-        if (rc == GL_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
-            rc = set_err(ctx, GL_ERR_CUDA, "sync failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    dfree(ctx, d);
-    return rc;
+    if (cudaMemcpy2DAsync(d.get(), n * 8, data, pitch, n * 8, batch, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
+        return set_err(ctx, GL_ERR_CUDA, "H2D: %s", cudaGetErrorString(cudaGetLastError()));
+    TRY(ntt_natural(ctx, d.get(), n, d.get(), n, (int)log_n, batch, inverse != 0, coset_shift));
+    cudaError_t e = cudaMemcpy2DAsync(data, pitch, d.get(), n * 8, n * 8, batch, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e != cudaSuccess) return set_err(ctx, GL_ERR_CUDA, "D2H: %s", cudaGetErrorString(e));
+    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+        return set_err(ctx, GL_ERR_CUDA, "sync failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return GL_OK;
 }
 
 void* gl_ctx_stream(const gl_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
@@ -1493,21 +1606,9 @@ int gl_commit_begin(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits,
     uint32_t shard_log = 0;
     TRY(commit_check_shape(ctx, B, log_n, rate_bits, cap_height, shard_index, num_shards, &shard_log));
     CK(ctx, cudaSetDevice(ctx->device));
-    gl_commit* c = new gl_commit();
-    c->ctx = ctx;
-    c->B = B;
-    c->W = B + (blinding ? GL_SALT_SIZE : 0);
-    c->degree_log = log_n;
-    c->rate_bits = rate_bits;
-    c->blinding = blinding != 0;
-    c->shard_index = shard_index;
-    c->shard_log = shard_log;
-    int rc = commit_alloc(ctx, c, cap_height, coeff_storage);
-    if (rc != GL_OK) {
-        gl_commit_destroy(c);
-        return rc;
-    }
-    *out = c;
+    CommitPtr c = commit_new(ctx, B, log_n, rate_bits, blinding != 0, shard_index, shard_log);
+    TRY(commit_alloc(ctx, c.get(), cap_height, coeff_storage));
+    *out = c.release();
     return GL_OK;
 }
 int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, const uint64_t* cols, size_t col_stride,
@@ -1552,21 +1653,9 @@ int gl_commit_create_sharded(gl_ctx* ctx, const uint64_t* cols, size_t col_strid
     CK(ctx, cudaSetDevice(ctx->device));
     if (B > 1 && col_stride < ((size_t)1 << log_n))
         return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent (stride < n)");
-    gl_commit* c = new gl_commit();
-    c->ctx = ctx;
-    c->B = B;
-    c->W = B + (salt ? GL_SALT_SIZE : 0);
-    c->degree_log = log_n;
-    c->rate_bits = rate_bits;
-    c->blinding = salt != nullptr;
-    c->shard_index = shard_index;
-    c->shard_log = shard_log;
-    int rc = commit_build(ctx, c, cols, col_stride, salt, is_coeffs, mem, cap_height);
-    if (rc != GL_OK) {
-        gl_commit_destroy(c);
-        return rc;
-    }
-    *out = c;
+    CommitPtr c = commit_new(ctx, B, log_n, rate_bits, salt != nullptr, shard_index, shard_log);
+    TRY(commit_build(ctx, c.get(), cols, col_stride, salt, is_coeffs, mem, cap_height));
+    *out = c.release();
     return GL_OK;
 }
 void gl_commit_destroy(gl_commit* c) {
@@ -1599,20 +1688,17 @@ int gl_commit_leaves(gl_commit* c, size_t row_begin, size_t row_count, uint64_t*
     CK(ctx, cudaSetDevice(ctx->device));
     // the LDE is column-major on the device; the reference's row-major leaves are produced on demand, in slabs
     const size_t slab = ((size_t)1 << 27) / c->W + 1;  // ~1 GiB of staging at most
-    u64* stage = nullptr;
-    if (mem == GL_MEM_HOST) TRY(dmalloc(ctx, &stage, (row_count < slab ? row_count : slab) * c->W));
-    int rc = GL_OK;
-    for (size_t r0 = 0; r0 < row_count && rc == GL_OK; r0 += slab) {
+    DevBuf stage(ctx);
+    if (mem == GL_MEM_HOST) TRY(stage.alloc((row_count < slab ? row_count : slab) * c->W));
+    for (size_t r0 = 0; r0 < row_count; r0 += slab) {
         const size_t rows = row_count - r0 < slab ? row_count - r0 : slab;
-        u64* dst = mem == GL_MEM_HOST ? stage : out + r0 * c->W;
+        u64* dst = mem == GL_MEM_HOST ? stage.get() : out + r0 * c->W;
         k_rows_from_columns<<<dim3((unsigned)((rows + 31) / 32), (c->W + 31) / 32), dim3(32, 8), 0, ctx->stream>>>(
             c->tree.leaves, c->tree.es, row_begin + r0, rows, c->W, dst);
-        ctx->launches++;
-        if (cudaGetLastError() != cudaSuccess) rc = set_err(ctx, GL_ERR_CUDA, "k_rows_from_columns launch failed");
-        if (rc == GL_OK && mem == GL_MEM_HOST) rc = d2h(ctx, out + r0 * c->W, stage, rows * c->W);
+        CKL(ctx);
+        if (mem == GL_MEM_HOST) TRY(d2h(ctx, out + r0 * c->W, stage.get(), rows * c->W));
     }
-    dfree(ctx, stage);
-    return rc;
+    return GL_OK;
 }
 int gl_commit_digests(gl_commit* c, uint64_t* out, int mem) {
     NEED_FINISHED(c);
@@ -1641,34 +1727,8 @@ int gl_commit_open(gl_commit* c, const uint64_t* leaf_indices, size_t count, uin
     return tree_open(c->ctx, c->tree, leaf_indices, count, out_leaves, out_paths);
 }
 int gl_commit_eval_ext(gl_commit* c, const uint64_t point[2], uint64_t* out) {
-    gl_ctx* ctx = c->ctx;
-    if (!point || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
-    CK(ctx, cudaSetDevice(ctx->device));
-    const size_t n = (size_t)1 << c->degree_log;
-    const E2 z = {canon(point[0]), canon(point[1])};
-    const size_t hi_cnt = (n >> 12) + 1;
-    u64 *zhi = nullptr, *zlo = nullptr, *zt = nullptr, *dout = nullptr;
-    auto body = [&]() -> int {
-        TRY(dmalloc(ctx, &zhi, 2 * hi_cnt));
-        TRY(dmalloc(ctx, &zlo, 2 * 4096));
-        TRY(dmalloc(ctx, &zt, 2 * n));
-        TRY(dmalloc(ctx, &dout, 2 * (size_t)c->B));
-        k_fill_e2_pows<<<(unsigned)((hi_cnt + 127) / 128), 128, 0, ctx->stream>>>(e2_pow(z, 4096), hi_cnt, zhi);
-        CKL(ctx);
-        k_fill_e2_pows<<<32, 128, 0, ctx->stream>>>(z, 4096, zlo);
-        CKL(ctx);
-        k_e2_pow_table<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(zhi, zlo, n, zt);
-        CKL(ctx);
-        k_eval_ext<<<c->B, 256, 0, ctx->stream>>>(c->coeffs, n, n, zt, dout);
-        CKL(ctx);
-        return d2h(ctx, out, dout, 2 * (size_t)c->B);
-    };
-    int rc = body();
-    dfree(ctx, zhi);
-    dfree(ctx, zlo);
-    dfree(ctx, zt);
-    dfree(ctx, dout);
-    return rc;
+    const uint32_t point_index = 0;
+    return gl_openings(c->ctx, &c, &point_index, 1, point, 1, out, GL_MEM_HOST);
 }
 // OpeningSet::new / StarkOpeningSet::new (plonk/proof.rs:313-351, starky/src/proof.rs:221-260) in ONE call: every
 // polynomial of commits[i] evaluated at points[point_index[i]], results concatenated in request order, one D2H.
@@ -1686,44 +1746,36 @@ int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_in
         total += commits[i]->B;
     }
     const size_t n = (size_t)1 << max_log, hi_cnt = (n >> 12) + 1;
-    u64 *zhi = nullptr, *zlo = nullptr, *zt = nullptr, *dout = nullptr;
-    auto body = [&]() -> int {
-        TRY(dmalloc(ctx, &zhi, 2 * hi_cnt));
-        TRY(dmalloc(ctx, &zlo, 2 * 4096));
-        TRY(dmalloc(ctx, &zt, 2 * n));
-        if (mem == GL_MEM_HOST) TRY(dmalloc(ctx, &dout, 2 * total));
-        else dout = out;
-        for (size_t p = 0; p < n_points; p++) {  // one power table per distinct point, shared by every request at it
-            bool used = false;
-            for (size_t i = 0; i < n_evals; i++) used |= point_index[i] == p;
-            if (!used) continue;
-            const E2 z = {canon(points[2 * p]), canon(points[2 * p + 1])};
-            k_fill_e2_pows<<<(unsigned)((hi_cnt + 127) / 128), 128, 0, ctx->stream>>>(e2_pow(z, 4096), hi_cnt, zhi);
-            CKL(ctx);
-            k_fill_e2_pows<<<32, 128, 0, ctx->stream>>>(z, 4096, zlo);
-            CKL(ctx);
-            k_e2_pow_table<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(zhi, zlo, n, zt);
-            CKL(ctx);
-            size_t off = 0;
-            for (size_t i = 0; i < n_evals; i++) {
-                const gl_commit* c = commits[i];
-                if (point_index[i] == p) {
-                    const size_t nc = (size_t)1 << c->degree_log;
-                    k_eval_ext<<<c->B, 256, 0, ctx->stream>>>(c->coeffs, nc, nc, zt, dout + 2 * off);
-                    CKL(ctx);
-                }
-                off += c->B;
+    DevBuf zhi(ctx), zlo(ctx), zt(ctx), stage(ctx);
+    TRY(zhi.alloc(2 * hi_cnt));
+    TRY(zlo.alloc(2 * 4096));
+    TRY(zt.alloc(2 * n));
+    u64* dout;
+    TRY(device_out(out, 2 * total, mem, stage, &dout));
+    for (size_t p = 0; p < n_points; p++) {  // one power table per distinct point, shared by every request at it
+        bool used = false;
+        for (size_t i = 0; i < n_evals; i++) used |= point_index[i] == p;
+        if (!used) continue;
+        const E2 z = {canon(points[2 * p]), canon(points[2 * p + 1])};
+        k_fill_e2_pows<<<(unsigned)((hi_cnt + 127) / 128), 128, 0, ctx->stream>>>(e2_pow(z, 4096), hi_cnt, zhi.get());
+        CKL(ctx);
+        k_fill_e2_pows<<<32, 128, 0, ctx->stream>>>(z, 4096, zlo.get());
+        CKL(ctx);
+        k_e2_pow_table<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(zhi.get(), zlo.get(), n, zt.get());
+        CKL(ctx);
+        size_t off = 0;
+        for (size_t i = 0; i < n_evals; i++) {
+            const gl_commit* c = commits[i];
+            if (point_index[i] == p) {
+                const size_t nc = (size_t)1 << c->degree_log;
+                k_eval_ext<<<c->B, 256, 0, ctx->stream>>>(c->coeffs, nc, nc, zt.get(), dout + 2 * off);
+                CKL(ctx);
             }
+            off += c->B;
         }
-        if (mem == GL_MEM_HOST) return d2h(ctx, out, dout, 2 * total);
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, zhi);
-    dfree(ctx, zlo);
-    dfree(ctx, zt);
-    if (mem == GL_MEM_HOST) dfree(ctx, dout);
-    return rc;
+    }
+    if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, 2 * total));
+    return GL_OK;
 }
 const uint64_t* gl_commit_dev_lde(const gl_commit* c, size_t* col_stride) {
     if (col_stride) *col_stride = c->tree.es;
@@ -1742,56 +1794,30 @@ int gl_partial_products_and_zs(gl_ctx* ctx, const uint64_t* wires, const uint64_
     const size_t n = (size_t)1 << log_n;
     const uint32_t M = (num_routed + degree - 1) / degree;
     const size_t L = n * M, nchunks = (L + SCAN_CHUNK - 1) / SCAN_CHUNK;
-    u64 *dw = nullptr, *ds = nullptr, *dk = nullptr, *seq = nullptr, *tot = nullptr, *dout = nullptr, *dflag = nullptr;
-    u64* xtab = nullptr;
-    auto body = [&]() -> int {
-        const u64 *pw = wires, *ps = sigmas;
-        if (mem == GL_MEM_HOST) {
-            TRY(dmalloc(ctx, &dw, (size_t)num_routed * n));
-            TRY(dmalloc(ctx, &ds, (size_t)num_routed * n));
-            TRY(h2d(ctx, dw, wires, (size_t)num_routed * n));
-            TRY(h2d(ctx, ds, sigmas, (size_t)num_routed * n));
-            pw = dw;
-            ps = ds;
-            TRY(dmalloc(ctx, &dout, (size_t)M * n));
-        } else {
-            dout = out;
-        }
-        TRY(dmalloc(ctx, &dk, num_routed));
-        TRY(h2d(ctx, dk, k_is, num_routed));  // k_is is a small host array in both modes
-        TRY(dmalloc(ctx, &seq, L));
-        TRY(dmalloc(ctx, &tot, nchunks));
-        TRY(dmalloc(ctx, &dflag, 1));
-        CK(ctx, cudaMemsetAsync(dflag, 0, 8, ctx->stream));
-        const u64 wn = root_of_unity(log_n);
-        const size_t tcnt = 4096 > (n >> 12) + 1 ? 4096 : (n >> 12) + 1;
-        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(wn, 4096), wn}, tcnt, &xtab));
-        PPParams pp{pw, ps, dk, n, log_n, num_routed, degree, M, canon(beta), canon(gamma), xtab, xtab + tcnt, seq,
-                    (unsigned int*)dflag};
-        k_pp_chunks<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(pp);
-        CKL(ctx);
-        k_mscan_phase1<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq, L, tot);
-        CKL(ctx);
-        k_mscan_phase2<<<1, 1024, 0, ctx->stream>>>(tot, nchunks);
-        CKL(ctx);
-        k_mscan_phase3<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq, L, tot, n, M, dout);
-        CKL(ctx);
-        u64 flag = 0;
-        TRY(d2h(ctx, &flag, dflag, 1));
-        if (flag & 0xFFFFFFFFu) return set_err(ctx, GL_ERR_DIV_ZERO, "Tried to invert zero");
-        if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)M * n));
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, dw);
-    dfree(ctx, ds);
-    dfree(ctx, dk);
-    dfree(ctx, seq);
-    dfree(ctx, tot);
-    dfree(ctx, dflag);
-    dfree(ctx, xtab);
-    if (mem == GL_MEM_HOST) dfree(ctx, dout);
-    return rc;
+    DevBuf dw(ctx), ds(ctx), dout_stage(ctx), dk(ctx), seq(ctx), tot(ctx), dflag(ctx), xtab(ctx);
+    u64 *pw, *ps, *dout;
+    TRY(device_in(ctx, wires, (size_t)num_routed * n, mem, dw, &pw));
+    TRY(device_in(ctx, sigmas, (size_t)num_routed * n, mem, ds, &ps));
+    TRY(device_out(out, (size_t)M * n, mem, dout_stage, &dout));
+    TRY(dk.alloc(num_routed));
+    TRY(h2d(ctx, dk.get(), k_is, num_routed));  // k_is is a small host array in both modes
+    TRY(seq.alloc(L));
+    TRY(tot.alloc(nchunks));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(x_pow_tables(ctx, root_of_unity(log_n), n, xtab));
+    PPParams pp{pw, ps, dk.get(), n, log_n, num_routed, degree, M, canon(beta), canon(gamma), xtab.get(),
+                xtab.get() + x_pow_table_len(n), seq.get(), (unsigned int*)dflag.get()};
+    k_pp_chunks<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(pp);
+    CKL(ctx);
+    k_mscan_phase1<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq.get(), L, tot.get());
+    CKL(ctx);
+    k_mscan_phase2<<<1, 1024, 0, ctx->stream>>>(tot.get(), nchunks);
+    CKL(ctx);
+    k_mscan_phase3<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq.get(), L, tot.get(), n, M, dout);
+    CKL(ctx);
+    TRY(flag_status(ctx, dflag, {{0xFFFFFFFFu, GL_ERR_DIV_ZERO, "Tried to invert zero"}}));
+    if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)M * n));
+    return GL_OK;
 }
 
 int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t num_routed_wires,
@@ -1813,72 +1839,53 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
             return set_err(ctx, GL_ERR_BAD_ARG, "lookup rows %u: need last_lu <= last_lut <= first_lut < n - 1", k);
     }
     CK(ctx, cudaSetDevice(ctx->device));
-    u64 *dw = nullptr, *dout = nullptr, *term = nullptr, *reh = nullptr, *dflag = nullptr;
-    auto body = [&]() -> int {
-        const u64* pw = wires;
-        if (mem == GL_MEM_HOST) {
-            TRY(dmalloc(ctx, &dw, (size_t)num_wires_read * n));
-            TRY(h2d(ctx, dw, wires, (size_t)num_wires_read * n));
-            pw = dw;
-            TRY(dmalloc(ctx, &dout, (size_t)(P + 1) * n));
-        } else {
-            dout = out;
-        }
-        CK(ctx, cudaMemsetAsync(dout, 0, (size_t)(P + 1) * n * 8, ctx->stream));  // vec![F::ZERO; degree]
-        TRY(dmalloc(ctx, &dflag, 1));
-        CK(ctx, cudaMemsetAsync(dflag, 0, 8, ctx->stream));
-        u64 dL = 1;  // delta^num_lut_slots
-        for (uint32_t s = 0; s < num_lut_slots; s++) dL = mul(dL, canon(deltas[3]));
-        for (uint32_t k = 0; k < n_lookup_wires; k++) {
-            LookupParams p;
-            p.wires = pw;
-            p.n = n;
-            p.num_lu_slots = num_lu_slots;
-            p.num_lut_slots = num_lut_slots;
-            p.P = P;
-            p.max_lookup_degree = max_lookup_degree;
-            p.max_lookup_table_degree = max_lookup_table_degree;
-            p.dA = canon(deltas[0]);
-            p.dB = canon(deltas[1]);
-            p.dAlpha = canon(deltas[2]);
-            p.dDelta = canon(deltas[3]);
-            p.last_lu = lookup_rows[3 * k];
-            p.last_lut = lookup_rows[3 * k + 1];
-            p.first_lut = lookup_rows[3 * k + 2];
-            const uint32_t rows_lut = p.first_lut - p.last_lut + 1, T = rows_lut + (p.last_lut - p.last_lu);
-            dfree(ctx, term);
-            dfree(ctx, reh);
-            term = reh = nullptr;
-            TRY(dmalloc(ctx, &term, (size_t)T * P));
-            TRY(dmalloc(ctx, &reh, rows_lut));
-            p.term = term;
-            p.reh = reh;
-            p.flag = (unsigned int*)dflag;
-            k_lookup_terms<<<(T + 127) / 128, 128, 0, ctx->stream>>>(p);
-            CKL(ctx);
-            // initial values: the arrays' entries at first_lut_row + 1 (zero unless an earlier LookupWire wrote them)
-            u64 init[2];
-            CK(ctx, cudaMemcpyAsync(&init[0], dout + p.first_lut + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(ctx, cudaMemcpyAsync(&init[1], dout + (size_t)P * n + p.first_lut + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(ctx, cudaStreamSynchronize(ctx->stream));
-            k_affine_scan<<<1, 1024, 0, ctx->stream>>>(reh, rows_lut, dL, init[0], p, 1, dout);
-            CKL(ctx);
-            k_affine_scan<<<1, 1024, 0, ctx->stream>>>(term, (size_t)T * P, 1, init[1], p, 0, dout);
-            CKL(ctx);
-        }
-        u64 flag = 0;
-        TRY(d2h(ctx, &flag, dflag, 1));
-        if (flag & 1u) return set_err(ctx, GL_ERR_DIV_ZERO, "Tried to invert zero");
-        if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)(P + 1) * n));
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, dw);
-    dfree(ctx, term);
-    dfree(ctx, reh);
-    dfree(ctx, dflag);
-    if (mem == GL_MEM_HOST) dfree(ctx, dout);
-    return rc;
+    DevBuf dw(ctx), dout_stage(ctx), dflag(ctx), term(ctx), reh(ctx);
+    u64 *pw, *dout;
+    TRY(device_in(ctx, wires, (size_t)num_wires_read * n, mem, dw, &pw));
+    TRY(device_out(out, (size_t)(P + 1) * n, mem, dout_stage, &dout));
+    CK(ctx, cudaMemsetAsync(dout, 0, (size_t)(P + 1) * n * 8, ctx->stream));  // vec![F::ZERO; degree]
+    TRY(flag_alloc(ctx, dflag));
+    u64 dL = 1;  // delta^num_lut_slots
+    for (uint32_t s = 0; s < num_lut_slots; s++) dL = mul(dL, canon(deltas[3]));
+    for (uint32_t k = 0; k < n_lookup_wires; k++) {
+        LookupParams p;
+        p.wires = pw;
+        p.n = n;
+        p.num_lu_slots = num_lu_slots;
+        p.num_lut_slots = num_lut_slots;
+        p.P = P;
+        p.max_lookup_degree = max_lookup_degree;
+        p.max_lookup_table_degree = max_lookup_table_degree;
+        p.dA = canon(deltas[0]);
+        p.dB = canon(deltas[1]);
+        p.dAlpha = canon(deltas[2]);
+        p.dDelta = canon(deltas[3]);
+        p.last_lu = lookup_rows[3 * k];
+        p.last_lut = lookup_rows[3 * k + 1];
+        p.first_lut = lookup_rows[3 * k + 2];
+        const uint32_t rows_lut = p.first_lut - p.last_lut + 1, T = rows_lut + (p.last_lut - p.last_lu);
+        term.reset();  // both of the previous LookupWire's buffers go before either new one is allocated
+        reh.reset();
+        TRY(term.alloc((size_t)T * P));
+        TRY(reh.alloc(rows_lut));
+        p.term = term.get();
+        p.reh = reh.get();
+        p.flag = (unsigned int*)dflag.get();
+        k_lookup_terms<<<(T + 127) / 128, 128, 0, ctx->stream>>>(p);
+        CKL(ctx);
+        // initial values: the arrays' entries at first_lut_row + 1 (zero unless an earlier LookupWire wrote them)
+        u64 init[2];
+        CK(ctx, cudaMemcpyAsync(&init[0], dout + p.first_lut + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(ctx, cudaMemcpyAsync(&init[1], dout + (size_t)P * n + p.first_lut + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(ctx, cudaStreamSynchronize(ctx->stream));
+        k_affine_scan<<<1, 1024, 0, ctx->stream>>>(reh.get(), rows_lut, dL, init[0], p, 1, dout);
+        CKL(ctx);
+        k_affine_scan<<<1, 1024, 0, ctx->stream>>>(term.get(), (size_t)T * P, 1, init[1], p, 0, dout);
+        CKL(ctx);
+    }
+    TRY(flag_status(ctx, dflag, {INVERT_ZERO}));
+    if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)(P + 1) * n));
+    return GL_OK;
 }
 
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
@@ -1910,68 +1917,41 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
     CK(ctx, cudaSetDevice(ctx->device));
     const uint32_t db = trace->degree_log, size_log = db + qd_bits;
     const size_t size = (size_t)1 << size_log;
-    u64 *dprog = nullptr, *dconst = nullptr, *xtab = nullptr, *dflag = nullptr;
-    auto body = [&]() -> int {
-        const size_t prog_words = ((size_t)n_instr * sizeof(gl_stark_instr) + 7) / 8;
-        TRY(dmalloc(ctx, &dprog, prog_words));
-        CK(ctx, cudaMemcpyAsync(dprog, program, (size_t)n_instr * sizeof(gl_stark_instr), cudaMemcpyHostToDevice, ctx->stream));
-        TRY(dmalloc(ctx, &dconst, n_consts ? n_consts : 1));
-        if (n_consts) TRY(h2d(ctx, dconst, consts, n_consts));
-        TRY(dmalloc(ctx, &dflag, 1));
-        CK(ctx, cudaMemsetAsync(dflag, 0, 8, ctx->stream));
-        const u64 ws = root_of_unity(size_log);
-        const size_t tcnt = 4096 > (size >> 12) + 1 ? 4096 : (size >> 12) + 1;
-        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(ws, 4096), ws}, tcnt, &xtab));
-        StarkQuotientParams p;
-        p.lde = trace->tree.leaves;
-        p.lde_stride = trace->tree.es;
-        p.log_N = db + trace->rate_bits;
-        p.degree_bits = db;
-        p.qd_bits = qd_bits;
-        p.prog = (const gl_stark_instr*)dprog;
-        p.n_instr = n_instr;
-        p.consts = dconst;
-        p.n_alphas = n_alphas;
-        for (uint32_t a = 0; a < GL_STARK_MAX_ALPHAS; a++) p.alphas[a] = a < n_alphas ? canon(alphas[a]) : 0;
-        p.xhi = xtab;
-        p.xlo = xtab + tcnt;
-        p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
-        p.last = gl::inv(root_of_unity(db));
-        p.n_field = canon((u64)1 << db);
-        // ZeroPolyOnCoset::new(degree_bits, qd_bits) (field/src/zero_poly_coset.rs:20-34)
-        u64 g_pow_n = MULTIPLICATIVE_GROUP_GENERATOR;
-        for (uint32_t k = 0; k < db; k++) g_pow_n = sqr(g_pow_n);
-        const u64 wq = root_of_unity(qd_bits);
-        u64 xq = 1;
-        for (uint32_t j = 0; j < (1u << qd_bits); j++, xq = mul(xq, wq)) {
-            p.zh[j] = canon(sub(mul(g_pow_n, xq), 1));
-            p.zh_inv[j] = canon(gl::inv(p.zh[j]));
-        }
-        p.out = out_coeffs;
-        p.flag = (unsigned int*)dflag;
-        k_stark_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    DevBuf dprog(ctx), dconst(ctx), dflag(ctx), xtab(ctx);
+    TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_stark_instr), consts, n_consts, dprog, dconst));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(x_pow_tables(ctx, root_of_unity(size_log), size, xtab));
+    StarkQuotientParams p;
+    p.lde = trace->tree.leaves;
+    p.lde_stride = trace->tree.es;
+    p.log_N = db + trace->rate_bits;
+    p.degree_bits = db;
+    p.qd_bits = qd_bits;
+    p.prog = (const gl_stark_instr*)dprog.get();
+    p.n_instr = n_instr;
+    p.consts = dconst.get();
+    p.n_alphas = n_alphas;
+    for (uint32_t a = 0; a < GL_STARK_MAX_ALPHAS; a++) p.alphas[a] = a < n_alphas ? canon(alphas[a]) : 0;
+    p.xhi = xtab.get();
+    p.xlo = xtab.get() + x_pow_table_len(size);
+    p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
+    p.last = gl::inv(root_of_unity(db));
+    p.n_field = canon((u64)1 << db);
+    zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
+    p.out = out_coeffs;
+    p.flag = (unsigned int*)dflag.get();
+    k_stark_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    CKL(ctx);
+    // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:661-667)
+    TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
+    // trim_to_len(degree * quotient_degree_factor) (prover.rs:396-401): the rest must vanish
+    const size_t keep = ((size_t)quotient_degree_factor) << db;
+    if (keep < size) {
+        k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
+                                                                                               size - keep, (unsigned int*)dflag.get());
         CKL(ctx);
-        // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:661-667)
-        TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
-        // trim_to_len(degree * quotient_degree_factor) (prover.rs:396-401): the rest must vanish
-        const size_t keep = ((size_t)quotient_degree_factor) << db;
-        if (keep < size) {
-            k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
-                                                                                                   size - keep, (unsigned int*)dflag);
-            CKL(ctx);
-        }
-        u64 flag = 0;
-        TRY(d2h(ctx, &flag, dflag, 1));
-        if (flag & 1u) return set_err(ctx, GL_ERR_DIV_ZERO, "Tried to invert zero");
-        if (flag & 2u) return set_err(ctx, GL_ERR_BAD_ARG, "Quotient has failed, the vanishing polynomial is not divisible by Z_H");
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, dprog);
-    dfree(ctx, dconst);
-    dfree(ctx, xtab);
-    dfree(ctx, dflag);
-    return rc;
+    }
+    return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
 }
 
 int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
@@ -2019,79 +1999,51 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
     CK(ctx, cudaSetDevice(ctx->device));
     const uint32_t size_log = db + qd_bits;
     const size_t size = (size_t)1 << size_log;
-    u64 *dprog = nullptr, *dconst = nullptr, *dapow = nullptr, *xtab = nullptr, *dflag = nullptr;
-    auto body = [&]() -> int {
-        const size_t prog_words = ((size_t)n_instr * sizeof(gl_vp_instr) + 7) / 8;
-        TRY(dmalloc(ctx, &dprog, prog_words));
-        TRY(h2d(ctx, dprog, (const u64*)program, prog_words));
-        TRY(dmalloc(ctx, &dconst, n_consts ? n_consts : 1));
-        if (n_consts) TRY(h2d(ctx, dconst, consts, n_consts));
-        std::vector<u64> apow((size_t)n_alphas * n_terms);
-        for (uint32_t a = 0; a < n_alphas; a++) {
-            u64 pw = 1;
-            for (uint32_t t = 0; t < n_terms; t++, pw = mul(pw, alphas[a])) apow[(size_t)a * n_terms + t] = canon(pw);
-        }
-        TRY(dmalloc(ctx, &dapow, apow.size()));
-        TRY(h2d(ctx, dapow, apow.data(), apow.size()));
-        TRY(dmalloc(ctx, &dflag, 1));
-        CK(ctx, cudaMemsetAsync(dflag, 0, 8, ctx->stream));
-        const u64 ws = root_of_unity(size_log);
-        const size_t tcnt = 4096 > (size >> 12) + 1 ? 4096 : (size >> 12) + 1;
-        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(ws, 4096), ws}, tcnt, &xtab));
-        VanishingParams p;
-        for (uint32_t c = 0; c < GL_VP_MAX_COMMITS; c++) {
-            p.lde[c] = c < n_commits ? commits[c]->tree.leaves : nullptr;
-            p.lde_stride[c] = c < n_commits ? commits[c]->tree.es : 0;
-        }
-        p.log_N = db + rate_bits;
-        p.degree_bits = db;
-        p.qd_bits = qd_bits;
-        p.prog = (const gl_vp_instr*)dprog;
-        p.n_instr = n_instr;
-        p.consts = dconst;
-        p.apow = dapow;
-        p.n_alphas = n_alphas;
-        p.n_terms = n_terms;
-        p.xhi = xtab;
-        p.xlo = xtab + tcnt;
-        p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
-        p.n_field = canon((u64)1 << db);
-        // ZeroPolyOnCoset::new(degree_bits, qd_bits) (field/src/zero_poly_coset.rs:20-34)
-        u64 g_pow_n = MULTIPLICATIVE_GROUP_GENERATOR;
-        for (uint32_t k = 0; k < db; k++) g_pow_n = sqr(g_pow_n);
-        const u64 wq = root_of_unity(qd_bits);
-        u64 xq = 1;
-        for (uint32_t j = 0; j < GL_VP_MAX_QD; j++) p.zh[j] = p.zh_inv[j] = 0;
-        for (uint32_t j = 0; j < (1u << qd_bits); j++, xq = mul(xq, wq)) {
-            p.zh[j] = canon(sub(mul(g_pow_n, xq), 1));
-            p.zh_inv[j] = canon(gl::inv(p.zh[j]));
-        }
-        p.out = out_coeffs;
-        p.flag = (unsigned int*)dflag;
-        k_plonk_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    DevBuf dprog(ctx), dconst(ctx), dapow(ctx), dflag(ctx), xtab(ctx);
+    TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_vp_instr), consts, n_consts, dprog, dconst));
+    std::vector<u64> apow((size_t)n_alphas * n_terms);
+    for (uint32_t a = 0; a < n_alphas; a++) {
+        u64 pw = 1;
+        for (uint32_t t = 0; t < n_terms; t++, pw = mul(pw, alphas[a])) apow[(size_t)a * n_terms + t] = canon(pw);
+    }
+    TRY(dapow.alloc(apow.size()));
+    TRY(h2d(ctx, dapow.get(), apow.data(), apow.size()));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(x_pow_tables(ctx, root_of_unity(size_log), size, xtab));
+    VanishingParams p;
+    for (uint32_t c = 0; c < GL_VP_MAX_COMMITS; c++) {
+        p.lde[c] = c < n_commits ? commits[c]->tree.leaves : nullptr;
+        p.lde_stride[c] = c < n_commits ? commits[c]->tree.es : 0;
+    }
+    p.log_N = db + rate_bits;
+    p.degree_bits = db;
+    p.qd_bits = qd_bits;
+    p.prog = (const gl_vp_instr*)dprog.get();
+    p.n_instr = n_instr;
+    p.consts = dconst.get();
+    p.apow = dapow.get();
+    p.n_alphas = n_alphas;
+    p.n_terms = n_terms;
+    p.xhi = xtab.get();
+    p.xlo = xtab.get() + x_pow_table_len(size);
+    p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
+    p.n_field = canon((u64)1 << db);
+    for (uint32_t j = 0; j < GL_VP_MAX_QD; j++) p.zh[j] = p.zh_inv[j] = 0;
+    zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
+    p.out = out_coeffs;
+    p.flag = (unsigned int*)dflag.get();
+    k_plonk_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    CKL(ctx);
+    // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:811-814)
+    TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
+    // trim_to_len(quotient_degree) (prover.rs:327-331): the rest must vanish
+    const size_t keep = ((size_t)quotient_degree_factor) << db;
+    if (keep < size) {
+        k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
+                                                                                               size - keep, (unsigned int*)dflag.get());
         CKL(ctx);
-        // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:811-814)
-        TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
-        // trim_to_len(quotient_degree) (prover.rs:327-331): the rest must vanish
-        const size_t keep = ((size_t)quotient_degree_factor) << db;
-        if (keep < size) {
-            k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
-                                                                                                   size - keep, (unsigned int*)dflag);
-            CKL(ctx);
-        }
-        u64 flag = 0;
-        TRY(d2h(ctx, &flag, dflag, 1));  // synchronises: the host tables above outlive the copies
-        if (flag & 1u) return set_err(ctx, GL_ERR_DIV_ZERO, "Tried to invert zero");
-        if (flag & 2u) return set_err(ctx, GL_ERR_BAD_ARG, "Quotient has failed, the vanishing polynomial is not divisible by Z_H");
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, dprog);
-    dfree(ctx, dconst);
-    dfree(ctx, dapow);
-    dfree(ctx, xtab);
-    dfree(ctx, dflag);
-    return rc;
+    }
+    return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
 }
 
 void gl_poseidon_permute_host(uint64_t state[12]) {
@@ -2102,14 +2054,10 @@ void gl_poseidon_permute_host(uint64_t state[12]) {
 static int hash_many_impl(gl_ctx* ctx, const u64* in, size_t n_items, size_t in_words_per_item, u64* out, int mem,
                           int which, uint32_t W) {
     if (n_items == 0) return GL_OK;
-    const u64* din = in;
-    u64 *tin = nullptr, *dout = out;
-    if (mem == GL_MEM_HOST) {
-        TRY(dmalloc(ctx, &tin, n_items * in_words_per_item));
-        TRY(h2d(ctx, tin, in, n_items * in_words_per_item));
-        din = tin;
-        TRY(dmalloc(ctx, &dout, n_items * 4));
-    }
+    DevBuf tin(ctx), tout(ctx);
+    u64 *din, *dout;
+    TRY(device_in(ctx, in, n_items * in_words_per_item, mem, tin, &din));
+    TRY(device_out(out, n_items * 4, mem, tout, &dout));
     if (which == 0)
         k_hash_many<true><<<(unsigned)((n_items + 127) / 128), 128, 0, ctx->stream>>>(din, n_items, W, dout);
     else if (which == 2)
@@ -2117,12 +2065,7 @@ static int hash_many_impl(gl_ctx* ctx, const u64* in, size_t n_items, size_t in_
     else
         k_two_to_one_many<<<(unsigned)((n_items + 127) / 128), 128, 0, ctx->stream>>>(din, n_items, dout);
     CKL(ctx);
-    if (mem == GL_MEM_HOST) {
-        int rc = d2h(ctx, out, dout, n_items * 4);
-        dfree(ctx, tin);
-        dfree(ctx, dout);
-        return rc;
-    }
+    if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, n_items * 4));
     return GL_OK;
 }
 int gl_poseidon_hash_many(gl_ctx* ctx, const uint64_t* in, size_t n_items, uint32_t W, uint64_t* out, int mem) {
@@ -2145,23 +2088,13 @@ int gl_poseidon_permute_many(gl_ctx* ctx, uint64_t* states, size_t n_items, int 
     if (!ctx || !states) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     CK(ctx, cudaSetDevice(ctx->device));
     if (n_items == 0) return GL_OK;
-    u64* d = states;
-    if (mem == GL_MEM_HOST) {
-        TRY(dmalloc(ctx, &d, n_items * 12));
-        int rc = h2d(ctx, d, states, n_items * 12);
-        if (rc != GL_OK) {
-            dfree(ctx, d);
-            return rc;
-        }
-    }
+    DevBuf stage(ctx);
+    u64* d;
+    TRY(device_in(ctx, states, n_items * 12, mem, stage, &d));
     k_permute_many<<<(unsigned)((n_items + 127) / 128), 128, 0, ctx->stream>>>(d, n_items);
-    ctx->launches++;
-    int rc = cudaGetLastError() == cudaSuccess ? GL_OK : set_err(ctx, GL_ERR_CUDA, "k_permute_many launch failed");
-    if (mem == GL_MEM_HOST) {
-        if (rc == GL_OK) rc = d2h(ctx, states, d, n_items * 12);
-        dfree(ctx, d);
-    }
-    return rc;
+    CKL(ctx);
+    if (mem == GL_MEM_HOST) TRY(d2h(ctx, states, d, n_items * 12));
+    return GL_OK;
 }
 
 struct gl_merkle {
@@ -2177,25 +2110,17 @@ int gl_merkle_build(gl_ctx* ctx, const uint64_t* leaves, size_t N, uint32_t W, u
     if (log2_exact(N, &lg)) return set_err(ctx, GL_ERR_BAD_SHAPE, "Not a power of two: %zu", N);
     if (cap_height > lg)
         return set_err(ctx, GL_ERR_BAD_SHAPE, "cap_height=%u should be at most log2(leaves.len())=%u", cap_height, lg);
-    gl_merkle* m = new gl_merkle();
+    std::unique_ptr<gl_merkle, void (*)(gl_merkle*)> m(new gl_merkle(), gl_merkle_destroy);
     m->ctx = ctx;
     m->tree.N = N;
     m->tree.W = W;
     m->tree.cap_height = cap_height;
-    int rc = GL_OK;
-    if (mem == GL_MEM_HOST) {
-        m->tree.own_leaves = true;
-        rc = dmalloc(ctx, &m->tree.leaves, N * (size_t)W);
-        if (rc == GL_OK) rc = h2d(ctx, m->tree.leaves, leaves, N * (size_t)W);
-    } else {
-        m->tree.leaves = const_cast<u64*>(leaves);  // caller keeps the buffer alive
-    }
-    if (rc == GL_OK) rc = tree_build(ctx, m->tree);
-    if (rc != GL_OK) {
-        gl_merkle_destroy(m);
-        return rc;
-    }
-    *out = m;
+    DevBuf dleaves(ctx);  // GL_MEM_DEVICE: the caller keeps its buffer alive for the life of the tree
+    TRY(device_in(ctx, leaves, N * (size_t)W, mem, dleaves, &m->tree.leaves));
+    TRY(tree_build(ctx, m->tree));
+    m->tree.own_leaves = mem == GL_MEM_HOST;
+    dleaves.release();
+    *out = m.release();
     return GL_OK;
 }
 void gl_merkle_destroy(gl_merkle* m) {
@@ -2223,83 +2148,66 @@ int gl_fri_begin(gl_ctx* ctx, gl_commit* const* oracles, size_t n_oracles, const
     const size_t n = (size_t)1 << log_n;
     for (size_t o = 0; o < n_oracles; o++)
         if (oracles[o]->degree_log != log_n) return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent");
-    gl_fri* f = new gl_fri();
-    f->ctx = ctx;
-    f->log_n = log_n;
-    f->rate_bits = rate_bits;
-    f->cap_height = cap_height;
-    int rc = GL_OK;
-    u64 *comp = nullptr, *chunk = nullptr, *drefs = nullptr, *ztab = nullptr;
+    FriPtr f = fri_new(ctx, log_n, rate_bits, cap_height);
     const E2 alpha = {canon(alpha_in[0]), canon(alpha_in[1])};
     const size_t nchunks = (n + SCAN_CHUNK - 1) / SCAN_CHUNK;
     const size_t hi_cnt = (n >> 12) + 1;
-    auto body = [&]() -> int {
-        TRY(dmalloc(ctx, &f->coeff_cols, 2 * n));
-        TRY(dmalloc(ctx, &comp, 2 * n));
-        TRY(dmalloc(ctx, &chunk, 2 * nchunks));
-        // z / z^-1 power tables: [zhi | zlo | zihi | zilo], one allocation reused by every batch (stream-ordered)
-        TRY(dmalloc(ctx, &ztab, 2 * (2 * hi_cnt + 2 * 4096)));
-        u64 *zhi = ztab, *zlo = zhi + 2 * hi_cnt, *zihi = zlo + 2 * 4096, *zilo = zihi + 2 * hi_cnt;
-        // alpha^j per polynomial (ReducingFactor restarts at alpha^0 for every batch): the references of ALL batches
-        // go up in one copy (a pageable source is staged by the runtime before cudaMemcpyAsync returns)
-        size_t total_polys = 0;
-        for (size_t b = 0; b < n_batches; b++) total_polys += batches[b].num_polys;
-        std::vector<PolyRef> refs(total_polys);
-        std::vector<E2> shiftmuls(n_batches);
-        for (size_t b = 0, at = 0; b < n_batches; b++) {
-            const gl_fri_batch& batch = batches[b];
-            E2 ap = {1, 0};
-            for (size_t j = 0; j < batch.num_polys; j++, at++) {
-                const uint32_t oi = batch.oracle_index[j], pi = batch.poly_index[j];
-                if (oi >= n_oracles || pi >= oracles[oi]->B) return set_err(ctx, GL_ERR_BAD_ARG, "bad polynomial reference");
-                refs[at].ptr = oracles[oi]->coeffs + (size_t)pi * n;
-                refs[at].a0 = canon(ap.a);
-                refs[at].a1 = canon(ap.b);
-                ap = e2_mul(ap, alpha);
-            }
-            shiftmuls[b] = E2{canon(ap.a), canon(ap.b)};  // alpha^count: alpha.shift_poly (reducing.rs:102-106)
+    DevBuf comp(ctx), chunk(ctx), ztab(ctx), drefs(ctx);
+    TRY(dmalloc(ctx, &f->coeff_cols, 2 * n));
+    TRY(comp.alloc(2 * n));
+    TRY(chunk.alloc(2 * nchunks));
+    // z / z^-1 power tables: [zhi | zlo | zihi | zilo], one allocation reused by every batch (stream-ordered)
+    TRY(ztab.alloc(2 * (2 * hi_cnt + 2 * 4096)));
+    u64 *zhi = ztab.get(), *zlo = zhi + 2 * hi_cnt, *zihi = zlo + 2 * 4096, *zilo = zihi + 2 * hi_cnt;
+    // alpha^j per polynomial (ReducingFactor restarts at alpha^0 for every batch): the references of ALL batches
+    // go up in one copy (a pageable source is staged by the runtime before cudaMemcpyAsync returns)
+    size_t total_polys = 0;
+    for (size_t b = 0; b < n_batches; b++) total_polys += batches[b].num_polys;
+    std::vector<PolyRef> refs(total_polys);
+    std::vector<E2> shiftmuls(n_batches);
+    for (size_t b = 0, at = 0; b < n_batches; b++) {
+        const gl_fri_batch& batch = batches[b];
+        E2 ap = {1, 0};
+        for (size_t j = 0; j < batch.num_polys; j++, at++) {
+            const uint32_t oi = batch.oracle_index[j], pi = batch.poly_index[j];
+            if (oi >= n_oracles || pi >= oracles[oi]->B) return set_err(ctx, GL_ERR_BAD_ARG, "bad polynomial reference");
+            refs[at].ptr = oracles[oi]->coeffs + (size_t)pi * n;
+            refs[at].a0 = canon(ap.a);
+            refs[at].a1 = canon(ap.b);
+            ap = e2_mul(ap, alpha);
         }
-        const size_t ref_words = total_polys * sizeof(PolyRef) / 8;
-        TRY(dmalloc(ctx, &drefs, ref_words));
-        if (ref_words) TRY(h2d(ctx, drefs, (const u64*)refs.data(), ref_words));
-        for (size_t b = 0, at = 0; b < n_batches; at += batches[b].num_polys, b++) {
-            const gl_fri_batch& batch = batches[b];
-            const E2 shiftmul = shiftmuls[b];
-            k_fri_compose<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>((const PolyRef*)drefs + at,
-                                                                              (uint32_t)batch.num_polys, n, comp);
-            CKL(ctx);
-            const E2 z = {canon(batch.point[0]), canon(batch.point[1])};
-            if (z.a == 0 && z.b == 0) {
-                k_div_by_x<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(comp, n, shiftmul, b == 0, f->coeff_cols);
-                CKL(ctx);
-                continue;
-            }
-            const E2 zi = e2_inv(z);
-            E2Pows4 pw{{e2_pow(z, 4096), z, e2_pow(zi, 4096), zi}, {hi_cnt, 4096, hi_cnt, 4096}, {zhi, zlo, zihi, zilo}};
-            const size_t fill_total = 2 * hi_cnt + 2 * 4096;
-            k_fill_e2_pows4<<<(unsigned)((fill_total + 127) / 128), 128, 0, ctx->stream>>>(pw);
-            CKL(ctx);
-            k_scan_phase1<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(comp, n, zhi, zlo, chunk);
-            CKL(ctx);
-            k_scan_phase2<<<1, 1024, 0, ctx->stream>>>(chunk, nchunks);
-            CKL(ctx);
-            k_scan_phase3<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(comp, n, chunk, zihi, zilo, shiftmul,
-                                                                              b == 0, f->coeff_cols);
-            CKL(ctx);
-        }
-        TRY(fri_finish_begin(ctx, f));
-        return GL_OK;
-    };
-    rc = body();
-    dfree(ctx, comp);
-    dfree(ctx, chunk);
-    dfree(ctx, drefs);
-    dfree(ctx, ztab);
-    if (rc != GL_OK) {
-        gl_fri_destroy(f);
-        return rc;
+        shiftmuls[b] = E2{canon(ap.a), canon(ap.b)};  // alpha^count: alpha.shift_poly (reducing.rs:102-106)
     }
-    *out = f;
+    const size_t ref_words = total_polys * sizeof(PolyRef) / 8;
+    TRY(drefs.alloc(ref_words));
+    TRY(h2d(ctx, drefs.get(), (const u64*)refs.data(), ref_words));
+    for (size_t b = 0, at = 0; b < n_batches; at += batches[b].num_polys, b++) {
+        const gl_fri_batch& batch = batches[b];
+        const E2 shiftmul = shiftmuls[b];
+        k_fri_compose<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>((const PolyRef*)drefs.get() + at,
+                                                                          (uint32_t)batch.num_polys, n, comp.get());
+        CKL(ctx);
+        const E2 z = {canon(batch.point[0]), canon(batch.point[1])};
+        if (z.a == 0 && z.b == 0) {
+            k_div_by_x<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(comp.get(), n, shiftmul, b == 0, f->coeff_cols);
+            CKL(ctx);
+            continue;
+        }
+        const E2 zi = e2_inv(z);
+        E2Pows4 pw{{e2_pow(z, 4096), z, e2_pow(zi, 4096), zi}, {hi_cnt, 4096, hi_cnt, 4096}, {zhi, zlo, zihi, zilo}};
+        const size_t fill_total = 2 * hi_cnt + 2 * 4096;
+        k_fill_e2_pows4<<<(unsigned)((fill_total + 127) / 128), 128, 0, ctx->stream>>>(pw);
+        CKL(ctx);
+        k_scan_phase1<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(comp.get(), n, zhi, zlo, chunk.get());
+        CKL(ctx);
+        k_scan_phase2<<<1, 1024, 0, ctx->stream>>>(chunk.get(), nchunks);
+        CKL(ctx);
+        k_scan_phase3<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(comp.get(), n, chunk.get(), zihi, zilo, shiftmul,
+                                                                          b == 0, f->coeff_cols);
+        CKL(ctx);
+    }
+    TRY(fri_finish_begin(ctx, f.get()));
+    *out = f.release();
     return GL_OK;
 }
 
@@ -2368,78 +2276,58 @@ int gl_fri_begin_values(gl_ctx* ctx, gl_commit* const* oracles, size_t n_oracles
             return set_err(ctx, GL_ERR_BAD_SHAPE, "commitments are sharded differently");
     }
     if (c0->shard_log > cap_height) return set_err(ctx, GL_ERR_BAD_SHAPE, "more shards than cap entries");
-    gl_fri* f = new gl_fri();
-    f->ctx = ctx;
-    f->log_n = c0->degree_log;
-    f->rate_bits = c0->rate_bits;
-    f->cap_height = cap_height;
+    FriPtr f = fri_new(ctx, c0->degree_log, c0->rate_bits, cap_height);
     f->vshard_index = c0->shard_index;
     f->vshard_log = c0->shard_log;
     f->log_cur = c0->degree_log + c0->rate_bits;
     f->shift = MULTIPLICATIVE_GROUP_GENERATOR;
     const size_t rows = c0->tree.N;
     const E2 alpha = {canon(alpha_in[0]), canon(alpha_in[1])};
-    u64 *drefs = nullptr, *xtab = nullptr, *dflag = nullptr;
-    auto body = [&]() -> int {
-        size_t total = 0;
-        for (size_t b = 0; b < n_batches; b++) total += batches[b].num_polys;
-        std::vector<ValRef> refs(total);
-        ComposeValuesParams p;
-        p.n_batches = (uint32_t)n_batches;
-        for (size_t b = 0, at = 0; b < n_batches; b++) {
-            const gl_fri_batch& batch = batches[b];
-            E2 ap = {1, 0}, y = {0, 0};
-            p.batch[b].first = (uint32_t)at;
-            p.batch[b].count = (uint32_t)batch.num_polys;
-            for (size_t k = 0; k < batch.num_polys; k++, at++) {
-                const uint32_t oi = batch.oracle_index[k], pi = batch.poly_index[k];
-                if (oi >= n_oracles || pi >= oracles[oi]->B) return set_err(ctx, GL_ERR_BAD_ARG, "bad polynomial reference");
-                refs[at].col = oracles[oi]->tree.leaves + (size_t)pi * oracles[oi]->tree.es;
-                const E2 yv = {canon(opened[2 * at]), canon(opened[2 * at + 1])};
-                y = e2_add(y, e2_mul(ap, yv));
-                ap = e2_mul(ap, alpha);
-            }
-            p.batch[b].z = E2{canon(batch.point[0]), canon(batch.point[1])};
-            p.batch[b].y = E2{canon(y.a), canon(y.b)};
-            p.batch[b].shiftmul = E2{canon(ap.a), canon(ap.b)};
+    size_t total = 0;
+    for (size_t b = 0; b < n_batches; b++) total += batches[b].num_polys;
+    std::vector<ValRef> refs(total);
+    ComposeValuesParams p;
+    p.n_batches = (uint32_t)n_batches;
+    for (size_t b = 0, at = 0; b < n_batches; b++) {
+        const gl_fri_batch& batch = batches[b];
+        E2 ap = {1, 0}, y = {0, 0};
+        p.batch[b].first = (uint32_t)at;
+        p.batch[b].count = (uint32_t)batch.num_polys;
+        for (size_t k = 0; k < batch.num_polys; k++, at++) {
+            const uint32_t oi = batch.oracle_index[k], pi = batch.poly_index[k];
+            if (oi >= n_oracles || pi >= oracles[oi]->B) return set_err(ctx, GL_ERR_BAD_ARG, "bad polynomial reference");
+            refs[at].col = oracles[oi]->tree.leaves + (size_t)pi * oracles[oi]->tree.es;
+            const E2 yv = {canon(opened[2 * at]), canon(opened[2 * at + 1])};
+            y = e2_add(y, e2_mul(ap, yv));
+            ap = e2_mul(ap, alpha);
         }
-        const size_t ref_words = total * sizeof(ValRef) / 8;
-        TRY(dmalloc(ctx, &drefs, ref_words ? ref_words : 1));
-        if (ref_words) TRY(h2d(ctx, drefs, (const u64*)refs.data(), ref_words));
-        const uint32_t log_N = f->log_cur;
-        const size_t N = (size_t)1 << log_N;
-        const u64 wN = root_of_unity(log_N);
-        const size_t tcnt = 4096 > (N >> 12) + 1 ? 4096 : (N >> 12) + 1;
-        TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(wN, 4096), wN}, tcnt, &xtab));
-        TRY(dmalloc(ctx, &dflag, 1));
-        CK(ctx, cudaMemsetAsync(dflag, 0, 8, ctx->stream));
-        TRY(dmalloc(ctx, &f->values, 2 * rows));
-        p.refs = (const ValRef*)drefs;
-        p.rows = rows;
-        p.row0 = (size_t)c0->shard_index * rows;
-        p.log_N = log_N;
-        p.xhi = xtab;
-        p.xlo = xtab + tcnt;
-        p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
-        p.alpha = alpha;
-        p.out = f->values;
-        p.flag = (unsigned int*)dflag;
-        k_fri_compose_values<<<(unsigned)((rows + 127) / 128), 128, 0, ctx->stream>>>(p);
-        CKL(ctx);
-        u64 flag = 0;
-        TRY(d2h(ctx, &flag, dflag, 1));
-        if (flag & 1u) return set_err(ctx, GL_ERR_DIV_ZERO, "Opening point is in the LDE domain");
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, drefs);
-    dfree(ctx, xtab);
-    dfree(ctx, dflag);
-    if (rc != GL_OK) {
-        gl_fri_destroy(f);
-        return rc;
+        p.batch[b].z = E2{canon(batch.point[0]), canon(batch.point[1])};
+        p.batch[b].y = E2{canon(y.a), canon(y.b)};
+        p.batch[b].shiftmul = E2{canon(ap.a), canon(ap.b)};
     }
-    *out = f;
+    DevBuf drefs(ctx), xtab(ctx), dflag(ctx);
+    const size_t ref_words = total * sizeof(ValRef) / 8;
+    TRY(drefs.alloc(ref_words ? ref_words : 1));
+    TRY(h2d(ctx, drefs.get(), (const u64*)refs.data(), ref_words));
+    const uint32_t log_N = f->log_cur;
+    const size_t N = (size_t)1 << log_N;
+    TRY(x_pow_tables(ctx, root_of_unity(log_N), N, xtab));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(dmalloc(ctx, &f->values, 2 * rows));
+    p.refs = (const ValRef*)drefs.get();
+    p.rows = rows;
+    p.row0 = (size_t)c0->shard_index * rows;
+    p.log_N = log_N;
+    p.xhi = xtab.get();
+    p.xlo = xtab.get() + x_pow_table_len(N);
+    p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
+    p.alpha = alpha;
+    p.out = f->values;
+    p.flag = (unsigned int*)dflag.get();
+    k_fri_compose_values<<<(unsigned)((rows + 127) / 128), 128, 0, ctx->stream>>>(p);
+    CKL(ctx);
+    TRY(flag_status(ctx, dflag, {{1, GL_ERR_DIV_ZERO, "Opening point is in the LDE domain"}}));
+    *out = f.release();
     return GL_OK;
 }
 // the local block of the current codeword (between rounds): 2^(log_cur - shard_log) F_{p^2} values, bit-reversed order
@@ -2466,28 +2354,15 @@ int gl_fri_begin_from_coeffs(gl_ctx* ctx, const uint64_t* coeffs_ext, uint32_t l
     CK(ctx, cudaSetDevice(ctx->device));
     if (log_n > 3 * NTT_MAX_LOG_PASS) return set_err(ctx, GL_ERR_UNSUPPORTED, "log_n %u > 30", log_n);
     const size_t n = (size_t)1 << log_n;
-    gl_fri* f = new gl_fri();
-    f->ctx = ctx;
-    f->log_n = log_n;
-    f->rate_bits = rate_bits;
-    f->cap_height = cap_height;
-    u64* tmp = nullptr;
-    auto body = [&]() -> int {
-        TRY(dmalloc(ctx, &f->coeff_cols, 2 * n));
-        TRY(dmalloc(ctx, &tmp, 2 * n));
-        TRY(h2d(ctx, tmp, coeffs_ext, 2 * n));
-        k_split_ext<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(tmp, n, f->coeff_cols);
-        CKL(ctx);
-        TRY(fri_finish_begin(ctx, f));
-        return GL_OK;
-    };
-    int rc = body();
-    dfree(ctx, tmp);
-    if (rc != GL_OK) {
-        gl_fri_destroy(f);
-        return rc;
-    }
-    *out = f;
+    FriPtr f = fri_new(ctx, log_n, rate_bits, cap_height);
+    DevBuf tmp(ctx);
+    TRY(dmalloc(ctx, &f->coeff_cols, 2 * n));
+    TRY(tmp.alloc(2 * n));
+    TRY(h2d(ctx, tmp.get(), coeffs_ext, 2 * n));
+    k_split_ext<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(tmp.get(), n, f->coeff_cols);
+    CKL(ctx);
+    TRY(fri_finish_begin(ctx, f.get()));
+    *out = f.release();
     return GL_OK;
 }
 void gl_fri_destroy(gl_fri* f) {
@@ -2502,13 +2377,11 @@ int gl_fri_coeffs(gl_fri* f, uint64_t* out) {
     gl_ctx* ctx = f->ctx;
     if (!f->coeff_cols) return set_err(ctx, GL_ERR_BAD_ARG, "this FRI state was built in the value domain: no coefficients");
     const size_t n = (size_t)1 << f->log_n;
-    u64* tmp;
-    TRY(dmalloc(ctx, &tmp, 2 * n));
-    k_interleave<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(f->coeff_cols, n, n, tmp);
+    DevBuf tmp(ctx);
+    TRY(tmp.alloc(2 * n));
+    k_interleave<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(f->coeff_cols, n, n, tmp.get());
     CKL(ctx);
-    int rc = d2h(ctx, out, tmp, 2 * n);
-    dfree(ctx, tmp);
-    return rc;
+    return d2h(ctx, out, tmp.get(), 2 * n);
 }
 uint32_t gl_fri_num_rounds(const gl_fri* f) { return (uint32_t)f->trees.size(); }
 
@@ -2570,30 +2443,23 @@ int gl_fri_fold(gl_fri* f, const uint64_t beta[2]) {
     if (!f->committed) return set_err(ctx, GL_ERR_BAD_ARG, "commit the round first");
     const uint32_t ab = f->pending_arity_bits;
     const size_t leaves = f->round_leaves;
-    u64* out;
-    TRY(dmalloc(ctx, &out, 2 * leaves));
+    DevBuf out(ctx);
+    TRY(out.alloc(2 * leaves));
     FoldParams fp{};
     fp.values = f->round_values;
-    fp.out = out;
+    fp.out = out.get();
     fp.n_leaves = leaves;
     fp.leaf0 = (size_t)f->vshard_index * leaves;
     fp.log_leaves = f->log_cur - ab;
-    const u64 wN = root_of_unity(f->log_cur);
-    const u64 winv = gl::inv(wN);
-    const size_t hi_cnt = ((size_t)1 << (f->log_cur > 12 ? f->log_cur - 12 : 0)) + 1;  // covers any arity
-    const size_t tcnt = hi_cnt > 4096 ? hi_cnt : 4096;
-    u64* tabs;
-    {
-        auto it = ctx->fold_tabs.find((int)f->log_cur);
-        if (it == ctx->fold_tabs.end()) {
-            TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(winv, 4096), winv}, tcnt, &tabs));
-            ctx->fold_tabs[(int)f->log_cur] = tabs;
-        } else {
-            tabs = it->second;
-        }
+    const size_t N = (size_t)1 << f->log_cur;  // w_N^-i for every i < N covers any arity
+    auto it = ctx->fold_tabs.find((int)f->log_cur);
+    if (it == ctx->fold_tabs.end()) {
+        DevBuf tabs(ctx);
+        TRY(x_pow_tables(ctx, gl::inv(root_of_unity(f->log_cur)), N, tabs));
+        it = ctx->fold_tabs.emplace((int)f->log_cur, tabs.release()).first;
     }
-    fp.winv_hi = tabs;
-    fp.winv_lo = tabs + tcnt;
+    fp.winv_hi = it->second;
+    fp.winv_lo = it->second + x_pow_table_len(N);
     fp.shift_inv = gl::inv(f->shift);
     fp.beta0 = canon(beta[0]);
     fp.beta1 = canon(beta[1]);
@@ -2609,7 +2475,7 @@ int gl_fri_fold(gl_fri* f, const uint64_t beta[2]) {
         case 5: k_fri_fold<5><<<nb, 128, 0, ctx->stream>>>(fp); break;
     }
     CKL(ctx);
-    f->values = out;
+    f->values = out.release();
     f->log_cur -= ab;
     f->shift = gl::pow(f->shift, (u64)1 << ab);  // shift = shift.exp_u64(arity), prover.rs:118
     f->committed = false;
@@ -2650,22 +2516,18 @@ int gl_fri_final_poly(gl_fri* f, uint64_t* out, size_t cap_words, size_t* len_ou
     if (f->log_cur < f->rate_bits) return set_err(ctx, GL_ERR_BAD_SHAPE, "codeword shorter than the blowup");
     const size_t len = Nf >> f->rate_bits;
     if (cap_words < 2 * len) return set_err(ctx, GL_ERR_BAD_ARG, "output buffer too small");
-    u64 *cols, *inter;
-    TRY(dmalloc(ctx, &cols, 2 * Nf));
-    TRY(dmalloc(ctx, &inter, 2 * len));
-    k_unbitrev_split<<<(unsigned)((Nf + 255) / 256), 256, 0, ctx->stream>>>(f->values, Nf, f->log_cur, cols);
+    DevBuf cols(ctx), inter(ctx);
+    TRY(cols.alloc(2 * Nf));
+    TRY(inter.alloc(2 * len));
+    k_unbitrev_split<<<(unsigned)((Nf + 255) / 256), 256, 0, ctx->stream>>>(f->values, Nf, f->log_cur, cols.get());
     CKL(ctx);
     // coset_ifft on the current coset (the reference keeps coefficients; we recover them once)
-    int rc = ntt_natural(ctx, cols, Nf, cols, Nf, (int)f->log_cur, 2, true, f->shift);
-    if (rc == GL_OK) {
-        k_interleave<<<(unsigned)((len + 255) / 256), 256, 0, ctx->stream>>>(cols, Nf, len, inter);
-        ctx->launches++;
-        rc = d2h(ctx, out, inter, 2 * len);
-    }
-    dfree(ctx, cols);
-    dfree(ctx, inter);
-    if (rc == GL_OK && len_out) *len_out = len;
-    return rc;
+    TRY(ntt_natural(ctx, cols.get(), Nf, cols.get(), Nf, (int)f->log_cur, 2, true, f->shift));
+    k_interleave<<<(unsigned)((len + 255) / 256), 256, 0, ctx->stream>>>(cols.get(), Nf, len, inter.get());
+    CKL(ctx);
+    TRY(d2h(ctx, out, inter.get(), 2 * len));
+    if (len_out) *len_out = len;
+    return GL_OK;
 }
 
 int gl_fri_open(gl_fri* f, uint32_t round, const uint64_t* leaf_indices, size_t count, uint64_t* out_leaves,
@@ -2678,8 +2540,8 @@ int gl_fri_open(gl_fri* f, uint32_t round, const uint64_t* leaf_indices, size_t 
 int gl_fri_pow(gl_ctx* ctx, const uint64_t state[12], uint32_t pos, uint32_t min_leading_zeros, uint64_t* nonce_out) {
     if (!ctx || !state || !nonce_out || pos >= 8) return set_err(ctx, GL_ERR_BAD_ARG, "bad argument");
     CK(ctx, cudaSetDevice(ctx->device));
-    unsigned long long* dres;
-    TRY(dmalloc(ctx, (u64**)&dres, 1));
+    DevBuf dres(ctx);
+    TRY(dres.alloc(1));
     PowParams pp;
     for (int i = 0; i < 12; i++) pp.state[i] = canon(state[i]);
     pp.pos = pos;
@@ -2688,33 +2550,22 @@ int gl_fri_pow(gl_ctx* ctx, const uint64_t state[12], uint32_t pos, uint32_t min
     // small launch; candidates are scanned in increasing order, so the first hit batch holds the minimum.
     u64 batch = (u64)2 << (min_leading_zeros < 24 ? min_leading_zeros : 24);
     if (batch < 4096) batch = 4096;
-    int rc = GL_OK;
     u64 found = ~0ULL;
     for (u64 start = 0; start < P; start += batch, batch = batch < ((u64)1 << 24) ? batch * 4 : batch) {
-        if (cudaMemsetAsync(dres, 0xFF, 8, ctx->stream) != cudaSuccess) {
-            rc = set_err(ctx, GL_ERR_CUDA, "cudaMemsetAsync failed: %s", cudaGetErrorString(cudaGetLastError()));
-            break;
-        }
+        if (cudaMemsetAsync(dres.get(), 0xFF, 8, ctx->stream) != cudaSuccess)
+            return set_err(ctx, GL_ERR_CUDA, "cudaMemsetAsync failed: %s", cudaGetErrorString(cudaGetLastError()));
         pp.start = start;
         pp.count = (P - start < batch) ? P - start : batch;
         const u64 nb_max = (u64)ctx->sm_count * 8;
         const unsigned nb = (unsigned)((pp.count + 127) / 128 < nb_max ? (pp.count + 127) / 128 : nb_max);
-        k_fri_pow<<<nb, 128, 0, ctx->stream>>>(pp, dres);
-        ctx->launches++;
-        if (cudaGetLastError() != cudaSuccess) {
-            rc = set_err(ctx, GL_ERR_CUDA, "k_fri_pow launch failed");
-            break;
-        }
-        rc = d2h(ctx, &found, (u64*)dres, 1);
-        if (rc != GL_OK || found != ~0ULL) break;
-        if (start > ((u64)1 << 40)) {
-            rc = set_err(ctx, GL_ERR_POW_FAILED, "Proof of work failed. This is highly unlikely!");
-            break;
-        }
+        k_fri_pow<<<nb, 128, 0, ctx->stream>>>(pp, (unsigned long long*)dres.get());
+        CKL(ctx);
+        TRY(d2h(ctx, &found, dres.get(), 1));
+        if (found != ~0ULL) break;
+        if (start > ((u64)1 << 40)) return set_err(ctx, GL_ERR_POW_FAILED, "Proof of work failed. This is highly unlikely!");
     }
-    dfree(ctx, (u64*)dres);
-    if (rc == GL_OK) *nonce_out = found;
-    return rc;
+    *nonce_out = found;
+    return GL_OK;
 }
 
 }  // extern "C"
