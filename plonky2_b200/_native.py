@@ -162,8 +162,27 @@ def np_ptr(a):
     return a.ctypes.data_as(vp)
 
 
-class Context:
+class Handle:
+    """Owner of one library handle `h`, destroyed by the library function named `destroyer`. close() is idempotent;
+    collecting the object closes it too."""
+    destroyer = None
+    h = None
+
+    def close(self):
+        if self.h:
+            getattr(lib(), self.destroyer)(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Context(Handle):
     """One gl_ctx per (device, stream) (SURVEY.md section 8b, threading row)."""
+    destroyer = "gl_ctx_destroy"
 
     def __init__(self, device=0, stream=None):
         h = vp()
@@ -202,17 +221,6 @@ class Context:
             check(lib().gl_ctx_phase_ms(self.h, pid, C.byref(ms), C.byref(cnt)), self.h)
             out[name] = (ms.value, cnt.value)
         return out
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().gl_ctx_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 _default_ctx = {}

@@ -4,16 +4,15 @@ them, the lower-degree instances being mixed into the folded codeword when it re
 
 Device path: every degree group is a PolynomialBatch (coefficients and LDE stay on the device); the batch tree's first
 stage IS the tallest group's own Merkle tree built to the height of the next group, later stages hash `previous cap ||
-group rows`; every instance's composed polynomial comes from gl_fri_begin, the rounds are gl_fri_commit_round /
-gl_fri_fold plus gl_fri_mix at the mixing points."""
-import ctypes as C
-
+group rows`; every instance's composed polynomial comes from gl_fri_begin, and the rounds are fri.fri_committed_trees
+with the lower-degree instances mixed in at their LDE sizes."""
 import numpy as np
 
 from . import _native as N
 from . import fri as F
+from .batch_merkle_tree import _stage_chain
 from .field import log2_strict
-from .hash import MerkleCap, MerkleProof, MerkleTree
+from .hash import NUM_HASH_OUT_ELTS, MerkleProof
 from .polynomial_batch import PolynomialBatch
 
 
@@ -26,19 +25,10 @@ class BatchFriOracle:
         self.blinding = False
         heights = [d + rate_bits for d in degree_bits]
         self.leaf_heights = heights
-        self.stages = []
-        cap = None
-        for k, g in enumerate(groups):
-            nxt = heights[k + 1] if k + 1 < len(groups) else cap_height
-            if k == 0:
-                self.stages.append(g)       # the tallest group's own tree, built with cap height = next stage's height
-                cap = g.merkle_tree.cap.hashes
-            else:
-                rows = g.merkle_tree.get_rows(0, 1 << heights[k])
-                t = MerkleTree(np.ascontiguousarray(np.concatenate([cap, rows], axis=1)), nxt, ctx)
-                self.stages.append(t)
-                cap = t.cap.hashes
-        self.cap = MerkleCap(cap)
+        # stage 0 is the tallest group's own tree, built with cap height = next stage's height; the later groups' rows
+        # are read back as their stage is built
+        rows = (g.merkle_tree.get_rows(0, 1 << h) for g, h in zip(groups[1:], heights[1:]))
+        self.stages, self.cap = _stage_chain(groups[0].merkle_tree, rows, heights, cap_height, ctx)
 
     @classmethod
     def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None):
@@ -87,12 +77,22 @@ class BatchFriOracle:
 
     def open_batch(self, leaf_index):
         """BatchMerkleTree::open_batch (batch_merkle_tree.rs:131-152)."""
+        return MerkleProof(self.open_many([leaf_index])[1][0])
+
+    @property
+    def merkle_tree(self):
+        """The initial-tree view fri_prover_query_rounds opens (open_many)."""
+        return self
+
+    def open_many(self, indices):
+        """For leaf indices of the tallest matrix, one opening per stage: (per index, `values` back to back (q, W);
+        per index, `open_batch` siblings (q, L, 4))."""
+        idx = np.asarray(indices, dtype=np.uint64)
         h0 = self.leaf_heights[0]
-        sib = []
-        for k, (st, hk) in enumerate(zip(self.stages, self.leaf_heights)):
-            idx = leaf_index >> (h0 - hk)
-            sib.append((st.merkle_tree if k == 0 else st).open_many([idx])[1][0])
-        return MerkleProof(np.concatenate(sib) if sib else np.zeros((0, 4), dtype=np.uint64))
+        opened = [st.open_many(idx >> np.uint64(h0 - hk)) for st, hk in zip(self.stages, self.leaf_heights)]
+        # a later stage's leaf is `previous cap digest || the group's row`
+        rows = [lv if k == 0 else lv[:, NUM_HASH_OUT_ELTS:] for k, (lv, _) in enumerate(opened)]
+        return np.concatenate(rows, axis=1), np.concatenate([pt for _, pt in opened], axis=1)
 
     def get_lde_values(self, degree_bits_index, index, step, slice_start, slice_len):
         """get_lde_values (oracle.rs:186-199)."""
@@ -109,10 +109,9 @@ def batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params
     """BatchFriOracle::prove_openings + batch_fri_proof (oracle.rs:124-183, prover.rs:30-147). instances[i] opens the
     polynomials of degree 2^degree_bits[i]; polynomial indices are indices into each oracle's full polynomial list."""
     assert len(degree_bits) == len(instances)
-    L = N.lib()
     ctx = oracles[0].ctx
     alpha = challenger.get_extension_challenge()
-    states = []
+    states, params = [], []
     try:
         for db, inst in zip(degree_bits, instances):
             # the polynomials of this instance live in the degree-`db` group of their oracle
@@ -129,52 +128,14 @@ def batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params
                     polys.append(F.FriPolynomialInfo(index_of[p.oracle_index], j))
                 group_batches.append(F.FriBatchInfo(b.point, polys))
             sub = F.FriInstanceInfo([F.FriOracleInfo(h.num_polys, False) for h in handles], group_batches)
-            params_i = F.FriParams(fri_params.config, fri_params.hiding, db, fri_params.reduction_arity_bits)
-            states.append(F._begin(sub, handles, alpha, params_i))
-        # batch_fri_committed_trees (prover.rs:88-147)
-        main = states[0]
-        cap_words = 4 << fri_params.config.cap_height
-        caps, nxt = [], 1
-        log_cur = degree_bits[0] + fri_params.config.rate_bits
-        for arity_bits in fri_params.reduction_arity_bits:
-            cap = np.empty(cap_words, dtype=np.uint64)
-            N.check(L.gl_fri_commit_round(main.h, arity_bits, N.np_ptr(cap)), ctx.h)
-            cap = MerkleCap(cap)
-            challenger.observe_cap(cap)
-            caps.append(cap)
-            beta = challenger.get_extension_challenge()
-            b = np.array(beta, dtype=np.uint64)
-            N.check(L.gl_fri_fold(main.h, N.np_ptr(b)), ctx.h)
-            log_cur -= arity_bits
-            if nxt < len(states) and log_cur == degree_bits[nxt] + fri_params.config.rate_bits:
-                N.check(L.gl_fri_mix(main.h, states[nxt].h, N.np_ptr(b)), ctx.h)
-                nxt += 1
-        assert nxt == len(states), "reduction_arity_bits must pass through every instance's LDE size (prover.rs:44-57)"
-        n_final = 1 << (log_cur - fri_params.config.rate_bits)
-        buf = np.empty(2 * max(n_final, 1), dtype=np.uint64)
-        ln = C.c_size_t()
-        N.check(L.gl_fri_final_poly(main.h, N.np_ptr(buf), buf.size, C.byref(ln)), ctx.h)
-        final = buf[:2 * ln.value].reshape(-1, 2).copy()
-        challenger.observe_extension_elements([(int(c[0]), int(c[1])) for c in final])
+            params.append(F.FriParams(fri_params.config, fri_params.hiding, db, fri_params.reduction_arity_bits))
+            states.append(F._begin(sub, handles, alpha, params[-1]))
+        # batch_fri_committed_trees (prover.rs:88-147) and batch_fri_prover_query_rounds (prover.rs:149-215)
+        rate_bits = fri_params.config.rate_bits
+        mixes = [(db + rate_bits, st) for db, st in zip(degree_bits[1:], states[1:])]
+        caps, final = F.fri_committed_trees(states[0], challenger, params[0], mixes=mixes)
         pow_witness = F.fri_proof_of_work(challenger, fri_params.config, ctx)
-        # batch_fri_prover_query_rounds (prover.rs:149-215)
-        n = 1 << (degree_bits[0] + fri_params.config.rate_bits)
-        nq = fri_params.config.num_query_rounds
-        x_indices = [c % n for c in challenger.get_n_challenges(nq)]
-        rounds = []
-        for x in x_indices:
-            init = F.FriInitialTreeProof([(np.concatenate(o.values(x)), o.open_batch(x).siblings) for o in oracles])
-            steps, xi, lc = [], x, degree_bits[0] + fri_params.config.rate_bits
-            for r, arity_bits in enumerate(fri_params.reduction_arity_bits):
-                xi >>= arity_bits
-                layers = lc - arity_bits - fri_params.config.cap_height
-                leaf = np.empty((1, 2 << arity_bits), dtype=np.uint64)
-                path = np.empty((1, layers, 4), dtype=np.uint64)
-                idx = np.array([xi], dtype=np.uint64)
-                N.check(L.gl_fri_open(main.h, r, N.np_ptr(idx), 1, N.np_ptr(leaf), N.np_ptr(path) if path.size else None), ctx.h)
-                steps.append(F.FriQueryStep(leaf[0].reshape(-1, 2), path[0]))
-                lc -= arity_bits
-            rounds.append(F.FriQueryRound(init, steps))
+        rounds, _ = F.fri_prover_query_rounds(oracles, states[0], challenger, params[0].lde_size(), params[0])
         return F.FriProof(caps, rounds, final, pow_witness)
     finally:
         for st in states:

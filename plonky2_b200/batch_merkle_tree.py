@@ -25,15 +25,8 @@ class BatchMerkleTree:
         if cap_height > heights[-1]:
             raise N.ShapeError("cap_height=%d should be at most last_leaves_cap_height=%d" % (cap_height, heights[-1]))
         self.leaves, self.leaf_heights, self.cap_height = leaves, heights, cap_height
-        self.stages = []
-        cap = None
-        for k, m in enumerate(leaves):
-            next_height = heights[k + 1] if k + 1 < len(leaves) else cap_height
-            rows = m if cap is None else np.ascontiguousarray(np.concatenate([cap, m], axis=1))  # cap_hash || cur[i]
-            t = MerkleTree(rows, next_height, self.ctx)
-            self.stages.append(t)
-            cap = t.cap.hashes
-        self.cap = MerkleCap(cap)
+        first = MerkleTree(leaves[0], heights[1] if len(leaves) > 1 else cap_height, self.ctx)
+        self.stages, self.cap = _stage_chain(first, leaves[1:], heights, cap_height, self.ctx)
 
     @property
     def digests(self):
@@ -55,6 +48,20 @@ class BatchMerkleTree:
     def close(self):
         for t in self.stages:
             t.close()
+
+
+def _stage_chain(first, later, heights, cap_height, ctx):
+    """The stages of a batch tree whose matrices have leaf heights `heights`: `first` is stage 0 (any tree with a
+    `cap`), stage k >= 1 hashes the rows `previous stage's cap digest || later[k - 1][i]` (cap_hash || cur[i]) up to
+    the height of the next matrix, or to cap_height after the last. `later` is read one matrix per stage, so it may be
+    a generator. Returns (stages, the batch tree's cap)."""
+    stages, cap = [first], first.cap.hashes
+    for k, m in enumerate(later, 1):
+        t = MerkleTree(np.ascontiguousarray(np.concatenate([cap, m], axis=1)),
+                       heights[k + 1] if k + 1 < len(heights) else cap_height, ctx)
+        stages.append(t)
+        cap = t.cap.hashes
+    return stages, MerkleCap(cap)
 
 
 def verify_batch_merkle_proof_to_cap(leaf_data, leaf_heights, leaf_index, merkle_cap, proof, ctx=None):

@@ -365,26 +365,18 @@ def fri_challenges(challenger, commit_phase_merkle_caps, final_poly, pow_witness
 
 
 # ------------------------------------------------------------------ prover
-class _FriState:
-    """Owner of a gl_fri handle."""
+class _FriState(N.Handle):
+    """Owner of a gl_fri handle. value_sharded = (shard, num_shards) when the codeword is row-block sharded
+    (_begin_values)."""
+    destroyer = "gl_fri_destroy"
 
-    def __init__(self, h, ctx):
-        self.h, self.ctx = h, ctx
-
-    def close(self):
-        if getattr(self, "h", None):
-            N.lib().gl_fri_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def __init__(self, h, ctx, value_sharded=None):
+        self.h, self.ctx, self.value_sharded = h, ctx, value_sharded
 
 
-def _begin(instance, oracles, alpha, fri_params):
-    ctx = oracles[0].ctx
+def _fri_batches(instance, oracles):
+    """The gl_fri_begin* inputs of an instance: the oracles' handle array, the FriBatch array and the index arrays the
+    batches point into (keep them alive until the call returns)."""
     handles = (N.vp * len(oracles))(*[o.h for o in oracles])
     barr = (N.FriBatch * len(instance.batches))()
     keep = []
@@ -396,6 +388,12 @@ def _begin(instance, oracles, alpha, fri_params):
         barr[i].num_polys = len(b.polynomials)
         barr[i].oracle_index = oi.ctypes.data_as(N.u32p)
         barr[i].poly_index = pi.ctypes.data_as(N.u32p)
+    return handles, barr, keep
+
+
+def _begin(instance, oracles, alpha, fri_params):
+    ctx = oracles[0].ctx
+    handles, barr, keep = _fri_batches(instance, oracles)
     al = np.array([alpha[0], alpha[1]], dtype=np.uint64)
     h = N.vp()
     N.check(N.lib().gl_fri_begin(ctx.h, handles, len(oracles), barr, len(instance.batches), N.np_ptr(al),
@@ -408,26 +406,14 @@ def _begin_values(instance, oracles, alpha, opened, fri_params):
     [(num_polys_b, 2) array per batch], the openings f_{b,j}(z_b) the prover already holds (OpeningSet). With row-block
     sharded oracles the state holds this rank's rows only."""
     ctx = oracles[0].ctx
-    handles = (N.vp * len(oracles))(*[o.h for o in oracles])
-    barr = (N.FriBatch * len(instance.batches))()
-    keep = []
-    for i, b in enumerate(instance.batches):
-        oi = np.array([p.oracle_index for p in b.polynomials], dtype=np.uint32)
-        pi = np.array([p.polynomial_index for p in b.polynomials], dtype=np.uint32)
-        keep += [oi, pi]
-        barr[i].point[0], barr[i].point[1] = int(b.point[0]) % ORDER, int(b.point[1]) % ORDER
-        barr[i].num_polys = len(b.polynomials)
-        barr[i].oracle_index = oi.ctypes.data_as(N.u32p)
-        barr[i].poly_index = pi.ctypes.data_as(N.u32p)
+    handles, barr, keep = _fri_batches(instance, oracles)
     op = np.ascontiguousarray(np.concatenate([np.asarray(o, dtype=np.uint64).reshape(-1, 2) for o in opened]), dtype=np.uint64)
     assert len(op) == sum(len(b.polynomials) for b in instance.batches)
     al = np.array([alpha[0], alpha[1]], dtype=np.uint64)
     h = N.vp()
     N.check(N.lib().gl_fri_begin_values(ctx.h, handles, len(oracles), barr, len(instance.batches), N.np_ptr(op.reshape(-1)),
                                         N.np_ptr(al), fri_params.config.cap_height, C.byref(h)), ctx.h)
-    st = _FriState(h, ctx)
-    st.value_sharded = (oracles[0].shard_index, oracles[0].num_shards)
-    return st
+    return _FriState(h, ctx, (oracles[0].shard_index, oracles[0].num_shards))
 
 
 def _final_poly_from_values(values, log_len, shift, rate_bits, ctx):
@@ -446,15 +432,19 @@ def _final_poly_from_values(values, log_len, shift, rate_bits, ctx):
 
 
 def fri_committed_trees(state, challenger, fri_params, final_poly_coeff_len=None, max_num_query_steps=None,
-                        shard=None, gather=None):
+                        shard=None, gather=None, mixes=()):
     """fri_committed_trees (prover.rs:84-150): returns (caps, final_poly coefficients (len, 2)).
     shard=(g, G), gather=fn(local cap words) -> full cap words: every round's tree is row-block sharded over the G
     ranks (this rank hashes only its block of leaves; the values and the fold stay replicated) and the ranks
-    all-gather their cap entries -- rounds too small to shard are built whole on every rank."""
+    all-gather their cap entries -- rounds too small to shard are built whole on every rank.
+    mixes=[(log LDE size, state)], sizes decreasing: the lower-degree instances of batch FRI (batch_fri/prover.rs:88-147),
+    each mixed into the codeword (gl_fri_mix) after the fold that reaches its size."""
     L, ctx = N.lib(), state.ctx
     cap_words = NUM_HASH_OUT_ELTS << fri_params.config.cap_height
     caps = []
-    vs = getattr(state, "value_sharded", None)
+    vs = state.value_sharded
+    mixes = list(mixes)
+    log_cur = fri_params.lde_bits()
     for arity_bits in fri_params.reduction_arity_bits:
         cap = np.empty(cap_words, dtype=np.uint64)
         if vs is not None and vs[1] > 1:  # the codeword itself is row-block sharded: everything is rank-local
@@ -475,6 +465,10 @@ def fri_committed_trees(state, challenger, fri_params, final_poly_coeff_len=None
         beta = challenger.get_extension_challenge()
         b = np.array(beta, dtype=np.uint64)
         N.check(L.gl_fri_fold(state.h, N.np_ptr(b)), ctx.h)
+        log_cur -= arity_bits
+        if mixes and mixes[0][0] == log_cur:
+            N.check(L.gl_fri_mix(state.h, mixes.pop(0)[1].h, N.np_ptr(b)), ctx.h)
+    assert not mixes, "reduction_arity_bits must pass through every instance's LDE size (prover.rs:44-57)"
     if max_num_query_steps is not None:
         zero_cap = [0] * cap_words
         for _ in range(len(fri_params.reduction_arity_bits), max_num_query_steps):

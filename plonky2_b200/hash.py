@@ -48,6 +48,17 @@ class PoseidonPermutation:
         return p
 
 
+def _hash_rows(fn, rows, ctx):
+    """One digest per row of an (n_items, W) array from the library's batch hash `fn` -> (n_items, 4)."""
+    ctx = ctx or N.default_context()
+    rows = np.ascontiguousarray(rows, dtype=np.uint64)
+    n, w = rows.shape
+    out = np.empty((n, 4), dtype=np.uint64)
+    if n:
+        N.check(fn(ctx.h, N.np_ptr(rows) if w else None, n, w, N.np_ptr(out), N.MEM_HOST), ctx.h)
+    return out
+
+
 class PoseidonHash:
     """Hasher<GoldilocksField> (config.rs:36-77, poseidon.rs:872-887). Hash = 4 canonical u64."""
 
@@ -65,14 +76,7 @@ class PoseidonHash:
     @staticmethod
     def hash_many(rows, ctx=None):
         """hash_or_noop for every row of an (n_items, W) array -> (n_items, 4)."""
-        ctx = ctx or N.default_context()
-        rows = np.ascontiguousarray(rows, dtype=np.uint64)
-        n, w = rows.shape
-        out = np.empty((n, 4), dtype=np.uint64)
-        if n:
-            N.check(N.lib().gl_poseidon_hash_many(ctx.h, N.np_ptr(rows) if w else None, n, w, N.np_ptr(out),
-                                                  N.MEM_HOST), ctx.h)
-        return out
+        return _hash_rows(N.lib().gl_poseidon_hash_many, rows, ctx)
 
     @staticmethod
     def hash_or_noop(inputs, ctx=None):
@@ -81,14 +85,7 @@ class PoseidonHash:
     @staticmethod
     def hash_no_pad_many(rows, ctx=None):
         """hash_no_pad (always the sponge) for every row of an (n_items, W) array -> (n_items, 4)."""
-        ctx = ctx or N.default_context()
-        rows = np.ascontiguousarray(rows, dtype=np.uint64)
-        n, w = rows.shape
-        out = np.empty((n, 4), dtype=np.uint64)
-        if n:
-            N.check(N.lib().gl_poseidon_hash_no_pad_many(ctx.h, N.np_ptr(rows) if w else None, n, w,
-                                                         N.np_ptr(out), N.MEM_HOST), ctx.h)
-        return out
+        return _hash_rows(N.lib().gl_poseidon_hash_no_pad_many, rows, ctx)
 
     @staticmethod
     def hash_no_pad(inputs, ctx=None):
@@ -154,9 +151,29 @@ class MerkleProof:
         self.siblings = np.asarray(siblings, dtype=np.uint64).reshape(-1, 4)
 
 
-class MerkleTree:
+def _read_digests(fn, h, ctx, count):
+    """The (count, 4) digest buffer of a device tree through the library's digest read-back `fn`."""
+    out = np.empty((count, 4), dtype=np.uint64)
+    if out.size:
+        N.check(fn(h, N.np_ptr(out), N.MEM_HOST), ctx.h)
+    return out
+
+
+def _open_leaves(fn, h, ctx, indices, width, layers):
+    """(leaves (q, width), sibling paths (q, layers, 4)) of a device tree at `indices` through the library's opening
+    `fn`."""
+    idx = np.ascontiguousarray(indices, dtype=np.uint64)
+    leaves = np.empty((len(idx), width), dtype=np.uint64)
+    paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
+    if len(idx):
+        N.check(fn(h, N.np_ptr(idx), len(idx), N.np_ptr(leaves), N.np_ptr(paths) if paths.size else None), ctx.h)
+    return leaves, paths
+
+
+class MerkleTree(N.Handle):
     """MerkleTree<F, PoseidonHash> built on the GPU (merkle_tree.rs:46-62,193-237). The public fields of
     the reference (`leaves`, `digests`, `cap`) are properties that copy from the device on demand."""
+    destroyer = "gl_merkle_destroy"
 
     def __init__(self, leaves, cap_height, ctx=None):
         self.ctx = ctx or N.default_context()
@@ -183,37 +200,17 @@ class MerkleTree:
 
     @property
     def digests(self):
-        out = np.empty((2 * (self.N - (1 << self.cap_height)), 4), dtype=np.uint64)
-        if out.size:
-            N.check(N.lib().gl_merkle_digests(self.h, N.np_ptr(out), N.MEM_HOST), self.ctx.h)
-        return out
+        return _read_digests(N.lib().gl_merkle_digests, self.h, self.ctx, 2 * (self.N - (1 << self.cap_height)))
 
     def get(self, i):
         return self._leaves[i]
 
     def open_many(self, indices):
-        idx = np.ascontiguousarray(indices, dtype=np.uint64)
-        layers = log2_strict(self.N) - self.cap_height
-        leaves = np.empty((len(idx), self.W), dtype=np.uint64)
-        paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
-        if len(idx):
-            N.check(N.lib().gl_merkle_open(self.h, N.np_ptr(idx), len(idx), N.np_ptr(leaves),
-                                           N.np_ptr(paths) if paths.size else None), self.ctx.h)
-        return leaves, paths
+        return _open_leaves(N.lib().gl_merkle_open, self.h, self.ctx, indices, self.W,
+                            log2_strict(self.N) - self.cap_height)
 
     def prove(self, leaf_index):
         return MerkleProof(self.open_many([leaf_index])[1][0])
-
-    def close(self):
-        if getattr(self, "h", None):
-            N.lib().gl_merkle_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def verify_merkle_proof_to_cap(leaf_data, leaf_index, merkle_cap, proof, ctx=None):

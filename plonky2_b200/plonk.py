@@ -1440,24 +1440,9 @@ def commit_quotient_polys(common_data, quotient_polys, ctx=None):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients (trim_to_len(quotient_degree) was checked by the kernel call), all
     chunks committed with from_coeffs -- straight from the device tensor compute_quotient_polys returned."""
-    ctx = ctx or N.default_context()
     cfg = common_data.config
-    qdf, n = common_data.quotient_degree_factor, 1 << common_data.degree_bits
-    num = quotient_polys.shape[0]
-    B = num * qdf
-    L = N.lib()
-    h = N.vp()
-    N.check(L.gl_commit_begin(ctx.h, B, common_data.degree_bits, cfg.rate_bits, cfg.cap_height, 0, 0, 1, None, C.byref(h)), ctx.h)
-    try:
-        for j in range(num):
-            N.check(L.gl_commit_add_columns(h, j * qdf, qdf, N.vp(quotient_polys[j].data_ptr()), n, N.COLS_COEFFS,
-                                            N.MEM_DEVICE), ctx.h)
-        N.check(L.gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
-        ctx.synchronize()
-    except Exception:
-        L.gl_commit_destroy(h)
-        raise
-    return PolynomialBatch(h, ctx, B, common_data.degree_bits, cfg.rate_bits, cfg.cap_height, False)
+    return PolynomialBatch._from_coeff_chunks(quotient_polys, common_data.quotient_degree_factor,
+                                              common_data.degree_bits, cfg.rate_bits, cfg.cap_height, ctx)
 
 
 # ------------------------------------------------------------------ prove (plonk/prover.rs:113-360)

@@ -7,7 +7,8 @@ import numpy as np
 
 from . import _native as N
 from .field import log2_strict
-from .hash import MerkleCap, MerkleProof
+from .hash import MerkleCap, MerkleProof, _open_leaves, _read_digests
+from .proof import eval_commitments
 
 SALT_SIZE = 4  # oracle.rs:26
 
@@ -58,31 +59,24 @@ class _DeviceMerkleTree:
     @property
     def digests(self):
         b = self._b
-        out = np.empty((2 * (b.local_rows - (1 << b.cap_height) // b.num_shards), 4), dtype=np.uint64)
-        if out.size:
-            N.check(N.lib().gl_commit_digests(b.h, N.np_ptr(out), N.MEM_HOST), b.ctx.h)
-        return out
+        count = 2 * (b.local_rows - (1 << b.cap_height) // b.num_shards)
+        return _read_digests(N.lib().gl_commit_digests, b.h, b.ctx, count)
 
     def get(self, i):
         return self.get_rows(i, 1)[0]
 
     def open_many(self, indices):
         b = self._b
-        idx = np.ascontiguousarray(indices, dtype=np.uint64)
         layers = b.degree_log + b.rate_bits - b.cap_height  # local rows and local cap shrink together
-        leaves = np.empty((len(idx), b.leaf_width), dtype=np.uint64)
-        paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
-        if len(idx):
-            N.check(N.lib().gl_commit_open(b.h, N.np_ptr(idx), len(idx), N.np_ptr(leaves),
-                                           N.np_ptr(paths) if paths.size else None), b.ctx.h)
-        return leaves, paths
+        return _open_leaves(N.lib().gl_commit_open, b.h, b.ctx, indices, b.leaf_width, layers)
 
     def prove(self, leaf_index):
         return MerkleProof(self.open_many([leaf_index])[1][0])
 
 
-class PolynomialBatch:
+class PolynomialBatch(N.Handle):
     """PolynomialBatch<F, PoseidonGoldilocksConfig, 2> (oracle.rs:30-37)."""
+    destroyer = "gl_commit_destroy"
 
     def __init__(self, handle, ctx, num_polys, degree_log, rate_bits, cap_height, blinding, shard=(0, 1)):
         self.h, self.ctx = handle, ctx
@@ -118,6 +112,38 @@ class PolynomialBatch:
         return cls(h, ctx, B, log_n, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
 
     @classmethod
+    def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns):
+        """An unblinded batch committed incrementally from device memory: gl_commit_begin, then add_columns(h) issues
+        the gl_commit_add_columns calls on the unfinished handle h, then gl_commit_finish. The columns' device memory
+        only has to live until this returns."""
+        h = N.vp()
+        N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, 0, 0, 1, None, C.byref(h)),
+                ctx.h)
+        batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, False)
+        try:
+            add_columns(h)
+            N.check(N.lib().gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
+            ctx.synchronize()  # the library's stream-ordered reads of the caller's (torch) columns are done
+        except Exception:
+            batch.close()
+            raise
+        return batch
+
+    @classmethod
+    def _from_coeff_chunks(cls, polys, chunks, degree_log, rate_bits, cap_height, ctx=None):
+        """Every row of the device tensor `polys` cut into `chunks` coefficient polynomials of 2^degree_log, committed
+        in row order: the quotient commitment of plonky2 and starky (plonk/prover.rs:319-352, starky/prover.rs:391-421)."""
+        ctx = ctx or N.default_context()
+        n = 1 << degree_log
+
+        def add_columns(h):
+            for j in range(polys.shape[0]):
+                N.check(N.lib().gl_commit_add_columns(h, j * chunks, chunks, N.vp(polys[j].data_ptr()), n,
+                                                      N.COLS_COEFFS, N.MEM_DEVICE), ctx.h)
+
+        return cls._from_device(ctx, polys.shape[0] * chunks, degree_log, rate_bits, cap_height, add_columns)
+
+    @classmethod
     def from_values(cls, values, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,
                     salt=None, ctx=None, shard=(0, 1)):
         """from_values (oracle.rs:57-79). `timing`/`fft_root_table` are accepted for signature parity.
@@ -145,10 +171,7 @@ class PolynomialBatch:
     def eval_commitment(self, z):
         """eval_commitment of OpeningSet::new (plonk/proof.rs:313-351): every polynomial at z in F_{p^2};
         returns (num_polys, 2)."""
-        pt = np.array([int(z[0]), int(z[1])], dtype=np.uint64)
-        out = np.empty((self.num_polys, 2), dtype=np.uint64)
-        N.check(N.lib().gl_commit_eval_ext(self.h, N.np_ptr(pt), N.np_ptr(out)), self.ctx.h)
-        return out
+        return eval_commitments([(self, z)])[0]
 
     @staticmethod
     def prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len=None,
@@ -158,14 +181,3 @@ class PolynomialBatch:
 
         return prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len,
                               max_num_query_steps)
-
-    def close(self):
-        if getattr(self, "h", None):
-            N.lib().gl_commit_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -36,8 +36,6 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
     then handed to the incremental commitment (gl_commit_add_columns, GL_MEM_DEVICE): no H2D, no D2H.
     The caller's tensors must be complete (their producing stream synchronised or ordered before ctx's stream).
     Returns the PolynomialBatch (num_challenges * (num_partial_products + 1) polynomials)."""
-    import ctypes as C
-
     import torch
 
     from .polynomial_batch import PolynomialBatch
@@ -50,12 +48,10 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
     k_is = np.ascontiguousarray(k_is, dtype=np.uint64)
     nch = len(betas)
     M = (R + degree - 1) // degree          # columns per challenge: M - 1 partial products, then Z
-    B = nch * M
     L = N.lib()
-    h = N.vp()
-    N.check(L.gl_commit_begin(ctx.h, B, log_n, rate_bits, cap_height, 0, 0, 1, None, C.byref(h)), ctx.h)
-    try:
-        stage = torch.empty((M, n), dtype=torch.int64, device=wires_dev.device)
+    stage = torch.empty((M, n), dtype=torch.int64, device=wires_dev.device)  # must outlive _from_device's synchronise
+
+    def add_columns(h):
         for i in range(nch):
             N.check(L.gl_partial_products_and_zs(ctx.h, N.vp(wires_dev.data_ptr()), N.vp(sigmas_dev.data_ptr()),
                                                  N.np_ptr(k_is), log_n, R, int(betas[i]), int(gammas[i]), int(degree),
@@ -65,12 +61,8 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
             if M > 1:
                 N.check(L.gl_commit_add_columns(h, nch + i * (M - 1), M - 1, N.vp(stage.data_ptr()), n, N.COLS_VALUES,
                                                 N.MEM_DEVICE), ctx.h)
-        N.check(L.gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
-        ctx.synchronize()  # the staging matrix (a torch allocation) must outlive the library's stream-ordered reads
-    except Exception:
-        L.gl_commit_destroy(h)
-        raise
-    return PolynomialBatch(h, ctx, B, log_n, rate_bits, cap_height, False)
+
+    return PolynomialBatch._from_device(ctx, nch * M, log_n, rate_bits, cap_height, add_columns)
 
 
 def compute_lookup_polys(wires, num_routed_wires, max_quotient_degree_factor, deltas, lookup_rows, ctx=None):

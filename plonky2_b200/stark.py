@@ -180,21 +180,5 @@ def commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_hei
     """'split quotient polys' + 'compute quotient commitment' (prover.rs:391-421): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients, all chunks are committed with from_coeffs -- straight from the
     device tensor compute_quotient_polys returned."""
-    ctx = ctx or N.default_context()
-    qdf = stark.quotient_degree_factor()
-    n = 1 << degree_bits
-    num, size = quotient_polys.shape
-    B = num * qdf
-    L = N.lib()
-    h = N.vp()
-    N.check(L.gl_commit_begin(ctx.h, B, degree_bits, rate_bits, cap_height, 0, 0, 1, None, C.byref(h)), ctx.h)
-    try:
-        for j in range(num):
-            N.check(L.gl_commit_add_columns(h, j * qdf, qdf, N.vp(quotient_polys[j].data_ptr()), n, N.COLS_COEFFS,
-                                            N.MEM_DEVICE), ctx.h)
-        N.check(L.gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
-        ctx.synchronize()
-    except Exception:
-        L.gl_commit_destroy(h)
-        raise
-    return PolynomialBatch(h, ctx, B, degree_bits, rate_bits, cap_height, False)
+    return PolynomialBatch._from_coeff_chunks(quotient_polys, stark.quotient_degree_factor(), degree_bits, rate_bits,
+                                              cap_height, ctx)
