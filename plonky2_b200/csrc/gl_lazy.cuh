@@ -8,9 +8,9 @@
 // 64x64 multiplication needs it (l3_norm). Power-of-two twiddles (w_32 = 2^6 ... w_4 = 2^48, SURVEY appendix A.2)
 // act directly on the lazy form: the 128-bit signed product v*2^r is folded with 2^64 = 2^32 - 1, 2^96 = -1
 // (X^2 = X - 1, X^3 = -1 for X = 2^32) back into three words (l3_shift) -- no separate reduction before or after.
-// Range discipline (checked by gl_selftest_lazy on the device and by the parity suite): inputs of a radix-2^M
-// transform have e = 0; every level at most doubles |v|; l3_shift accepts |v| < 2^94 and returns |v| < 2^67,
-// so e stays far below the 2^20 that l3_norm allows.
+// Range discipline (checked on the device by tests/test_gpu_field_lazy.py, which runs tests/cuda/field_lazy_device.cu,
+// and by the parity suite): inputs of a radix-2^M transform have e = 0; every level at most doubles |v|; l3_shift
+// accepts |v| < 2^94 and returns |v| < 2^67, so e stays far below the 2^20 that l3_norm allows.
 #pragma once
 #include "gl_field.cuh"
 

@@ -471,9 +471,12 @@ static int ntt_natural(gl_ctx* ctx, const u64* in, size_t in_stride, u64* out, s
         const size_t tcnt = lo_cnt > hi_cnt ? lo_cnt : hi_cnt;
         DevBuf tabs(ctx);
         TRY(build_pow_tables(ctx, std::vector<u64>{gl::pow(sinv, lo_cnt), sinv}, tcnt, tabs));
-        k_mul_pows<<<dim3((unsigned)((n + 255) / 256), ncols), 256, 0, ctx->stream>>>(out, out_stride, n, tabs.get(),
-                                                                                     tabs.get() + tcnt, lowbits);
-        CKL(ctx);
+        for (uint32_t b0 = 0; b0 < ncols; b0 += MAX_GRID_Y) {  // one column per blockIdx.y, which is capped
+            const uint32_t bc = (ncols - b0 < MAX_GRID_Y) ? ncols - b0 : MAX_GRID_Y;
+            k_mul_pows<<<dim3((unsigned)((n + 255) / 256), bc), 256, 0, ctx->stream>>>(
+                out + (size_t)b0 * out_stride, out_stride, n, tabs.get(), tabs.get() + tcnt, lowbits);
+            CKL(ctx);
+        }
     }
     return GL_OK;
 }

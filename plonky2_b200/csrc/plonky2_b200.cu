@@ -115,6 +115,8 @@ static int set_err(gl_ctx* ctx, int code, const char* fmt, ...) {
         int rc_ = (expr);          \
         if (rc_ != GL_OK) return rc_; \
     } while (0)
+// CUDA's limit on gridDim.y: kernels with one column per blockIdx.y are launched in chunks of at most this many
+constexpr uint32_t MAX_GRID_Y = 65535;
 
 static int dmalloc(gl_ctx* ctx, u64** p, size_t words) {
     *p = nullptr;
@@ -604,9 +606,12 @@ static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int
         const size_t M = (size_t)1 << logM;
         DevBuf folded(ctx);
         TRY(folded.alloc((size_t)gc * M));
-        k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), gc), 128, 0, ctx->stream>>>(cg, n, n, M, gl::pow(c->sg, M),
-                                                                                     folded.get());
-        CKL(ctx);
+        for (uint32_t b0 = 0; b0 < gc; b0 += MAX_GRID_Y) {
+            const uint32_t bc = (gc - b0 < MAX_GRID_Y) ? gc - b0 : MAX_GRID_Y;
+            k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), bc), 128, 0, ctx->stream>>>(
+                cg + (size_t)b0 * n, n, n, M, gl::pow(c->sg, M), folded.get() + (size_t)b0 * M);
+            CKL(ctx);
+        }
         TRY(lde_columns(ctx, folded.get(), M, gc, (int)logM, 0, c->sg, t.leaves + (size_t)g0 * Nloc, Nloc));
     }
     return GL_OK;
