@@ -135,6 +135,12 @@ int gl_commit_begin(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits,
 int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, const uint64_t* cols, size_t col_stride,
                           int kind, int mem);
 int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem);
+/* gl_commit_finish for a commitment begun with blinding = 1, with the salt drawn ON THE DEVICE from a ChaCha20 keystream
+ * (gl_random_field_elements below): salt column s at LDE row i is element (s, i) of the key, so every shard of a sharded
+ * begin produces the leaves of the unsharded commitment, and the result equals gl_commit_finish with the explicit salt
+ * array salt[s * N + i] = element (s, i). key = 32 bytes, or NULL: the library draws a fresh key from the OS CSPRNG
+ * (getrandom(2)) for this commitment and forgets it (the reference's OsRng salt, oracle.rs:133-137). */
+int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]);
 int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_shards);
 void gl_commit_destroy(gl_commit* c);
 /* shape queries */
@@ -173,6 +179,15 @@ int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_in
  * reference's row-major MerkleTree.leaves is what gl_commit_leaves / gl_commit_open return. */
 const uint64_t* gl_commit_dev_lde(const gl_commit* c, size_t* col_stride);
 const uint64_t* gl_commit_dev_coeffs(const gl_commit* c);
+
+/* ---- random field elements (F::rand, field/src/goldilocks_field.rs:61-67) ------------------------------------------ */
+/* out[j] = element (column, first + j) of the keystream of `key` (32 bytes), j < count: uniform canonical field elements,
+ * ChaCha20 (RFC 8439 section 2.3) with the sampling rule of plonky2_b200/csrc/gl_chacha.cuh -- position i takes the
+ * little-endian word i mod 8 of block i / 8 of the stream with nonce (column, a, 0), for the first attempt a = 0, 1, ...
+ * whose word is below p. Each element depends only on (key, column, position), so ranges can be drawn in any split.
+ * Positions must stay below 2^35. */
+int gl_random_field_elements(gl_ctx* ctx, const uint8_t key[32], uint32_t column, uint64_t first, size_t count,
+                             uint64_t* out, int mem);
 
 /* ---- "next" rows (SURVEY.md section 8f) ------------------------------------------------------------------ */
 /* wires_permutation_partial_products_and_zs (plonky2/src/plonk/prover.rs:387-449, util/partial_products.rs:13-37):

@@ -17,6 +17,7 @@
 // Shape violations that panic in the reference throw ShapeError; other failures throw Error. There is no CPU
 // fallback: constructing a Context without a CUDA device throws.
 #pragma once
+#include <array>
 #include <cstdint>
 #include <cstring>
 #include <memory>
@@ -284,9 +285,32 @@ struct FriProof {
     }
 };
 
+// The salt of a zero-knowledge commitment drawn on the device (gl_commit_finish_keyed): a 32-byte ChaCha20 key, which
+// makes the commitment reproducible, or fresh entropy from the OS CSPRNG for each commitment (the reference's OsRng).
+struct SaltKey {
+    std::array<uint8_t, 32> key{};
+    bool fresh = true;
+    static SaltKey of(const std::array<uint8_t, 32>& k) {
+        SaltKey s;
+        s.key = k;
+        s.fresh = false;
+        return s;
+    }
+    static SaltKey os_entropy() { return SaltKey(); }
+};
+
 // ---- PolynomialBatch (fri/oracle.rs:30-237) ----
 class PolynomialBatch {
    public:
+    // from_values / from_coeffs with blinding and the salt drawn on the device from `key`
+    static PolynomialBatch from_values(Context& ctx, const std::vector<std::vector<F>>& values, uint32_t rate_bits,
+                                       bool blinding, uint32_t cap_height, const SaltKey& key) {
+        return create_keyed(ctx, values, rate_bits, blinding, cap_height, key, false);
+    }
+    static PolynomialBatch from_coeffs(Context& ctx, const std::vector<std::vector<F>>& polynomials, uint32_t rate_bits,
+                                       bool blinding, uint32_t cap_height, const SaltKey& key) {
+        return create_keyed(ctx, polynomials, rate_bits, blinding, cap_height, key, true);
+    }
     // from_values (oracle.rs:57-79): one Vec per polynomial; `salt` = SALT_SIZE columns of n << rate_bits
     // values when blinding (the reference draws them from OsRng).
     static PolynomialBatch from_values(Context& ctx, const std::vector<std::vector<F>>& values, uint32_t rate_bits,
@@ -526,6 +550,27 @@ class PolynomialBatch {
         pb.ctx_ = &ctx;
         check(gl_commit_create(ctx.get(), flat.data(), n, (uint32_t)cols.size(), log_n, rate_bits, cap_height,
                                blinding ? salt->data() : nullptr, is_coeffs ? 1 : 0, GL_MEM_HOST, &pb.h_), ctx.get());
+        return pb;
+    }
+    // gl_commit_begin -> gl_commit_add_columns -> gl_commit_finish_keyed
+    static PolynomialBatch create_keyed(Context& ctx, const std::vector<std::vector<F>>& cols, uint32_t rate_bits,
+                                        bool blinding, uint32_t cap_height, const SaltKey& key, bool is_coeffs) {
+        if (!blinding) throw ShapeError(GL_ERR_BAD_SHAPE, "a salt key needs blinding");
+        if (cols.empty()) throw ShapeError(GL_ERR_BAD_SHAPE, "empty polynomial batch");
+        const size_t n = cols[0].size();
+        const uint32_t log_n = log2_strict(n);
+        std::vector<F> flat(cols.size() * n);
+        for (size_t b = 0; b < cols.size(); b++) {
+            if (cols[b].size() != n) throw ShapeError(GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent");  // oracle.rs:128
+            std::memcpy(&flat[b * n], cols[b].data(), n * 8);
+        }
+        PolynomialBatch pb;
+        pb.ctx_ = &ctx;
+        check(gl_commit_begin(ctx.get(), (uint32_t)cols.size(), log_n, rate_bits, cap_height, 1, 0, 1, nullptr, &pb.h_),
+              ctx.get());
+        check(gl_commit_add_columns(pb.h_, 0, (uint32_t)cols.size(), flat.data(), n,
+                                    is_coeffs ? GL_COLS_COEFFS : GL_COLS_VALUES, GL_MEM_HOST), ctx.get());
+        check(gl_commit_finish_keyed(pb.h_, key.fresh ? nullptr : key.key.data()), ctx.get());
         return pb;
     }
     gl_commit* h_ = nullptr;

@@ -12,7 +12,7 @@ from .fri import (FriBatchInfo, FriConfig, FriInstanceInfo, FriOracleInfo, FriPa
                   starky_standard_fast_fri_config)
 from .hash import (MerkleCap, MerkleProof, MerkleTree, PoseidonHash, PoseidonPermutation,  # noqa: F401
                    verify_merkle_proof_to_cap)
-from .polynomial_batch import SALT_SIZE, PolynomialBatch  # noqa: F401
+from .polynomial_batch import SALT_SIZE, PolynomialBatch, random_field_elements_keyed  # noqa: F401
 from .proof import OpeningSet, StarkOpeningSet, eval_commitments  # noqa: F401
 from .stark import FibonacciStark, Stark, commit_quotient_polys, compute_quotient_polys  # noqa: F401
 from . import plonk  # noqa: F401  (plonk.compute_quotient_polys: the plonky2 circuit quotient)

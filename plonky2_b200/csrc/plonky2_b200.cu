@@ -20,7 +20,12 @@
 #include <tuple>
 #include <vector>
 
+#include <sys/random.h>
+
+#include <cerrno>
+
 #include "../../include/plonky2_b200.h"
+#include "gl_chacha.cuh"
 #include "gl_field.cuh"
 #include "gl_ntt.cuh"
 #include "gl_poseidon.cuh"
@@ -632,6 +637,32 @@ static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem) {
     }
     TRY(tree_build(ctx, t));
     c->finished = true;
+    return GL_OK;
+}
+// salt columns drawn on the device from a ChaCha20 key (gl_chacha.cuh), this shard's leaves only, + "build Merkle tree"
+static int commit_finish_keyed(gl_ctx* ctx, gl_commit* c, const ChaChaKey& key) {
+    Tree& t = c->tree;
+    const size_t Nloc = t.N;
+    const uint32_t log_N = c->degree_log + c->rate_bits;
+    const size_t items = salt_fill_items(log_N, Nloc);
+    k_chacha_salt<<<dim3((unsigned)((items + 255) / 256), GL_SALT_SIZE), 256, 0, ctx->stream>>>(
+        key, log_N, (u64)c->shard_index * Nloc, Nloc, t.leaves + (size_t)c->B * Nloc, Nloc);
+    CKL(ctx);
+    TRY(tree_build(ctx, t));
+    c->finished = true;
+    return GL_OK;
+}
+// 32 bytes from the OS CSPRNG
+static int os_random_key(gl_ctx* ctx, uint8_t out[32]) {
+    size_t got = 0;
+    while (got < 32) {
+        const ssize_t r = getrandom(out + got, 32 - got, 0);
+        if (r < 0) {
+            if (errno == EINTR) continue;
+            return set_err(ctx, GL_ERR_UNSUPPORTED, "getrandom failed: %s", strerror(errno));
+        }
+        got += (size_t)r;
+    }
     return GL_OK;
 }
 
@@ -1640,6 +1671,39 @@ int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem) {
     if (c->blinding != (salt != nullptr)) return set_err(ctx, GL_ERR_BAD_ARG, "salt must be given exactly when blinding was requested");
     CK(ctx, cudaSetDevice(ctx->device));
     return commit_finish(ctx, c, salt, mem);
+}
+int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]) {
+    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    gl_ctx* ctx = c->ctx;
+    if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
+    if (!c->blinding) return set_err(ctx, GL_ERR_BAD_ARG, "a salt key was given for a commitment begun without blinding");
+    uint8_t fresh[32];
+    if (!key) {
+        TRY(os_random_key(ctx, fresh));
+        key = fresh;
+    }
+    const ChaChaKey k = chacha_key_from_bytes(key);
+    memset(fresh, 0, sizeof(fresh));
+    CK(ctx, cudaSetDevice(ctx->device));
+    return commit_finish_keyed(ctx, c, k);
+}
+int gl_random_field_elements(gl_ctx* ctx, const uint8_t key[32], uint32_t column, uint64_t first, size_t count,
+                             uint64_t* out, int mem) {
+    if (!ctx || !key || (!out && count)) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (first > CHACHA_MAX_POSITION || count > CHACHA_MAX_POSITION - first)
+        return set_err(ctx, GL_ERR_BAD_ARG, "positions %llu + %zu exceed the 2^35 of one stream", (unsigned long long)first,
+                       count);
+    if (count == 0) return GL_OK;
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf stage(ctx);
+    u64* dout;
+    TRY(device_out(out, count, mem, stage, &dout));
+    const u64 blocks = ((first + count - 1) >> 3) - (first >> 3) + 1;
+    k_chacha_elements<<<(unsigned)((blocks + 255) / 256), 256, 0, ctx->stream>>>(chacha_key_from_bytes(key), column, first,
+                                                                               count, dout);
+    CKL(ctx);
+    if (mem == GL_MEM_HOST) return d2h(ctx, out, dout, count);
+    return GL_OK;
 }
 
 int gl_commit_create(gl_ctx* ctx, const uint64_t* cols, size_t col_stride, uint32_t B, uint32_t log_n,

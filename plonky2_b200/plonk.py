@@ -20,7 +20,7 @@ import numpy as np
 
 from . import _native as N
 from . import field as F
-from .polynomial_batch import PolynomialBatch
+from .polynomial_batch import SALT_SIZE, PolynomialBatch
 
 OP_LOCAL, OP_NEXT, OP_CONST, OP_X, OP_L0, OP_ADD, OP_SUB, OP_MUL, OP_TERM, OP_ADDC, OP_MULC = range(11)
 _BINARY, _UNARY_CONST = (OP_ADD, OP_SUB, OP_MUL), (OP_ADDC, OP_MULC)
@@ -42,10 +42,38 @@ class CircuitConfig:
     """CircuitConfig (plonk/circuit_data.rs:60-131); defaults = standard_recursion_config."""
 
     def __init__(self, num_wires=135, num_routed_wires=80, num_constants=2, num_challenges=2,
-                 max_quotient_degree_factor=8, rate_bits=3, cap_height=4):
+                 max_quotient_degree_factor=8, rate_bits=3, cap_height=4, *, zero_knowledge=False):
         self.num_wires, self.num_routed_wires, self.num_constants = num_wires, num_routed_wires, num_constants
         self.num_challenges, self.max_quotient_degree_factor = num_challenges, max_quotient_degree_factor
         self.rate_bits, self.cap_height = rate_bits, cap_height
+        self.zero_knowledge = bool(zero_knowledge)
+
+
+def standard_recursion_zk_config():
+    """CircuitConfig::standard_recursion_zk_config (plonk/circuit_data.rs:135-140)."""
+    return CircuitConfig(zero_knowledge=True)
+
+
+def blinding_counts(config, fri_config, num_gates):
+    """CircuitBuilder::blinding_counts with num_blinding_gates (plonk/circuit_builder.rs:866-909): (regular_poly_openings,
+    z_openings), the number of values a proof reveals per "regular" polynomial (opened at zeta and in the FRI queries) and
+    per Z polynomial (also at g zeta), for a circuit of num_gates gates before blinding, under the FRI config fri_config.
+    A zero-knowledge circuit (CircuitBuilder::blind, :911-970) then gets regular_poly_openings NoopGate rows with random
+    values on every wire, and z_openings pairs of NoopGate rows with the same random value on each routed wire of the
+    pair and a copy constraint between them; filling them is witness generation (RandomValueGenerator)."""
+    degree_estimate = 1 << max(0, int(num_gates) - 1).bit_length()
+    while True:
+        arities = [1 << b for b in fri_config.fri_params(F.log2_strict(degree_estimate),
+                                                         config.zero_knowledge).reduction_arity_bits]
+        product = 1
+        for a in arities:
+            product *= a
+        fri_openings = fri_config.num_query_rounds * (1 + F.D * sum(a - 1 for a in arities)
+                                                      + F.D * (degree_estimate // product))
+        regular_poly_openings, z_openings = F.D + fri_openings, 2 * F.D + fri_openings
+        if num_gates + regular_poly_openings + 2 * z_openings <= degree_estimate:
+            return regular_poly_openings, z_openings
+        degree_estimate *= 2
 
 
 # ------------------------------------------------------------------ expressions
@@ -1436,13 +1464,15 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
     return out
 
 
-def commit_quotient_polys(common_data, quotient_polys, ctx=None):
+def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients (trim_to_len(quotient_degree) was checked by the kernel call), all
-    chunks committed with from_coeffs -- straight from the device tensor compute_quotient_polys returned."""
+    chunks committed with from_coeffs -- straight from the device tensor compute_quotient_polys returned. With blinding
+    the salt is drawn on the device from salt_key (PolynomialBatch._from_device)."""
     cfg = common_data.config
     return PolynomialBatch._from_coeff_chunks(quotient_polys, common_data.quotient_degree_factor,
-                                              common_data.degree_bits, cfg.rate_bits, cfg.cap_height, ctx)
+                                              common_data.degree_bits, cfg.rate_bits, cfg.cap_height, ctx,
+                                              blinding=blinding, salt_key=salt_key)
 
 
 # ------------------------------------------------------------------ prove (plonk/prover.rs:113-360)
@@ -1512,8 +1542,9 @@ class Proof:
         pps, quot = ext_vec(nc * cd.num_partial_products), ext_vec(nc * cd.quotient_degree_factor)
         openings = OpeningSet(constants=constants, plonk_sigmas=sigmas, wires=wires, plonk_zs=zs, plonk_zs_next=zs_next,
                               partial_products=pps, quotient_polys=quot, lookup_zs=lk, lookup_zs_next=lk_next)
-        widths = [cd.num_constants + cfg.num_routed_wires, cfg.num_wires,
-                  nc * (1 + cd.num_partial_products + cd.num_lookup_polys), nc * cd.quotient_degree_factor]
+        salt = SALT_SIZE if fri_params.hiding else 0          # salt_size(hiding): the salted oracles' leaves
+        widths = [cd.num_constants + cfg.num_routed_wires, cfg.num_wires + salt,
+                  nc * (1 + cd.num_partial_products + cd.num_lookup_polys) + salt, nc * cd.quotient_degree_factor + salt]
         fri, pos = FriProof.from_bytes(buf, widths, fri_params, pos)
         return cls(caps[0], caps[1], caps[2], openings, fri), pos
 
@@ -1595,7 +1626,8 @@ class CompressedProofWithPublicInputs(ProofWithPublicInputs):
 
 def get_fri_instance(cd, zeta):
     """CommonCircuitData::get_fri_instance (plonk/circuit_data.rs:530-660): every polynomial at zeta, the Z's and the
-    lookup polynomials also at g * zeta."""
+    lookup polynomials also at g * zeta. The wires, Z / partial-product and quotient oracles are blinded in a
+    zero-knowledge circuit (fri_oracles, :575-600); the constants / sigmas never are."""
     from .fri import FriBatchInfo, FriInstanceInfo, FriOracleInfo, FriPolynomialInfo
 
     cfg = cd.config
@@ -1608,8 +1640,9 @@ def get_fri_instance(cd, zeta):
                  + FriPolynomialInfo.from_range(2, range(n_zs_pp)) + FriPolynomialInfo.from_range(3, range(n_quot)) + lookup)
     g = F.primitive_root_of_unity(cd.degree_bits)
     zeta_next = F.ext_mul((g, 0), zeta)
-    oracles = [FriOracleInfo(n_pre, False), FriOracleInfo(cfg.num_wires, False), FriOracleInfo(n_zs_pp + n_lookup, False),
-               FriOracleInfo(n_quot, False)]
+    zk = cfg.zero_knowledge
+    oracles = [FriOracleInfo(n_pre, False), FriOracleInfo(cfg.num_wires, zk), FriOracleInfo(n_zs_pp + n_lookup, zk),
+               FriOracleInfo(n_quot, zk)]
     return FriInstanceInfo(oracles, [FriBatchInfo(zeta, all_polys),
                                      FriBatchInfo(zeta_next, FriPolynomialInfo.from_range(2, range(nc)) + lookup)])
 
@@ -1624,12 +1657,17 @@ def _to_device(columns, ctx):
     return t
 
 
-def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None):
+def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None, *, salt_keys=None):
     """prove_with_partition_witness (plonk/prover.rs:132-360) from the full witness matrix `wires` (num_wires, n) -- the
     generators' output -- to ProofWithPublicInputs, every array-sized step on the device: wires commitment, Z / partial
     products (+ lookup) commitment, quotient polynomials from the LDEs in place and their commitment, the openings at
     zeta and g zeta, the FRI opening proof. The transcript runs on the host exactly as in the reference.
-    zero_knowledge = false (no blinding)."""
+
+    With config.zero_knowledge the wires, Z / partial-product (+ lookup) and quotient commitments are salted, as
+    prover.rs:179,249,297 do (the constants / sigmas commitment never is), and prover_data.fri_params.hiding must be set.
+    The salt is drawn on the device: salt_keys = three 32-byte keys (wires, Z's, quotient) give a reproducible proof;
+    None draws a fresh key from the OS CSPRNG per commitment. The blinding rows of the circuit (blinding_counts) are part
+    of the witness, which the caller generates."""
     from .challenger import Challenger
     from .fri import prove_openings
     from .hash import PoseidonHash
@@ -1643,8 +1681,16 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None)
     wires = np.ascontiguousarray(wires, dtype=np.uint64)
     if wires.shape != (cfg.num_wires, 1 << cd.degree_bits):
         raise N.ShapeError("the witness must be (num_wires, n)")
+    zk = cfg.zero_knowledge
+    if bool(prover_data.fri_params.hiding) != zk:
+        raise N.ShapeError("fri_params.hiding (%s) must equal config.zero_knowledge (%s)"
+                           % (bool(prover_data.fri_params.hiding), zk))
+    if salt_keys is not None and (not zk or len(salt_keys) != 3):
+        raise N.ShapeError("salt_keys: three 32-byte keys (wires, Z's, quotient), for a zero-knowledge config only")
+    # keyword arguments of the three salted commitments (none without zero knowledge)
+    salted = [dict(salt_key=salt_keys[i] if salt_keys is not None else "fresh") if zk else {} for i in range(3)]
     public_inputs_hash = [int(x) for x in PoseidonHash.hash_no_pad(np.array(public_inputs, dtype=np.uint64), ctx)]
-    wires_commitment = PolynomialBatch.from_values(wires, cfg.rate_bits, False, cfg.cap_height, ctx=ctx)
+    wires_commitment = PolynomialBatch.from_values(wires, cfg.rate_bits, zk, cfg.cap_height, ctx=ctx, **salted[0])
     commitments = [wires_commitment]
     try:
         challenger = Challenger()
@@ -1668,18 +1714,20 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None)
                 pps += list(out[:-1])
             lookup_polys = compute_all_lookup_polys(wires, nr, cfg.max_quotient_degree_factor, deltas, cd.lookup_rows, nc, ctx)
             zs_commitment = PolynomialBatch.from_values(np.concatenate([np.stack(zs + pps), lookup_polys]), cfg.rate_bits,
-                                                        False, cfg.cap_height, ctx=ctx)
+                                                        zk, cfg.cap_height, ctx=ctx, **salted[1])
         else:
             wires_dev, sigmas_dev = _to_device(wires[:nr], ctx), _to_device(prover_data.sigmas, ctx)
             zs_commitment = commit_zs_partial_products(wires_dev, sigmas_dev, cd.k_is, betas, gammas,
-                                                       cd.quotient_degree_factor, cfg.rate_bits, cfg.cap_height, ctx)
+                                                       cd.quotient_degree_factor, cfg.rate_bits, cfg.cap_height, ctx,
+                                                       **(dict(blinding=True, **salted[1]) if zk else {}))
         commitments.append(zs_commitment)
         challenger.observe_cap(zs_commitment.merkle_tree.cap)
         alphas = challenger.get_n_challenges(nc)
         cs = prover_data.constants_sigmas_commitment
         quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas, gammas,
                                                 alphas, deltas)
-        quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx)
+        quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx,
+                                                    **(dict(blinding=True, **salted[2]) if zk else {}))
         commitments.append(quotient_commitment)
         challenger.observe_cap(quotient_commitment.merkle_tree.cap)
         zeta = challenger.get_extension_challenge()

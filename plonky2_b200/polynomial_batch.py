@@ -15,7 +15,8 @@ SALT_SIZE = 4  # oracle.rs:26
 
 def random_field_elements(count):
     """Uniform canonical field elements from the OS CSPRNG (F::rand, field/src/goldilocks_field.rs:61-64):
-    64-bit draws, rejecting values >= p -- vectorised (a 2^23 x 4 salt takes ~0.3 s, not minutes)."""
+    64-bit draws, rejecting values >= p -- vectorised. A 2^23 x 4 salt takes about 0.8 s on a 16-core host
+    (not minutes); salt_key= draws it on the device in under a millisecond instead."""
     import os
 
     from .field import ORDER
@@ -28,6 +29,31 @@ def random_field_elements(count):
         cand = cand[cand < np.uint64(ORDER)][:need]
         out[filled:filled + len(cand)] = cand
         filled += len(cand)
+    return out
+
+
+def _salt_key(salt_key):
+    """A salt_key argument as the C ABI takes it: the 32 key bytes, or None for "fresh" (the library draws a key from
+    the OS CSPRNG)."""
+    if isinstance(salt_key, str) and salt_key == "fresh":
+        return None
+    if isinstance(salt_key, (bytes, bytearray)) and len(salt_key) == 32:
+        return bytes(salt_key)
+    raise N.ShapeError("salt_key must be 32 bytes or 'fresh'")
+
+
+def random_field_elements_keyed(key, column, first, count, ctx=None):
+    """Elements first .. first + count - 1 of stream `column` of the device salt sampler for a 32-byte key
+    (gl_random_field_elements; the sampling rule is documented in csrc/gl_chacha.cuh): uniform canonical field elements,
+    each a function of (key, column, position) alone. A keyed commitment's salt column s at LDE row i is element i of
+    stream s."""
+    ctx = ctx or N.default_context()
+    key = _salt_key(key)
+    if key is None:
+        raise N.ShapeError("random_field_elements_keyed needs an explicit 32-byte key")
+    out = np.empty(int(count), dtype=np.uint64)
+    N.check(N.lib().gl_random_field_elements(ctx.h, key, int(column), int(first), int(count), N.np_ptr(out),
+                                             N.MEM_HOST), ctx.h)
     return out
 
 
@@ -89,13 +115,23 @@ class PolynomialBatch(N.Handle):
         self.merkle_tree = _DeviceMerkleTree(self)
 
     @classmethod
-    def _create(cls, cols, rate_bits, blinding, cap_height, is_coeffs, salt, ctx, shard=(0, 1)):
+    def _create(cls, cols, rate_bits, blinding, cap_height, is_coeffs, salt, ctx, shard=(0, 1), salt_key=None):
         ctx = ctx or N.default_context()
         cols = np.ascontiguousarray(cols, dtype=np.uint64)
         if cols.ndim != 2 or cols.shape[0] == 0:
             raise N.ShapeError("expected a non-empty (num_polys, degree) array")
         B, n = cols.shape
         log_n = log2_strict(n)
+        if salt_key is not None:
+            if salt is not None:
+                raise N.ShapeError("salt= and salt_key= are exclusive")
+            kind = N.COLS_COEFFS if is_coeffs else N.COLS_VALUES
+
+            def add_columns(h):
+                N.check(N.lib().gl_commit_add_columns(h, 0, B, N.np_ptr(cols), n, kind, N.MEM_HOST), ctx.h)
+
+            return cls._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, blinding=blinding,
+                                    salt_key=salt_key, shard=shard)
         sp = None
         if blinding:
             if salt is None:
@@ -112,17 +148,25 @@ class PolynomialBatch(N.Handle):
         return cls(h, ctx, B, log_n, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
 
     @classmethod
-    def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns):
-        """An unblinded batch committed incrementally from device memory: gl_commit_begin, then add_columns(h) issues
-        the gl_commit_add_columns calls on the unfinished handle h, then gl_commit_finish. The columns' device memory
-        only has to live until this returns."""
+    def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns, *, blinding=False,
+                     salt_key=None, shard=(0, 1)):
+        """A batch committed incrementally: gl_commit_begin, then add_columns(h) issues the gl_commit_add_columns calls
+        on the unfinished handle h, then gl_commit_finish -- or, with blinding, gl_commit_finish_keyed: the salt is
+        drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). The columns' device
+        memory only has to live until this returns."""
+        if salt_key is not None and not blinding:
+            raise N.ShapeError("salt_key= needs blinding=True")
+        key = _salt_key(salt_key) if salt_key is not None else None
         h = N.vp()
-        N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, 0, 0, 1, None, C.byref(h)),
-                ctx.h)
-        batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, False)
+        N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, int(bool(blinding)),
+                                        int(shard[0]), int(shard[1]), None, C.byref(h)), ctx.h)
+        batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
         try:
             add_columns(h)
-            N.check(N.lib().gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
+            if blinding:
+                N.check(N.lib().gl_commit_finish_keyed(h, key), ctx.h)
+            else:
+                N.check(N.lib().gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
             ctx.synchronize()  # the library's stream-ordered reads of the caller's (torch) columns are done
         except Exception:
             batch.close()
@@ -130,9 +174,11 @@ class PolynomialBatch(N.Handle):
         return batch
 
     @classmethod
-    def _from_coeff_chunks(cls, polys, chunks, degree_log, rate_bits, cap_height, ctx=None):
+    def _from_coeff_chunks(cls, polys, chunks, degree_log, rate_bits, cap_height, ctx=None, *, blinding=False,
+                           salt_key=None):
         """Every row of the device tensor `polys` cut into `chunks` coefficient polynomials of 2^degree_log, committed
-        in row order: the quotient commitment of plonky2 and starky (plonk/prover.rs:319-352, starky/prover.rs:391-421)."""
+        in row order: the quotient commitment of plonky2 and starky (plonk/prover.rs:319-352, starky/prover.rs:391-421).
+        blinding / salt_key: as in _from_device."""
         ctx = ctx or N.default_context()
         n = 1 << degree_log
 
@@ -141,20 +187,24 @@ class PolynomialBatch(N.Handle):
                 N.check(N.lib().gl_commit_add_columns(h, j * chunks, chunks, N.vp(polys[j].data_ptr()), n,
                                                       N.COLS_COEFFS, N.MEM_DEVICE), ctx.h)
 
-        return cls._from_device(ctx, polys.shape[0] * chunks, degree_log, rate_bits, cap_height, add_columns)
+        return cls._from_device(ctx, polys.shape[0] * chunks, degree_log, rate_bits, cap_height, add_columns,
+                                blinding=blinding, salt_key=salt_key)
 
     @classmethod
     def from_values(cls, values, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,
-                    salt=None, ctx=None, shard=(0, 1)):
+                    salt=None, ctx=None, shard=(0, 1), salt_key=None):
         """from_values (oracle.rs:57-79). `timing`/`fft_root_table` are accepted for signature parity.
-        shard=(g, G): build only leaf rows [g*N/G, (g+1)*N/G) on this device (multi-GPU row-block sharding)."""
-        return cls._create(values, rate_bits, blinding, cap_height, False, salt, ctx, shard)
+        shard=(g, G): build only leaf rows [g*N/G, (g+1)*N/G) on this device (multi-GPU row-block sharding).
+        With blinding, the salt is `salt` (4 x N, by LDE row), else, with salt_key (32 bytes, or "fresh" for a key from
+        the OS CSPRNG), drawn on the device: salt column s at LDE row i = random_field_elements_keyed(key, s, i, 1);
+        else drawn on the host from the OS CSPRNG."""
+        return cls._create(values, rate_bits, blinding, cap_height, False, salt, ctx, shard, salt_key)
 
     @classmethod
     def from_coeffs(cls, polynomials, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,
-                    salt=None, ctx=None, shard=(0, 1)):
-        """from_coeffs (oracle.rs:82-112)."""
-        return cls._create(polynomials, rate_bits, blinding, cap_height, True, salt, ctx, shard)
+                    salt=None, ctx=None, shard=(0, 1), salt_key=None):
+        """from_coeffs (oracle.rs:82-112); salt / salt_key as in from_values."""
+        return cls._create(polynomials, rate_bits, blinding, cap_height, True, salt, ctx, shard, salt_key)
 
     @property
     def polynomials(self):
