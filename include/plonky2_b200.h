@@ -230,7 +230,9 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
 #define GL_STARK_TRANSITION 1
 #define GL_STARK_FIRST_ROW 2
 #define GL_STARK_LAST_ROW 3
-#define GL_STARK_MAX_INSTR 256
+/* every instruction's value lives in thread-local memory (8 B each); 512 fits two transition constraints on each of
+ * 64 columns (a 64-column STARK of 32 Fibonacci pairs is 288 instructions) */
+#define GL_STARK_MAX_INSTR 512
 #define GL_STARK_MAX_ALPHAS 4
 #define GL_STARK_MAX_QD 8
 typedef struct {

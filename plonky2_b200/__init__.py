@@ -14,7 +14,9 @@ from .hash import (MerkleCap, MerkleProof, MerkleTree, PoseidonHash, PoseidonPer
                    verify_merkle_proof_to_cap)
 from .polynomial_batch import SALT_SIZE, PolynomialBatch, random_field_elements_keyed  # noqa: F401
 from .proof import OpeningSet, StarkOpeningSet, eval_commitments  # noqa: F401
-from .stark import FibonacciStark, Stark, commit_quotient_polys, compute_quotient_polys  # noqa: F401
+from .stark import (FibonacciStark, Stark, StarkConfig, StarkProof, StarkProofWithPublicInputs,  # noqa: F401
+                    commit_quotient_polys, compute_quotient_polys, eval_l_0_and_l_last, eval_vanishing_poly)
+from . import stark  # noqa: F401  (stark.prove: the starky prover, next to plonk.prove_with_witness)
 from . import plonk  # noqa: F401  (plonk.compute_quotient_polys: the plonky2 circuit quotient)
 from .batch_merkle_tree import (BatchMerkleTree, compress_merkle_proofs, decompress_merkle_proofs,  # noqa: F401
                                 verify_batch_merkle_proof_to_cap)

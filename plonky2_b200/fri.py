@@ -348,16 +348,28 @@ class CompressedFriProof:
         return FriProof(self.commit_phase_merkle_caps, rounds, self.final_poly, self.pow_witness)
 
 
-def fri_challenges(challenger, commit_phase_merkle_caps, final_poly, pow_witness, degree_bits, config):
-    """Challenger::fri_challenges (fri/challenges.rs:28-75): what the verifier (and ProofWithPublicInputs::compress)
-    re-derives from a proof. Returns (fri_alpha, fri_betas, fri_pow_response, fri_query_indices)."""
+def fri_challenges(challenger, commit_phase_merkle_caps, final_poly, pow_witness, degree_bits, config,
+                   final_poly_coeff_len=None, max_num_query_steps=None):
+    """Challenger::fri_challenges (fri/challenges.rs:28-89): what the verifier (and ProofWithPublicInputs::compress)
+    re-derives from a proof. final_poly_coeff_len / max_num_query_steps: the zero caps and zero coefficients a proof
+    made for a verifier circuit of other FRI parameters observes (as fri_committed_trees does).
+    Returns (fri_alpha, fri_betas, fri_pow_response, fri_query_indices)."""
     lde_size = 1 << (degree_bits + config.rate_bits)
     fri_alpha = challenger.get_extension_challenge()
     fri_betas = []
     for cap in commit_phase_merkle_caps:
         challenger.observe_cap(cap)
         fri_betas.append(challenger.get_extension_challenge())
-    challenger.observe_elements(np.asarray(final_poly, dtype=np.uint64).reshape(-1))
+    if max_num_query_steps is not None:
+        zero_cap = [0] * (NUM_HASH_OUT_ELTS << config.cap_height)
+        for _ in range(len(commit_phase_merkle_caps), max_num_query_steps):
+            challenger.observe_elements(zero_cap)
+            challenger.get_extension_challenge()
+    final_poly = np.asarray(final_poly, dtype=np.uint64).reshape(-1, 2)
+    challenger.observe_elements(final_poly.reshape(-1))
+    if final_poly_coeff_len is not None:
+        for _ in range(len(final_poly), final_poly_coeff_len):
+            challenger.observe_extension_element((0, 0))
     challenger.observe_element(pow_witness)
     fri_pow_response = challenger.get_challenge()
     fri_query_indices = [challenger.get_challenge() % lde_size for _ in range(config.num_query_rounds)]

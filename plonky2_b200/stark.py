@@ -1,14 +1,19 @@
-"""starky's prover path adjacent to the commitment kernels (SURVEY.md section 8f row 1): Stark constraints, the quotient
-polynomials and their commitment, mirroring starky/src/{stark.rs, constraint_consumer.rs, prover.rs:391-421,488-668,
-fibonacci_stark.rs}. The constraints of a Stark are recorded ONCE as a straight-line program (ConstraintBuilder) and
-evaluated by gl_stark_quotient on every point of the quotient coset, reading the trace LDE in place on the device."""
+"""starky's prover (SURVEY.md section 8f rows 1 and 1'), mirroring starky/src/{config.rs, stark.rs,
+constraint_consumer.rs, vanishing_poly.rs, prover.rs, proof.rs, get_challenges.rs, fibonacci_stark.rs} for STARKs
+without lookups or cross-table lookups. The constraints of a Stark are recorded ONCE as a straight-line program
+(ConstraintBuilder): gl_stark_quotient evaluates it on every point of the quotient coset, reading the trace LDE in place
+on the device, and eval_vanishing_poly evaluates the same instructions at one point of F_{p^2} on the host (the
+constraint-binding step of `prove`, and any verifier). `prove` strings the device steps together in the reference's
+order with the transcript on the host."""
 import ctypes as C
 
 import numpy as np
 
 from . import _native as N
 from . import field as F
+from .fri import starky_standard_fast_fri_config
 from .polynomial_batch import PolynomialBatch
+from .proof import StarkOpeningSet
 
 OP_LOCAL, OP_NEXT, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_EMIT = range(7)
 KIND_CONSTRAINT, KIND_TRANSITION, KIND_FIRST_ROW, KIND_LAST_ROW = range(4)
@@ -118,6 +123,25 @@ class Stark:
         self.eval(b, b)
         return b
 
+    def num_quotient_polys(self, config):
+        """stark.rs:95-98"""
+        return self.quotient_degree_factor() * config.num_challenges
+
+    def fri_instance(self, zeta, g, config):
+        """fri_instance (stark.rs:101-170) without auxiliary (lookup / CTL) polynomials: the trace oracle opened at zeta
+        and g * zeta, the quotient oracle -- present only when the Stark has constraints -- at zeta."""
+        from .fri import FriBatchInfo, FriInstanceInfo, FriOracleInfo, FriPolynomialInfo
+
+        trace_info = FriPolynomialInfo.from_range(0, range(self.COLUMNS))
+        oracles = [FriOracleInfo(self.COLUMNS, False)]
+        quotient_info = []
+        nq = self.num_quotient_polys(config)
+        if nq > 0:
+            quotient_info = FriPolynomialInfo.from_range(len(oracles), range(nq))
+            oracles.append(FriOracleInfo(nq, False))
+        zeta_next = F.ext_mul((int(g) % F.ORDER, 0), zeta)
+        return FriInstanceInfo(oracles, [FriBatchInfo(zeta, trace_info + quotient_info), FriBatchInfo(zeta_next, trace_info)])
+
 
 class FibonacciStark(Stark):
     """FibonacciStark (starky/src/fibonacci_stark.rs:19-120): columns (x0, x1), x0' = x1, x1' = x0 + x1; public inputs
@@ -182,3 +206,248 @@ def commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_hei
     device tensor compute_quotient_polys returned."""
     return PolynomialBatch._from_coeff_chunks(quotient_polys, stark.quotient_degree_factor(), degree_bits, rate_bits,
                                               cap_height, ctx)
+
+
+class StarkConfig:
+    """StarkConfig (starky/src/config.rs:21-117): target security, number of challenges, FRI configuration."""
+
+    def __init__(self, security_bits, num_challenges, fri_config):
+        self.security_bits, self.num_challenges, self.fri_config = security_bits, num_challenges, fri_config
+
+    @classmethod
+    def standard_fast_config(cls):
+        """config.rs:52-64: rate 1/2, ~100 bits of conjectured security."""
+        return cls(100, 2, starky_standard_fast_fri_config())
+
+    def fri_params(self, degree_bits):
+        """config.rs:67-69: starky never hides."""
+        return self.fri_config.fri_params(degree_bits, False)
+
+    def observe(self, challenger):
+        """config.rs:102-107"""
+        challenger.observe_element(self.security_bits)
+        challenger.observe_element(self.num_challenges)
+        self.fri_config.observe(challenger)
+
+
+def eval_l_0_and_l_last(log_n, x):
+    """eval_l_0_and_l_last (vanishing_poly.rs:96-106) at x in F_{p^2}: L_0(x) = (x^n - 1) / (n (x - 1)),
+    L_{n-1}(x) = (x^n - 1) / (n (g x - 1))."""
+    n = ((1 << log_n) % F.ORDER, 0)
+    g = (F.primitive_root_of_unity(log_n), 0)
+    z_x = F.ext_sub(F.ext_pow(x, 1 << log_n), (1, 0))
+    l_0 = F.ext_mul(z_x, F.ext_inverse(F.ext_mul(n, F.ext_sub(x, (1, 0)))))
+    l_last = F.ext_mul(z_x, F.ext_inverse(F.ext_mul(n, F.ext_sub(F.ext_mul(g, x), (1, 0)))))
+    return l_0, l_last
+
+
+def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas, x, degree_bits):
+    """compute_eval_vanishing_poly (vanishing_poly.rs:108-173) without lookups or CTLs: the Stark's constraint program
+    -- the instructions gl_stark_quotient runs -- evaluated at one point x of F_{p^2}, with the local and next rows as
+    F_{p^2} values and the public inputs and program constants as base-field values; the constraints are filtered by
+    z_last = x - g^{-1}, L_0(x), L_{n-1}(x) and folded with every alpha as ConstraintConsumer does
+    (constraint_consumer.rs:46-84). Returns num_challenges F_{p^2} values (c0, c1)."""
+    b = stark.constraint_program()
+    if len(public_inputs) != stark.PUBLIC_INPUTS:
+        raise N.ShapeError("expected %d public inputs, got %d" % (stark.PUBLIC_INPUTS, len(public_inputs)))
+    consts = [int(v) % F.ORDER for v in public_inputs] + b.consts[b.num_pi:]
+    x = (int(x[0]) % F.ORDER, int(x[1]) % F.ORDER)
+    l_0, l_last = eval_l_0_and_l_last(degree_bits, x)
+    z_last = F.ext_sub(x, (F.inverse(F.primitive_root_of_unity(degree_bits)), 0))
+    filters = {KIND_CONSTRAINT: None, KIND_TRANSITION: z_last, KIND_FIRST_ROW: l_0, KIND_LAST_ROW: l_last}
+
+    def ext(v):
+        return (int(v[0]) % F.ORDER, int(v[1]) % F.ORDER)
+
+    acc = [(0, 0)] * len(alphas)
+    vals = []
+    for op, a, c in b.instrs:
+        r = (0, 0)
+        if op == OP_LOCAL:
+            r = ext(local_values[a])
+        elif op == OP_NEXT:
+            r = ext(next_values[a])
+        elif op == OP_CONST:
+            r = (consts[a], 0)
+        elif op == OP_ADD:
+            r = F.ext_add(vals[a], vals[c])
+        elif op == OP_SUB:
+            r = F.ext_sub(vals[a], vals[c])
+        elif op == OP_MUL:
+            r = F.ext_mul(vals[a], vals[c])
+        else:  # OP_EMIT
+            e = vals[a] if filters[c] is None else F.ext_mul(vals[a], filters[c])
+            acc = [F.ext_add(F.ext_mul(s, (int(al) % F.ORDER, 0)), e) for s, al in zip(acc, alphas)]
+        vals.append(r)
+    return acc
+
+
+def _dummy_openings(challenger, num_trace_polys, pow_degree):
+    """get_dummy_polys (get_challenges.rs:201-256, prover.rs:272-319) without auxiliary polynomials: simulated local and
+    next values c_i, c_i^d, c_i^{d^2}, ... from fresh extension challenges c_i, d = pow_degree."""
+    log_pow_degree = (pow_degree - 1).bit_length()
+    num_extension_powers = max(1, 50 // log_pow_degree - 1)
+    total = 2 * num_trace_polys
+    zetas = challenger.get_n_extension_challenges(-(-total // num_extension_powers))
+    per_zeta = min(num_extension_powers + 1, total)
+    evals = []
+    for z in zetas:
+        for _ in range(per_zeta):
+            evals.append(z)
+            z = F.ext_pow(z, pow_degree)
+    return evals[:num_trace_polys], evals[num_trace_polys:total]
+
+
+def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_bits):
+    """The constraint-binding step (prover.rs:239-370, get_challenges.rs:94-163): alphas', simulated openings, zeta',
+    the vanishing polynomial there observed; returns the alphas the quotient uses."""
+    alphas_prime = challenger.get_n_challenges(num_challenges)
+    pow_degree = max(2, stark.constraint_degree() + 1)
+    local, nxt = _dummy_openings(challenger, stark.COLUMNS, pow_degree)
+    zeta_prime = challenger.get_extension_challenge()
+    challenger.observe_extension_elements(eval_vanishing_poly(stark, local, nxt, public_inputs, alphas_prime, zeta_prime,
+                                                              degree_bits))
+    return challenger.get_n_challenges(num_challenges)
+
+
+class StarkProof:
+    """StarkProof (starky/src/proof.rs:30-53) without auxiliary polynomials: trace cap, quotient cap (None for a Stark
+    without constraints), StarkOpeningSet, FriProof. The reference has no byte format for it (serde only);
+    opening_proof.to_bytes() is write_fri_proof."""
+
+    def __init__(self, trace_cap, quotient_polys_cap, openings, opening_proof):
+        self.trace_cap, self.quotient_polys_cap = trace_cap, quotient_polys_cap
+        self.openings, self.opening_proof = openings, opening_proof
+
+    def recover_degree_bits(self, config):
+        """proof.rs:45-52: from the length of the first initial-tree Merkle proof."""
+        siblings = self.opening_proof.query_round_proofs[0].initial_trees_proof.evals_proofs[0][1]
+        return config.fri_config.cap_height + len(siblings) - config.fri_config.rate_bits
+
+
+class StarkProofWithPublicInputs:
+    """StarkProofWithPublicInputs (proof.rs:133-145)."""
+
+    def __init__(self, proof, public_inputs):
+        self.proof, self.public_inputs = proof, [int(v) % F.ORDER for v in public_inputs]
+
+    def get_challenges(self, stark, config, verifier_circuit_fri_params=None):
+        """get_challenges (get_challenges.rs:37-199,323-357) replayed from the proof alone: the public inputs, the
+        config, the trace cap, the constraint-binding step, the quotient cap, zeta, the openings, then FRI's challenges.
+        Returns a dict: stark_alphas, stark_zeta, fri_alpha, fri_betas, fri_pow_response, fri_query_indices."""
+        from .challenger import Challenger
+        from .fri import fri_challenges
+
+        p = self.proof
+        degree_bits = p.recover_degree_bits(config)
+        ch = Challenger()
+        ch.observe_elements(self.public_inputs)
+        config.observe(ch)
+        ch.observe_cap(p.trace_cap)
+        alphas = _bind_constraints(stark, ch, self.public_inputs, config.num_challenges, degree_bits)
+        if p.quotient_polys_cap is not None:
+            ch.observe_cap(p.quotient_polys_cap)
+        zeta = ch.get_extension_challenge()
+        for batch in p.openings.to_fri_openings():                      # Challenger::observe_openings
+            ch.observe_elements(batch.reshape(-1))
+        final_len = steps = None
+        if verifier_circuit_fri_params is not None:
+            vp = verifier_circuit_fri_params
+            final_len, steps = 1 << (vp.degree_bits - vp.total_arities()), len(vp.reduction_arity_bits)
+        fp = p.opening_proof
+        fri_alpha, fri_betas, pow_response, indices = fri_challenges(ch, fp.commit_phase_merkle_caps, fp.final_poly,
+                                                                     fp.pow_witness, degree_bits, config.fri_config,
+                                                                     final_len, steps)
+        return dict(stark_alphas=alphas, stark_zeta=zeta, fri_alpha=fri_alpha, fri_betas=fri_betas,
+                    fri_pow_response=pow_response, fri_query_indices=indices)
+
+
+def _commit_trace(trace, rate_bits, cap_height, ctx):
+    """The trace commitment (prover.rs:83-94) from host columns or from a (COLUMNS, n) torch CUDA tensor on the context's
+    device (read in place, never copied to the host)."""
+    if hasattr(trace, "data_ptr"):
+        import torch
+
+        if not trace.is_cuda or trace.dim() != 2 or trace.element_size() != 8:
+            raise N.ShapeError("a torch trace must be a (COLUMNS, n) CUDA tensor of 64-bit words")
+        cols = trace.contiguous().view(torch.int64)
+        B, n = cols.shape
+        log_n = F.log2_strict(n)
+
+        def add_columns(h):
+            N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(cols.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE), ctx.h)
+
+        return PolynomialBatch._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns)
+    return PolynomialBatch.from_values(trace, rate_bits, False, cap_height, ctx=ctx)
+
+
+def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None):
+    """prove + prove_with_commitment (starky/src/prover.rs:40-114,125-484) for a Stark without lookups or CTLs:
+    trace = (COLUMNS, n) host columns or torch CUDA tensor -> StarkProofWithPublicInputs. Every array-sized step runs on
+    the device (trace commitment, quotient from the LDE in place, quotient commitment, openings, FRI); the transcript and
+    the constraint-binding step run on the host. verifier_circuit_fri_params: the FRI parameters of a verifier circuit
+    made for another degree (ConstantArityBits only); the transcript then observes the zero caps and coefficients that
+    verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment is released on
+    every exit path."""
+    from .challenger import Challenger
+    from .fri import prove_openings
+
+    ctx = ctx or N.default_context()
+    shape = tuple(trace.shape)
+    if len(shape) != 2 or shape[0] != stark.COLUMNS:
+        raise N.ShapeError("the trace must be (COLUMNS = %d, n), got %r" % (stark.COLUMNS, shape))
+    if len(public_inputs) != stark.PUBLIC_INPUTS:
+        raise N.ShapeError("expected %d public inputs, got %d" % (stark.PUBLIC_INPUTS, len(public_inputs)))
+    public_inputs = [int(v) % F.ORDER for v in public_inputs]
+    degree_bits = F.log2_strict(shape[1])
+    fri_params = config.fri_params(degree_bits)
+    rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
+    if fri_params.total_arities() > degree_bits + rate_bits - cap_height:
+        raise N.ShapeError("FRI total reduction arity is too large.")
+    if stark.constraint_degree() > (1 << rate_bits) + 1:
+        raise N.ShapeError("The degree of the Stark constraints must be <= blowup_factor + 1")
+    final_poly_coeff_len = max_num_query_steps = None
+    if verifier_circuit_fri_params is not None:
+        vp = verifier_circuit_fri_params
+        if vp.config != fri_params.config:
+            raise N.ShapeError("verifier_circuit_fri_params.config differs from the proof's FRI config")
+        strategy = config.fri_config.reduction_strategy
+        if strategy[0] != "ConstantArityBits":
+            raise N.ShapeError("Fri Reduction Strategy is not ConstantArityBits")
+        final_poly_coeff_len = 1 << (vp.degree_bits - vp.total_arities())       # final_poly_coeff_len (fri/prover.rs:77)
+        if final_poly_coeff_len != 1 << (1 + strategy[2]):
+            raise N.ShapeError("the verifier circuit's final polynomial has %d coefficients, expected %d"
+                               % (final_poly_coeff_len, 1 << (1 + strategy[2])))
+        max_num_query_steps = len(vp.reduction_arity_bits)
+
+    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx)
+    commitments = [trace_commitment]
+    try:
+        challenger = Challenger()
+        challenger.observe_elements(public_inputs)
+        config.observe(challenger)
+        challenger.observe_cap(trace_commitment.merkle_tree.cap)
+        alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits)
+        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas)
+        quotient_commitment = None
+        if quotient_polys is not None:
+            quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx)
+            commitments.append(quotient_commitment)
+            del quotient_polys
+            challenger.observe_cap(quotient_commitment.merkle_tree.cap)
+        zeta = challenger.get_extension_challenge()
+        if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
+            raise N.NativeError("Opening point is in the subgroup.")
+        g = F.primitive_root_of_unity(degree_bits)
+        openings = StarkOpeningSet.new(zeta, g, trace_commitment, None, quotient_commitment)
+        for batch in openings.to_fri_openings():                        # Challenger::observe_openings
+            challenger.observe_elements(batch.reshape(-1))
+        opening_proof = prove_openings(stark.fri_instance(zeta, g, config), commitments, challenger, fri_params,
+                                       final_poly_coeff_len, max_num_query_steps)
+        proof = StarkProof(trace_commitment.merkle_tree.cap,
+                           quotient_commitment.merkle_tree.cap if quotient_commitment is not None else None,
+                           openings, opening_proof)
+        return StarkProofWithPublicInputs(proof, public_inputs)
+    finally:
+        for c in commitments:
+            c.close()
