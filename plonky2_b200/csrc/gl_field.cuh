@@ -244,11 +244,11 @@ GL_HD void mul_wide(uint64_t a, uint64_t b, uint64_t& lo, uint64_t& hi) {
     hi = (uint64_t)(p >> 64);
 #endif
 }
-GL_HD void sqr_wide(uint64_t a, uint64_t& lo, uint64_t& hi) {
-#if defined(__CUDA_ARCH__) && defined(GL_SQR_3WIDE)
-    // Variant: a^2 = a0^2 + 2*a0*a1*2^32 + a1^2*2^64 with THREE IMAD.WIDE.U32 and the cross term added twice on
-    // the ALU pipe. Off by default: with both integer pipes busy, the extra ALU work can cost more than the saved
-    // IMAD.WIDE (tools/variants ranks the two forms on the GPU at hand).
+// a^2 = a0^2 + 2*a0*a1*2^32 + a1^2*2^64 with THREE IMAD.WIDE.U32, the cross term added twice on the ALU pipe.
+// Poseidon's S-box squares with it (sqr_3w): with 4 CTAs/SM of 128 threads (no spills) it ranks above the
+// four-product form in tools/variants (DESIGN.md §4). The generic sqr keeps mul_wide unless GL_SQR_3WIDE.
+GL_HD void sqr_wide_3w(uint64_t a, uint64_t& lo, uint64_t& hi) {
+#if defined(__CUDA_ARCH__)
     uint32_t r0, r1, r2, r3;
     asm("{\n\t.reg .u64 z, c, w;\n\t.reg .u32 z1, c0, c1, w0, w1;\n\t"
         "mul.wide.u32 z, %4, %4;\n\t"
@@ -267,8 +267,6 @@ GL_HD void sqr_wide(uint64_t a, uint64_t& lo, uint64_t& hi) {
         : "r"(lo32(a)), "r"(hi32(a)));
     lo = pack64(r0, r1);
     hi = pack64(r2, r3);
-#elif defined(__CUDA_ARCH__)
-    mul_wide(a, a, lo, hi);
 #elif defined(GL_FORCE_32BIT_PATH)
     uint32_t a0 = (uint32_t)a, a1 = (uint32_t)(a >> 32);
     uint64_t p00 = (uint64_t)a0 * a0;
@@ -279,6 +277,15 @@ GL_HD void sqr_wide(uint64_t a, uint64_t& lo, uint64_t& hi) {
     uint64_t m2 = p01 + (uint32_t)m;                          // < 2^64
     hi = p11 + (m >> 32) + (m2 >> 32);
     lo = (m2 << 32) | (uint32_t)p00;
+#else
+    unsigned __int128 p = (unsigned __int128)a * a;
+    lo = (uint64_t)p;
+    hi = (uint64_t)(p >> 64);
+#endif
+}
+GL_HD void sqr_wide(uint64_t a, uint64_t& lo, uint64_t& hi) {
+#if defined(GL_SQR_3WIDE) || (defined(GL_FORCE_32BIT_PATH) && !defined(__CUDA_ARCH__))
+    sqr_wide_3w(a, lo, hi);
 #else
     mul_wide(a, a, lo, hi);
 #endif
@@ -292,6 +299,11 @@ GL_HD uint64_t mul(uint64_t a, uint64_t b) {
 GL_HD uint64_t sqr(uint64_t a) {
     uint64_t lo, hi;
     sqr_wide(a, lo, hi);
+    return reduce128(lo, hi);
+}
+GL_HD uint64_t sqr_3w(uint64_t a) {
+    uint64_t lo, hi;
+    sqr_wide_3w(a, lo, hi);
     return reduce128(lo, hi);
 }
 // a * b + c (mod p) with one reduction (multiply_accumulate, goldilocks_field.rs:184-188)

@@ -14,7 +14,8 @@
 //  * partial rounds: lanes 1..11 never leave the FP64 pipe for all 22 rounds and two rounds are one linear step
 //    (poseidon_partial_rounds_f64) -- the reference's "fast" w_hat / v factorisation (23 64x64 products per
 //    round) is only used on the host and under -DGL_PARTIAL_FAST;
-//  * u32 <-> f64 conversions are I2F / F2I on the XU pipe.
+//  * f64 -> u64 conversions are F2I on the XU pipe; the S-box's u32 words enter the FP64 pipe as 2^52-offset doubles
+//    built by register moves (sbox7_f64), the squarings are three 32x32 products each (sqr_3w).
 // The rounds are rolled loops (one copy of each round body) so the permutation fits the instruction cache.
 // Each of these steps (single 128-bit product, FP64-resident partial rounds, two rounds per step, split circulant
 // MDS) was kept because it raised the leaf-hash permutation rate over the integer fast form; tools/variants/
@@ -27,7 +28,8 @@
 // IMAD on its own pipe (tools/pipe_mix.cu: a DFMA + IMAD stream runs at the speed of either alone), and every
 // sum is < 2^53, so doubles are exact. Define GL_MDS_INT to force the integer (IMAD.WIDE) formulation.
 // Other measured alternatives kept as switches: GL_PARTIAL_FAST (integer rounds everywhere),
-// GL_CVT_MAGIC (2^52 magic-number conversions on the FP64 pipe); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT,
+// GL_CVT_MAGIC (2^52 magic-number conversions on the FP64 pipe everywhere), GL_SBOX_I2F (I2F in the S-box),
+// GL_SBOX_SQR4 (four-product squarings in the S-box); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT,
 // GL_REDUCE_V1. tools/variants/ ranks them with one GPU call.
 #if !defined(GL_MDS_INT) && !defined(GL_MDS_FP64)
 #define GL_MDS_FP64 1
@@ -232,6 +234,17 @@ GL_HD double u32_to_f64(uint32_t x) {
     return (double)x;  // I2F.F64.U32 on the (idle) XU pipe: one instruction, exact
 #endif
 }
+// The double 2^52 + x (bit pattern 0x43300000:x), exact for any 32-bit x.
+GL_HD double u32_magic_f64(uint32_t x) {
+#if defined(__CUDA_ARCH__)
+    return __hiloint2double(0x43300000, (int)x);
+#else
+    const uint64_t b = 0x4330000000000000ULL | x;
+    double d;
+    __builtin_memcpy(&d, &b, 8);
+    return d;
+#endif
+}
 // al + 2^32 * ah (mod p) for NON-NEGATIVE integers al, ah < 2^52 held in doubles.
 GL_HD uint64_t f64_pair_to_u64(double al, double ah) {
 #if defined(__CUDA_ARCH__) && !defined(GL_CVT_MAGIC)
@@ -291,16 +304,33 @@ GL_HD uint64_t sbox7(uint64_t x) {  // sbox_monomial, poseidon.rs:689-696
 // words, 2^64 = 2^32 - 1 and 2^96 = -1 give  x^7 = (p0 - p2 - p3) + 2^32 * (p1 + p2)  (mod p), i.e. exactly a
 // (signed) limb pair (L, H), |L| < 2^33.6, 0 <= H < 2^33: three FP64 adds replace the 11-instruction integer
 // reduce128, and the MDS constants carry a bias = 0 (mod p) that makes its outputs positive again.
+// The squarings are the three-product form (sqr_3w; -DGL_SBOX_SQR4 restores mul_wide's four), and the four words
+// enter the FP64 pipe as 2^52 + w (bits 0x43300000:w, a register move each) instead of through four I2F.F64, which
+// cost about 6 issue clocks each when mixed with IMAD.WIDE (tools/pipe_mix2.cu); -DGL_SBOX_I2F restores them. The
+// 2^52 offsets cancel inside the same adds: H = (m1 - 2^53) + m2, L = (m0 - m2) - (m3 - 2^52); every intermediate
+// is an integer below 2^53 in magnitude, so all five adds are exact.
 GL_HD void sbox7_f64(uint64_t x, double& L, double& H) {
+#if defined(GL_SBOX_SQR4)
     const uint64_t x2 = sqr(x);
     const uint64_t x4 = sqr(x2);
+#else
+    const uint64_t x2 = sqr_3w(x);
+    const uint64_t x4 = sqr_3w(x2);
+#endif
     const uint64_t x3 = mul(x, x2);
     uint64_t lo, hi;
     mul_wide(x3, x4, lo, hi);
+#if !defined(GL_SBOX_I2F)
+    const double m0 = u32_magic_f64((uint32_t)lo), m1 = u32_magic_f64((uint32_t)(lo >> 32));
+    const double m2 = u32_magic_f64((uint32_t)hi), m3 = u32_magic_f64((uint32_t)(hi >> 32));
+    H = (m1 - 9007199254740992.0) + m2;
+    L = (m0 - m2) - (m3 - 4503599627370496.0);
+#else
     const double d0 = u32_to_f64((uint32_t)lo), d1 = u32_to_f64((uint32_t)(lo >> 32));
     const double d2 = u32_to_f64((uint32_t)hi), d3 = u32_to_f64((uint32_t)(hi >> 32));
     L = (d0 - d2) - d3;
     H = d1 + d2;
+#endif
 }
 #endif
 

@@ -287,7 +287,12 @@ __host__ __device__ __forceinline__ size_t digest_pos(size_t q, uint32_t i) {
 }
 
 constexpr int HASH_CTA = 128;   // CTA size of the barrier-synchronised Poseidon kernels
-constexpr int HASH_MINB = 5;    // 5 CTAs/SM => up to 96 registers/thread (best of the microbench sweep: 820 M perm/s)
+// 4 CTAs/SM => up to 128 registers/thread: the permutation runs without spills (at 5 CTAs / 96 registers both round
+// loops spill); -DGL_HASH_MINB=5 restores the former budget for tools/lib_variants.py.
+#ifndef GL_HASH_MINB
+#define GL_HASH_MINB 4
+#endif
+constexpr int HASH_MINB = GL_HASH_MINB;
 __global__ void __launch_bounds__(HASH_CTA, HASH_MINB) k_leaf_hash(TreeView t) {
     size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool live = j < t.N;

@@ -24,6 +24,10 @@ VARIANTS = {
     "sqr3": ["-DGL_SQR_3WIDE"],
     "mulx": ["-DGL_MUL_EXPLICIT"],
     "pfast": ["-DGL_PARTIAL_FAST"],
+    "minb5": ["-DGL_HASH_MINB=5"],
+    "sboxsqr4": ["-DGL_SBOX_SQR4"],
+    "sboxi2f": ["-DGL_SBOX_I2F"],
+    "parent": ["-DGL_HASH_MINB=5", "-DGL_SBOX_SQR4", "-DGL_SBOX_I2F"],
 }
 
 

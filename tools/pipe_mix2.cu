@@ -1,5 +1,9 @@
 // Round-2 follow-up to pipe_mix.cu: issue cost of the instruction classes the NTT / Poseidon rewrites lean on
 // (IMAD.HI, IMAD.WIDE without addend, funnel shifts, carry chains, PRMT, SHFL, LDS) alone and mixed.
+// Also: the 64x64->128 product as ptxas builds it from unsigned __int128 (IMAD.WIDE.U32 + IMAD.WIDE.U32.X, with the
+// moves and carry materialisation it brings), mixed at the full-round body's ratios with IADD3, DFMA and I2F;
+// mul.lo.u32 + mul.hi.u32 of the same operands (ptxas may fuse them back into one IMAD.WIDE: check the SASS); and
+// LDC.64 from a __constant__ table at a loop-variant index, the form the rolled round loops load constants in.
 // Each stream has ILP independent chains per thread; 16 warps per SMSP hide latency, so the numbers are
 // issue/pipe throughput: cycles per warp-instruction per SMSP.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/pipe_mix2 tools/pipe_mix2.cu
@@ -9,7 +13,9 @@
 constexpr int ILP = 8, ITERS = 2048;
 
 enum { S_HI = 1, S_MULHI = 2, S_WIDE_ACC = 4, S_WIDE_NOACC = 8, S_SHF = 16, S_CARRY = 32, S_PRMT = 64, S_SHFL = 128,
-       S_LO = 256, S_LOP = 512, S_DFMA = 1024, S_LDS = 2048, S_IADD3 = 4096, S_SEL = 8192 };
+       S_LO = 256, S_LOP = 512, S_DFMA = 1024, S_LDS = 2048, S_IADD3 = 4096, S_SEL = 8192, S_MUL128 = 16384,
+       S_LOHI = 32768, S_LDC = 65536, S_I2F = 131072 };
+__constant__ double c_tab[64];
 
 template <int M>
 __global__ void k_mix(uint64_t* out, uint32_t ix, double dx) {
@@ -39,6 +45,13 @@ __global__ void k_mix(uint64_t* out, uint32_t ix, double dx) {
             if (M & S_DFMA) asm volatile("fma.rn.f64 %0, %0, %1, %2;" : "+d"(d[i]) : "d"(dx), "d"(1.0));
             if (M & S_LDS) { uint32_t idx = (c[i] & 255u); uint64_t v; asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"((uint32_t)__cvta_generic_to_shared(&sh[idx]))); c[i] = (uint32_t)v + (uint32_t)(v >> 32); }
             if (M & S_IADD3) asm volatile("{\n\t.reg .u32 t;\n\tadd.u32 t, %0, %1;\n\tadd.u32 %0, t, %2;\n\t}" : "+r"(a[i]) : "r"(ix), "r"(b[i]));
+            if (M & S_MUL128) {
+                const unsigned __int128 q = (unsigned __int128)w[i] * (w[i] ^ ((uint64_t)ix << 32 | 0x9E3779B9u));
+                w[i] = (uint64_t)q ^ (uint64_t)(q >> 64);
+            }
+            if (M & S_LOHI) asm volatile("{\n\t.reg .u32 t, u;\n\tmul.lo.u32 t, %0, %1;\n\tmul.hi.u32 u, %0, %1;\n\txor.b32 %0, t, u;\n\t}" : "+r"(h[i]) : "r"(ix * 0x85EBCA6Bu + 0xF0000001u));
+            if (M & S_LDC) d[i] += c_tab[(it + i) & 63];
+            if (M & S_I2F) d[i] += (double)(b[i] += ix);
             if (M & S_SEL) asm volatile("{\n\t.reg .pred p;\n\tsetp.lt.u32 p, %0, %1;\n\tselp.u32 %0, %2, %0, p;\n\t}" : "+r"(a[i]) : "r"(ix + 77), "r"(b[i]));
         }
     }
@@ -92,5 +105,16 @@ int main() {
     RUN(S_SHFL | S_LO | S_LOP, "SHFL + IMAD + LOP3");
     RUN(S_LDS | S_LO, "LDS.64 + 2 int + IMAD");
     RUN(S_LOP | S_LO | S_DFMA | S_SHF, "LOP3 + IMAD + DFMA + SHF");
+    // one group of these = one 128-bit product (4 IMAD.WIDE) plus its companions; the full-round body has per
+    // product about 2.4 IADD3, 0.6 IMAD.MOV, 1.2 DFMA, 0.4 I2F, 0.13 LDC.64
+    RUN(S_MUL128, "128-bit product (u128)");
+    RUN(S_LOHI, "mul.lo + mul.hi same operands");
+    RUN(S_LDC, "LDC.64 (loop-variant index) + DADD");
+    RUN(S_I2F, "IADD + I2F.F64.U32 + DADD");
+    RUN(S_MUL128 | S_IADD3, "128-bit product + 2 IADD3");
+    RUN(S_MUL128 | S_IADD3 | S_DFMA, "128-bit product + 2 IADD3 + DFMA");
+    RUN(S_MUL128 | S_IADD3 | S_DFMA | S_I2F, "128-bit + 2 IADD3 + DFMA + I2F");
+    RUN(S_MUL128 | S_LDC, "128-bit product + LDC.64");
+    RUN(S_WIDE_ACC | S_IADD3 | S_DFMA, "IMAD.WIDE acc + 2 IADD3 + DFMA");
     return 0;
 }

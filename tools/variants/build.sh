@@ -12,9 +12,13 @@ v pfast -DGL_PARTIAL_FAST
 v mdsint -DGL_MDS_INT
 v mulx -DGL_MUL_EXPLICIT
 v sqr3 -DGL_SQR_3WIDE
+v sboxsqr4 -DGL_SBOX_SQR4
+v sboxi2f -DGL_SBOX_I2F
+v parent -DGL_SBOX_SQR4 -DGL_SBOX_I2F -DVB_MINB=5      # the S-box and budget before the spill-free change
+v parentb4 -DGL_SBOX_SQR4 -DGL_SBOX_I2F                # that S-box at the shipped budget
 v redv1 -DGL_REDUCE_V1
 v nosync -DVB_SYNC=0
-v t128b4 -DVB_MINB=4
+v t128b5 -DVB_MINB=5
 v t128b6 -DVB_MINB=6
 v t256b2 -DVB_THREADS=256 -DVB_MINB=2
 v t64b10 -DVB_THREADS=64 -DVB_MINB=10

@@ -6,7 +6,7 @@
 #define VB_THREADS 128
 #endif
 #ifndef VB_MINB
-#define VB_MINB 5
+#define VB_MINB 4  // HASH_MINB of plonky2_b200.cu
 #endif
 #ifndef VB_SYNC
 #define VB_SYNC 1
