@@ -219,7 +219,7 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
  * result of instruction k; GL_STARK_EMIT feeds a value to the ConstraintConsumer (constraint_consumer.rs:46-84).
  * consts = the public inputs followed by the program's constants. Split the result into degree-n chunks with
  * gl_commit_begin / gl_commit_add_columns(GL_COLS_COEFFS) to obtain the quotient commitment (prover.rs:391-421). */
-#define GL_STARK_LOCAL 0 /* a = trace column: local row value */
+#define GL_STARK_LOCAL 0 /* a = trace column: local row value (opcodes 7 and 8: gl_stark_quotient_aux below) */
 #define GL_STARK_NEXT 1  /* a = trace column: next row value */
 #define GL_STARK_CONST 2 /* a = index into consts */
 #define GL_STARK_ADD 3   /* values a + b */
@@ -241,6 +241,39 @@ typedef struct {
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
                       const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
                       uint32_t quotient_degree_factor, uint64_t* out_coeffs);
+/* gl_stark_quotient for a STARK with an auxiliary commitment (the logUp helper columns, starky/src/prover.rs:216-230):
+ * the program may also read the auxiliary polynomials' LDE in place, at the same leaves as the trace. `aux` must be
+ * finished, whole on this device and of the trace's degree and rate. The lookup constraints (lookup.rs:804-863) follow
+ * the STARK's own in the program; the lookup challenges are bound in consts like the public inputs. */
+#define GL_STARK_AUX_LOCAL 7 /* a = auxiliary column: local row value */
+#define GL_STARK_AUX_NEXT 8  /* a = auxiliary column: next row value */
+int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                          uint32_t quotient_degree_factor, uint64_t* out_coeffs);
+
+/* starky's logUp helper columns (lookup_helper_columns, starky/src/lookup.rs:579-652, for every Lookup and every challenge
+ * in the reference's order, prover.rs:178-195) on the device. trace: COLUMNS value columns of n = 2^log_n words at
+ * trace + k*col_stride; out: the auxiliary polynomials' values, column j at out + j*n. Both are DEVICE memory.
+ * Lookup l (l < n_lookups) is the row program program[lookup_offsets[l] .. lookup_offsets[l + 1]) in the gl_stark_instr
+ * format, instruction operands relative to its first instruction: GL_STARK_LOCAL reads row i, GL_STARK_NEXT row
+ * (i + 1) mod n (Column::eval_table / Filter::eval_table, lookup.rs:118-129,323-335), GL_STARK_CONST reads consts, and
+ * GL_STARK_EMIT hands value a to the argument in role b: one GL_LOGUP_LOOKED and one GL_LOGUP_FILTER per looking column
+ * (in column order), exactly one GL_LOGUP_TABLE (t) and one GL_LOGUP_FREQUENCIES (m). For each lookup, for each
+ * challenge gamma, the output holds ceil(L / chunk) columns h_k = sum_{j in chunk k} filter_j / (f_j + gamma), chunk =
+ * constraint_degree - 1 (1 when that is 0), then Z with Z[0] = 0, Z[i + 1] = Z[i] + sum_k h_k[i] - m[i] / (t[i] + gamma).
+ * Errors: a zero denominator -> GL_ERR_DIV_ZERO ("Tried to invert zero"); constraint_degree 1 -> GL_ERR_BAD_SHAPE (the
+ * reference divides by zero); more than GL_LOGUP_MAX_COLUMNS looking columns, GL_LOGUP_MAX_INSTR instructions in a
+ * lookup or GL_STARK_MAX_ALPHAS challenges -> GL_ERR_UNSUPPORTED. */
+#define GL_LOGUP_LOOKED 0
+#define GL_LOGUP_FILTER 1
+#define GL_LOGUP_TABLE 2
+#define GL_LOGUP_FREQUENCIES 3
+#define GL_LOGUP_MAX_COLUMNS 16
+#define GL_LOGUP_MAX_INSTR 256
+int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,
+                            const gl_stark_instr* program, const uint32_t* lookup_offsets, uint32_t n_lookups,
+                            const uint64_t* consts, uint32_t n_consts, const uint64_t* challenges, uint32_t n_challenges,
+                            uint32_t constraint_degree, uint64_t* out);
 
 /* compute_quotient_polys of a plonky2 circuit (plonky2/src/plonk/prover.rs:609-815): for every challenge alpha_k the
  * values eval_vanishing_poly_base_batch(x) / Z_H(x) (plonky2/src/plonk/vanishing_poly.rs:167-340) on the coset g<w_size>,

@@ -16,6 +16,7 @@ from .polynomial_batch import SALT_SIZE, PolynomialBatch, random_field_elements_
 from .proof import OpeningSet, StarkOpeningSet, eval_commitments  # noqa: F401
 from .stark import (FibonacciStark, Stark, StarkConfig, StarkProof, StarkProofWithPublicInputs,  # noqa: F401
                     commit_quotient_polys, compute_quotient_polys, eval_l_0_and_l_last, eval_vanishing_poly)
+from .lookup import Column, Filter, GrandProductChallenge, Lookup, get_grand_product_challenge_set  # noqa: F401
 from . import stark  # noqa: F401  (stark.prove: the starky prover, next to plonk.prove_with_witness)
 from . import plonk  # noqa: F401  (plonk.compute_quotient_polys: the plonky2 circuit quotient)
 from .batch_merkle_tree import (BatchMerkleTree, compress_merkle_proofs, decompress_merkle_proofs,  # noqa: F401

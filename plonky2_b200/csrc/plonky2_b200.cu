@@ -27,6 +27,7 @@
 #include "../../include/plonky2_b200.h"
 #include "gl_chacha.cuh"
 #include "gl_field.cuh"
+#include "gl_logup.cuh"
 #include "gl_ntt.cuh"
 #include "gl_poseidon.cuh"
 #include "gl_vanishing.cuh"
@@ -1046,36 +1047,47 @@ __global__ void __launch_bounds__(128) k_pp_chunks(PPParams p) {
         inv_run = mul(inv_run, den[m]);
     }
 }
-// multiplicative inclusive prefix scan, 3 phases
+// inclusive prefix scan under an associative operator Op (ScanMul: the running products of Z and the partial products;
+// ScanAdd: logUp's running sum Z), 3 phases
+struct ScanMul {
+    static constexpr u64 identity = 1;
+    static __device__ __forceinline__ u64 op(u64 a, u64 b) { return mul(a, b); }
+};
+struct ScanAdd {
+    static constexpr u64 identity = 0;
+    static __device__ __forceinline__ u64 op(u64 a, u64 b) { return add(a, b); }
+};
+template <class Op>
 __global__ void __launch_bounds__(SCAN_THREADS) k_mscan_phase1(const u64* seq, size_t L, u64* chunk_tot) {
     __shared__ u64 sh[SCAN_THREADS];
     const size_t base = (size_t)blockIdx.x * SCAN_CHUNK + (size_t)threadIdx.x * SCAN_ITEMS;
-    u64 t = 1;
+    u64 t = Op::identity;
     for (int k = 0; k < SCAN_ITEMS; k++)
-        if (base + k < L) t = mul(t, seq[base + k]);
+        if (base + k < L) t = Op::op(t, seq[base + k]);
     sh[threadIdx.x] = t;
     __syncthreads();
     for (int off = SCAN_THREADS / 2; off > 0; off >>= 1) {
-        if ((int)threadIdx.x < off) sh[threadIdx.x] = mul(sh[threadIdx.x], sh[threadIdx.x + off]);
+        if ((int)threadIdx.x < off) sh[threadIdx.x] = Op::op(sh[threadIdx.x], sh[threadIdx.x + off]);
         __syncthreads();
     }
     if (threadIdx.x == 0) chunk_tot[blockIdx.x] = sh[0];
 }
-// exclusive prefix products of the chunk totals, one CTA: each thread owns a contiguous run
+// exclusive prefix of the chunk totals, one CTA: each thread owns a contiguous run
+template <class Op>
 __global__ void __launch_bounds__(1024) k_mscan_phase2(u64* chunk_tot, size_t nchunks) {
     __shared__ u64 sh[1024];
     const size_t per = (nchunks + 1023) / 1024;
     const size_t lo = (size_t)threadIdx.x * per, hi = lo + per < nchunks ? lo + per : nchunks;
-    u64 t = 1;
-    for (size_t k = lo; k < hi; k++) t = mul(t, chunk_tot[k]);
+    u64 t = Op::identity;
+    for (size_t k = lo; k < hi; k++) t = Op::op(t, chunk_tot[k]);
     sh[threadIdx.x] = t;
     __syncthreads();
-    if (threadIdx.x == 0) {  // 1024 sequential multiplies
-        u64 run = 1;
+    if (threadIdx.x == 0) {  // 1024 sequential steps
+        u64 run = Op::identity;
         for (int k = 0; k < 1024; k++) {
             u64 v = sh[k];
             sh[k] = run;
-            run = mul(run, v);
+            run = Op::op(run, v);
         }
     }
     __syncthreads();
@@ -1083,19 +1095,21 @@ __global__ void __launch_bounds__(1024) k_mscan_phase2(u64* chunk_tot, size_t nc
     for (size_t k = lo; k < hi; k++) {
         u64 v = chunk_tot[k];
         chunk_tot[k] = run;
-        run = mul(run, v);
+        run = Op::op(run, v);
     }
 }
-// phase 3: inclusive products inside each chunk; scatter to the output columns:
-// acc(i, m) -> partial product column m (m < M-1) at row i, or Z at row i+1 (m == M-1); Z(0) = 1.
+// phase 3: inclusive scan inside each chunk; scatter to the output columns:
+// acc(i, m) -> partial product column m (m < M-1) at row i, or Z at row i+1 (m == M-1); Z(0) = the identity.
+// (M = 1: out = the exclusive scan of the n items, the shape of logUp's Z.)
+template <class Op>
 __global__ void __launch_bounds__(SCAN_THREADS) k_mscan_phase3(const u64* seq, size_t L, const u64* chunk_carry, size_t n,
                                                              uint32_t M, u64* out) {
     __shared__ u64 sh[SCAN_THREADS];
     const size_t base = (size_t)blockIdx.x * SCAN_CHUNK + (size_t)threadIdx.x * SCAN_ITEMS;
     u64 loc[SCAN_ITEMS];
-    u64 run = 1;
+    u64 run = Op::identity;
     for (int k = 0; k < SCAN_ITEMS; k++) {
-        if (base + k < L) run = mul(run, seq[base + k]);
+        if (base + k < L) run = Op::op(run, seq[base + k]);
         loc[k] = run;
     }
     sh[threadIdx.x] = run;
@@ -1105,7 +1119,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_mscan_phase3(const u64* seq, s
         for (int t = 0; t < SCAN_THREADS; t++) {
             u64 v = sh[t];
             sh[t] = r;
-            r = mul(r, v);
+            r = Op::op(r, v);
         }
     }
     __syncthreads();
@@ -1113,12 +1127,24 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_mscan_phase3(const u64* seq, s
     for (int k = 0; k < SCAN_ITEMS; k++) {
         const size_t t = base + k;
         if (t >= L) break;
-        const u64 acc = canon(mul(carry, loc[k]));
+        const u64 acc = canon(Op::op(carry, loc[k]));
         const size_t i = t / M, m = t % M;
         if (m + 1 < M) out[m * n + i] = acc;
         else if (i + 1 < n) out[(size_t)(M - 1) * n + i + 1] = acc;
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) out[(size_t)(M - 1) * n] = 1;
+    if (blockIdx.x == 0 && threadIdx.x == 0) out[(size_t)(M - 1) * n] = Op::identity;
+}
+// the three phases over L items; tot = (L + SCAN_CHUNK - 1) / SCAN_CHUNK words of scratch
+template <class Op>
+static int mscan(gl_ctx* ctx, const u64* seq, size_t L, u64* tot, size_t n, uint32_t M, u64* out) {
+    const size_t nchunks = (L + SCAN_CHUNK - 1) / SCAN_CHUNK;
+    k_mscan_phase1<Op><<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq, L, tot);
+    CKL(ctx);
+    k_mscan_phase2<Op><<<1, 1024, 0, ctx->stream>>>(tot, nchunks);
+    CKL(ctx);
+    k_mscan_phase3<Op><<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq, L, tot, n, M, out);
+    CKL(ctx);
+    return GL_OK;
 }
 
 // ---- lookup argument helper columns (compute_lookup_polys, plonk/prover.rs:458-577; SURVEY 8(f) row 3) ----
@@ -1223,6 +1249,8 @@ __global__ void __launch_bounds__(1024) k_affine_scan(const u64* b, size_t len, 
 struct StarkQuotientParams {
     const u64* lde;        // trace LDE, column k at lde + k*lde_stride, leaf order
     size_t lde_stride;
+    const u64* aux;        // auxiliary LDE (logUp helper columns; NULL without), same layout and leaves
+    size_t aux_stride;
     uint32_t log_N;        // log2 of the LDE size
     uint32_t degree_bits, qd_bits;
     const gl_stark_instr* prog;
@@ -1267,6 +1295,8 @@ __global__ void __launch_bounds__(128) k_stark_quotient(StarkQuotientParams p) {
         switch (in.op) {
             case GL_STARK_LOCAL: r = p.lde[(size_t)in.a * p.lde_stride + jl]; break;
             case GL_STARK_NEXT: r = p.lde[(size_t)in.a * p.lde_stride + jn]; break;
+            case GL_STARK_AUX_LOCAL: r = p.aux[(size_t)in.a * p.aux_stride + jl]; break;
+            case GL_STARK_AUX_NEXT: r = p.aux[(size_t)in.a * p.aux_stride + jn]; break;
             case GL_STARK_CONST: r = p.consts[in.a]; break;
             case GL_STARK_ADD: r = add(v[in.a], v[in.b]); break;
             case GL_STARK_SUB: r = sub(v[in.a], v[in.b]); break;
@@ -1283,6 +1313,14 @@ __global__ void __launch_bounds__(128) k_stark_quotient(StarkQuotientParams p) {
     }
     const u64 zi = p.zh_inv[i & (((size_t)1 << p.qd_bits) - 1)];
     for (uint32_t a = 0; a < p.n_alphas; a++) p.out[(size_t)a * size + i] = canon(mul(acc[a], zi));
+}
+// ---- starky's logUp helper columns (lookup_helper_columns, starky/src/lookup.rs:579-652): one thread per row of one
+// Lookup, every challenge; the row's arithmetic is gl_logup.cuh. Z is the additive mscan of the `term` sequences.
+__global__ void __launch_bounds__(128) k_logup_rows(LogupParams p, unsigned int* flag) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ((size_t)1 << p.log_n)) return;
+    u64 v[GL_LOGUP_MAX_INSTR];
+    if (!logup_row(p, i, v)) atomicOr(flag, 1u);
 }
 // any non-zero word in [begin, begin + count) of each of `cols` columns (stride `stride`) -> flag
 __global__ void k_any_nonzero(const u64* data, size_t stride, size_t begin, size_t count, unsigned int* flag) {
@@ -1883,12 +1921,7 @@ int gl_partial_products_and_zs(gl_ctx* ctx, const uint64_t* wires, const uint64_
                 xtab.get() + x_pow_table_len(n), seq.get(), (unsigned int*)dflag.get()};
     k_pp_chunks<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(pp);
     CKL(ctx);
-    k_mscan_phase1<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq.get(), L, tot.get());
-    CKL(ctx);
-    k_mscan_phase2<<<1, 1024, 0, ctx->stream>>>(tot.get(), nchunks);
-    CKL(ctx);
-    k_mscan_phase3<<<(unsigned)nchunks, SCAN_THREADS, 0, ctx->stream>>>(seq.get(), L, tot.get(), n, M, dout);
-    CKL(ctx);
+    TRY(mscan<ScanMul>(ctx, seq.get(), L, tot.get(), n, M, dout));
     TRY(flag_status(ctx, dflag, {{0xFFFFFFFFu, GL_ERR_DIV_ZERO, "Tried to invert zero"}}));
     if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)M * n));
     return GL_OK;
@@ -1962,15 +1995,24 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
     return GL_OK;
 }
 
-int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
-                      const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
-                      uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+// gl_stark_quotient and gl_stark_quotient_aux (aux = NULL: the program may not read auxiliary columns)
+static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                          uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
     if (!ctx || !trace || !program || !alphas || !out_coeffs) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     if (n_instr == 0 || n_instr > GL_STARK_MAX_INSTR) return set_err(ctx, GL_ERR_UNSUPPORTED, "program of %u instructions (max %d)", n_instr, GL_STARK_MAX_INSTR);
     if (n_alphas == 0 || n_alphas > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
     if (quotient_degree_factor == 0) return set_err(ctx, GL_ERR_BAD_ARG, "quotient_degree_factor is 0: the STARK has no quotient");
     if (trace->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
-    NEED_FINISHED(trace);
+    // unfinished handles: the error goes to `ctx`, the context the caller reads it from
+    if (!trace->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the trace commitment");
+    if (aux) {
+        if (aux->ctx->device != ctx->device) return set_err(ctx, GL_ERR_BAD_ARG, "the auxiliary commitment is on another device");
+        if (aux->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole auxiliary LDE on this device");
+        if (aux->degree_log != trace->degree_log || aux->rate_bits != trace->rate_bits)
+            return set_err(ctx, GL_ERR_BAD_SHAPE, "the auxiliary commitment's degree or rate differs from the trace's");
+        if (!aux->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the auxiliary commitment");
+    }
     uint32_t qd_bits = 0;
     while ((1u << qd_bits) < quotient_degree_factor) qd_bits++;  // log2_ceil
     if (qd_bits > trace->rate_bits)
@@ -1981,6 +2023,7 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
         bool ok = true;
         switch (in.op) {
             case GL_STARK_LOCAL: case GL_STARK_NEXT: ok = in.a < trace->B; break;
+            case GL_STARK_AUX_LOCAL: case GL_STARK_AUX_NEXT: ok = aux && in.a < aux->B; break;
             case GL_STARK_CONST: ok = in.a < n_consts; break;
             case GL_STARK_ADD: case GL_STARK_SUB: case GL_STARK_MUL: ok = in.a < k && in.b < k; break;
             case GL_STARK_EMIT: ok = in.a < k && in.b <= GL_STARK_LAST_ROW; break;
@@ -1998,6 +2041,8 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
     StarkQuotientParams p;
     p.lde = trace->tree.leaves;
     p.lde_stride = trace->tree.es;
+    p.aux = aux ? aux->tree.leaves : nullptr;
+    p.aux_stride = aux ? aux->tree.es : 0;
     p.log_N = db + trace->rate_bits;
     p.degree_bits = db;
     p.qd_bits = qd_bits;
@@ -2026,6 +2071,90 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
         CKL(ctx);
     }
     return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
+}
+int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
+                      const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                      uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+    return stark_quotient(ctx, trace, nullptr, program, n_instr, consts, n_consts, alphas, n_alphas,
+                          quotient_degree_factor, out_coeffs);
+}
+int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                          uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+    if (!aux) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    return stark_quotient(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, quotient_degree_factor,
+                          out_coeffs);
+}
+
+int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,
+                            const gl_stark_instr* program, const uint32_t* lookup_offsets, uint32_t n_lookups,
+                            const uint64_t* consts, uint32_t n_consts, const uint64_t* challenges, uint32_t n_challenges,
+                            uint32_t constraint_degree, uint64_t* out) {
+    if (!ctx || !trace || !program || !lookup_offsets || !challenges || !out || (n_consts && !consts))
+        return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (n_lookups == 0) return set_err(ctx, GL_ERR_BAD_ARG, "no lookups");
+    if (constraint_degree == 1) return set_err(ctx, GL_ERR_BAD_SHAPE, "attempt to divide by zero: constraint degree 1 leaves no looking columns per helper column");
+    if (n_challenges == 0 || n_challenges > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
+    if (log_n > 3 * NTT_MAX_LOG_PASS) return set_err(ctx, GL_ERR_UNSUPPORTED, "log_n %u > 30", log_n);
+    const size_t n = (size_t)1 << log_n;
+    if (num_columns > 1 && col_stride < n) return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent (stride < n)");
+    const uint32_t chunk = constraint_degree == 0 ? 1 : constraint_degree - 1;  // lookup.rs:757
+    // validate every lookup's row program once on the host: the kernel trusts it
+    std::vector<uint32_t> num_h(n_lookups);
+    for (uint32_t l = 0; l < n_lookups; l++) {
+        const uint32_t b = lookup_offsets[l], e = lookup_offsets[l + 1];
+        if (e <= b || e - b > GL_LOGUP_MAX_INSTR)
+            return set_err(ctx, GL_ERR_UNSUPPORTED, "lookup %u: row program of 1..%d instructions", l, GL_LOGUP_MAX_INSTR);
+        uint32_t roles[4] = {0, 0, 0, 0};
+        for (uint32_t k = 0; k < e - b; k++) {
+            const gl_stark_instr in = program[b + k];
+            bool ok = true;
+            switch (in.op) {
+                case GL_STARK_LOCAL: case GL_STARK_NEXT: ok = in.a < num_columns; break;
+                case GL_STARK_CONST: ok = in.a < n_consts; break;
+                case GL_STARK_ADD: case GL_STARK_SUB: case GL_STARK_MUL: ok = in.a < k && in.b < k; break;
+                case GL_STARK_EMIT: ok = in.a < k && in.b <= GL_LOGUP_FREQUENCIES; if (ok) roles[in.b]++; break;
+                default: ok = false;
+            }
+            if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "lookup %u: bad row instruction %u", l, k);
+        }
+        if (roles[GL_LOGUP_LOOKED] > GL_LOGUP_MAX_COLUMNS)
+            return set_err(ctx, GL_ERR_UNSUPPORTED, "lookup %u: more than %d looking columns", l, GL_LOGUP_MAX_COLUMNS);
+        if (roles[GL_LOGUP_FILTER] != roles[GL_LOGUP_LOOKED] || roles[GL_LOGUP_TABLE] != 1 || roles[GL_LOGUP_FREQUENCIES] != 1)
+            return set_err(ctx, GL_ERR_BAD_ARG, "lookup %u: need one filter per looking column, one table, one frequencies column", l);
+        num_h[l] = (roles[GL_LOGUP_LOOKED] + chunk - 1) / chunk;
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    const size_t nchunks = (n + SCAN_CHUNK - 1) / SCAN_CHUNK;
+    const size_t n_prog = lookup_offsets[n_lookups] - lookup_offsets[0];
+    DevBuf dprog(ctx), dconst(ctx), dflag(ctx), term(ctx), tot(ctx);
+    TRY(upload_program(ctx, program + lookup_offsets[0], n_prog * sizeof(gl_stark_instr), consts, n_consts, dprog, dconst));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(term.alloc((size_t)n_challenges * n));
+    TRY(tot.alloc(nchunks));
+    size_t col = 0;
+    for (uint32_t l = 0; l < n_lookups; l++) {
+        LogupParams p;
+        p.trace = trace;
+        p.trace_stride = col_stride;
+        p.log_n = log_n;
+        p.prog = (const gl_stark_instr*)dprog.get() + (lookup_offsets[l] - lookup_offsets[0]);
+        p.n_instr = lookup_offsets[l + 1] - lookup_offsets[l];
+        p.consts = dconst.get();
+        p.chunk = chunk;
+        p.num_h = num_h[l];
+        for (uint32_t c = 0; c < GL_STARK_MAX_ALPHAS; c++) p.gammas[c] = c < n_challenges ? canon(challenges[c]) : 0;
+        p.n_challenges = n_challenges;
+        p.h_out = out + col * n;
+        p.term = term.get();
+        k_logup_rows<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(p, (unsigned int*)dflag.get());
+        CKL(ctx);
+        for (uint32_t c = 0; c < n_challenges; c++)  // Z of (lookup l, challenge c): the column after its h_k
+            TRY(mscan<ScanAdd>(ctx, term.get() + (size_t)c * n, n, tot.get(), n, 1,
+                               out + (col + (size_t)c * (num_h[l] + 1) + num_h[l]) * n));
+        col += (size_t)n_challenges * (num_h[l] + 1);
+    }
+    return flag_status(ctx, dflag, {INVERT_ZERO});
 }
 
 int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,

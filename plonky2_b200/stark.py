@@ -1,10 +1,11 @@
 """starky's prover (SURVEY.md section 8f rows 1 and 1'), mirroring starky/src/{config.rs, stark.rs,
 constraint_consumer.rs, vanishing_poly.rs, prover.rs, proof.rs, get_challenges.rs, fibonacci_stark.rs} for STARKs
-without lookups or cross-table lookups. The constraints of a Stark are recorded ONCE as a straight-line program
-(ConstraintBuilder): gl_stark_quotient evaluates it on every point of the quotient coset, reading the trace LDE in place
-on the device, and eval_vanishing_poly evaluates the same instructions at one point of F_{p^2} on the host (the
-constraint-binding step of `prove`, and any verifier). `prove` strings the device steps together in the reference's
-order with the transcript on the host."""
+with or without logUp lookups (lookup.py), without cross-table lookups. The constraints of a Stark -- its own, then
+those of its lookups -- are recorded ONCE as a straight-line program (ConstraintBuilder): gl_stark_quotient[_aux]
+evaluates it on every point of the quotient coset, reading the trace and auxiliary LDEs in place on the device, and
+eval_vanishing_poly evaluates the same instructions at one point of F_{p^2} on the host (the constraint-binding step of
+`prove`, and any verifier). `prove` strings the device steps together in the reference's order with the transcript on
+the host; the lookup helper columns are written on the device by gl_stark_lookup_helpers."""
 import ctypes as C
 
 import numpy as np
@@ -15,7 +16,7 @@ from .fri import starky_standard_fast_fri_config
 from .polynomial_batch import PolynomialBatch
 from .proof import StarkOpeningSet
 
-OP_LOCAL, OP_NEXT, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_EMIT = range(7)
+OP_LOCAL, OP_NEXT, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_EMIT, OP_AUX_LOCAL, OP_AUX_NEXT = range(9)
 KIND_CONSTRAINT, KIND_TRANSITION, KIND_FIRST_ROW, KIND_LAST_ROW = range(4)
 
 
@@ -48,9 +49,11 @@ class Expr:
 class ConstraintBuilder:
     """Records eval_packed_generic as instructions; doubles as the ConstraintConsumer (constraint_consumer.rs:46-84)."""
 
-    def __init__(self, num_columns, num_public_inputs):
-        self.instrs, self.consts = [], [None] * num_public_inputs  # consts[0:num_pi] are bound at evaluation time
-        self.num_columns, self.num_pi = num_columns, num_public_inputs
+    def __init__(self, num_columns, num_public_inputs, num_aux=0, num_lookup_challenges=0):
+        # consts[0:num_bound] -- the public inputs, then the lookup challenges -- are bound at evaluation time
+        self.num_bound = num_public_inputs + num_lookup_challenges
+        self.instrs, self.consts = [], [None] * self.num_bound
+        self.num_columns, self.num_pi, self.num_aux = num_columns, num_public_inputs, num_aux
         self._cache = {}
 
     def _push(self, op, a=0, b=0):
@@ -76,11 +79,24 @@ class ConstraintBuilder:
         assert 0 <= k < self.num_pi
         return self._push(OP_CONST, k)
 
+    # the auxiliary polynomials (LookupCheckVars, lookup.rs:791-801)
+    def aux_local(self, col):
+        assert 0 <= col < self.num_aux
+        return self._push(OP_AUX_LOCAL, col)
+
+    def aux_next(self, col):
+        assert 0 <= col < self.num_aux
+        return self._push(OP_AUX_NEXT, col)
+
+    def lookup_challenge(self, c):
+        assert 0 <= c < self.num_bound - self.num_pi
+        return self._push(OP_CONST, self.num_pi + c)
+
     def constant(self, v):
         v = int(v) % F.ORDER
-        if v not in self.consts[self.num_pi:]:
+        if v not in self.consts[self.num_bound:]:
             self.consts.append(v)
-        return self._push(OP_CONST, self.num_pi + self.consts[self.num_pi:].index(v))
+        return self._push(OP_CONST, self.num_bound + self.consts[self.num_bound:].index(v))
 
     # ConstraintConsumer
     def constraint(self, e):
@@ -118,9 +134,35 @@ class Stark:
         d = self.constraint_degree()
         return 0 if d == 0 else max(1, d - 1)
 
-    def constraint_program(self):
-        b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS)
+    def lookups(self):
+        """stark.rs:251-254: the Stark's logUp lookups (lookup.Lookup), none by default."""
+        return []
+
+    def uses_lookups(self):
+        """stark.rs:266-270"""
+        return len(self.lookups()) > 0
+
+    def num_lookup_helper_columns(self, config):
+        """stark.rs:256-264: the auxiliary polynomials of all lookups and challenges."""
+        return self._helper_columns_per_challenge() * config.num_challenges
+
+    def _helper_columns_per_challenge(self):
+        return sum(lookup.num_helper_columns(self.constraint_degree()) for lookup in self.lookups())
+
+    def constraint_program(self, num_lookup_challenges=0):
+        """The Stark's constraints (eval_packed_generic), then -- with lookups -- those of the logUp argument for
+        num_lookup_challenges challenges (eval_vanishing_poly, vanishing_poly.rs:41-52): the order of the alpha-fold."""
+        if not self.uses_lookups():
+            b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS)
+            self.eval(b, b)
+            return b
+        from .lookup import eval_packed_lookups_generic
+
+        lookups = self.lookups()
+        b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS, self._helper_columns_per_challenge() * num_lookup_challenges,
+                              num_lookup_challenges)
         self.eval(b, b)
+        eval_packed_lookups_generic(self, lookups, b, num_lookup_challenges, b)
         return b
 
     def num_quotient_polys(self, config):
@@ -128,12 +170,16 @@ class Stark:
         return self.quotient_degree_factor() * config.num_challenges
 
     def fri_instance(self, zeta, g, config):
-        """fri_instance (stark.rs:101-170) without auxiliary (lookup / CTL) polynomials: the trace oracle opened at zeta
-        and g * zeta, the quotient oracle -- present only when the Stark has constraints -- at zeta."""
+        """fri_instance (stark.rs:101-170) without CTLs: the trace oracle and -- with lookups -- the auxiliary oracle
+        opened at zeta and g * zeta, the quotient oracle -- present only when the Stark has constraints -- at zeta."""
         from .fri import FriBatchInfo, FriInstanceInfo, FriOracleInfo, FriPolynomialInfo
 
         trace_info = FriPolynomialInfo.from_range(0, range(self.COLUMNS))
         oracles = [FriOracleInfo(self.COLUMNS, False)]
+        if self.uses_lookups():
+            num_aux = self.num_lookup_helper_columns(config)
+            trace_info = trace_info + FriPolynomialInfo.from_range(len(oracles), range(num_aux))
+            oracles.append(FriOracleInfo(num_aux, False))
         quotient_info = []
         nq = self.num_quotient_polys(config)
         if nq > 0:
@@ -175,17 +221,22 @@ class FibonacciStark(Stark):
         return 2
 
 
-def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas):
+def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxiliary_polys_commitment=None,
+                           lookup_challenges=None):
     """compute_quotient_polys (prover.rs:488-668) on the device. Returns a torch int64 CUDA tensor (num_challenges, size)
     of quotient-polynomial coefficients, size = n << log2_ceil(quotient_degree_factor), or None if the Stark has no
-    quotient. Raises if the vanishing polynomial is not divisible by Z_H."""
+    quotient. Raises if the vanishing polynomial is not divisible by Z_H. A Stark with lookups also needs the auxiliary
+    commitment (its LDE is read in place, like the trace's) and the lookup challenges."""
     import torch
 
     qdf = stark.quotient_degree_factor()
     if qdf == 0:
         return None
-    b = stark.constraint_program()
-    consts = np.array([int(x) % F.ORDER for x in public_inputs] + b.consts[b.num_pi:], dtype=np.uint64)
+    if stark.uses_lookups() and (auxiliary_polys_commitment is None or lookup_challenges is None):
+        raise N.ShapeError("a Stark with lookups needs the auxiliary commitment and the lookup challenges")
+    challenges = [int(c) % F.ORDER for c in lookup_challenges] if stark.uses_lookups() else []
+    b = stark.constraint_program(len(challenges))
+    consts = np.array([int(x) % F.ORDER for x in public_inputs] + challenges + b.consts[b.num_bound:], dtype=np.uint64)
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs" % stark.PUBLIC_INPUTS)
     al = np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
@@ -194,10 +245,55 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas):
     ctx = trace_commitment.ctx
     out = torch.empty((len(al), size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     prog = b.program()
-    N.check(N.lib().gl_stark_quotient(ctx.h, trace_commitment.h, prog, len(b.instrs), N.np_ptr(consts), len(consts),
-                                      N.np_ptr(al), len(al), qdf, N.vp(out.data_ptr())), ctx.h)
+    if stark.uses_lookups():
+        N.check(N.lib().gl_stark_quotient_aux(ctx.h, trace_commitment.h, auxiliary_polys_commitment.h, prog,
+                                              len(b.instrs), N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
+                                              N.vp(out.data_ptr())), ctx.h)
+    else:
+        N.check(N.lib().gl_stark_quotient(ctx.h, trace_commitment.h, prog, len(b.instrs), N.np_ptr(consts), len(consts),
+                                          N.np_ptr(al), len(al), qdf, N.vp(out.data_ptr())), ctx.h)
     ctx.synchronize()
     return out
+
+
+def check_lookup_shapes(stark):
+    """The reference's panics for a Stark's lookups, raised before any device work: constraint degree 1 (division by
+    zero in num_helper_columns) and chunks of more than two looking columns (todo! in eval_helper_columns)."""
+    for lookup in stark.lookups():
+        lookup.check_chunks(stark.constraint_degree())
+
+
+def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx):
+    """The lookup helper columns (prover.rs:177-195, lookup_helper_columns) on the device: for every lookup, for every
+    challenge, the h_k columns and Z, from the trace values `trace` -- a (COLUMNS, n) int64 CUDA tensor, read in place.
+    Returns a (num_lookup_helper_columns, n) int64 CUDA tensor of values."""
+    import torch
+
+    from .lookup import row_programs
+
+    check_lookup_shapes(stark)
+    cols, n = trace.shape
+    prog, offsets, consts = row_programs(stark.lookups(), stark.COLUMNS)
+    ch = np.array([int(c) % F.ORDER for c in lookup_challenges], dtype=np.uint64)
+    out = torch.empty((stark._helper_columns_per_challenge() * len(ch), n), dtype=torch.int64, device=trace.device)
+    N.check(N.lib().gl_stark_lookup_helpers(ctx.h, N.vp(trace.data_ptr()), n, cols, F.log2_strict(n), prog,
+                                            offsets.ctypes.data_as(N.u32p), len(offsets) - 1,
+                                            N.np_ptr(consts) if len(consts) else None, len(consts), N.np_ptr(ch), len(ch),
+                                            stark.constraint_degree(), N.vp(out.data_ptr())), ctx.h)
+    ctx.synchronize()
+    return out
+
+
+def commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx):
+    """The auxiliary commitment (prover.rs:216-230): PolynomialBatch::from_values of the helper columns, never blinded,
+    committed straight from the device tensor compute_lookup_helper_columns returned."""
+    B, n = helper_columns.shape
+
+    def add_columns(h):
+        N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(helper_columns.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE),
+                ctx.h)
+
+    return PolynomialBatch._from_device(ctx, B, F.log2_strict(n), rate_bits, cap_height, add_columns)
 
 
 def commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx=None):
@@ -241,16 +337,25 @@ def eval_l_0_and_l_last(log_n, x):
     return l_0, l_last
 
 
-def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas, x, degree_bits):
-    """compute_eval_vanishing_poly (vanishing_poly.rs:108-173) without lookups or CTLs: the Stark's constraint program
-    -- the instructions gl_stark_quotient runs -- evaluated at one point x of F_{p^2}, with the local and next rows as
-    F_{p^2} values and the public inputs and program constants as base-field values; the constraints are filtered by
-    z_last = x - g^{-1}, L_0(x), L_{n-1}(x) and folded with every alpha as ConstraintConsumer does
-    (constraint_consumer.rs:46-84). Returns num_challenges F_{p^2} values (c0, c1)."""
-    b = stark.constraint_program()
+def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas, x, degree_bits, auxiliary_polys=None,
+                        auxiliary_polys_next=None, lookup_challenges=None):
+    """compute_eval_vanishing_poly (vanishing_poly.rs:108-173) without CTLs: the Stark's constraint program -- the
+    instructions gl_stark_quotient runs -- evaluated at one point x of F_{p^2}, with the local and next rows (and, with
+    lookups, the auxiliary polynomials' local and next values) as F_{p^2} values and the public inputs, lookup challenges
+    and program constants as base-field values; the constraints are filtered by z_last = x - g^{-1}, L_0(x), L_{n-1}(x)
+    and folded with every alpha as ConstraintConsumer does (constraint_consumer.rs:46-84). Returns num_challenges F_{p^2}
+    values (c0, c1)."""
+    challenges = []
+    if stark.uses_lookups():
+        if auxiliary_polys is None or auxiliary_polys_next is None or lookup_challenges is None:
+            raise N.ShapeError("a Stark with lookups needs the auxiliary values and the lookup challenges")
+        challenges = [int(c) % F.ORDER for c in lookup_challenges]
+    b = stark.constraint_program(len(challenges))
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs, got %d" % (stark.PUBLIC_INPUTS, len(public_inputs)))
-    consts = [int(v) % F.ORDER for v in public_inputs] + b.consts[b.num_pi:]
+    if challenges and (len(auxiliary_polys) != b.num_aux or len(auxiliary_polys_next) != b.num_aux):
+        raise N.ShapeError("expected %d auxiliary values" % b.num_aux)
+    consts = [int(v) % F.ORDER for v in public_inputs] + challenges + b.consts[b.num_bound:]
     x = (int(x[0]) % F.ORDER, int(x[1]) % F.ORDER)
     l_0, l_last = eval_l_0_and_l_last(degree_bits, x)
     z_last = F.ext_sub(x, (F.inverse(F.primitive_root_of_unity(degree_bits)), 0))
@@ -267,6 +372,10 @@ def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas,
             r = ext(local_values[a])
         elif op == OP_NEXT:
             r = ext(next_values[a])
+        elif op == OP_AUX_LOCAL:
+            r = ext(auxiliary_polys[a])
+        elif op == OP_AUX_NEXT:
+            r = ext(auxiliary_polys_next[a])
         elif op == OP_CONST:
             r = (consts[a], 0)
         elif op == OP_ADD:
@@ -282,12 +391,13 @@ def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas,
     return acc
 
 
-def _dummy_openings(challenger, num_trace_polys, pow_degree):
-    """get_dummy_polys (get_challenges.rs:201-256, prover.rs:272-319) without auxiliary polynomials: simulated local and
-    next values c_i, c_i^d, c_i^{d^2}, ... from fresh extension challenges c_i, d = pow_degree."""
+def _dummy_openings(challenger, num_trace_polys, pow_degree, num_aux_polys=0):
+    """get_dummy_polys (get_challenges.rs:201-256, prover.rs:272-319): simulated local, next, auxiliary and next
+    auxiliary values c_i, c_i^d, c_i^{d^2}, ... from fresh extension challenges c_i, d = pow_degree. Returns (local,
+    next) without auxiliary polynomials, else (local, next, aux, aux_next)."""
     log_pow_degree = (pow_degree - 1).bit_length()
     num_extension_powers = max(1, 50 // log_pow_degree - 1)
-    total = 2 * num_trace_polys
+    total = 2 * num_trace_polys + 2 * num_aux_polys
     zetas = challenger.get_n_extension_challenges(-(-total // num_extension_powers))
     per_zeta = min(num_extension_powers + 1, total)
     evals = []
@@ -295,29 +405,40 @@ def _dummy_openings(challenger, num_trace_polys, pow_degree):
         for _ in range(per_zeta):
             evals.append(z)
             z = F.ext_pow(z, pow_degree)
-    return evals[:num_trace_polys], evals[num_trace_polys:total]
+    t, a = num_trace_polys, num_aux_polys
+    if a == 0:
+        return evals[:t], evals[t:2 * t]
+    return evals[:t], evals[t:2 * t], evals[2 * t:2 * t + a], evals[2 * t + a:total]
 
 
-def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_bits):
+def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_bits, lookup_challenges=None):
     """The constraint-binding step (prover.rs:239-370, get_challenges.rs:94-163): alphas', simulated openings, zeta',
-    the vanishing polynomial there observed; returns the alphas the quotient uses."""
+    the vanishing polynomial there observed; returns the alphas the quotient uses. A Stark with lookups also simulates
+    its auxiliary polynomials and evaluates the lookup constraints with the lookup challenges."""
     alphas_prime = challenger.get_n_challenges(num_challenges)
     pow_degree = max(2, stark.constraint_degree() + 1)
-    local, nxt = _dummy_openings(challenger, stark.COLUMNS, pow_degree)
+    if lookup_challenges is None:
+        local, nxt = _dummy_openings(challenger, stark.COLUMNS, pow_degree)
+        aux = {}
+    else:
+        num_aux = stark._helper_columns_per_challenge() * len(lookup_challenges)
+        local, nxt, a, a_next = _dummy_openings(challenger, stark.COLUMNS, pow_degree, num_aux)
+        aux = dict(auxiliary_polys=a, auxiliary_polys_next=a_next, lookup_challenges=lookup_challenges)
     zeta_prime = challenger.get_extension_challenge()
     challenger.observe_extension_elements(eval_vanishing_poly(stark, local, nxt, public_inputs, alphas_prime, zeta_prime,
-                                                              degree_bits))
+                                                              degree_bits, **aux))
     return challenger.get_n_challenges(num_challenges)
 
 
 class StarkProof:
-    """StarkProof (starky/src/proof.rs:30-53) without auxiliary polynomials: trace cap, quotient cap (None for a Stark
-    without constraints), StarkOpeningSet, FriProof. The reference has no byte format for it (serde only);
-    opening_proof.to_bytes() is write_fri_proof."""
+    """StarkProof (starky/src/proof.rs:30-53) without CTLs: trace cap, quotient cap (None for a Stark without
+    constraints), StarkOpeningSet, FriProof, and the auxiliary polynomials' cap (None for a Stark without lookups). The
+    reference has no byte format for it (serde only); opening_proof.to_bytes() is write_fri_proof."""
 
-    def __init__(self, trace_cap, quotient_polys_cap, openings, opening_proof):
+    def __init__(self, trace_cap, quotient_polys_cap, openings, opening_proof, auxiliary_polys_cap=None):
         self.trace_cap, self.quotient_polys_cap = trace_cap, quotient_polys_cap
         self.openings, self.opening_proof = openings, opening_proof
+        self.auxiliary_polys_cap = auxiliary_polys_cap
 
     def recover_degree_bits(self, config):
         """proof.rs:45-52: from the length of the first initial-tree Merkle proof."""
@@ -333,10 +454,13 @@ class StarkProofWithPublicInputs:
 
     def get_challenges(self, stark, config, verifier_circuit_fri_params=None):
         """get_challenges (get_challenges.rs:37-199,323-357) replayed from the proof alone: the public inputs, the
-        config, the trace cap, the constraint-binding step, the quotient cap, zeta, the openings, then FRI's challenges.
-        Returns a dict: stark_alphas, stark_zeta, fri_alpha, fri_betas, fri_pow_response, fri_query_indices."""
+        config, the trace cap, the lookup challenges and the auxiliary cap (get_challenges.rs:67-92), the
+        constraint-binding step, the quotient cap, zeta, the openings, then FRI's challenges. Returns a dict:
+        lookup_challenge_set (None without an auxiliary cap), stark_alphas, stark_zeta, fri_alpha, fri_betas,
+        fri_pow_response, fri_query_indices."""
         from .challenger import Challenger
         from .fri import fri_challenges
+        from .lookup import get_grand_product_challenge_set
 
         p = self.proof
         degree_bits = p.recover_degree_bits(config)
@@ -344,7 +468,15 @@ class StarkProofWithPublicInputs:
         ch.observe_elements(self.public_inputs)
         config.observe(ch)
         ch.observe_cap(p.trace_cap)
-        alphas = _bind_constraints(stark, ch, self.public_inputs, config.num_challenges, degree_bits)
+        lookup_challenge_set = lookup_challenges = None
+        if p.auxiliary_polys_cap is not None:
+            lookup_challenge_set = get_grand_product_challenge_set(ch, config.num_challenges)
+            ch.observe_cap(p.auxiliary_polys_cap)
+        if stark.uses_lookups():
+            if lookup_challenge_set is None:
+                raise N.ShapeError("Missing auxiliary_polys_cap")
+            lookup_challenges = [c.beta for c in lookup_challenge_set]
+        alphas = _bind_constraints(stark, ch, self.public_inputs, config.num_challenges, degree_bits, lookup_challenges)
         if p.quotient_polys_cap is not None:
             ch.observe_cap(p.quotient_polys_cap)
         zeta = ch.get_extension_challenge()
@@ -358,8 +490,8 @@ class StarkProofWithPublicInputs:
         fri_alpha, fri_betas, pow_response, indices = fri_challenges(ch, fp.commit_phase_merkle_caps, fp.final_poly,
                                                                      fp.pow_witness, degree_bits, config.fri_config,
                                                                      final_len, steps)
-        return dict(stark_alphas=alphas, stark_zeta=zeta, fri_alpha=fri_alpha, fri_betas=fri_betas,
-                    fri_pow_response=pow_response, fri_query_indices=indices)
+        return dict(lookup_challenge_set=lookup_challenge_set, stark_alphas=alphas, stark_zeta=zeta, fri_alpha=fri_alpha,
+                    fri_betas=fri_betas, fri_pow_response=pow_response, fri_query_indices=indices)
 
 
 def _commit_trace(trace, rate_bits, cap_height, ctx):
@@ -381,16 +513,32 @@ def _commit_trace(trace, rate_bits, cap_height, ctx):
     return PolynomialBatch.from_values(trace, rate_bits, False, cap_height, ctx=ctx)
 
 
+def _device_trace(trace, ctx):
+    """The trace as ONE (COLUMNS, n) int64 CUDA tensor that the trace commitment and the lookup helper columns both read:
+    a torch CUDA trace as it is (made contiguous), host columns copied to the context's device once."""
+    import torch
+
+    if hasattr(trace, "data_ptr"):
+        if not trace.is_cuda or trace.dim() != 2 or trace.element_size() != 8:
+            raise N.ShapeError("a torch trace must be a (COLUMNS, n) CUDA tensor of 64-bit words")
+        return trace.contiguous().view(torch.int64)
+    host = np.ascontiguousarray(trace, dtype=np.uint64).view(np.int64)
+    dev = torch.from_numpy(host).to("cuda:%d" % ctx.device)
+    torch.cuda.synchronize(dev.device)  # the copy is on torch's stream; the library reads it on the context's
+    return dev
+
+
 def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None):
-    """prove + prove_with_commitment (starky/src/prover.rs:40-114,125-484) for a Stark without lookups or CTLs:
-    trace = (COLUMNS, n) host columns or torch CUDA tensor -> StarkProofWithPublicInputs. Every array-sized step runs on
-    the device (trace commitment, quotient from the LDE in place, quotient commitment, openings, FRI); the transcript and
-    the constraint-binding step run on the host. verifier_circuit_fri_params: the FRI parameters of a verifier circuit
-    made for another degree (ConstantArityBits only); the transcript then observes the zero caps and coefficients that
-    verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment is released on
-    every exit path."""
+    """prove + prove_with_commitment (starky/src/prover.rs:40-114,125-484) for a Stark without CTLs: trace = (COLUMNS, n)
+    host columns or torch CUDA tensor -> StarkProofWithPublicInputs. Every array-sized step runs on the device (trace
+    commitment, lookup helper columns and their commitment, quotient from the LDEs in place, quotient commitment,
+    openings, FRI); the transcript and the constraint-binding step run on the host. verifier_circuit_fri_params: the
+    FRI parameters of a verifier circuit made for another degree (ConstantArityBits only); the transcript then observes
+    the zero caps and coefficients that verifier expects. Raises ShapeError / NativeError with the reference's
+    messages; every commitment is released on every exit path."""
     from .challenger import Challenger
     from .fri import prove_openings
+    from .lookup import get_grand_product_challenge_set
 
     ctx = ctx or N.default_context()
     shape = tuple(trace.shape)
@@ -420,6 +568,10 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
                                % (final_poly_coeff_len, 1 << (1 + strategy[2])))
         max_num_query_steps = len(vp.reduction_arity_bits)
 
+    uses_lookups = stark.uses_lookups()
+    if uses_lookups:
+        check_lookup_shapes(stark)
+        trace = _device_trace(trace, ctx)
     trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx)
     commitments = [trace_commitment]
     try:
@@ -427,8 +579,19 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
         challenger.observe_elements(public_inputs)
         config.observe(challenger)
         challenger.observe_cap(trace_commitment.merkle_tree.cap)
-        alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits)
-        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas)
+        aux_commitment = lookup_challenges = None
+        lookup_args = {}
+        if uses_lookups:                                                # prover.rs:164-237
+            lookup_challenges = [c.beta for c in get_grand_product_challenge_set(challenger, config.num_challenges)]
+            helper_columns = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
+            aux_commitment = commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx)
+            commitments.append(aux_commitment)
+            del helper_columns
+            challenger.observe_cap(aux_commitment.merkle_tree.cap)
+            lookup_args = dict(auxiliary_polys_commitment=aux_commitment, lookup_challenges=lookup_challenges)
+        alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
+                                   lookup_challenges)
+        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **lookup_args)
         quotient_commitment = None
         if quotient_polys is not None:
             quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx)
@@ -439,14 +602,15 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
         if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
             raise N.NativeError("Opening point is in the subgroup.")
         g = F.primitive_root_of_unity(degree_bits)
-        openings = StarkOpeningSet.new(zeta, g, trace_commitment, None, quotient_commitment)
+        openings = StarkOpeningSet.new(zeta, g, trace_commitment, aux_commitment, quotient_commitment)
         for batch in openings.to_fri_openings():                        # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         opening_proof = prove_openings(stark.fri_instance(zeta, g, config), commitments, challenger, fri_params,
                                        final_poly_coeff_len, max_num_query_steps)
         proof = StarkProof(trace_commitment.merkle_tree.cap,
                            quotient_commitment.merkle_tree.cap if quotient_commitment is not None else None,
-                           openings, opening_proof)
+                           openings, opening_proof,
+                           aux_commitment.merkle_tree.cap if aux_commitment is not None else None)
         return StarkProofWithPublicInputs(proof, public_inputs)
     finally:
         for c in commitments:
