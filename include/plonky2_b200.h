@@ -275,6 +275,40 @@ int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_strid
                             const uint64_t* consts, uint32_t n_consts, const uint64_t* challenges, uint32_t n_challenges,
                             uint32_t constraint_degree, uint64_t* out);
 
+/* starky's cross-table lookup helper and Z columns of ONE table (partial_sums / get_helper_cols,
+ * starky/src/cross_table_lookup.rs:270-414, lookup.rs:746-789: the table's part of cross_table_lookup_data) on the
+ * device, for every CtlZData group of the table and every challenge. trace: num_columns value columns of n = 2^log_n
+ * words at trace + k*col_stride; out: the table's CTL auxiliary polynomials' values, column j at out + j*n. Both are
+ * DEVICE memory. Group g (g < n_groups) -- the table's consecutive looking entries of one CrossTableLookup, or its
+ * looked entry -- is the row program program[group_offsets[g] .. group_offsets[g + 1]) in the gl_stark_instr format,
+ * operands relative to its first instruction: GL_STARK_LOCAL reads row i, GL_STARK_NEXT row (i + 1) mod n
+ * (Column::eval_table / Filter::eval_table), GL_STARK_CONST reads consts, and GL_STARK_EMIT hands value a to the
+ * argument in role b: for each entry in order, its tuple's values in order (GL_CTL_VALUE), then its filter
+ * (GL_CTL_FILTER), which closes the entry. challenges: n_challenges (beta, gamma) pairs, 2 * n_challenges words.
+ * For each group and challenge, combine_j = gamma + sum_k beta^k v_{j,k} (GrandProductChallenge::combine); a group of
+ * more than one entry has ceil(entries / chunk) helper columns h_k = sum_{j in chunk k} filter_j / combine_j, chunk =
+ * constraint_degree - 1 (1 when that is 0), and Z[i] = sum_{i' >= i} sum_k h_k[i']; a group of one entry has no helper
+ * column and Z[i] = sum_{i' >= i} filter[i'] / combine[i']. zs_index[g * n_challenges + c] is the position of (group g,
+ * challenge c) in the table's zs_columns order, a permutation of 0 .. n_groups * n_challenges - 1; out holds
+ * ctl_helper_polys() then ctl_z_polys() in that order (get_ctl_auxiliary_polys): the helper columns of every position,
+ * then one Z column per position.
+ * Errors: a zero denominator -> GL_ERR_DIV_ZERO ("Tried to invert zero"); constraint_degree 1 with a group of more than
+ * one entry -> GL_ERR_BAD_SHAPE (the reference's chunks(0)); more than GL_CTL_MAX_GROUPS groups, GL_CTL_MAX_ENTRIES
+ * entries in a group, GL_CTL_MAX_VALUES values in an entry, GL_CTL_MAX_INSTR instructions in a group or
+ * GL_STARK_MAX_ALPHAS challenges -> GL_ERR_UNSUPPORTED; an invalid program (an operand out of range, an unknown opcode
+ * or role, values after the last filter, a group without entries) or zs_index that is not a permutation ->
+ * GL_ERR_BAD_ARG. */
+#define GL_CTL_VALUE 0
+#define GL_CTL_FILTER 1
+#define GL_CTL_MAX_GROUPS 16
+#define GL_CTL_MAX_ENTRIES 8
+#define GL_CTL_MAX_VALUES 32
+#define GL_CTL_MAX_INSTR 256
+int gl_stark_ctl_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,
+                         const gl_stark_instr* program, const uint32_t* group_offsets, uint32_t n_groups,
+                         const uint64_t* consts, uint32_t n_consts, const uint64_t* challenges, uint32_t n_challenges,
+                         uint32_t constraint_degree, const uint32_t* zs_index, uint64_t* out);
+
 /* compute_quotient_polys of a plonky2 circuit (plonky2/src/plonk/prover.rs:609-815): for every challenge alpha_k the
  * values eval_vanishing_poly_base_batch(x) / Z_H(x) (plonky2/src/plonk/vanishing_poly.rs:167-340) on the coset g<w_size>,
  * size = n << log2_ceil(quotient_degree_factor), then coset_ifft: n_alphas polynomials of `size` coefficients at

@@ -17,6 +17,8 @@ from .proof import OpeningSet, StarkOpeningSet, eval_commitments  # noqa: F401
 from .stark import (FibonacciStark, Stark, StarkConfig, StarkProof, StarkProofWithPublicInputs,  # noqa: F401
                     commit_quotient_polys, compute_quotient_polys, eval_l_0_and_l_last, eval_vanishing_poly)
 from .lookup import Column, Filter, GrandProductChallenge, Lookup, get_grand_product_challenge_set  # noqa: F401
+from .cross_table_lookup import (CrossTableLookup, CtlCheckVars, CtlData, CtlZData, MultiStarkProof,  # noqa: F401
+                                 TableWithColumns, check_ctls, prove_with_ctls)
 from . import stark  # noqa: F401  (stark.prove: the starky prover, next to plonk.prove_with_witness)
 from . import plonk  # noqa: F401  (plonk.compute_quotient_polys: the plonky2 circuit quotient)
 from .batch_merkle_tree import (BatchMerkleTree, compress_merkle_proofs, decompress_merkle_proofs,  # noqa: F401

@@ -28,6 +28,7 @@
 #include "gl_chacha.cuh"
 #include "gl_field.cuh"
 #include "gl_logup.cuh"
+#include "gl_ctl.cuh"
 #include "gl_ntt.cuh"
 #include "gl_poseidon.cuh"
 #include "gl_vanishing.cuh"
@@ -1322,6 +1323,22 @@ __global__ void __launch_bounds__(128) k_logup_rows(LogupParams p, unsigned int*
     u64 v[GL_LOGUP_MAX_INSTR];
     if (!logup_row(p, i, v)) atomicOr(flag, 1u);
 }
+// ---- starky's cross-table lookup helper columns (partial_sums, starky/src/cross_table_lookup.rs:383-414): one thread
+// per row of one table, every CtlZData group and challenge; the row's arithmetic is gl_ctl.cuh. Z is the suffix sum of
+// the `term` sequences: total - (the additive mscan's exclusive prefix), k_ctl_suffix.
+__global__ void __launch_bounds__(128) k_ctl_rows(CtlParams p, unsigned int* flag) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ((size_t)1 << p.log_n)) return;
+    u64 v[GL_CTL_MAX_INSTR];
+    if (!ctl_row(p, i, v)) atomicOr(flag, 1u);
+}
+// z[i] = sum_{i' >= i} term[i'] from pre[i] = sum_{i' < i} term[i']: the total minus the exclusive prefix
+__global__ void k_ctl_suffix(const u64* term, const u64* pre, size_t n, u64* z) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u64 total = add(pre[n - 1], term[n - 1]);
+    z[i] = canon(sub(total, pre[i]));
+}
 // any non-zero word in [begin, begin + count) of each of `cols` columns (stride `stride`) -> flag
 __global__ void k_any_nonzero(const u64* data, size_t stride, size_t begin, size_t count, unsigned int* flag) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -2153,6 +2170,102 @@ int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_strid
             TRY(mscan<ScanAdd>(ctx, term.get() + (size_t)c * n, n, tot.get(), n, 1,
                                out + (col + (size_t)c * (num_h[l] + 1) + num_h[l]) * n));
         col += (size_t)n_challenges * (num_h[l] + 1);
+    }
+    return flag_status(ctx, dflag, {INVERT_ZERO});
+}
+
+int gl_stark_ctl_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,
+                         const gl_stark_instr* program, const uint32_t* group_offsets, uint32_t n_groups,
+                         const uint64_t* consts, uint32_t n_consts, const uint64_t* challenges, uint32_t n_challenges,
+                         uint32_t constraint_degree, const uint32_t* zs_index, uint64_t* out) {
+    if (!ctx || !trace || !program || !group_offsets || !challenges || !zs_index || !out || (n_consts && !consts))
+        return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (n_groups == 0) return set_err(ctx, GL_ERR_BAD_ARG, "no CTL groups");
+    if (n_groups > GL_CTL_MAX_GROUPS) return set_err(ctx, GL_ERR_UNSUPPORTED, "%u CTL groups (max %d)", n_groups, GL_CTL_MAX_GROUPS);
+    if (n_challenges == 0 || n_challenges > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
+    if (log_n > 3 * NTT_MAX_LOG_PASS) return set_err(ctx, GL_ERR_UNSUPPORTED, "log_n %u > 30", log_n);
+    const size_t n = (size_t)1 << log_n;
+    if (num_columns > 1 && col_stride < n) return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent (stride < n)");
+    const uint32_t chunk = constraint_degree == 0 ? 1 : constraint_degree - 1;  // lookup.rs:757
+    // validate every group's row program once on the host: the kernel trusts it
+    std::vector<uint32_t> num_h(n_groups);
+    for (uint32_t g = 0; g < n_groups; g++) {
+        const uint32_t b = group_offsets[g], e = group_offsets[g + 1];
+        if (e <= b || e - b > GL_CTL_MAX_INSTR)
+            return set_err(ctx, GL_ERR_UNSUPPORTED, "CTL group %u: row program of 1..%d instructions", g, GL_CTL_MAX_INSTR);
+        uint32_t entries = 0, values = 0;
+        for (uint32_t k = 0; k < e - b; k++) {
+            const gl_stark_instr in = program[b + k];
+            bool ok = true;
+            switch (in.op) {
+                case GL_STARK_LOCAL: case GL_STARK_NEXT: ok = in.a < num_columns; break;
+                case GL_STARK_CONST: ok = in.a < n_consts; break;
+                case GL_STARK_ADD: case GL_STARK_SUB: case GL_STARK_MUL: ok = in.a < k && in.b < k; break;
+                case GL_STARK_EMIT: ok = in.a < k && in.b <= GL_CTL_FILTER; break;
+                default: ok = false;
+            }
+            if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "CTL group %u: bad row instruction %u", g, k);
+            if (in.op != GL_STARK_EMIT) continue;
+            if (in.b == GL_CTL_VALUE && ++values > GL_CTL_MAX_VALUES)
+                return set_err(ctx, GL_ERR_UNSUPPORTED, "CTL group %u: more than %d values in an entry", g, GL_CTL_MAX_VALUES);
+            if (in.b == GL_CTL_FILTER) {
+                if (++entries > GL_CTL_MAX_ENTRIES)
+                    return set_err(ctx, GL_ERR_UNSUPPORTED, "CTL group %u: more than %d entries", g, GL_CTL_MAX_ENTRIES);
+                values = 0;
+            }
+        }
+        if (entries == 0 || values != 0)
+            return set_err(ctx, GL_ERR_BAD_ARG, "CTL group %u: every entry needs its values, then one filter", g);
+        if (entries > 1 && constraint_degree == 1)
+            return set_err(ctx, GL_ERR_BAD_SHAPE, "attempt to divide by zero: constraint degree 1 leaves no entries per helper column");
+        num_h[g] = entries > 1 ? (entries + chunk - 1) / chunk : 0;
+    }
+    // zs position -> (group, challenge); helper columns of the positions in order, then the Z columns
+    const uint32_t n_zs = n_groups * n_challenges;
+    std::vector<int64_t> at(n_zs, -1);
+    for (uint32_t k = 0; k < n_zs; k++) {
+        if (zs_index[k] >= n_zs || at[zs_index[k]] >= 0) return set_err(ctx, GL_ERR_BAD_ARG, "zs_index is not a permutation");
+        at[zs_index[k]] = k;
+    }
+    CtlParams p;
+    uint32_t total_h = 0;
+    for (uint32_t z = 0; z < n_zs; z++) {
+        const uint32_t g = (uint32_t)(at[z] / n_challenges), c = (uint32_t)(at[z] % n_challenges);
+        p.helper_col[g][c] = total_h;
+        total_h += num_h[g];
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    const size_t nchunks = (n + SCAN_CHUNK - 1) / SCAN_CHUNK;
+    const size_t n_prog = group_offsets[n_groups] - group_offsets[0];
+    DevBuf dprog(ctx), dconst(ctx), dflag(ctx), term(ctx), pre(ctx), tot(ctx);
+    TRY(upload_program(ctx, program + group_offsets[0], n_prog * sizeof(gl_stark_instr), consts, n_consts, dprog, dconst));
+    TRY(flag_alloc(ctx, dflag));
+    TRY(term.alloc((size_t)n_zs * n));
+    TRY(pre.alloc(n));
+    TRY(tot.alloc(nchunks));
+    p.trace = trace;
+    p.trace_stride = col_stride;
+    p.log_n = log_n;
+    p.prog = (const gl_stark_instr*)dprog.get();
+    for (uint32_t g = 0; g <= n_groups; g++) p.offsets[g] = group_offsets[g] - group_offsets[0];
+    p.n_groups = n_groups;
+    p.consts = dconst.get();
+    p.chunk = chunk;
+    for (uint32_t c = 0; c < GL_STARK_MAX_ALPHAS; c++) {
+        p.betas[c] = c < n_challenges ? canon(challenges[2 * c]) : 0;
+        p.gammas[c] = c < n_challenges ? canon(challenges[2 * c + 1]) : 0;
+    }
+    p.n_challenges = n_challenges;
+    p.out = out;
+    p.term = term.get();
+    k_ctl_rows<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(p, (unsigned int*)dflag.get());
+    CKL(ctx);
+    for (uint32_t k = 0; k < n_zs; k++) {  // Z of zs position zs_index[k]: the suffix sum of (group, challenge) k's terms
+        const u64* t = term.get() + (size_t)k * n;
+        TRY(mscan<ScanAdd>(ctx, t, n, tot.get(), n, 1, pre.get()));
+        k_ctl_suffix<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(t, pre.get(), n,
+                                                                         out + ((size_t)total_h + zs_index[k]) * n);
+        CKL(ctx);
     }
     return flag_status(ctx, dflag, {INVERT_ZERO});
 }

@@ -1,7 +1,8 @@
-"""starky's logUp lookup argument (starky/src/lookup.rs:33-863, https://eprint.iacr.org/2022/1530) without cross-table
-lookups: Column / Filter / Lookup, the grand-product challenges, the lookup constraints recorded into a STARK's constraint
-program (eval_packed_lookups_generic) and the row programs gl_stark_lookup_helpers runs to write the helper columns on
-the device (lookup_helper_columns)."""
+"""starky's logUp lookup argument (starky/src/lookup.rs:33-863, https://eprint.iacr.org/2022/1530) within one STARK (the
+cross-table lookups, which reuse Column / Filter and eval_helper_columns, are cross_table_lookup.py): Column / Filter /
+Lookup, the grand-product challenges, the lookup constraints recorded into a STARK's constraint program
+(eval_packed_lookups_generic) and the row programs gl_stark_lookup_helpers runs to write the helper columns on the
+device (lookup_helper_columns)."""
 import numpy as np
 
 from . import _native as N
@@ -190,19 +191,23 @@ def get_grand_product_challenge_set(challenger, num_challenges):
     return out
 
 
-def eval_helper_columns(filters, columns, helper_columns, constraint_degree, challenge, consumer, vars):
-    """eval_helper_columns (lookup.rs:655-695) with the challenge (beta = 1, gamma = challenge): combine(x) = x + gamma."""
+def eval_helper_columns(filters, columns, helper_columns, constraint_degree, challenge, consumer, vars, combine=None):
+    """eval_helper_columns (lookup.rs:655-695). A lookup's columns are single values combined with its challenge
+    (beta = 1, gamma = challenge): combine(x) = x + gamma; a cross-table lookup passes its own combine (a tuple's
+    GrandProductChallenge::combine)."""
     if not helper_columns:
         return
+    if combine is None:
+        combine = lambda x: x + challenge  # noqa: E731
     chunk_size = helper_chunk_size(constraint_degree)
     for k, h in enumerate(helper_columns):
         chunk, fs = columns[k * chunk_size:(k + 1) * chunk_size], filters[k * chunk_size:(k + 1) * chunk_size]
         if len(chunk) == 2:
-            combin0, combin1 = chunk[0] + challenge, chunk[1] + challenge
+            combin0, combin1 = combine(chunk[0]), combine(chunk[1])
             f0, f1 = fs[0].eval_filter(vars), fs[1].eval_filter(vars)
             consumer.constraint(combin1 * combin0 * h - f0 * combin1 - f1 * combin0)
         elif len(chunk) == 1:
-            combin = chunk[0] + challenge
+            combin = combine(chunk[0])
             consumer.constraint(combin * h - fs[0].eval_filter(vars))
         else:
             raise N.ShapeError("Allow other constraint degrees: a chunk of %d looking columns" % len(chunk))

@@ -79,39 +79,54 @@ class OpeningSet:
 
 @dataclass
 class StarkOpeningSet:
-    """StarkOpeningSet<F, D> (starky/src/proof.rs:205-219) without cross-table lookups."""
+    """StarkOpeningSet<F, D> (starky/src/proof.rs:205-219). ctl_zs_first: the CTL Z polynomials at 1, base-field values
+    (uint64), for a Stark with cross-table lookups; None otherwise."""
     local_values: np.ndarray
     next_values: np.ndarray
     auxiliary_polys: np.ndarray = None
     auxiliary_polys_next: np.ndarray = None
     quotient_polys: np.ndarray = None
+    ctl_zs_first: np.ndarray = None
 
     @classmethod
-    def new(cls, zeta, g, trace_commitment, auxiliary_polys_commitment=None, quotient_commitment=None):
-        """StarkOpeningSet::new (starky/src/proof.rs:221-260): trace (and auxiliary) polynomials at zeta and g*zeta,
-        quotient polynomials at zeta."""
+    def new(cls, zeta, g, trace_commitment, auxiliary_polys_commitment=None, quotient_commitment=None,
+            num_ctl_zs_first=None):
+        """StarkOpeningSet::new (starky/src/proof.rs:221-265): trace (and auxiliary) polynomials at zeta and g*zeta,
+        quotient polynomials at zeta; with num_ctl_zs_first = (first, count), the auxiliary polynomials first ..
+        first + count (the CTL Zs) at 1."""
         g_zeta = F.ext_mul((int(g), 0), zeta)
         req = [(trace_commitment, zeta), (trace_commitment, g_zeta)]
         if auxiliary_polys_commitment is not None:
             req += [(auxiliary_polys_commitment, zeta), (auxiliary_polys_commitment, g_zeta)]
         if quotient_commitment is not None:
             req.append((quotient_commitment, zeta))
+        if num_ctl_zs_first is not None:
+            req.append((auxiliary_polys_commitment, (1, 0)))
         res = eval_commitments(req)
         k = 2
-        aux = aux_next = quot = None
+        aux = aux_next = quot = first = None
         if auxiliary_polys_commitment is not None:
             aux, aux_next = res[k], res[k + 1]
             k += 2
         if quotient_commitment is not None:
             quot = res[k]
-        return cls(res[0], res[1], aux, aux_next, quot)
+            k += 1
+        if num_ctl_zs_first is not None:
+            start, count = num_ctl_zs_first
+            first = np.ascontiguousarray(np.asarray(res[k])[start:start + count, 0], dtype=np.uint64)
+        return cls(res[0], res[1], aux, aux_next, quot, first)
 
     def to_fri_openings(self):
-        """to_fri_openings (starky/src/proof.rs:263-290), no CTLs: [zeta batch, zeta_next batch]."""
+        """to_fri_openings (starky/src/proof.rs:267-307): [zeta batch, zeta_next batch] and, with CTLs, the CTL Zs
+        at 1 as extension values."""
         zeta_batch = [self.local_values]
         if self.auxiliary_polys is not None:
             zeta_batch.append(self.auxiliary_polys)
         if self.quotient_polys is not None:
             zeta_batch.append(self.quotient_polys)
         next_batch = [self.next_values] + ([self.auxiliary_polys_next] if self.auxiliary_polys_next is not None else [])
-        return [np.concatenate(zeta_batch), np.concatenate(next_batch)]
+        out = [np.concatenate(zeta_batch), np.concatenate(next_batch)]
+        if self.ctl_zs_first is not None:
+            first = np.asarray(self.ctl_zs_first, dtype=np.uint64)
+            out.append(np.stack([first, np.zeros_like(first)], axis=1))
+        return out

@@ -1,11 +1,13 @@
 """starky's prover (SURVEY.md section 8f rows 1 and 1'), mirroring starky/src/{config.rs, stark.rs,
 constraint_consumer.rs, vanishing_poly.rs, prover.rs, proof.rs, get_challenges.rs, fibonacci_stark.rs} for STARKs
-with or without logUp lookups (lookup.py), without cross-table lookups. The constraints of a Stark -- its own, then
-those of its lookups -- are recorded ONCE as a straight-line program (ConstraintBuilder): gl_stark_quotient[_aux]
-evaluates it on every point of the quotient coset, reading the trace and auxiliary LDEs in place on the device, and
-eval_vanishing_poly evaluates the same instructions at one point of F_{p^2} on the host (the constraint-binding step of
-`prove`, and any verifier). `prove` strings the device steps together in the reference's order with the transcript on
-the host; the lookup helper columns are written on the device by gl_stark_lookup_helpers."""
+with or without logUp lookups (lookup.py) and cross-table lookups (cross_table_lookup.py). The constraints of a Stark --
+its own, then those of its lookups, then those of its CTLs -- are recorded ONCE as a straight-line program
+(ConstraintBuilder): gl_stark_quotient[_aux] evaluates it on every point of the quotient coset, reading the trace and
+auxiliary LDEs in place on the device, and eval_vanishing_poly evaluates the same instructions at one point of F_{p^2}
+on the host (the constraint-binding step of the prover, and any verifier). `prove` (one STARK) and
+cross_table_lookup.prove_with_ctls (several) both run prove_with_commitment, which strings the device steps together in
+the reference's order with the transcript on the host; the lookup helper columns are written on the device by
+gl_stark_lookup_helpers, the CTL helper and Z columns by gl_stark_ctl_helpers."""
 import ctypes as C
 
 import numpy as np
@@ -49,9 +51,11 @@ class Expr:
 class ConstraintBuilder:
     """Records eval_packed_generic as instructions; doubles as the ConstraintConsumer (constraint_consumer.rs:46-84)."""
 
-    def __init__(self, num_columns, num_public_inputs, num_aux=0, num_lookup_challenges=0):
-        # consts[0:num_bound] -- the public inputs, then the lookup challenges -- are bound at evaluation time
-        self.num_bound = num_public_inputs + num_lookup_challenges
+    def __init__(self, num_columns, num_public_inputs, num_aux=0, num_lookup_challenges=0, num_ctl_vars=0):
+        # consts[0:num_bound] -- the public inputs, the lookup challenges, then each CTL Z's (beta, gamma) -- are bound
+        # at evaluation time
+        self.num_lookup_challenges = num_lookup_challenges
+        self.num_bound = num_public_inputs + num_lookup_challenges + 2 * num_ctl_vars
         self.instrs, self.consts = [], [None] * self.num_bound
         self.num_columns, self.num_pi, self.num_aux = num_columns, num_public_inputs, num_aux
         self._cache = {}
@@ -89,8 +93,14 @@ class ConstraintBuilder:
         return self._push(OP_AUX_NEXT, col)
 
     def lookup_challenge(self, c):
-        assert 0 <= c < self.num_bound - self.num_pi
+        assert 0 <= c < self.num_lookup_challenges
         return self._push(OP_CONST, self.num_pi + c)
+
+    def ctl_challenge(self, k):
+        """(beta, gamma) of the program's k-th CTL Z polynomial."""
+        base = self.num_pi + self.num_lookup_challenges + 2 * k
+        assert base + 2 <= self.num_bound
+        return self._push(OP_CONST, base), self._push(OP_CONST, base + 1)
 
     def constant(self, v):
         v = int(v) % F.ORDER
@@ -149,35 +159,50 @@ class Stark:
     def _helper_columns_per_challenge(self):
         return sum(lookup.num_helper_columns(self.constraint_degree()) for lookup in self.lookups())
 
-    def constraint_program(self, num_lookup_challenges=0):
+    def requires_ctls(self):
+        """stark.rs:272-278: whether the Stark takes part in cross-table lookups; False by default."""
+        return False
+
+    def constraint_program(self, num_lookup_challenges=0, ctl_vars=None):
         """The Stark's constraints (eval_packed_generic), then -- with lookups -- those of the logUp argument for
-        num_lookup_challenges challenges (eval_vanishing_poly, vanishing_poly.rs:41-52): the order of the alpha-fold."""
-        if not self.uses_lookups():
+        num_lookup_challenges challenges, then -- with ctl_vars (CtlCheckVars; only their shape is read) -- those of
+        its cross-table lookups (eval_vanishing_poly, vanishing_poly.rs:41-61): the order of the alpha-fold. The
+        auxiliary columns are [lookup helpers | CTL helpers | CTL Zs]."""
+        if not self.uses_lookups() and ctl_vars is None:
             b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS)
             self.eval(b, b)
             return b
         from .lookup import eval_packed_lookups_generic
 
-        lookups = self.lookups()
-        b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS, self._helper_columns_per_challenge() * num_lookup_challenges,
-                              num_lookup_challenges)
+        nl = self._helper_columns_per_challenge() * num_lookup_challenges if self.uses_lookups() else 0
+        ctl_vars = ctl_vars or []
+        num_ctl = sum(len(v.helper_columns) for v in ctl_vars) + len(ctl_vars)
+        b = ConstraintBuilder(self.COLUMNS, self.PUBLIC_INPUTS, nl + num_ctl,
+                              num_lookup_challenges if self.uses_lookups() else 0, len(ctl_vars))
         self.eval(b, b)
-        eval_packed_lookups_generic(self, lookups, b, num_lookup_challenges, b)
+        if self.uses_lookups():
+            eval_packed_lookups_generic(self, self.lookups(), b, num_lookup_challenges, b)
+        if ctl_vars:
+            from .cross_table_lookup import eval_cross_table_lookup_checks
+
+            eval_cross_table_lookup_checks(b, ctl_vars, b, self.constraint_degree(), nl)
         return b
 
     def num_quotient_polys(self, config):
         """stark.rs:95-98"""
         return self.quotient_degree_factor() * config.num_challenges
 
-    def fri_instance(self, zeta, g, config):
-        """fri_instance (stark.rs:101-170) without CTLs: the trace oracle and -- with lookups -- the auxiliary oracle
-        opened at zeta and g * zeta, the quotient oracle -- present only when the Stark has constraints -- at zeta."""
+    def fri_instance(self, zeta, g, config, num_ctl_helpers=0, num_ctl_zs=0):
+        """fri_instance (stark.rs:101-170): the trace oracle and -- with lookups or CTLs -- the auxiliary oracle opened
+        at zeta and g * zeta, the quotient oracle -- present only when the Stark has constraints -- at zeta, and -- with
+        CTLs -- the auxiliary oracle's CTL Z columns at 1."""
         from .fri import FriBatchInfo, FriInstanceInfo, FriOracleInfo, FriPolynomialInfo
 
         trace_info = FriPolynomialInfo.from_range(0, range(self.COLUMNS))
         oracles = [FriOracleInfo(self.COLUMNS, False)]
-        if self.uses_lookups():
-            num_aux = self.num_lookup_helper_columns(config)
+        nl = self.num_lookup_helper_columns(config) if self.uses_lookups() else 0
+        if self.uses_lookups() or self.requires_ctls():
+            num_aux = nl + num_ctl_helpers + num_ctl_zs
             trace_info = trace_info + FriPolynomialInfo.from_range(len(oracles), range(num_aux))
             oracles.append(FriOracleInfo(num_aux, False))
         quotient_info = []
@@ -186,7 +211,11 @@ class Stark:
             quotient_info = FriPolynomialInfo.from_range(len(oracles), range(nq))
             oracles.append(FriOracleInfo(nq, False))
         zeta_next = F.ext_mul((int(g) % F.ORDER, 0), zeta)
-        return FriInstanceInfo(oracles, [FriBatchInfo(zeta, trace_info + quotient_info), FriBatchInfo(zeta_next, trace_info)])
+        batches = [FriBatchInfo(zeta, trace_info + quotient_info), FriBatchInfo(zeta_next, trace_info)]
+        if self.requires_ctls():
+            batches.append(FriBatchInfo((1, 0), FriPolynomialInfo.from_range(
+                1, range(nl + num_ctl_helpers, nl + num_ctl_helpers + num_ctl_zs))))
+        return FriInstanceInfo(oracles, batches)
 
 
 class FibonacciStark(Stark):
@@ -222,11 +251,13 @@ class FibonacciStark(Stark):
 
 
 def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxiliary_polys_commitment=None,
-                           lookup_challenges=None):
+                           lookup_challenges=None, ctl_vars=None):
     """compute_quotient_polys (prover.rs:488-668) on the device. Returns a torch int64 CUDA tensor (num_challenges, size)
     of quotient-polynomial coefficients, size = n << log2_ceil(quotient_degree_factor), or None if the Stark has no
     quotient. Raises if the vanishing polynomial is not divisible by Z_H. A Stark with lookups also needs the auxiliary
-    commitment (its LDE is read in place, like the trace's) and the lookup challenges."""
+    commitment (its LDE is read in place, like the trace's) and the lookup challenges; one with CTLs the auxiliary
+    commitment and ctl_vars (CtlCheckVars of its CTL data's shape; their challenges are bound like the public
+    inputs)."""
     import torch
 
     qdf = stark.quotient_degree_factor()
@@ -234,9 +265,12 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
         return None
     if stark.uses_lookups() and (auxiliary_polys_commitment is None or lookup_challenges is None):
         raise N.ShapeError("a Stark with lookups needs the auxiliary commitment and the lookup challenges")
+    if ctl_vars is not None and auxiliary_polys_commitment is None:
+        raise N.ShapeError("a Stark with CTLs needs the auxiliary commitment")
     challenges = [int(c) % F.ORDER for c in lookup_challenges] if stark.uses_lookups() else []
-    b = stark.constraint_program(len(challenges))
-    consts = np.array([int(x) % F.ORDER for x in public_inputs] + challenges + b.consts[b.num_bound:], dtype=np.uint64)
+    b = stark.constraint_program(len(challenges), ctl_vars)
+    consts = np.array([int(x) % F.ORDER for x in public_inputs] + challenges + _ctl_bound(ctl_vars) + b.consts[b.num_bound:],
+                      dtype=np.uint64)
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs" % stark.PUBLIC_INPUTS)
     al = np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
@@ -245,7 +279,7 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
     ctx = trace_commitment.ctx
     out = torch.empty((len(al), size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     prog = b.program()
-    if stark.uses_lookups():
+    if stark.uses_lookups() or ctl_vars is not None:
         N.check(N.lib().gl_stark_quotient_aux(ctx.h, trace_commitment.h, auxiliary_polys_commitment.h, prog,
                                               len(b.instrs), N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
                                               N.vp(out.data_ptr())), ctx.h)
@@ -256,6 +290,11 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
     return out
 
 
+def _ctl_bound(ctl_vars):
+    """The CTL challenges a constraint program binds after the public inputs and lookup challenges."""
+    return [int(v) % F.ORDER for c in (ctl_vars or []) for v in (c.challenges.beta, c.challenges.gamma)]
+
+
 def check_lookup_shapes(stark):
     """The reference's panics for a Stark's lookups, raised before any device work: constraint degree 1 (division by
     zero in num_helper_columns) and chunks of more than two looking columns (todo! in eval_helper_columns)."""
@@ -263,10 +302,11 @@ def check_lookup_shapes(stark):
         lookup.check_chunks(stark.constraint_degree())
 
 
-def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx):
+def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx, out=None):
     """The lookup helper columns (prover.rs:177-195, lookup_helper_columns) on the device: for every lookup, for every
     challenge, the h_k columns and Z, from the trace values `trace` -- a (COLUMNS, n) int64 CUDA tensor, read in place.
-    Returns a (num_lookup_helper_columns, n) int64 CUDA tensor of values."""
+    Returns a (num_lookup_helper_columns, n) int64 CUDA tensor of values: `out` if given (a contiguous view, e.g. the
+    first rows of a table's auxiliary buffer), else a new one."""
     import torch
 
     from .lookup import row_programs
@@ -275,7 +315,11 @@ def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx):
     cols, n = trace.shape
     prog, offsets, consts = row_programs(stark.lookups(), stark.COLUMNS)
     ch = np.array([int(c) % F.ORDER for c in lookup_challenges], dtype=np.uint64)
-    out = torch.empty((stark._helper_columns_per_challenge() * len(ch), n), dtype=torch.int64, device=trace.device)
+    shape = (stark._helper_columns_per_challenge() * len(ch), n)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.int64, device=trace.device)
+    elif tuple(out.shape) != shape or not out.is_contiguous():
+        raise N.ShapeError("the lookup helper output must be a contiguous %r tensor" % (shape,))
     N.check(N.lib().gl_stark_lookup_helpers(ctx.h, N.vp(trace.data_ptr()), n, cols, F.log2_strict(n), prog,
                                             offsets.ctypes.data_as(N.u32p), len(offsets) - 1,
                                             N.np_ptr(consts) if len(consts) else None, len(consts), N.np_ptr(ch), len(ch),
@@ -338,24 +382,33 @@ def eval_l_0_and_l_last(log_n, x):
 
 
 def eval_vanishing_poly(stark, local_values, next_values, public_inputs, alphas, x, degree_bits, auxiliary_polys=None,
-                        auxiliary_polys_next=None, lookup_challenges=None):
-    """compute_eval_vanishing_poly (vanishing_poly.rs:108-173) without CTLs: the Stark's constraint program -- the
-    instructions gl_stark_quotient runs -- evaluated at one point x of F_{p^2}, with the local and next rows (and, with
-    lookups, the auxiliary polynomials' local and next values) as F_{p^2} values and the public inputs, lookup challenges
-    and program constants as base-field values; the constraints are filtered by z_last = x - g^{-1}, L_0(x), L_{n-1}(x)
-    and folded with every alpha as ConstraintConsumer does (constraint_consumer.rs:46-84). Returns num_challenges F_{p^2}
+                        auxiliary_polys_next=None, lookup_challenges=None, ctl_vars=None):
+    """compute_eval_vanishing_poly (vanishing_poly.rs:108-173): the Stark's constraint program -- the instructions
+    gl_stark_quotient runs -- evaluated at one point x of F_{p^2}, with the local and next rows (with lookups, the
+    auxiliary polynomials' local and next values, of which the lookup helper columns are read; with CTLs, the
+    CtlCheckVars' helper and Z values) as F_{p^2} values and the public inputs, lookup challenges, CTL challenges and
+    program constants as base-field values; the constraints are filtered by z_last = x - g^{-1}, L_0(x), L_{n-1}(x) and
+    folded with every alpha as ConstraintConsumer does (constraint_consumer.rs:46-84). Returns num_challenges F_{p^2}
     values (c0, c1)."""
     challenges = []
     if stark.uses_lookups():
         if auxiliary_polys is None or auxiliary_polys_next is None or lookup_challenges is None:
             raise N.ShapeError("a Stark with lookups needs the auxiliary values and the lookup challenges")
         challenges = [int(c) % F.ORDER for c in lookup_challenges]
-    b = stark.constraint_program(len(challenges))
+    b = stark.constraint_program(len(challenges), ctl_vars)
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs, got %d" % (stark.PUBLIC_INPUTS, len(public_inputs)))
-    if challenges and (len(auxiliary_polys) != b.num_aux or len(auxiliary_polys_next) != b.num_aux):
+    if ctl_vars is not None:     # [lookup helpers | CTL helpers | CTL Zs], as the program reads them
+        nl = stark._helper_columns_per_challenge() * len(challenges)
+        if challenges and (len(auxiliary_polys) < nl or len(auxiliary_polys_next) < nl):
+            raise N.ShapeError("expected %d lookup auxiliary values" % nl)
+        helpers = [h for v in ctl_vars for h in v.helper_columns]
+        auxiliary_polys = list(auxiliary_polys[:nl] if challenges else []) + helpers + [v.local_z for v in ctl_vars]
+        auxiliary_polys_next = (list(auxiliary_polys_next[:nl] if challenges else []) + [(0, 0)] * len(helpers)
+                                + [v.next_z for v in ctl_vars])
+    elif challenges and (len(auxiliary_polys) != b.num_aux or len(auxiliary_polys_next) != b.num_aux):
         raise N.ShapeError("expected %d auxiliary values" % b.num_aux)
-    consts = [int(v) % F.ORDER for v in public_inputs] + challenges + b.consts[b.num_bound:]
+    consts = [int(v) % F.ORDER for v in public_inputs] + challenges + _ctl_bound(ctl_vars) + b.consts[b.num_bound:]
     x = (int(x[0]) % F.ORDER, int(x[1]) % F.ORDER)
     l_0, l_last = eval_l_0_and_l_last(degree_bits, x)
     z_last = F.ext_sub(x, (F.inverse(F.primitive_root_of_unity(degree_bits)), 0))
@@ -411,19 +464,35 @@ def _dummy_openings(challenger, num_trace_polys, pow_degree, num_aux_polys=0):
     return evals[:t], evals[t:2 * t], evals[2 * t:2 * t + a], evals[2 * t + a:total]
 
 
-def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_bits, lookup_challenges=None):
+def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_bits, lookup_challenges=None,
+                      ctl_vars=None, num_aux=None):
     """The constraint-binding step (prover.rs:239-370, get_challenges.rs:94-163): alphas', simulated openings, zeta',
     the vanishing polynomial there observed; returns the alphas the quotient uses. A Stark with lookups also simulates
-    its auxiliary polynomials and evaluates the lookup constraints with the lookup challenges."""
+    its auxiliary polynomials and evaluates the lookup constraints with the lookup challenges; with ctl_vars (the shape
+    of its CTL data) the CTL helper and Z values are read from the simulated auxiliary polynomials too
+    (prover.rs:321-350), of which there are num_aux."""
+    from .cross_table_lookup import CtlCheckVars
+
     alphas_prime = challenger.get_n_challenges(num_challenges)
     pow_degree = max(2, stark.constraint_degree() + 1)
-    if lookup_challenges is None:
+    if num_aux is None:
+        num_aux = 0 if lookup_challenges is None else stark._helper_columns_per_challenge() * len(lookup_challenges)
+    if num_aux == 0:
         local, nxt = _dummy_openings(challenger, stark.COLUMNS, pow_degree)
         aux = {}
     else:
-        num_aux = stark._helper_columns_per_challenge() * len(lookup_challenges)
         local, nxt, a, a_next = _dummy_openings(challenger, stark.COLUMNS, pow_degree, num_aux)
         aux = dict(auxiliary_polys=a, auxiliary_polys_next=a_next, lookup_challenges=lookup_challenges)
+        if ctl_vars is not None:
+            nl = stark._helper_columns_per_challenge() * len(lookup_challenges) if lookup_challenges is not None else 0
+            total = sum(len(v.helper_columns) for v in ctl_vars)
+            dummy, start = [], nl
+            for i, v in enumerate(ctl_vars):
+                k = len(v.helper_columns)
+                dummy.append(CtlCheckVars(a[start:start + k], a[nl + total + i], a_next[nl + total + i], v.challenges,
+                                          v.columns, v.filter))
+                start += k
+            aux["ctl_vars"] = dummy
     zeta_prime = challenger.get_extension_challenge()
     challenger.observe_extension_elements(eval_vanishing_poly(stark, local, nxt, public_inputs, alphas_prime, zeta_prime,
                                                               degree_bits, **aux))
@@ -431,8 +500,8 @@ def _bind_constraints(stark, challenger, public_inputs, num_challenges, degree_b
 
 
 class StarkProof:
-    """StarkProof (starky/src/proof.rs:30-53) without CTLs: trace cap, quotient cap (None for a Stark without
-    constraints), StarkOpeningSet, FriProof, and the auxiliary polynomials' cap (None for a Stark without lookups). The
+    """StarkProof (starky/src/proof.rs:30-53): trace cap, quotient cap (None for a Stark without
+    constraints), StarkOpeningSet, FriProof, and the auxiliary polynomials' cap (None for a Stark without lookups or CTLs). The
     reference has no byte format for it (serde only); opening_proof.to_bytes() is write_fri_proof."""
 
     def __init__(self, trace_cap, quotient_polys_cap, openings, opening_proof, auxiliary_polys_cap=None):
@@ -452,31 +521,41 @@ class StarkProofWithPublicInputs:
     def __init__(self, proof, public_inputs):
         self.proof, self.public_inputs = proof, [int(v) % F.ORDER for v in public_inputs]
 
-    def get_challenges(self, stark, config, verifier_circuit_fri_params=None):
+    def get_challenges(self, stark, config, verifier_circuit_fri_params=None, challenger=None, ctl_challenges=None,
+                       ctl_vars=None, ignore_trace_cap=False):
         """get_challenges (get_challenges.rs:37-199,323-357) replayed from the proof alone: the public inputs, the
-        config, the trace cap, the lookup challenges and the auxiliary cap (get_challenges.rs:67-92), the
-        constraint-binding step, the quotient cap, zeta, the openings, then FRI's challenges. Returns a dict:
-        lookup_challenge_set (None without an auxiliary cap), stark_alphas, stark_zeta, fri_alpha, fri_betas,
-        fri_pow_response, fri_query_indices."""
+        config, the trace cap (unless ignore_trace_cap), the lookup challenges -- ctl_challenges when given, else drawn
+        if there is an auxiliary cap -- and the auxiliary cap (get_challenges.rs:67-92), the constraint-binding step
+        (with ctl_vars, the table's CtlCheckVars), the quotient cap, zeta, the openings, then FRI's challenges. A
+        multi-STARK replay passes its challenger. Returns a dict: lookup_challenge_set (None without an auxiliary cap
+        or CTL challenges), stark_alphas, stark_zeta, fri_alpha, fri_betas, fri_pow_response, fri_query_indices."""
         from .challenger import Challenger
         from .fri import fri_challenges
         from .lookup import get_grand_product_challenge_set
 
         p = self.proof
         degree_bits = p.recover_degree_bits(config)
-        ch = Challenger()
+        ch = challenger if challenger is not None else Challenger()
         ch.observe_elements(self.public_inputs)
         config.observe(ch)
-        ch.observe_cap(p.trace_cap)
+        if not ignore_trace_cap:
+            ch.observe_cap(p.trace_cap)
         lookup_challenge_set = lookup_challenges = None
-        if p.auxiliary_polys_cap is not None:
+        if ctl_challenges is not None:
+            lookup_challenge_set = list(ctl_challenges)
+        elif p.auxiliary_polys_cap is not None:
             lookup_challenge_set = get_grand_product_challenge_set(ch, config.num_challenges)
+        if p.auxiliary_polys_cap is not None:
             ch.observe_cap(p.auxiliary_polys_cap)
         if stark.uses_lookups():
             if lookup_challenge_set is None:
                 raise N.ShapeError("Missing auxiliary_polys_cap")
             lookup_challenges = [c.beta for c in lookup_challenge_set]
-        alphas = _bind_constraints(stark, ch, self.public_inputs, config.num_challenges, degree_bits, lookup_challenges)
+        num_aux = None
+        if ctl_vars is not None:
+            num_aux = len(p.openings.auxiliary_polys) if p.openings.auxiliary_polys is not None else 0
+        alphas = _bind_constraints(stark, ch, self.public_inputs, config.num_challenges, degree_bits, lookup_challenges,
+                                   ctl_vars, num_aux)
         if p.quotient_polys_cap is not None:
             ch.observe_cap(p.quotient_polys_cap)
         zeta = ch.get_extension_challenge()
@@ -528,25 +607,13 @@ def _device_trace(trace, ctx):
     return dev
 
 
-def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None):
-    """prove + prove_with_commitment (starky/src/prover.rs:40-114,125-484) for a Stark without CTLs: trace = (COLUMNS, n)
-    host columns or torch CUDA tensor -> StarkProofWithPublicInputs. Every array-sized step runs on the device (trace
-    commitment, lookup helper columns and their commitment, quotient from the LDEs in place, quotient commitment,
-    openings, FRI); the transcript and the constraint-binding step run on the host. verifier_circuit_fri_params: the
-    FRI parameters of a verifier circuit made for another degree (ConstantArityBits only); the transcript then observes
-    the zero caps and coefficients that verifier expects. Raises ShapeError / NativeError with the reference's
-    messages; every commitment is released on every exit path."""
-    from .challenger import Challenger
-    from .fri import prove_openings
-    from .lookup import get_grand_product_challenge_set
-
-    ctx = ctx or N.default_context()
+def _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params=None):
+    """prove's checks (prover.rs:53-81,153-162), before any device work. Returns the ProveParams of the trace."""
     shape = tuple(trace.shape)
     if len(shape) != 2 or shape[0] != stark.COLUMNS:
         raise N.ShapeError("the trace must be (COLUMNS = %d, n), got %r" % (stark.COLUMNS, shape))
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs, got %d" % (stark.PUBLIC_INPUTS, len(public_inputs)))
-    public_inputs = [int(v) % F.ORDER for v in public_inputs]
     degree_bits = F.log2_strict(shape[1])
     fri_params = config.fri_params(degree_bits)
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
@@ -567,31 +634,99 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
             raise N.ShapeError("the verifier circuit's final polynomial has %d coefficients, expected %d"
                                % (final_poly_coeff_len, 1 << (1 + strategy[2])))
         max_num_query_steps = len(vp.reduction_arity_bits)
+    return ProveParams(degree_bits, fri_params, final_poly_coeff_len, max_num_query_steps)
 
-    uses_lookups = stark.uses_lookups()
-    if uses_lookups:
+
+class ProveParams:
+    """What prove_with_commitment needs of the checks: degree_bits, the FRI parameters and the verifier-circuit FRI
+    shape (final_poly_coeff_len, max_num_query_steps; None without a verifier circuit)."""
+
+    def __init__(self, degree_bits, fri_params, final_poly_coeff_len, max_num_query_steps):
+        self.degree_bits, self.fri_params = degree_bits, fri_params
+        self.final_poly_coeff_len, self.max_num_query_steps = final_poly_coeff_len, max_num_query_steps
+
+
+def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None):
+    """prove (starky/src/prover.rs:40-114) for one Stark: trace = (COLUMNS, n) host columns or torch CUDA tensor ->
+    StarkProofWithPublicInputs. The trace commitment, then a fresh challenger observing the public inputs, the config
+    and the trace cap, then prove_with_commitment without CTLs. verifier_circuit_fri_params: the FRI parameters of a
+    verifier circuit made for another degree (ConstantArityBits only); the transcript then observes the zero caps and
+    coefficients that verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment
+    is released on every exit path."""
+    from .challenger import Challenger
+
+    ctx = ctx or N.default_context()
+    params = _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params)
+    public_inputs = [int(v) % F.ORDER for v in public_inputs]
+    rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
+    if stark.uses_lookups():
         check_lookup_shapes(stark)
         trace = _device_trace(trace, ctx)
     trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx)
-    commitments = [trace_commitment]
     try:
         challenger = Challenger()
         challenger.observe_elements(public_inputs)
         config.observe(challenger)
         challenger.observe_cap(trace_commitment.merkle_tree.cap)
-        aux_commitment = lookup_challenges = None
-        lookup_args = {}
-        if uses_lookups:                                                # prover.rs:164-237
-            lookup_challenges = [c.beta for c in get_grand_product_challenge_set(challenger, config.num_challenges)]
-            helper_columns = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
-            aux_commitment = commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx)
+        return prove_with_commitment(stark, config, trace, trace_commitment, None, None, challenger, public_inputs,
+                                     params, ctx=ctx)
+    finally:
+        trace_commitment.close()
+
+
+def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_challenges, challenger, public_inputs,
+                          params, ctx=None):
+    """prove_with_commitment (starky/src/prover.rs:125-484): one table's proof from its committed trace, on a challenger
+    that has already observed what precedes it (the config among them). Every array-sized step runs on the device
+    (lookup helper columns and the auxiliary commitment, quotient from the LDEs in place, quotient commitment, openings,
+    FRI); the transcript and the constraint-binding step run on the host. With ctl_challenges the lookups use their
+    betas (prover.rs:165-168). With ctl_data (cross_table_lookup.CtlData, its CTL columns already in its auxiliary
+    buffer) the auxiliary oracle is [lookup helpers | CTL helpers | CTL Zs], the CTL constraints join the quotient and
+    the openings carry ctl_zs_first. trace: the values the lookup helper columns read (a CUDA tensor when the Stark has
+    lookups). params: _check_prove_shapes's. Every commitment made here is released on every exit path; the trace
+    commitment stays the caller's."""
+    from .fri import prove_openings
+    from .lookup import get_grand_product_challenge_set
+
+    ctx = ctx or N.default_context()
+    degree_bits = params.degree_bits
+    rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
+    uses_lookups = stark.uses_lookups()
+    commitments = []
+    try:
+        aux_commitment = lookup_challenges = ctl_vars = None
+        nl = 0
+        quotient_args = {}
+        if uses_lookups:                                                # prover.rs:164-195
+            if ctl_challenges is not None:
+                lookup_challenges = [c.beta for c in ctl_challenges]
+            else:
+                lookup_challenges = [c.beta for c in get_grand_product_challenge_set(challenger, config.num_challenges)]
+            nl = stark._helper_columns_per_challenge() * len(lookup_challenges)
+            quotient_args = dict(lookup_challenges=lookup_challenges)
+        if ctl_data is not None:                                        # prover.rs:196-230
+            from .cross_table_lookup import ctl_shape_vars
+
+            auxiliary = ctl_data.auxiliary
+            if uses_lookups:
+                compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx, out=auxiliary[:nl])
+            ctl_vars = ctl_shape_vars(ctl_data)
+            quotient_args["ctl_vars"] = ctl_vars
+        elif uses_lookups:
+            auxiliary = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
+        if uses_lookups or ctl_data is not None:
+            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx)
             commitments.append(aux_commitment)
-            del helper_columns
+            del auxiliary
+            if ctl_data is not None:
+                ctl_data.auxiliary = None
             challenger.observe_cap(aux_commitment.merkle_tree.cap)
-            lookup_args = dict(auxiliary_polys_commitment=aux_commitment, lookup_challenges=lookup_challenges)
+            quotient_args["auxiliary_polys_commitment"] = aux_commitment
+        num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
+        num_ctl_helpers, num_ctl_zs = sum(num_ctl_polys), len(num_ctl_polys)
         alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
-                                   lookup_challenges)
-        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **lookup_args)
+                                   lookup_challenges, ctl_vars, nl + num_ctl_helpers + num_ctl_zs if ctl_vars else None)
+        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **quotient_args)
         quotient_commitment = None
         if quotient_polys is not None:
             quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx)
@@ -602,11 +737,13 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
         if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
             raise N.NativeError("Opening point is in the subgroup.")
         g = F.primitive_root_of_unity(degree_bits)
-        openings = StarkOpeningSet.new(zeta, g, trace_commitment, aux_commitment, quotient_commitment)
+        ctl_first = dict(num_ctl_zs_first=(nl + num_ctl_helpers, num_ctl_zs)) if stark.requires_ctls() else {}
+        openings = StarkOpeningSet.new(zeta, g, trace_commitment, aux_commitment, quotient_commitment, **ctl_first)
         for batch in openings.to_fri_openings():                        # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
-        opening_proof = prove_openings(stark.fri_instance(zeta, g, config), commitments, challenger, fri_params,
-                                       final_poly_coeff_len, max_num_query_steps)
+        instance = stark.fri_instance(zeta, g, config, num_ctl_helpers, num_ctl_zs)
+        opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
+                                       params.final_poly_coeff_len, params.max_num_query_steps)
         proof = StarkProof(trace_commitment.merkle_tree.cap,
                            quotient_commitment.merkle_tree.cap if quotient_commitment is not None else None,
                            openings, opening_proof,
