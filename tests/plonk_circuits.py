@@ -483,6 +483,91 @@ class ExtPointVars:
         return ExtPointVars(self.c, self.w, self.pih, self.prefix + n)
 
 
+def openings_at(cd, cs_coeffs, wires_coeffs, zs_coeffs, zeta, zeta_next, ev, pool=None):
+    """The openings vanishing_at reads (OpeningSet::new, plonk/proof.rs:313-351) from the coefficients of the
+    constants / sigmas, wires and Z / partial-products (+ lookup) polynomials: ev(coeffs, point) -> (a, b) evaluates one
+    polynomial at a point of F_{p^2}; `pool` (an Executor) runs the evaluations side by side."""
+    nc, n_zs_pp = cd.config.num_challenges, cd.num_zs_partial_products_polys()
+    jobs = [(p, zeta) for p in list(cs_coeffs) + list(wires_coeffs) + list(zs_coeffs)]
+    jobs += [(p, zeta_next) for p in list(zs_coeffs[:nc]) + list(zs_coeffs[n_zs_pp:])]
+    vals = [Fp2(*v) for v in (pool.map(lambda a: ev(*a), jobs) if pool else [ev(*a) for a in jobs])]
+    ncs, nw, nz = len(cs_coeffs), len(wires_coeffs), len(zs_coeffs)
+    cs, w, z, nxt = vals[:ncs], vals[ncs:ncs + nw], vals[ncs + nw:ncs + nw + nz], vals[ncs + nw + nz:]
+    return dict(constants=cs[:cd.num_constants], plonk_sigmas=cs[cd.num_constants:], wires=w, plonk_zs=z[:nc],
+                partial_products=z[nc:n_zs_pp], lookup_zs=z[n_zs_pp:], plonk_zs_next=nxt[:nc], lookup_zs_next=nxt[nc:])
+
+
+def vanishing_at(plonk, cd, x, o, public_inputs_hash, betas, gammas, alphas, deltas=()):
+    """eval_vanishing_poly (vanishing_poly.rs:57-164) at one point x, an Fp2 (a base-field point has b = 0), from the
+    polynomials' values there: `o` maps constants, plonk_sigmas, wires, plonk_zs, partial_products, lookup_zs (at x) and
+    plonk_zs_next, lookup_zs_next (at g x) to lists of Fp2. Gates: ConstantGate, PublicInputGate and ArithmeticGate are
+    restated here; the others run the product's value-generic gate code over F_{p^2} numbers (the oracle restates every
+    gate independently in C++). The cost does not depend on n. Returns ([vanishing(x) per challenge], Z_H(x), x^n)."""
+    cfg = cd.config
+    nc, n = cfg.num_challenges, 1 << cd.degree_bits
+    constants, sigmas, wires = o["constants"], o["plonk_sigmas"], o["wires"]
+    zs, zs_next, pps = o["plonk_zs"], o["plonk_zs_next"], o["partial_products"]
+    lk, lk_next = o["lookup_zs"], o["lookup_zs_next"]
+    nsel = cd.selectors_info.num_selectors()
+    local = constants[nsel + cd.num_lookup_selectors:]
+    vars_ = ExtPointVars(constants, wires, public_inputs_hash)
+    constraint_terms = [Fp2(0)] * cd.num_gate_constraints                     # evaluate_gate_constraints
+    for i, gate in enumerate(cd.gates):
+        sel = cd.selectors_info.selector_indices[i]
+        s = constants[sel]
+        filt = Fp2(1)
+        for j in list(cd.selectors_info.groups[sel]) + ([plonk.UNUSED_SELECTOR] if nsel > 1 else []):
+            if j != i:
+                filt = filt * (j - s)
+        kind, param = oracle_gate_kind(gate)[:2]
+        if kind == OL.GATE_CONSTANT:
+            res = [local[t] - wires[t] for t in range(param)]
+        elif kind == OL.GATE_PUBLIC_INPUT:
+            res = [wires[t] - public_inputs_hash[t] for t in range(4)]
+        elif kind == OL.GATE_ARITHMETIC:
+            res = [wires[4 * t + 3] - (wires[4 * t] * wires[4 * t + 1] * local[0] + wires[4 * t + 2] * local[1])
+                   for t in range(param)]
+        else:
+            res = gate.eval_unfiltered(vars_.remove_prefix(nsel + cd.num_lookup_selectors))
+        for t, r in enumerate(res):
+            constraint_terms[t] = constraint_terms[t] + Fp2.of(r) * filt
+    xn = x
+    for _ in range(cd.degree_bits):
+        xn = xn * xn
+    z_h = xn - 1
+    l_0_x = z_h * ((x - 1) * n).inverse()                                      # eval_l_0, plonk_common.rs:69-79
+    nr, qdf, nprod = cfg.num_routed_wires, cd.quotient_degree_factor, cd.num_partial_products
+    z1, pp_terms, lookup_terms = [], [], []
+
+    def product(vs):
+        acc = Fp2(1)
+        for v in vs:
+            acc = acc * v
+        return acc
+
+    for i in range(nc):
+        z1.append(l_0_x * (zs[i] - 1))
+        if cd.luts:
+            npoly = cd.num_lookup_polys
+            d = deltas[4 * i:4 * i + 4]
+            lookup_terms += [Fp2.of(v) for v in plonk.check_lookup_constraints(
+                cd, vars_, lk[npoly * i:npoly * (i + 1)], lk_next[npoly * i:npoly * (i + 1)],
+                constants[nsel:nsel + cd.num_lookup_selectors], d, cd.lut_re_poly_evals(d), product)]
+        num = [wires[j] + x * (betas[i] * cd.k_is[j] % P) + gammas[i] for j in range(nr)]
+        den = [wires[j] + sigmas[j] * betas[i] + gammas[i] for j in range(nr)]
+        accs = [zs[i]] + pps[i * nprod:(i + 1) * nprod] + [zs_next[i]]
+        for k in range(nprod + 1):
+            pp_terms.append(accs[k] * product(num[k * qdf:(k + 1) * qdf]) - accs[k + 1] * product(den[k * qdf:(k + 1) * qdf]))
+    terms = z1 + pp_terms + lookup_terms + constraint_terms
+    vanishing = []
+    for i in range(nc):
+        acc = Fp2(0)
+        for t in reversed(terms):                                              # reduce_with_powers_multi
+            acc = acc * alphas[i] + t
+        vanishing.append(acc)
+    return vanishing, z_h, xn
+
+
 def fri_batches(cd, zeta):
     """get_fri_instance (plonk/circuit_data.rs:530-660) as the oracle's (point, [(oracle, polynomial)]) lists."""
     import plonky2_b200.field as F
@@ -573,11 +658,9 @@ def oracle_prove(oracle, c, circuit_digest, fri_cfg, public_inputs, taps=False):
 
 def oracle_verify(oracle, plonk, c, circuit_digest, fri_cfg, parts):
     """verify (plonk/verifier.rs:20-120): get_challenges (plonk/get_challenges.rs:26-90) replayed on a fresh transcript,
-    eval_vanishing_poly at zeta in F_{p^2} (vanishing_poly.rs:57-164; the gates' and the lookup argument's formulas are
-    the product's value-generic ones, here over F_{p^2} numbers), the quotient identity, then verify_fri_proof (the
-    oracle's). Returns None or the reason of the rejection."""
+    eval_vanishing_poly at zeta in F_{p^2} (vanishing_at), the quotient identity, then verify_fri_proof (the oracle's). Returns None or the reason of the rejection."""
     cd, cfg = c.common, c.config
-    nc, n = cfg.num_challenges, c.n
+    nc = cfg.num_challenges
     o = parts["openings"]
     arity_bits = fri_cfg.fri_params(cd.degree_bits, False).reduction_arity_bits
     public_inputs_hash = [int(x) for x in oracle.hash_no_pad(np.array(parts["public_inputs"], dtype=np.uint64))]
@@ -601,58 +684,15 @@ def oracle_verify(oracle, plonk, c, circuit_digest, fri_cfg, parts):
     def E(arr):
         return [Fp2(int(v[0]), int(v[1])) for v in arr]
 
-    x = Fp2(*zeta)
-    constants, sigmas, wires = E(o["constants"]), E(o["plonk_sigmas"]), E(o["wires"])
-    zs, zs_next, pps, quot = E(o["plonk_zs"]), E(o["plonk_zs_next"]), E(o["partial_products"]), E(o["quotient_polys"])
-    lk, lk_next = E(o["lookup_zs"]), E(o["lookup_zs_next"])
-    nsel = cd.selectors_info.num_selectors()
-    vars_ = ExtPointVars(constants, wires, public_inputs_hash)
-    constraint_terms = [Fp2(0)] * cd.num_gate_constraints                     # evaluate_gate_constraints
-    for i, gate in enumerate(cd.gates):
-        sel = cd.selectors_info.selector_indices[i]
-        s = constants[sel]
-        filt = Fp2(1)
-        for j in list(cd.selectors_info.groups[sel]) + ([plonk.UNUSED_SELECTOR] if nsel > 1 else []):
-            if j != i:
-                filt = filt * (j - s)
-        for t, r in enumerate(gate.eval_unfiltered(vars_.remove_prefix(nsel + cd.num_lookup_selectors))):
-            constraint_terms[t] = constraint_terms[t] + Fp2.of(r) * filt
-    xn = x
-    for _ in range(cd.degree_bits):
-        xn = xn * xn
-    z_h_zeta = xn - 1
-    l_0_x = z_h_zeta * ((x - 1) * n).inverse()                                 # eval_l_0, plonk_common.rs:69-79
-    nr, qdf, nprod = cfg.num_routed_wires, cd.quotient_degree_factor, cd.num_partial_products
-    z1, pp_terms, lookup_terms = [], [], []
-
-    def product(vs):
-        acc = Fp2(1)
-        for v in vs:
-            acc = acc * v
-        return acc
-
+    qdf = cd.quotient_degree_factor
+    ev = {k: E(v) for k, v in o.items()}
+    vanishing, z_h_zeta, xn = vanishing_at(plonk, cd, Fp2(*zeta), ev, public_inputs_hash, betas, gammas, alphas, deltas)
+    quot = ev["quotient_polys"]
     for i in range(nc):
-        z1.append(l_0_x * (zs[i] - 1))
-        if cd.luts:
-            npoly = cd.num_lookup_polys
-            d = deltas[4 * i:4 * i + 4]
-            lookup_terms += [Fp2.of(v) for v in plonk.check_lookup_constraints(
-                cd, vars_, lk[npoly * i:npoly * (i + 1)], lk_next[npoly * i:npoly * (i + 1)],
-                constants[nsel:nsel + cd.num_lookup_selectors], d, cd.lut_re_poly_evals(d), product)]
-        num = [wires[j] + x * (betas[i] * cd.k_is[j] % P) + gammas[i] for j in range(nr)]
-        den = [wires[j] + sigmas[j] * betas[i] + gammas[i] for j in range(nr)]
-        accs = [zs[i]] + pps[i * nprod:(i + 1) * nprod] + [zs_next[i]]
-        for k in range(nprod + 1):
-            pp_terms.append(accs[k] * product(num[k * qdf:(k + 1) * qdf]) - accs[k + 1] * product(den[k * qdf:(k + 1) * qdf]))
-    terms = z1 + pp_terms + lookup_terms + constraint_terms
-    for i in range(nc):
-        vanishing = Fp2(0)
-        for t in reversed(terms):                                              # reduce_with_powers_multi
-            vanishing = vanishing * alphas[i] + t
         chunk = Fp2(0)
         for t in reversed(quot[i * qdf:(i + 1) * qdf]):                        # reduce_with_powers(chunk, zeta^n)
             chunk = chunk * xn + t
-        if not vanishing == z_h_zeta * chunk:
+        if not vanishing[i] == z_h_zeta * chunk:
             return "vanishing polynomial identity fails for challenge %d" % i
     batches, num_polys = fri_batches(cd, zeta)
     params = oracle.make_params(cfg.rate_bits, cfg.cap_height, fri_cfg.proof_of_work_bits, fri_cfg.num_query_rounds, arity_bits)

@@ -94,67 +94,11 @@ def _vanishing_at(c, cs, w, z, zeta, betas, gammas, alphas, deltas=()):
     """eval_vanishing_poly (vanishing_poly.rs:29-164) at a base-field point, from the committed polynomials."""
     import plonk_circuits as PC
 
-    cd, cfg = c.common, c.config
-    n = c.n
+    cd = c.common
     g = PC.root_of_unity(cd.degree_bits)
-    consts_sigmas = [_ev(p, zeta) for p in cs.coeffs]
-    wires = [_ev(p, zeta) for p in w.coeffs]
-    zs_pp = [_ev(p, zeta) for p in z.coeffs]
-    zs_pp_next = [_ev(p, zeta * g % P_) for p in z.coeffs]
-    nsel = cd.selectors_info.num_selectors()
-    circuit = c.oracle_circuit()
-    constraint_terms = [0] * cd.num_gate_constraints
-    for i, (kind, param, sel, g0, g1, *_) in enumerate(circuit["gates"]):
-        s = consts_sigmas[sel]
-        filt = 1
-        for j in list(range(g0, g1)) + ([0xFFFFFFFF] if nsel > 1 else []):
-            if j != i:
-                filt = filt * (j - s) % P_
-        k = consts_sigmas[nsel + cd.num_lookup_selectors:]
-        if kind == 1:
-            res = [k[t] - wires[t] for t in range(param)]
-        elif kind == 2:
-            res = [wires[t] - c.public_inputs_hash[t] for t in range(4)]
-        elif kind == 3:
-            res = [wires[4 * t + 3] - (wires[4 * t] * wires[4 * t + 1] * k[0] + wires[4 * t + 2] * k[1]) for t in range(param)]
-        elif kind == 0:
-            res = []
-        else:   # the product's own gate code, over numbers (the oracle restates these gates independently in C++)
-            pv = PC.PointVars(consts_sigmas, wires, c.public_inputs_hash).remove_prefix(nsel + cd.num_lookup_selectors)
-            res = [int(v) for v in cd.gates[i].eval_unfiltered(pv)]
-        for t, r in enumerate(res):
-            constraint_terms[t] = (constraint_terms[t] + r * filt) % P_
-    zh = (pow(zeta, n, P_) - 1) % P_
-    l_0 = zh * pow(n * (zeta - 1) % P_, P_ - 2, P_) % P_     # eval_l_0(n, x), plonk_common.rs:69-79
-    nc, nr, qdf, nprod = cfg.num_challenges, cfg.num_routed_wires, cd.quotient_degree_factor, cd.num_partial_products
-    z1, pp = [], []
-    for i in range(nc):
-        z_x, z_gx = zs_pp[i], zs_pp_next[i]
-        z1.append(l_0 * (z_x - 1) % P_)
-        num = [(wires[j] + betas[i] * (cd.k_is[j] * zeta % P_) + gammas[i]) % P_ for j in range(nr)]
-        den = [(wires[j] + betas[i] * consts_sigmas[cd.num_constants + j] + gammas[i]) % P_ for j in range(nr)]
-        accs = [z_x] + zs_pp[nc + i * nprod: nc + (i + 1) * nprod] + [z_gx]
-        for k in range(nprod + 1):
-            a = b = 1
-            for j in range(k * qdf, min((k + 1) * qdf, nr)):
-                a, b = a * num[j] % P_, b * den[j] % P_
-            pp.append((accs[k] * a - accs[k + 1] * b) % P_)
-    lk = []
-    for i in range(nc if cd.luts else 0):   # the product's check_lookup_constraints over numbers (the oracle restates it in C++)
-        def product(vs):
-            acc = PC.Fp(1)
-            for v in vs:
-                acc = acc * v
-            return acc
-        plonk = _plonk()
-        rng = cd.lookup_range(i)
-        d = deltas[4 * i:4 * i + 4]
-        lk += [int(v) for v in plonk.check_lookup_constraints(
-            cd, PC.PointVars(consts_sigmas, wires, c.public_inputs_hash), [PC.Fp(zs_pp[k]) for k in rng],
-            [PC.Fp(zs_pp_next[k]) for k in rng], [PC.Fp(consts_sigmas[nsel + r]) for r in range(cd.num_lookup_selectors)],
-            d, cd.lut_re_poly_evals(d), product)]
-    terms = z1 + pp + lk + constraint_terms
-    return [sum(pow(al, t, P_) * v for t, v in enumerate(terms)) % P_ for al in alphas], zh
+    o = PC.openings_at(cd, cs.coeffs, w.coeffs, z.coeffs, (zeta, 0), (zeta * g % P_, 0), lambda p, x: (_ev(p, x[0]), 0))
+    want, zh, _ = PC.vanishing_at(_plonk(), cd, PC.Fp2(zeta), o, c.public_inputs_hash, betas, gammas, alphas, deltas)
+    return [int(v) for v in want], int(zh)
 
 
 @pytest.mark.parametrize("shape", SHAPES)
