@@ -956,6 +956,37 @@ void glo_poseidon_naive(uint64_t st[12]) {
     poseidon_naive(st);
     for (int i = 0; i < 12; i++) st[i] = canon(st[i]);
 }
+void glo_poseidon_many(uint64_t* states, size_t n, int nthreads) {
+    parallel_for(n, std::max(1, nthreads), [&](size_t i) { glo_poseidon(states + 12 * i); }, 1024);
+}
+uint64_t glo_pow_min_nonce(const uint64_t state[12], uint32_t pos, uint32_t min_leading_zeros, uint64_t limit,
+                           int nthreads) {
+    // fri_proof_of_work (prover.rs:183-194): the first nonce in increasing order whose permuted lane 7 has enough
+    // leading zeros. Candidates go in blocks of increasing order; inside a block the threads keep the smallest hit.
+    const size_t GRAIN = 4096;
+    const int T = std::max(1, nthreads);
+    const u64 block = (u64)GRAIN * T * 4;
+    for (u64 start = 0; start < limit; start += block) {
+        const u64 count = std::min<u64>(block, limit - start);
+        std::atomic<u64> best{~0ULL};
+        parallel_for(count, T, [&](size_t i) {
+            const u64 cand = start + i;
+            if (cand >= best.load(std::memory_order_relaxed)) return;
+            u64 st[12];
+            memcpy(st, state, sizeof(st));
+            st[pos] = cand;
+            poseidon(st);
+            const u64 resp = canon(st[7]);
+            const uint32_t lz = resp == 0 ? 64 : (uint32_t)__builtin_clzll(resp);
+            if (lz < min_leading_zeros) return;
+            u64 cur = best.load();
+            while (cand < cur && !best.compare_exchange_weak(cur, cand)) {
+            }
+        }, GRAIN);
+        if (best.load() != ~0ULL) return best.load();
+    }
+    return ~0ULL;
+}
 void glo_hash_no_pad(const uint64_t* in, size_t len, uint64_t out[4]) {
     Hash h = hash_no_pad(in, len);
     memcpy(out, h.e, 32);

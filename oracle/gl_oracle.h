@@ -69,6 +69,12 @@ void glo_naive_coset_eval(const uint64_t* coeffs, uint32_t log_n, uint64_t shift
  *      plonk/config.rs:63-74) ---- */
 void glo_poseidon(uint64_t st[12]);        /* fast-partial-rounds form, poseidon.rs:766-777 */
 void glo_poseidon_naive(uint64_t st[12]);  /* textbook form, poseidon.rs:779-801 */
+/* glo_poseidon on n states of 12 words each, in place, split over nthreads */
+void glo_poseidon_many(uint64_t* states, size_t n, int nthreads);
+/* the smallest nonce < limit such that lane 7 of the permuted state (state with lane pos = nonce) has at least
+ * min_leading_zeros leading zeros (fri_proof_of_work, prover.rs:183-194); ~0 if there is none */
+uint64_t glo_pow_min_nonce(const uint64_t state[12], uint32_t pos, uint32_t min_leading_zeros, uint64_t limit,
+                           int nthreads);
 void glo_hash_no_pad(const uint64_t* in, size_t len, uint64_t out[4]);
 void glo_hash_or_noop(const uint64_t* in, size_t len, uint64_t out[4]);
 void glo_two_to_one(const uint64_t l[4], const uint64_t r[4], uint64_t out[4]);

@@ -86,6 +86,9 @@ def lib():
     L.glo_naive_coset_eval.argtypes = [u64p, C.c_uint32, u64, u64p]
     L.glo_poseidon.argtypes = [u64p]
     L.glo_poseidon_naive.argtypes = [u64p]
+    L.glo_poseidon_many.argtypes = [u64p, C.c_size_t, C.c_int]
+    L.glo_pow_min_nonce.restype = u64
+    L.glo_pow_min_nonce.argtypes = [u64p, C.c_uint32, C.c_uint32, u64, C.c_int]
     L.glo_hash_no_pad.argtypes = [u64p, C.c_size_t, u64p]
     L.glo_hash_or_noop.argtypes = [u64p, C.c_size_t, u64p]
     L.glo_two_to_one.argtypes = [u64p, u64p, u64p]
@@ -194,6 +197,24 @@ def poseidon(state, naive=False):
     s = np.array(state, dtype=np.uint64)
     (lib().glo_poseidon_naive if naive else lib().glo_poseidon)(ptr(s))
     return s
+
+
+def poseidon_many(states, nthreads=None):
+    """The permutation of every row of an (n, 12) array -> (n, 12), canonical."""
+    s = np.array(states, dtype=np.uint64).reshape(-1, 12).copy()
+    if len(s):
+        lib().glo_poseidon_many(ptr(s), len(s), nthreads or nproc())
+    return s
+
+
+NO_NONCE = 2**64 - 1
+
+
+def pow_min_nonce(state, pos, min_leading_zeros, limit, nthreads=None):
+    """The smallest nonce < limit whose permuted state (lane pos = nonce) has lane 7 with at least min_leading_zeros
+    leading zeros, or NO_NONCE."""
+    s = np.array(state, dtype=np.uint64).reshape(12)
+    return int(lib().glo_pow_min_nonce(ptr(s), pos, min_leading_zeros, limit, nthreads or nproc()))
 
 
 def hash_no_pad(x):

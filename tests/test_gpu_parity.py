@@ -115,8 +115,9 @@ def test_poseidon_kats_on_device(pb, oracle):
     st = synth(0x4B, (3000, 12), canonical=False)
     st[:len(EDGE)] = np.array([EDGE] * 12, dtype=np.uint64).T[:, :12]
     got = pb.PoseidonHash.permute_many(st)
-    for i in list(range(40)) + list(range(2990, 3000)):
-        assert got[i].tolist() == (oracle.poseidon(st[i]) % np.uint64(P)).tolist(), i
+    want = oracle.poseidon_many(st)
+    bad = np.argwhere(got != want)
+    assert not bad.size, "state %d lane %d" % tuple(bad[0])
     # host transcript permutation = the same function
     h = st[17].copy()
     pb._native.lib().gl_poseidon_permute_host(pb._native.np_ptr(h))

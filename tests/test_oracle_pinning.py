@@ -3,6 +3,7 @@ for the hot path (SURVEY.md section 8c). CPU only.
 
 Reference tests mirrored here:
   * Poseidon KATs + fast==naive      plonky2/src/hash/poseidon_goldilocks.rs:455-495, poseidon.rs:926-957
+    (and the batched permutation and the proof-of-work search the device tests take expected values from)
   * bit-reversal golden table         plonky2/src/util/mod.rs:60-126
   * prime-field edge arithmetic       field/src/prime_field_testing.rs:7-17,69-183
   * fft_and_ifft vs naive evaluation  field/src/fft.rs:215-282
@@ -35,6 +36,42 @@ def test_poseidon_fast_equals_naive(oracle):
     xs = synth(0x77, (200, 12), canonical=False)
     for row in xs:
         assert oracle.poseidon(row).tolist() == oracle.poseidon(row, naive=True).tolist()
+
+
+def test_poseidon_many_equals_one_state_at_a_time(oracle):
+    # the batched permutation the device tests take their expected values from, against the pinned single-state forms
+    kat = json.load(open(os.path.join(GOLD, "poseidon_kat.json")))
+    st = synth(0x78, (4096, 12), canonical=False)
+    st[:4] = np.array([[int(x) for x in v["input"]] for v in kat["vectors"]], dtype=np.uint64)
+    st[4:4 + len(EDGE)] = np.array([EDGE[i:] + EDGE[:i] for i in range(len(EDGE))], dtype=np.uint64)
+    st[100:600] |= np.uint64(0xFFFFFFF0FFFFFFF0)
+    st[600:1100] = np.uint64(2**64 - 1) - (st[600:1100] & np.uint64(0xFF))
+    st[1100:1600, :8] = 0
+    got = oracle.poseidon_many(st, nthreads=3)
+    assert got[:4].tolist() == [[int(x) for x in v["output"]] for v in kat["vectors"]]
+    for i, row in enumerate(st):
+        want = oracle.poseidon(row).tolist()
+        assert got[i].tolist() == want, i
+        assert oracle.poseidon(row, naive=True).tolist() == want, i
+    assert np.array_equal(oracle.poseidon_many(st, nthreads=1), got)
+
+
+def test_pow_min_nonce_is_the_first_qualifying_nonce(oracle):
+    # fri_proof_of_work's rule (prover.rs:183-194), restated as a plain loop over the oracle permutation
+    for bits in range(11):
+        pos = bits % 8
+        st = synth(0x79 + bits, (12,), canonical=False)
+        st[(pos + 3) % 12] = np.uint64(P + bits)  # a word that is not canonical
+        want = 0
+        while True:
+            s = st.copy()
+            s[pos] = want
+            if 64 - int(oracle.poseidon(s)[7]).bit_length() >= bits:
+                break
+            want += 1
+        assert oracle.pow_min_nonce(st, pos, bits, 1 << 20) == want, bits
+        assert oracle.pow_min_nonce(st, pos, bits, want + 1, nthreads=1) == want, bits
+        assert oracle.pow_min_nonce(st, pos, bits, want) == oracle.NO_NONCE, bits
 
 
 def test_bit_reversal_golden_table(oracle):
