@@ -250,6 +250,28 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
 int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
                           const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
                           uint32_t quotient_degree_factor, uint64_t* out_coeffs);
+/* The quotient of a STARK whose commitments are row-block shards (gl_commit_create_sharded / gl_commit_begin with
+ * num_shards = G), in two steps with an all-gather between them. With size = n << log2_ceil(quotient_degree_factor),
+ * shard g owns the points i = r + G*k (k < M = size / G, r = the s-bit reversal of g, G = 2^s) of the quotient coset
+ * g*<w_size>: the numbering of the commitments' own shards.
+ *   gl_stark_quotient_shard        writes shard g's values of C(x)/Z_H(x), n_alphas x M words in local natural order k
+ *                                  (challenge a at out_values + a*M, DEVICE memory). The shard is the handles': `aux`
+ *                                  (NULL: the program may not read auxiliary columns) must be a shard of the same index
+ *                                  and count as `trace`, else GL_ERR_BAD_ARG. Everything else is checked as in
+ *                                  gl_stark_quotient[_aux]. The local values are read in place from the trace's leaves
+ *                                  when the quotient coset is the LDE coset (quotient degree 2^rate_bits), else they are
+ *                                  the LDE of the handle's (replicated) coefficients onto the shard's coset; the next
+ *                                  row comes from the same buffer when G divides 2^log2_ceil(quotient_degree_factor),
+ *                                  else from an LDE onto the coset times w_n.
+ *   gl_stark_quotient_from_shards  takes the G shards' buffers concatenated in shard order (G x n_alphas x M words,
+ *                                  DEVICE memory) and writes gl_stark_quotient's result to out_coeffs (n_alphas x size,
+ *                                  DEVICE memory): the values in natural order, .coset_ifft(g), and the trim_to_len check
+ *                                  ("Quotient has failed", GL_ERR_BAD_ARG). */
+int gl_stark_quotient_shard(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
+                            uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                            uint32_t n_alphas, uint32_t quotient_degree_factor, uint64_t* out_values);
+int gl_stark_quotient_from_shards(gl_ctx* ctx, const uint64_t* values, uint32_t num_shards, uint32_t n_alphas,
+                                  uint32_t degree_bits, uint32_t quotient_degree_factor, uint64_t* out_coeffs);
 
 /* starky's logUp helper columns (lookup_helper_columns, starky/src/lookup.rs:579-652, for every Lookup and every challenge
  * in the reference's order, prover.rs:178-195) on the device. trace: COLUMNS value columns of n = 2^log_n words at

@@ -565,6 +565,24 @@ __global__ void k_canon(u64* data, size_t n) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) data[i] = canon(data[i]);
 }
+// Values of `ncols` polynomials of degree < n = 2^log_n (coefficients, column b at coeffs + b*n) on the coset
+// shift * <w_M>, M = 2^log_M, in leaf order: the point shift * w_M^bitrev(j) at out[j], column b at out + b*out_stride.
+// A coset LDE when M >= n; with fewer points than n the polynomials are restricted to the coset first.
+static int coset_lde_columns(gl_ctx* ctx, const u64* coeffs, uint32_t ncols, uint32_t log_n, uint32_t log_M, u64 shift,
+                             u64* out, size_t out_stride) {
+    const size_t n = (size_t)1 << log_n;
+    if (log_M >= log_n) return lde_columns(ctx, coeffs, n, ncols, (int)log_n, (int)(log_M - log_n), shift, out, out_stride);
+    const size_t M = (size_t)1 << log_M;
+    DevBuf folded(ctx);
+    TRY(folded.alloc((size_t)ncols * M));
+    for (uint32_t b0 = 0; b0 < ncols; b0 += MAX_GRID_Y) {
+        const uint32_t bc = (ncols - b0 < MAX_GRID_Y) ? ncols - b0 : MAX_GRID_Y;
+        k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), bc), 128, 0, ctx->stream>>>(
+            coeffs + (size_t)b0 * n, n, n, M, gl::pow(shift, M), folded.get() + (size_t)b0 * M);
+        CKL(ctx);
+    }
+    return lde_columns(ctx, folded.get(), M, ncols, (int)log_M, 0, shift, out, out_stride);
+}
 
 // Allocate the device state of a commitment: coefficients (or adopt the caller's matrix) and the column-major LDE.
 static int commit_alloc(gl_ctx* ctx, gl_commit* c, uint32_t cap_height, u64* ext_coeffs) {
@@ -609,24 +627,8 @@ static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int
         CKL(ctx);
     }
     PhaseScope ps(ctx, GL_PHASE_LDE);
-    if (sl <= c->rate_bits) {
-        const uint32_t rloc = c->rate_bits - sl;
-        TRY(lde_columns(ctx, cg, n, gc, (int)c->degree_log, (int)rloc, c->sg, t.leaves + (size_t)g0 * Nloc, Nloc));
-    } else {
-        // fewer than n points per shard: restrict the polynomials to the sub-coset first
-        const uint32_t logM = c->degree_log + c->rate_bits - sl;
-        const size_t M = (size_t)1 << logM;
-        DevBuf folded(ctx);
-        TRY(folded.alloc((size_t)gc * M));
-        for (uint32_t b0 = 0; b0 < gc; b0 += MAX_GRID_Y) {
-            const uint32_t bc = (gc - b0 < MAX_GRID_Y) ? gc - b0 : MAX_GRID_Y;
-            k_fold_coeffs<<<dim3((unsigned)((M + 127) / 128), bc), 128, 0, ctx->stream>>>(
-                cg + (size_t)b0 * n, n, n, M, gl::pow(c->sg, M), folded.get() + (size_t)b0 * M);
-            CKL(ctx);
-        }
-        TRY(lde_columns(ctx, folded.get(), M, gc, (int)logM, 0, c->sg, t.leaves + (size_t)g0 * Nloc, Nloc));
-    }
-    return GL_OK;
+    return coset_lde_columns(ctx, cg, gc, c->degree_log, c->degree_log + c->rate_bits - sl, c->sg,
+                             t.leaves + (size_t)g0 * Nloc, Nloc);
 }
 // salt columns (blinding) + "build Merkle tree"
 static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem) {
@@ -1244,15 +1246,22 @@ __global__ void __launch_bounds__(1024) k_affine_scan(const u64* b, size_t len, 
 
 // ---- STARK quotient evaluation (compute_quotient_polys, starky/src/prover.rs:488-668; SURVEY 8(f) row 1) ----
 // The constraints (Stark::eval_packed_generic, starky/src/stark.rs) arrive as a small straight-line program over the
-// local row, the next row and the public inputs; value k = result of instruction k. One thread per point of the
-// quotient coset g*<w_size>, size = n << quotient_degree_bits, reading the trace LDE in place (column-major leaves):
-//   local = leaf bitrev(i*step), next = leaf bitrev(((i + next_step) % size) * step)      (get_lde_values, oracle.rs:142-147)
+// local row, the next row and the public inputs; value k = result of instruction k. One thread per point of one shard of
+// the quotient coset g*<w_size>, size = n << quotient_degree_bits: shard s of G = 2^shard_log owns the points
+// i = r + G*k, r = bitrev(s), k < M = size / G, i.e. the coset g*w_size^r*<w_M> (the whole coset when G = 1). The
+// polynomials' values on it come in two buffers of column-major leaves (get_lde_values, oracle.rs:142-147):
+//   local = loc[leaf bitrev_M(k)],  next (the point times w_n) = nxt[leaf bitrev_M((k + next_off) mod M)]
+// The whole trace LDE's first `size` leaves are the quotient coset in leaf order, so one device reads both in place
+// (next_off = 2^qd_bits); a shard reads its commitment's leaves, or values computed on its coset.
 struct StarkQuotientParams {
-    const u64* lde;        // trace LDE, column k at lde + k*lde_stride, leaf order
-    size_t lde_stride;
-    const u64* aux;        // auxiliary LDE (logUp helper columns; NULL without), same layout and leaves
-    size_t aux_stride;
-    uint32_t log_N;        // log2 of the LDE size
+    const u64 *loc, *nxt;          // trace values, column k at + k*stride, leaf order
+    size_t loc_stride, nxt_stride;
+    const u64 *aux_loc, *aux_nxt;  // auxiliary values (logUp helper columns; NULL without), same layout and leaves
+    size_t aux_loc_stride, aux_nxt_stride;
+    uint32_t log_M;        // log2 of the points of this shard
+    uint32_t shard_log;    // G = 2^shard_log
+    size_t r;              // this shard's first global point
+    size_t next_off;       // local offset of the next row in the next buffer
     uint32_t degree_bits, qd_bits;
     const gl_stark_instr* prog;
     uint32_t n_instr;
@@ -1264,17 +1273,17 @@ struct StarkQuotientParams {
     u64 last;              // w_n^-1, the last element of the trace subgroup
     u64 n_field;           // n as a field element
     u64 zh[GL_STARK_MAX_QD], zh_inv[GL_STARK_MAX_QD];  // Z_H on the coset: g^n * w_{2^qd}^j - 1 and inverses (ZeroPolyOnCoset)
-    u64* out;              // n_alphas columns of `size` values
+    u64* out;              // n_alphas columns of M values, local natural order k
     unsigned int* flag;
 };
 __global__ void __launch_bounds__(128) k_stark_quotient(StarkQuotientParams p) {
-    const size_t size = (size_t)1 << (p.degree_bits + p.qd_bits);
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= size) return;
-    const uint32_t step_log = p.log_N - p.degree_bits - p.qd_bits;   // step = 2^(rate_bits - qd_bits)
-    const size_t inext = (i + ((size_t)1 << p.qd_bits)) & (size - 1);
-    const size_t jl = (size_t)(__brevll((unsigned long long)(i << step_log)) >> (64 - p.log_N));
-    const size_t jn = (size_t)(__brevll((unsigned long long)(inext << step_log)) >> (64 - p.log_N));
+    const size_t M = (size_t)1 << p.log_M;
+    const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= M) return;
+    const size_t i = p.r + (k << p.shard_log);   // the global point: x, Z_H and the Lagrange selectors
+    const size_t kn = (k + p.next_off) & (M - 1);
+    const size_t jl = p.log_M ? (size_t)(__brevll((unsigned long long)k) >> (64 - p.log_M)) : 0;
+    const size_t jn = p.log_M ? (size_t)(__brevll((unsigned long long)kn) >> (64 - p.log_M)) : 0;
     const u64 x = mul(p.shift, mul(p.xhi[i >> 12], p.xlo[i & 4095]));
     const u64 z_last = sub(x, p.last);
     const u64 zh = p.zh[i & (((size_t)1 << p.qd_bits) - 1)];
@@ -1294,10 +1303,10 @@ __global__ void __launch_bounds__(128) k_stark_quotient(StarkQuotientParams p) {
         const gl_stark_instr in = p.prog[k];
         u64 r = 0;
         switch (in.op) {
-            case GL_STARK_LOCAL: r = p.lde[(size_t)in.a * p.lde_stride + jl]; break;
-            case GL_STARK_NEXT: r = p.lde[(size_t)in.a * p.lde_stride + jn]; break;
-            case GL_STARK_AUX_LOCAL: r = p.aux[(size_t)in.a * p.aux_stride + jl]; break;
-            case GL_STARK_AUX_NEXT: r = p.aux[(size_t)in.a * p.aux_stride + jn]; break;
+            case GL_STARK_LOCAL: r = p.loc[(size_t)in.a * p.loc_stride + jl]; break;
+            case GL_STARK_NEXT: r = p.nxt[(size_t)in.a * p.nxt_stride + jn]; break;
+            case GL_STARK_AUX_LOCAL: r = p.aux_loc[(size_t)in.a * p.aux_loc_stride + jl]; break;
+            case GL_STARK_AUX_NEXT: r = p.aux_nxt[(size_t)in.a * p.aux_nxt_stride + jn]; break;
             case GL_STARK_CONST: r = p.consts[in.a]; break;
             case GL_STARK_ADD: r = add(v[in.a], v[in.b]); break;
             case GL_STARK_SUB: r = sub(v[in.a], v[in.b]); break;
@@ -1313,7 +1322,16 @@ __global__ void __launch_bounds__(128) k_stark_quotient(StarkQuotientParams p) {
         v[k] = r;
     }
     const u64 zi = p.zh_inv[i & (((size_t)1 << p.qd_bits) - 1)];
-    for (uint32_t a = 0; a < p.n_alphas; a++) p.out[(size_t)a * size + i] = canon(mul(acc[a], zi));
+    for (uint32_t a = 0; a < p.n_alphas; a++) p.out[(size_t)a * M + k] = canon(mul(acc[a], zi));
+}
+// the all-gathered shard-major buffer (shard s, challenge a, local point k) -> out[a][bitrev(s) + G*k]
+__global__ void k_stark_unshard(const u64* values, uint32_t log_M, uint32_t shard_log, u64* out) {
+    const size_t M = (size_t)1 << log_M;
+    const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= M) return;
+    const uint32_t s = blockIdx.y, a = blockIdx.z, n_alphas = gridDim.z;
+    const size_t r = bitrev32(s, shard_log);
+    out[((size_t)a << (log_M + shard_log)) + r + (k << shard_log)] = values[((size_t)s * n_alphas + a) * M + k];
 }
 // ---- starky's logUp helper columns (lookup_helper_columns, starky/src/lookup.rs:579-652): one thread per row of one
 // Lookup, every challenge; the row's arithmetic is gl_logup.cuh. Z is the additive mscan of the `term` sequences.
@@ -2012,29 +2030,41 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
     return GL_OK;
 }
 
-// gl_stark_quotient and gl_stark_quotient_aux (aux = NULL: the program may not read auxiliary columns)
-static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
-                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
-                          uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
-    if (!ctx || !trace || !program || !alphas || !out_coeffs) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+// log2_ceil(quotient_degree_factor)
+static uint32_t quotient_degree_bits(uint32_t quotient_degree_factor) {
+    uint32_t qd_bits = 0;
+    while (((size_t)1 << qd_bits) < quotient_degree_factor) qd_bits++;
+    return qd_bits;
+}
+// The checks of gl_stark_quotient[_aux] (whole = true: both LDEs whole on this device) and gl_stark_quotient_shard
+// (whole = false: the trace and the auxiliary commitment are shards of the same index and count). Sets *qd_bits.
+static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
+                                uint32_t n_instr, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                                uint32_t quotient_degree_factor, const uint64_t* out, bool whole, uint32_t* qd_bits_out) {
+    if (!ctx || !trace || !program || !alphas || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     if (n_instr == 0 || n_instr > GL_STARK_MAX_INSTR) return set_err(ctx, GL_ERR_UNSUPPORTED, "program of %u instructions (max %d)", n_instr, GL_STARK_MAX_INSTR);
     if (n_alphas == 0 || n_alphas > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
     if (quotient_degree_factor == 0) return set_err(ctx, GL_ERR_BAD_ARG, "quotient_degree_factor is 0: the STARK has no quotient");
-    if (trace->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
+    if (whole && trace->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
     // unfinished handles: the error goes to `ctx`, the context the caller reads it from
     if (!trace->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the trace commitment");
     if (aux) {
         if (aux->ctx->device != ctx->device) return set_err(ctx, GL_ERR_BAD_ARG, "the auxiliary commitment is on another device");
-        if (aux->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole auxiliary LDE on this device");
+        if (whole && aux->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole auxiliary LDE on this device");
+        if (!whole && (aux->shard_index != trace->shard_index || aux->shard_log != trace->shard_log))
+            return set_err(ctx, GL_ERR_BAD_ARG, "the auxiliary commitment is shard %u of %u, the trace shard %u of %u",
+                           aux->shard_index, 1u << aux->shard_log, trace->shard_index, 1u << trace->shard_log);
         if (aux->degree_log != trace->degree_log || aux->rate_bits != trace->rate_bits)
             return set_err(ctx, GL_ERR_BAD_SHAPE, "the auxiliary commitment's degree or rate differs from the trace's");
         if (!aux->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the auxiliary commitment");
     }
-    uint32_t qd_bits = 0;
-    while ((1u << qd_bits) < quotient_degree_factor) qd_bits++;  // log2_ceil
+    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
     if (qd_bits > trace->rate_bits)
         return set_err(ctx, GL_ERR_UNSUPPORTED, "Having constraints of degree higher than the rate is not supported yet.");
     if ((1u << qd_bits) > GL_STARK_MAX_QD) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
+    if (trace->shard_log > trace->degree_log + qd_bits)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", 1u << trace->shard_log,
+                       trace->degree_log + qd_bits);
     for (uint32_t k = 0; k < n_instr; k++) {  // validate once on the host: the kernel trusts the program
         const gl_stark_instr in = program[k];
         bool ok = true;
@@ -2048,19 +2078,61 @@ static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
         }
         if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "constraint program: bad instruction %u", k);
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    const uint32_t db = trace->degree_log, size_log = db + qd_bits;
-    const size_t size = (size_t)1 << size_log;
-    DevBuf dprog(ctx), dconst(ctx), dflag(ctx), xtab(ctx);
+    *qd_bits_out = qd_bits;
+    return GL_OK;
+}
+// C(x)/Z_H(x) on the trace handle's shard of the quotient coset (the whole coset for an unsharded handle): M values per
+// challenge in local natural order, at out + a*M. Division by zero sets bit 1 of dflag.
+static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
+                                 uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                                 uint32_t n_alphas, uint32_t qd_bits, uint64_t* out, const DevBuf& dflag) {
+    const uint32_t db = trace->degree_log, size_log = db + qd_bits, sl = trace->shard_log, log_M = size_log - sl;
+    const size_t size = (size_t)1 << size_log, M = (size_t)1 << log_M;
+    const size_t r = bitrev32(trace->shard_index, sl);
+    const u64 w_size = root_of_unity(size_log);
+    const u64 shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(w_size, r));  // this shard's coset g*w_size^r*<w_M>
+    // The local values: in place when the shard's coset is its commitment's -- always on one device (the LDE's first
+    // `size` leaves), and on every shard when the quotient coset is the LDE coset. Else the LDE onto the coset.
+    const bool local_in_place = sl == 0 || qd_bits == trace->rate_bits;
+    // The next row, point i + 2^qd_bits, lies in the same shard when G divides 2^qd_bits: local point k + 2^qd_bits / G.
+    // Else the values on the coset times w_n.
+    const bool next_in_local = sl <= qd_bits;
+    DevBuf dprog(ctx), dconst(ctx), xtab(ctx), tl(ctx), tn(ctx), al(ctx), an(ctx);
+    struct View {
+        const u64* p;
+        size_t stride;
+    };
+    auto values_on = [&](gl_commit* c, u64 s, DevBuf& buf, View* v) -> int {
+        TRY(buf.alloc((size_t)c->B * M));
+        TRY(coset_lde_columns(ctx, c->coeffs, c->B, c->degree_log, log_M, s, buf.get(), M));
+        *v = {buf.get(), M};
+        return GL_OK;
+    };
+    auto views = [&](gl_commit* c, DevBuf& lbuf, DevBuf& nbuf, View* vl, View* vn) -> int {
+        if (local_in_place) *vl = {c->tree.leaves, c->tree.es};
+        else TRY(values_on(c, shift, lbuf, vl));
+        if (next_in_local) *vn = *vl;
+        else TRY(values_on(c, mul(shift, root_of_unity(db)), nbuf, vn));
+        return GL_OK;
+    };
+    View trl, trn, axl = {nullptr, 0}, axn = {nullptr, 0};
+    TRY(views(trace, tl, tn, &trl, &trn));
+    if (aux) TRY(views(aux, al, an, &axl, &axn));
     TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_stark_instr), consts, n_consts, dprog, dconst));
-    TRY(flag_alloc(ctx, dflag));
-    TRY(x_pow_tables(ctx, root_of_unity(size_log), size, xtab));
+    TRY(x_pow_tables(ctx, w_size, size, xtab));
     StarkQuotientParams p;
-    p.lde = trace->tree.leaves;
-    p.lde_stride = trace->tree.es;
-    p.aux = aux ? aux->tree.leaves : nullptr;
-    p.aux_stride = aux ? aux->tree.es : 0;
-    p.log_N = db + trace->rate_bits;
+    p.loc = trl.p;
+    p.loc_stride = trl.stride;
+    p.nxt = trn.p;
+    p.nxt_stride = trn.stride;
+    p.aux_loc = axl.p;
+    p.aux_loc_stride = axl.stride;
+    p.aux_nxt = axn.p;
+    p.aux_nxt_stride = axn.stride;
+    p.log_M = log_M;
+    p.shard_log = sl;
+    p.r = r;
+    p.next_off = next_in_local ? ((size_t)1 << (qd_bits - sl)) : 0;
     p.degree_bits = db;
     p.qd_bits = qd_bits;
     p.prog = (const gl_stark_instr*)dprog.get();
@@ -2074,20 +2146,41 @@ static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
     p.last = gl::inv(root_of_unity(db));
     p.n_field = canon((u64)1 << db);
     zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
-    p.out = out_coeffs;
+    p.out = out;
     p.flag = (unsigned int*)dflag.get();
-    k_stark_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    k_stark_quotient<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p);
     CKL(ctx);
+    return GL_OK;
+}
+// The quotient's coefficients from its values on the whole coset, in place, then the flags of both steps
+static int stark_quotient_coeffs(gl_ctx* ctx, uint64_t* coeffs, uint32_t degree_bits, uint32_t n_alphas,
+                                 uint32_t quotient_degree_factor, const DevBuf& dflag) {
+    const uint32_t size_log = degree_bits + quotient_degree_bits(quotient_degree_factor);
+    const size_t size = (size_t)1 << size_log;
     // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:661-667)
-    TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
+    TRY(ntt_natural(ctx, coeffs, size, coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
     // trim_to_len(degree * quotient_degree_factor) (prover.rs:396-401): the rest must vanish
-    const size_t keep = ((size_t)quotient_degree_factor) << db;
+    const size_t keep = ((size_t)quotient_degree_factor) << degree_bits;
     if (keep < size) {
-        k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
+        k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(coeffs, size, keep,
                                                                                                size - keep, (unsigned int*)dflag.get());
         CKL(ctx);
     }
     return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
+}
+// gl_stark_quotient and gl_stark_quotient_aux (aux = NULL: the program may not read auxiliary columns)
+static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                          uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+    uint32_t qd_bits = 0;
+    TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor,
+                             out_coeffs, true, &qd_bits));
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf dflag(ctx);
+    TRY(flag_alloc(ctx, dflag));
+    TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out_coeffs,
+                              dflag));
+    return stark_quotient_coeffs(ctx, out_coeffs, trace->degree_log, n_alphas, quotient_degree_factor, dflag);
 }
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
                       const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
@@ -2101,6 +2194,41 @@ int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
     if (!aux) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     return stark_quotient(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, quotient_degree_factor,
                           out_coeffs);
+}
+int gl_stark_quotient_shard(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
+                            uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                            uint32_t n_alphas, uint32_t quotient_degree_factor, uint64_t* out_values) {
+    uint32_t qd_bits = 0;
+    TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor,
+                             out_values, false, &qd_bits));
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf dflag(ctx);
+    TRY(flag_alloc(ctx, dflag));
+    TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out_values,
+                              dflag));
+    return flag_status(ctx, dflag, {INVERT_ZERO});
+}
+int gl_stark_quotient_from_shards(gl_ctx* ctx, const uint64_t* values, uint32_t num_shards, uint32_t n_alphas,
+                                  uint32_t degree_bits, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+    if (!ctx || !values || !out_coeffs) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (n_alphas == 0 || n_alphas > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
+    if (quotient_degree_factor == 0) return set_err(ctx, GL_ERR_BAD_ARG, "quotient_degree_factor is 0: the STARK has no quotient");
+    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
+    if ((1u << qd_bits) > GL_STARK_MAX_QD) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
+    uint32_t sl = 0;
+    if (log2_exact(num_shards, &sl)) return set_err(ctx, GL_ERR_BAD_ARG, "num_shards = %u is not a power of two", num_shards);
+    if (degree_bits > 32) return set_err(ctx, GL_ERR_BAD_SHAPE, "degree_bits = %u", degree_bits);
+    const uint32_t size_log = degree_bits + qd_bits;
+    if (sl > size_log || num_shards > MAX_GRID_Y)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", num_shards, size_log);
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf dflag(ctx);
+    TRY(flag_alloc(ctx, dflag));
+    const uint32_t log_M = size_log - sl;
+    k_stark_unshard<<<dim3((unsigned)((((size_t)1 << log_M) + 127) / 128), num_shards, n_alphas), 128, 0, ctx->stream>>>(
+        values, log_M, sl, out_coeffs);
+    CKL(ctx);
+    return stark_quotient_coeffs(ctx, out_coeffs, degree_bits, n_alphas, quotient_degree_factor, dflag);
 }
 
 int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,

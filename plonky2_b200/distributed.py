@@ -4,7 +4,11 @@ Merkle-cap entries (2^cap_height x 32 bytes in total) -- and PipelinedCommitter 
 (column-sharded iNTT whose stores are the coefficient all-gather over NVLink).
 
 No LDE data ever crosses NVLink: shard g of G evaluates every column on its own coset
-(g_shift * w_N^{bitrev(g)}) <w_{N/G}>, hashes its leaves and reduces its own cap subtrees."""
+(g_shift * w_N^{bitrev(g)}) <w_{N/G}>, hashes its leaves and reduces its own cap subtrees.
+
+prove_stark proves one STARK on the ranks of a group with these shards: besides the caps, only the quotient's values on
+each rank's shard of the quotient coset (quotient_polys_sharded) and the FRI query openings (prove_openings_sharded)
+cross ranks."""
 import numpy as np
 
 from .hash import MerkleCap
@@ -83,18 +87,21 @@ def open_sharded(batch, leaf_indices, group=None):
     return leaves, paths
 
 
-def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None):
+def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None, final_poly_coeff_len=None,
+                           max_num_query_steps=None):
     """prove_openings (oracle.rs:176-237) when the initial oracles are row-block sharded over the ranks.
     Coefficients are replicated (every rank ran the iNTT), so every rank runs the (small, single-column) FRI
     commit phase and the transcript redundantly and deterministically; only the initial-tree openings cross
     ranks. The returned FriProof is identical on every rank and byte-identical to the single-device proof.
-    The caller must already have observed the FULL caps (gather_cap) in `challenger`."""
+    The caller must already have observed the FULL caps (gather_cap) in `challenger`. final_poly_coeff_len /
+    max_num_query_steps: as in fri.prove_openings (a verifier circuit's shape)."""
     from . import fri as F
 
     alpha = challenger.get_extension_challenge()
     state = F._begin(instance, oracles, alpha, fri_params)
     try:
-        caps, final_coeffs = F.fri_committed_trees(state, challenger, fri_params)
+        caps, final_coeffs = F.fri_committed_trees(state, challenger, fri_params, final_poly_coeff_len,
+                                                   max_num_query_steps)
         pow_witness = F.fri_proof_of_work(challenger, fri_params.config, state.ctx)
         n = fri_params.lde_size()
 
@@ -110,6 +117,101 @@ def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None
         return F.FriProof(caps, rounds, final_coeffs, pow_witness)
     finally:
         state.close()
+
+
+def all_gather_tensor(t, group=None):
+    """The ranks' tensors `t` (same shape on every rank) stacked in rank order: (world, *t.shape) on t's device, ready
+    for the library's stream. Under NCCL the exchange stays on the device; other backends go through the host."""
+    import torch
+    import torch.distributed as dist
+
+    world = dist.get_world_size(group)
+    src = (t.contiguous() if dist.get_backend(group) == "nccl" else t.cpu()).reshape(-1)
+    out = torch.empty(world * src.numel(), dtype=t.dtype, device=src.device)
+    dist.all_gather_into_tensor(out, src, group=group)
+    out = out.to(t.device).view((world,) + tuple(t.shape))
+    if out.is_cuda:
+        torch.cuda.synchronize(out.device)
+    return out
+
+
+def quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, group=None, auxiliary_polys_commitment=None,
+                           lookup_challenges=None, ctl_vars=None):
+    """stark.compute_quotient_polys when the trace (and auxiliary) commitments are this rank's row-block shard: each rank
+    evaluates C(x)/Z_H(x) on its shard of the quotient coset (gl_stark_quotient_shard), the ranks all-gather the values,
+    and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same torch
+    tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
+    import torch
+
+    from . import _native as N
+    from .stark import quotient_program
+
+    qdf = stark.quotient_degree_factor()
+    if qdf == 0:
+        return None
+    b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
+                                     ctl_vars)
+    ctx, G = trace_commitment.ctx, trace_commitment.num_shards
+    size = (1 << trace_commitment.degree_log) << (qdf - 1).bit_length()
+    dev = "cuda:%d" % ctx.device
+    local = torch.empty((len(al), size // G), dtype=torch.int64, device=dev)
+    aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
+    failure = None
+    try:
+        N.check(N.lib().gl_stark_quotient_shard(ctx.h, trace_commitment.h, aux_h, b.program(), len(b.instrs),
+                                                N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
+                                                N.vp(local.data_ptr())), ctx.h)
+    except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
+        failure = e
+    failed = all_gather_tensor(torch.tensor([int(failure is not None)], dtype=torch.int64, device=dev), group)
+    if failure is not None:
+        raise failure
+    if int(failed.sum()):
+        raise N.NativeError("the quotient failed on rank %d" % int(torch.nonzero(failed.view(-1))[0]))
+    values = all_gather_tensor(local, group)
+    out = torch.empty((len(al), size), dtype=torch.int64, device=dev)
+    N.check(N.lib().gl_stark_quotient_from_shards(ctx.h, N.vp(values.data_ptr()), G, len(al),
+                                                  trace_commitment.degree_log, qdf, N.vp(out.data_ptr())), ctx.h)
+    ctx.synchronize()
+    return out
+
+
+def check_prove_stark(stark, config, world):
+    """prove_stark's refusals, raised identically on every rank before any device work or collective."""
+    from . import _native as N
+
+    if world < 1 or world & (world - 1):
+        raise N.ShapeError("prove_stark needs a power-of-two number of ranks, got %d" % world)
+    if world > 1 << config.fri_config.cap_height:
+        raise N.ShapeError("%d ranks exceed the %d cap entries of a commitment (cap_height %d)"
+                           % (world, 1 << config.fri_config.cap_height, config.fri_config.cap_height))
+    if stark.requires_ctls():
+        raise N.ShapeError("prove_stark proves one STARK without cross-table lookups; see "
+                           "cross_table_lookup.prove_with_ctls")
+
+
+def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circuit_fri_params=None, ctx=None):
+    """stark.prove on the ranks of a torch.distributed group (the default group if None): rank g commits row block g
+    of the trace, auxiliary and quotient LDEs, evaluates the quotient on its shard of the quotient coset and answers the
+    FRI queries that land in its rows; the coefficients, openings and transcript are computed on every rank.
+    Collective: every rank passes the same full trace (host columns or a torch CUDA tensor) and returns the same
+    StarkProofWithPublicInputs, equal to what stark.prove returns on one device. The world size must be a power of two
+    of at most 2^cap_height, and the Stark must not take part in cross-table lookups (ShapeError otherwise, on every
+    rank). Without an initialised process group, or with one rank, this is stark.prove. ctx: this rank's context
+    (default: the current CUDA device's)."""
+    import torch.distributed as dist
+
+    from . import _native as N
+    from . import stark as S
+
+    world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    check_prove_stark(stark, config, world)
+    if ctx is None:
+        import torch
+
+        ctx = N.default_context(torch.cuda.current_device())
+    placement = ((dist.get_rank(group), world), group) if world > 1 else None
+    return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement)
 
 
 def chunk_layout(num_polys, world, chunk_cols=64):

@@ -152,8 +152,9 @@ class PolynomialBatch(N.Handle):
                      salt_key=None, shard=(0, 1)):
         """A batch committed incrementally: gl_commit_begin, then add_columns(h) issues the gl_commit_add_columns calls
         on the unfinished handle h, then gl_commit_finish -- or, with blinding, gl_commit_finish_keyed: the salt is
-        drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). The columns' device
-        memory only has to live until this returns."""
+        drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). shard=(g, G): only
+        leaf rows [g*N/G, (g+1)*N/G) on this device, as in from_values. The columns' device memory only has to live
+        until this returns."""
         if salt_key is not None and not blinding:
             raise N.ShapeError("salt_key= needs blinding=True")
         key = _salt_key(salt_key) if salt_key is not None else None
@@ -175,10 +176,10 @@ class PolynomialBatch(N.Handle):
 
     @classmethod
     def _from_coeff_chunks(cls, polys, chunks, degree_log, rate_bits, cap_height, ctx=None, *, blinding=False,
-                           salt_key=None):
+                           salt_key=None, shard=(0, 1)):
         """Every row of the device tensor `polys` cut into `chunks` coefficient polynomials of 2^degree_log, committed
         in row order: the quotient commitment of plonky2 and starky (plonk/prover.rs:319-352, starky/prover.rs:391-421).
-        blinding / salt_key: as in _from_device."""
+        blinding / salt_key / shard: as in _from_device."""
         ctx = ctx or N.default_context()
         n = 1 << degree_log
 
@@ -188,7 +189,7 @@ class PolynomialBatch(N.Handle):
                                                       N.COLS_COEFFS, N.MEM_DEVICE), ctx.h)
 
         return cls._from_device(ctx, polys.shape[0] * chunks, degree_log, rate_bits, cap_height, add_columns,
-                                blinding=blinding, salt_key=salt_key)
+                                blinding=blinding, salt_key=salt_key, shard=shard)
 
     @classmethod
     def from_values(cls, values, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,

@@ -7,7 +7,8 @@ auxiliary LDEs in place on the device, and eval_vanishing_poly evaluates the sam
 on the host (the constraint-binding step of the prover, and any verifier). `prove` (one STARK) and
 cross_table_lookup.prove_with_ctls (several) both run prove_with_commitment, which strings the device steps together in
 the reference's order with the transcript on the host; the lookup helper columns are written on the device by
-gl_stark_lookup_helpers, the CTL helper and Z columns by gl_stark_ctl_helpers."""
+gl_stark_lookup_helpers, the CTL helper and Z columns by gl_stark_ctl_helpers. distributed.prove_stark runs the same
+prove_with_commitment on row-block shards over several GPUs (its `placement`)."""
 import ctypes as C
 
 import numpy as np
@@ -263,17 +264,8 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
     qdf = stark.quotient_degree_factor()
     if qdf == 0:
         return None
-    if stark.uses_lookups() and (auxiliary_polys_commitment is None or lookup_challenges is None):
-        raise N.ShapeError("a Stark with lookups needs the auxiliary commitment and the lookup challenges")
-    if ctl_vars is not None and auxiliary_polys_commitment is None:
-        raise N.ShapeError("a Stark with CTLs needs the auxiliary commitment")
-    challenges = [int(c) % F.ORDER for c in lookup_challenges] if stark.uses_lookups() else []
-    b = stark.constraint_program(len(challenges), ctl_vars)
-    consts = np.array([int(x) % F.ORDER for x in public_inputs] + challenges + _ctl_bound(ctl_vars) + b.consts[b.num_bound:],
-                      dtype=np.uint64)
-    if len(public_inputs) != stark.PUBLIC_INPUTS:
-        raise N.ShapeError("expected %d public inputs" % stark.PUBLIC_INPUTS)
-    al = np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
+    b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
+                                     ctl_vars)
     qd_bits = (qdf - 1).bit_length()
     size = (1 << trace_commitment.degree_log) << qd_bits
     ctx = trace_commitment.ctx
@@ -288,6 +280,24 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
                                           N.np_ptr(al), len(al), qdf, N.vp(out.data_ptr())), ctx.h)
     ctx.synchronize()
     return out
+
+
+def quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment=None, lookup_challenges=None,
+                     ctl_vars=None):
+    """What gl_stark_quotient[_aux] and gl_stark_quotient_shard take besides the commitments: the constraint program
+    (ConstraintBuilder), its constants (public inputs, lookup challenges, CTL challenges, then the program's own) and
+    the alphas, as uint64 arrays. Raises ShapeError for missing auxiliary inputs or a wrong number of public inputs."""
+    if stark.uses_lookups() and (auxiliary_polys_commitment is None or lookup_challenges is None):
+        raise N.ShapeError("a Stark with lookups needs the auxiliary commitment and the lookup challenges")
+    if ctl_vars is not None and auxiliary_polys_commitment is None:
+        raise N.ShapeError("a Stark with CTLs needs the auxiliary commitment")
+    challenges = [int(c) % F.ORDER for c in lookup_challenges] if stark.uses_lookups() else []
+    b = stark.constraint_program(len(challenges), ctl_vars)
+    consts = np.array([int(x) % F.ORDER for x in public_inputs] + challenges + _ctl_bound(ctl_vars) + b.consts[b.num_bound:],
+                      dtype=np.uint64)
+    if len(public_inputs) != stark.PUBLIC_INPUTS:
+        raise N.ShapeError("expected %d public inputs" % stark.PUBLIC_INPUTS)
+    return b, consts, np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
 
 
 def _ctl_bound(ctl_vars):
@@ -328,24 +338,25 @@ def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx, out=None
     return out
 
 
-def commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx):
+def commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx, **on):
     """The auxiliary commitment (prover.rs:216-230): PolynomialBatch::from_values of the helper columns, never blinded,
-    committed straight from the device tensor compute_lookup_helper_columns returned."""
+    committed straight from the device tensor compute_lookup_helper_columns returned. on: shard=(g, G) commits row
+    block g of G only."""
     B, n = helper_columns.shape
 
     def add_columns(h):
         N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(helper_columns.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE),
                 ctx.h)
 
-    return PolynomialBatch._from_device(ctx, B, F.log2_strict(n), rate_bits, cap_height, add_columns)
+    return PolynomialBatch._from_device(ctx, B, F.log2_strict(n), rate_bits, cap_height, add_columns, **on)
 
 
-def commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx=None):
+def commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx=None, **on):
     """'split quotient polys' + 'compute quotient commitment' (prover.rs:391-421): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients, all chunks are committed with from_coeffs -- straight from the
-    device tensor compute_quotient_polys returned."""
+    device tensor compute_quotient_polys returned. on: shard=(g, G) commits row block g of G only."""
     return PolynomialBatch._from_coeff_chunks(quotient_polys, stark.quotient_degree_factor(), degree_bits, rate_bits,
-                                              cap_height, ctx)
+                                              cap_height, ctx, **on)
 
 
 class StarkConfig:
@@ -573,9 +584,9 @@ class StarkProofWithPublicInputs:
                     fri_betas=fri_betas, fri_pow_response=pow_response, fri_query_indices=indices)
 
 
-def _commit_trace(trace, rate_bits, cap_height, ctx):
+def _commit_trace(trace, rate_bits, cap_height, ctx, **on):
     """The trace commitment (prover.rs:83-94) from host columns or from a (COLUMNS, n) torch CUDA tensor on the context's
-    device (read in place, never copied to the host)."""
+    device (read in place, never copied to the host). on: shard=(g, G) commits row block g of G only."""
     if hasattr(trace, "data_ptr"):
         import torch
 
@@ -588,8 +599,8 @@ def _commit_trace(trace, rate_bits, cap_height, ctx):
         def add_columns(h):
             N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(cols.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE), ctx.h)
 
-        return PolynomialBatch._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns)
-    return PolynomialBatch.from_values(trace, rate_bits, False, cap_height, ctx=ctx)
+        return PolynomialBatch._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, **on)
+    return PolynomialBatch.from_values(trace, rate_bits, False, cap_height, ctx=ctx, **on)
 
 
 def _device_trace(trace, ctx):
@@ -653,6 +664,11 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     verifier circuit made for another degree (ConstantArityBits only); the transcript then observes the zero caps and
     coefficients that verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment
     is released on every exit path."""
+    return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, None)
+
+
+def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement):
+    """prove on the placement of prove_with_commitment (None: one device)."""
     from .challenger import Challenger
 
     ctx = ctx or N.default_context()
@@ -662,20 +678,47 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     if stark.uses_lookups():
         check_lookup_shapes(stark)
         trace = _device_trace(trace, ctx)
-    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx)
+    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx, **_on(placement))
     try:
         challenger = Challenger()
         challenger.observe_elements(public_inputs)
         config.observe(challenger)
-        challenger.observe_cap(trace_commitment.merkle_tree.cap)
+        challenger.observe_cap(_full_cap(trace_commitment, placement))
         return prove_with_commitment(stark, config, trace, trace_commitment, None, None, challenger, public_inputs,
-                                     params, ctx=ctx)
+                                     params, ctx=ctx, placement=placement)
     finally:
         trace_commitment.close()
 
 
+def _shard(placement):
+    """(g, G) of a placement: this rank's row block of every commitment."""
+    return (0, 1) if placement is None else placement[0]
+
+
+def _on(placement):
+    """The keyword arguments that build a commitment on the placement (none on one device)."""
+    return dict(shard=_shard(placement)) if _shard(placement)[1] > 1 else {}
+
+
+def _full_cap(commitment, placement):
+    """The commitment's Merkle cap; for a row-block shard, every rank's cap entries all-gathered."""
+    if _shard(placement)[1] == 1:
+        return commitment.merkle_tree.cap
+    from .distributed import gather_cap
+
+    group = placement[1]
+    return gather_cap(commitment.merkle_tree.cap, group, device=_comm_device(group, commitment.ctx))
+
+
+def _comm_device(group, ctx):
+    """Where `group`'s collectives take their tensors: the context's GPU under NCCL, the host otherwise."""
+    import torch.distributed as dist
+
+    return "cuda:%d" % ctx.device if dist.get_backend(group) == "nccl" else None
+
+
 def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_challenges, challenger, public_inputs,
-                          params, ctx=None):
+                          params, ctx=None, placement=None):
     """prove_with_commitment (starky/src/prover.rs:125-484): one table's proof from its committed trace, on a challenger
     that has already observed what precedes it (the config among them). Every array-sized step runs on the device
     (lookup helper columns and the auxiliary commitment, quotient from the LDEs in place, quotient commitment, openings,
@@ -683,12 +726,17 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
     betas (prover.rs:165-168). With ctl_data (cross_table_lookup.CtlData, its CTL columns already in its auxiliary
     buffer) the auxiliary oracle is [lookup helpers | CTL helpers | CTL Zs], the CTL constraints join the quotient and
     the openings carry ctl_zs_first. trace: the values the lookup helper columns read (a CUDA tensor when the Stark has
-    lookups). params: _check_prove_shapes's. Every commitment made here is released on every exit path; the trace
-    commitment stays the caller's."""
+    lookups). params: _check_prove_shapes's. placement=((g, G), group) proves on the G ranks of the torch.distributed
+    group, this one holding row block g of every commitment (trace_commitment too): the caps are all-gathered before
+    they are observed, the quotient is evaluated shard by shard and all-gathered (distributed.quotient_polys_sharded),
+    and FRI routes the query openings between the ranks (distributed.prove_openings_sharded). Everything else runs
+    redundantly on every rank, so every rank returns the same proof. None: one device. Every commitment made here is
+    released on every exit path; the trace commitment stays the caller's."""
     from .fri import prove_openings
     from .lookup import get_grand_product_challenge_set
 
     ctx = ctx or N.default_context()
+    shard = _shard(placement)
     degree_bits = params.degree_bits
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     uses_lookups = stark.uses_lookups()
@@ -715,24 +763,33 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         elif uses_lookups:
             auxiliary = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
         if uses_lookups or ctl_data is not None:
-            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx)
+            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx, **_on(placement))
             commitments.append(aux_commitment)
             del auxiliary
             if ctl_data is not None:
                 ctl_data.auxiliary = None
-            challenger.observe_cap(aux_commitment.merkle_tree.cap)
+            aux_cap = _full_cap(aux_commitment, placement)
+            challenger.observe_cap(aux_cap)
             quotient_args["auxiliary_polys_commitment"] = aux_commitment
         num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
         num_ctl_helpers, num_ctl_zs = sum(num_ctl_polys), len(num_ctl_polys)
         alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
                                    lookup_challenges, ctl_vars, nl + num_ctl_helpers + num_ctl_zs if ctl_vars else None)
-        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **quotient_args)
+        if shard[1] > 1:
+            from .distributed import quotient_polys_sharded
+
+            quotient_polys = quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, placement[1],
+                                                    **quotient_args)
+        else:
+            quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **quotient_args)
         quotient_commitment = None
         if quotient_polys is not None:
-            quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx)
+            quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx,
+                                                        **_on(placement))
             commitments.append(quotient_commitment)
             del quotient_polys
-            challenger.observe_cap(quotient_commitment.merkle_tree.cap)
+            quotient_cap = _full_cap(quotient_commitment, placement)
+            challenger.observe_cap(quotient_cap)
         zeta = challenger.get_extension_challenge()
         if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
             raise N.NativeError("Opening point is in the subgroup.")
@@ -742,12 +799,19 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         for batch in openings.to_fri_openings():                        # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         instance = stark.fri_instance(zeta, g, config, num_ctl_helpers, num_ctl_zs)
-        opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
-                                       params.final_poly_coeff_len, params.max_num_query_steps)
-        proof = StarkProof(trace_commitment.merkle_tree.cap,
-                           quotient_commitment.merkle_tree.cap if quotient_commitment is not None else None,
+        if shard[1] > 1:
+            from .distributed import prove_openings_sharded
+
+            opening_proof = prove_openings_sharded(instance, [trace_commitment] + commitments, challenger,
+                                                   params.fri_params, placement[1], params.final_poly_coeff_len,
+                                                   params.max_num_query_steps)
+        else:
+            opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
+                                           params.final_poly_coeff_len, params.max_num_query_steps)
+        proof = StarkProof(_full_cap(trace_commitment, placement),
+                           quotient_cap if quotient_commitment is not None else None,
                            openings, opening_proof,
-                           aux_commitment.merkle_tree.cap if aux_commitment is not None else None)
+                           aux_cap if aux_commitment is not None else None)
         return StarkProofWithPublicInputs(proof, public_inputs)
     finally:
         for c in commitments:
