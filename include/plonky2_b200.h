@@ -266,7 +266,9 @@ int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
  *   gl_stark_quotient_from_shards  takes the G shards' buffers concatenated in shard order (G x n_alphas x M words,
  *                                  DEVICE memory) and writes gl_stark_quotient's result to out_coeffs (n_alphas x size,
  *                                  DEVICE memory): the values in natural order, .coset_ifft(g), and the trim_to_len check
- *                                  ("Quotient has failed", GL_ERR_BAD_ARG). */
+ *                                  ("Quotient has failed", GL_ERR_BAD_ARG). It takes gl_plonk_quotient_shard's values
+ *                                  the same way and then writes gl_plonk_quotient's result: both shard numberings and
+ *                                  layouts are this one, and the limits are equal (GL_VP_MAX_ALPHAS and GL_VP_MAX_QD). */
 int gl_stark_quotient_shard(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                             uint32_t n_alphas, uint32_t quotient_degree_factor, uint64_t* out_values);
@@ -364,6 +366,21 @@ typedef struct {
 int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                       uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                       uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_coeffs);
+/* gl_plonk_quotient on commitments that are row-block shards (gl_commit_create_sharded / gl_commit_begin with
+ * num_shards = G = 2^s), the first of two steps with an all-gather between them. Shard g owns the points i = r + G*k
+ * (k < M = size / G, r = the s-bit reversal of g) of the quotient coset, the leaf rows g*M .. g*M + M - 1 of the
+ * commitments' own numbering. It writes shard g's values of the vanishing polynomial over Z_H, n_alphas x M words in
+ * local natural order k (challenge alpha_a at out_values + a*M, DEVICE memory); gl_stark_quotient_from_shards turns the
+ * G shards' buffers, concatenated in shard order, into gl_plonk_quotient's result. Every commitment must be a shard of
+ * the same index and count (whole handles are shard 0 of 1), else GL_ERR_BAD_ARG; everything else is checked as in
+ * gl_plonk_quotient. The local values are read in place from the commitments' leaves when the quotient coset is the LDE
+ * coset (quotient degree 2^rate_bits, as in the standard recursion config), else they are the LDE of the handles'
+ * (replicated) coefficients onto the shard's coset, and then the program may not read salt columns. The next row comes
+ * from the same buffers when G divides 2^log2_ceil(quotient_degree_factor), else from an LDE onto the coset times w_n
+ * of the commitments the program reads with GL_VP_NEXT. */
+int gl_plonk_quotient_shard(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                            uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                            uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_values);
 
 /* ---- Hasher / MerkleTree  (plonky2/src/plonk/config.rs:36-77, plonky2/src/hash/merkle_tree.rs:193-237) */
 /* PoseidonPermutation::permute on the HOST for the sequential Fiat-Shamir transcript

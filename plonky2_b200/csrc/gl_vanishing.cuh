@@ -29,8 +29,16 @@ struct VanishingParams {
     uint64_t shift;                   // F::coset_shift()
     uint64_t n_field;                 // n as a field element
     uint64_t zh[GL_VP_MAX_QD], zh_inv[GL_VP_MAX_QD];  // ZeroPolyOnCoset (field/src/zero_poly_coset.rs:20-61)
-    uint64_t* out;                    // n_alphas columns of `size` values
+    uint64_t* out;                    // n_alphas columns of M = size >> shard_log values, local natural order
     unsigned int* flag;               // bit 0: L_0 asked for at x = 1 ("Tried to invert zero")
+    // Shard addressing (gl_plonk_quotient_shard); the defaults are the whole coset, shard 0 of 1. Shard g of
+    // G = 2^shard_log owns the quotient-coset leaf rows row0 + j (row0 = g*M, j < M), i.e. the points
+    // i = bitrev(g) + G*bitrev_M(j); lde[c] then holds those rows at j.
+    size_t row0 = 0;
+    uint32_t shard_log = 0;
+    bool next_in_shard = true;        // the next point's leaf row is in this shard: lde[c] at its row - row0
+    const uint64_t* nxt[GL_VP_MAX_COMMITS] = {};  // else the values at x*w_n, leaf order j, column k at + k*nxt_stride
+    size_t nxt_stride[GL_VP_MAX_COMMITS] = {};
 };
 
 GL_HD size_t vp_bitrev(size_t x, uint32_t bits) {
@@ -47,16 +55,17 @@ GL_HD size_t vp_bitrev(size_t x, uint32_t bits) {
 // bitrev(i * step) = bitrev_{size_log}(i), i.e. exactly the first `size` leaf rows, so thread j takes point
 // i = bitrev_{size_log}(j): every LDE load of a warp is one contiguous 256-byte segment of a column, and only the
 // n_alphas result stores (and the few Z(g x) loads) are scattered. Returns false if the program divided by zero.
-// regs: GL_VP_MAX_REGS words of scratch.
+// regs: GL_VP_MAX_REGS words of scratch. On a shard, j is the local leaf row (p.row0 + j globally); x, Z_H and L_0
+// still come from the global point i.
 GL_HD bool vp_eval_point(const VanishingParams& p, size_t j, uint64_t* regs) {
     const uint32_t size_log = p.degree_bits + p.qd_bits;
     const size_t size = (size_t)1 << size_log;
-    const size_t i = vp_bitrev(j, size_log);
+    const size_t i = vp_bitrev(p.row0 + j, size_log);
     const size_t inext = (i + ((size_t)1 << p.qd_bits)) & (size - 1);  // next_step = 2^quotient_degree_bits, prover.rs:643
     // get_lde_values(i, step) with step = 2^(rate_bits - quotient_degree_bits) (prover.rs:640, fri/oracle.rs:142-147):
     // leaf row bitrev_{log_N}(i * step) = bitrev_{size_log}(i)
     const size_t jl = j;
-    const size_t jn = vp_bitrev(inext, size_log);
+    const size_t jn = p.next_in_shard ? vp_bitrev(inext, size_log) - p.row0 : j;
     const uint32_t qmask = (1u << p.qd_bits) - 1;
     const uint64_t x = mul(p.shift, mul(p.xhi[i >> 12], p.xlo[i & 4095]));
     uint64_t acc[GL_VP_MAX_ALPHAS];
@@ -68,7 +77,10 @@ GL_HD bool vp_eval_point(const VanishingParams& p, size_t j, uint64_t* regs) {
         uint64_t r;
         switch (in.op) {
             case GL_VP_LOCAL: r = p.lde[in.a][(size_t)in.b * p.lde_stride[in.a] + jl]; break;
-            case GL_VP_NEXT: r = p.lde[in.a][(size_t)in.b * p.lde_stride[in.a] + jn]; break;
+            case GL_VP_NEXT:
+                r = p.next_in_shard ? p.lde[in.a][(size_t)in.b * p.lde_stride[in.a] + jn]
+                                    : p.nxt[in.a][(size_t)in.b * p.nxt_stride[in.a] + jn];
+                break;
             case GL_VP_CONST: r = p.consts[(uint32_t)in.a | ((uint32_t)in.b << 16)]; break;
             case GL_VP_X: r = x; break;
             case GL_VP_L0: {  // eval_l_0: Z_H(x) / (n (x - 1)), zero_poly_coset.rs:58-61
@@ -91,7 +103,8 @@ GL_HD bool vp_eval_point(const VanishingParams& p, size_t j, uint64_t* regs) {
         regs[in.dst] = r;
     }
     const uint64_t zi = p.zh_inv[i & qmask];  // eval_inverse(i), prover.rs:796-802
-    for (uint32_t a = 0; a < p.n_alphas; a++) p.out[(size_t)a * size + i] = canon(mul(acc[a], zi));
+    const uint32_t log_M = size_log - p.shard_log;  // i = bitrev(g) + G*k: local point k = i >> shard_log
+    for (uint32_t a = 0; a < p.n_alphas; a++) p.out[((size_t)a << log_M) + (i >> p.shard_log)] = canon(mul(acc[a], zi));
     return ok;
 }
 

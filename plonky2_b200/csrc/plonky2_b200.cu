@@ -1365,13 +1365,14 @@ __global__ void k_any_nonzero(const u64* data, size_t stride, size_t begin, size
 }
 
 // ---- plonky2 quotient evaluation (compute_quotient_polys, plonk/prover.rs:609-815; SURVEY 8(f) row 1) ----
-// one thread per point of the quotient coset; the point's evaluation is gl_vanishing.cuh
+// one thread per point of the shard of the quotient coset (the whole coset on one device); the point's evaluation is
+// gl_vanishing.cuh
 __global__ void __launch_bounds__(128) k_plonk_quotient(VanishingParams p) {
-    const size_t size = (size_t)1 << (p.degree_bits + p.qd_bits);
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= size) return;
+    const size_t M = (size_t)1 << (p.degree_bits + p.qd_bits - p.shard_log);
+    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= M) return;
     u64 regs[GL_VP_MAX_REGS];
-    if (!vp_eval_point(p, i, regs)) atomicOr(p.flag, 1u);
+    if (!vp_eval_point(p, j, regs)) atomicOr(p.flag, 1u);
 }
 
 // proof-of-work grind (prover.rs:183-194): smallest qualifying nonce via atomicMin
@@ -2081,6 +2082,13 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
     *qd_bits_out = qd_bits;
     return GL_OK;
 }
+// The values of commitment c's polynomials (its replicated coefficients) on the coset shift*<w_M>, M = 2^log_M, in leaf
+// order, column k at buf + k*M: a shard's quotient-coset values when its commitment's leaves are another coset
+static int commit_coset_values(gl_ctx* ctx, const gl_commit* c, uint32_t log_M, u64 shift, DevBuf& buf) {
+    const size_t M = (size_t)1 << log_M;
+    TRY(buf.alloc((size_t)c->B * M));
+    return coset_lde_columns(ctx, c->coeffs, c->B, c->degree_log, log_M, shift, buf.get(), M);
+}
 // C(x)/Z_H(x) on the trace handle's shard of the quotient coset (the whole coset for an unsharded handle): M values per
 // challenge in local natural order, at out + a*M. Division by zero sets bit 1 of dflag.
 static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
@@ -2103,8 +2111,7 @@ static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, 
         size_t stride;
     };
     auto values_on = [&](gl_commit* c, u64 s, DevBuf& buf, View* v) -> int {
-        TRY(buf.alloc((size_t)c->B * M));
-        TRY(coset_lde_columns(ctx, c->coeffs, c->B, c->degree_log, log_M, s, buf.get(), M));
+        TRY(commit_coset_values(ctx, c, log_M, s, buf));
         *v = {buf.get(), M};
         return GL_OK;
     };
@@ -2152,14 +2159,15 @@ static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, 
     CKL(ctx);
     return GL_OK;
 }
-// The quotient's coefficients from its values on the whole coset, in place, then the flags of both steps
-static int stark_quotient_coeffs(gl_ctx* ctx, uint64_t* coeffs, uint32_t degree_bits, uint32_t n_alphas,
-                                 uint32_t quotient_degree_factor, const DevBuf& dflag) {
+// The quotient's coefficients from its values on the whole coset, in place, then the flags of both steps: the tail of
+// starky's and plonky2's quotient, one device or gathered shards
+static int quotient_coeffs(gl_ctx* ctx, uint64_t* coeffs, uint32_t degree_bits, uint32_t n_alphas,
+                           uint32_t quotient_degree_factor, const DevBuf& dflag) {
     const uint32_t size_log = degree_bits + quotient_degree_bits(quotient_degree_factor);
     const size_t size = (size_t)1 << size_log;
-    // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:661-667)
+    // .coset_ifft(F::coset_shift()) of every challenge's values (starky prover.rs:661-667, plonk/prover.rs:811-814)
     TRY(ntt_natural(ctx, coeffs, size, coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
-    // trim_to_len(degree * quotient_degree_factor) (prover.rs:396-401): the rest must vanish
+    // trim_to_len(degree * quotient_degree_factor) (starky prover.rs:396-401, plonk/prover.rs:327-331): the rest must vanish
     const size_t keep = ((size_t)quotient_degree_factor) << degree_bits;
     if (keep < size) {
         k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(coeffs, size, keep,
@@ -2180,7 +2188,7 @@ static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
     TRY(flag_alloc(ctx, dflag));
     TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out_coeffs,
                               dflag));
-    return stark_quotient_coeffs(ctx, out_coeffs, trace->degree_log, n_alphas, quotient_degree_factor, dflag);
+    return quotient_coeffs(ctx, out_coeffs, trace->degree_log, n_alphas, quotient_degree_factor, dflag);
 }
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
                       const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
@@ -2228,7 +2236,7 @@ int gl_stark_quotient_from_shards(gl_ctx* ctx, const uint64_t* values, uint32_t 
     k_stark_unshard<<<dim3((unsigned)((((size_t)1 << log_M) + 127) / 128), num_shards, n_alphas), 128, 0, ctx->stream>>>(
         values, log_M, sl, out_coeffs);
     CKL(ctx);
-    return stark_quotient_coeffs(ctx, out_coeffs, degree_bits, n_alphas, quotient_degree_factor, dflag);
+    return quotient_coeffs(ctx, out_coeffs, degree_bits, n_alphas, quotient_degree_factor, dflag);
 }
 
 int gl_stark_lookup_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, uint32_t num_columns, uint32_t log_n,
@@ -2398,10 +2406,14 @@ int gl_stark_ctl_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, 
     return flag_status(ctx, dflag, {INVERT_ZERO});
 }
 
-int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
-                      uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
-                      uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
-    if (!ctx || !commits || !program || !alphas || !out_coeffs) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+// The checks of gl_plonk_quotient (whole = true: every LDE whole on this device) and gl_plonk_quotient_shard
+// (whole = false: the commitments are shards of the same index and count). Sets *qd_bits_out and *next_mask_out (bit c:
+// the program reads commitment c's next row).
+static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                                uint32_t n_instr, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                                uint32_t n_terms, uint32_t quotient_degree_factor, const uint64_t* out, bool whole,
+                                uint32_t* qd_bits_out, uint32_t* next_mask_out) {
+    if (!ctx || !commits || !program || !alphas || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     if (n_commits == 0 || n_commits > GL_VP_MAX_COMMITS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d commitments", GL_VP_MAX_COMMITS);
     if (n_instr == 0) return set_err(ctx, GL_ERR_BAD_ARG, "empty program");
     if (n_alphas == 0 || n_alphas > GL_VP_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_VP_MAX_ALPHAS);
@@ -2410,17 +2422,25 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
     for (uint32_t c = 0; c < n_commits; c++) {
         if (!commits[c]) return set_err(ctx, GL_ERR_BAD_ARG, "null commitment");
         if (commits[c]->ctx != ctx) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u belongs to another context", c);
-        if (commits[c]->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
+        if (whole && commits[c]->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
+        if (!whole && (commits[c]->shard_index != commits[0]->shard_index || commits[c]->shard_log != commits[0]->shard_log))
+            return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is shard %u of %u, commitment 0 shard %u of %u", c,
+                           commits[c]->shard_index, 1u << commits[c]->shard_log, commits[0]->shard_index,
+                           1u << commits[0]->shard_log);
         NEED_FINISHED(commits[c]);
         if (commits[c]->degree_log != commits[0]->degree_log || commits[c]->rate_bits != commits[0]->rate_bits)
             return set_err(ctx, GL_ERR_BAD_SHAPE, "commitments of different degree or rate");
     }
-    const uint32_t db = commits[0]->degree_log, rate_bits = commits[0]->rate_bits;
-    uint32_t qd_bits = 0;
-    while ((1u << qd_bits) < quotient_degree_factor) qd_bits++;  // log2_ceil
+    const uint32_t db = commits[0]->degree_log, rate_bits = commits[0]->rate_bits, sl = commits[0]->shard_log;
+    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
     if (qd_bits > rate_bits)
         return set_err(ctx, GL_ERR_UNSUPPORTED, "Having constraints of degree higher than the rate is not supported yet.");
     if ((1u << qd_bits) > GL_VP_MAX_QD) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
+    if (sl > db + qd_bits)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", 1u << sl, db + qd_bits);
+    // a shard whose quotient coset is not its LDE coset reads values computed from the coefficients: no salt columns
+    const bool in_place = sl == 0 || qd_bits == rate_bits;
+    uint32_t next_mask = 0;
     {  // validate once on the host: the kernel trusts the program (operands in range, no register read before it is written)
         bool written[GL_VP_MAX_REGS] = {false};
         auto readable = [&](uint16_t r) { return r < GL_VP_MAX_REGS && written[r]; };
@@ -2428,7 +2448,10 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
             const gl_vp_instr in = program[k];
             bool ok = in.dst < GL_VP_MAX_REGS;
             switch (in.op) {
-                case GL_VP_LOCAL: case GL_VP_NEXT: ok = ok && in.a < n_commits && in.b < commits[in.a]->W; break;
+                case GL_VP_LOCAL: case GL_VP_NEXT:
+                    ok = ok && in.a < n_commits && in.b < (in_place ? commits[in.a]->W : commits[in.a]->B);
+                    if (ok && in.op == GL_VP_NEXT) next_mask |= 1u << in.a;
+                    break;
                 case GL_VP_CONST: ok = ok && ((uint32_t)in.a | ((uint32_t)in.b << 16)) < n_consts; break;
                 case GL_VP_X: case GL_VP_L0: break;
                 case GL_VP_ADD: case GL_VP_SUB: case GL_VP_MUL: ok = ok && readable(in.a) && readable(in.b); break;
@@ -2440,10 +2463,48 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
             if (in.op != GL_VP_TERM) written[in.dst] = true;
         }
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    const uint32_t size_log = db + qd_bits;
-    const size_t size = (size_t)1 << size_log;
-    DevBuf dprog(ctx), dconst(ctx), dapow(ctx), dflag(ctx), xtab(ctx);
+    *qd_bits_out = qd_bits;
+    *next_mask_out = next_mask;
+    return GL_OK;
+}
+// The vanishing polynomial over Z_H on the commitments' shard of the quotient coset (the whole coset for unsharded
+// handles): M values per challenge in local natural order, at out + a*M. L_0 asked for at x = 1 sets bit 0 of dflag.
+static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                                 uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                                 uint32_t n_alphas, uint32_t n_terms, uint32_t qd_bits, uint32_t next_mask, uint64_t* out,
+                                 const DevBuf& dflag) {
+    const gl_commit* c0 = commits[0];
+    const uint32_t db = c0->degree_log, size_log = db + qd_bits, sl = c0->shard_log, log_M = size_log - sl;
+    const size_t size = (size_t)1 << size_log, M = (size_t)1 << log_M;
+    const u64 w_size = root_of_unity(size_log);
+    // this shard's coset g*w_size^r*<w_M>, r = the sl-bit reversal of the shard index
+    const u64 shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(w_size, bitrev32(c0->shard_index, sl)));
+    // The local values: in place when the shard's coset is its commitments' -- always on one device (the LDE's first
+    // `size` leaves), and on every shard when the quotient coset is the LDE coset. Else the LDE onto the coset.
+    const bool local_in_place = sl == 0 || qd_bits == c0->rate_bits;
+    // The next row, point i + 2^qd_bits, lies in the same shard when G divides 2^qd_bits. Else the values on the coset
+    // times w_n, for the commitments the program reads there.
+    const bool next_in_shard = sl <= qd_bits;
+    VanishingParams p;
+    std::vector<DevBuf> bufs;
+    bufs.reserve(2 * GL_VP_MAX_COMMITS);
+    for (uint32_t c = 0; c < GL_VP_MAX_COMMITS; c++) {
+        p.lde[c] = c < n_commits && local_in_place ? commits[c]->tree.leaves : nullptr;
+        p.lde_stride[c] = c < n_commits && local_in_place ? commits[c]->tree.es : 0;
+        if (c < n_commits && !local_in_place) {
+            bufs.emplace_back(ctx);
+            TRY(commit_coset_values(ctx, commits[c], log_M, shift, bufs.back()));
+            p.lde[c] = bufs.back().get();
+            p.lde_stride[c] = M;
+        }
+        if (c < n_commits && !next_in_shard && ((next_mask >> c) & 1)) {
+            bufs.emplace_back(ctx);
+            TRY(commit_coset_values(ctx, commits[c], log_M, mul(shift, root_of_unity(db)), bufs.back()));
+            p.nxt[c] = bufs.back().get();
+            p.nxt_stride[c] = M;
+        }
+    }
+    DevBuf dprog(ctx), dconst(ctx), dapow(ctx), xtab(ctx);
     TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_vp_instr), consts, n_consts, dprog, dconst));
     std::vector<u64> apow((size_t)n_alphas * n_terms);
     for (uint32_t a = 0; a < n_alphas; a++) {
@@ -2452,14 +2513,8 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
     }
     TRY(dapow.alloc(apow.size()));
     TRY(h2d(ctx, dapow.get(), apow.data(), apow.size()));
-    TRY(flag_alloc(ctx, dflag));
-    TRY(x_pow_tables(ctx, root_of_unity(size_log), size, xtab));
-    VanishingParams p;
-    for (uint32_t c = 0; c < GL_VP_MAX_COMMITS; c++) {
-        p.lde[c] = c < n_commits ? commits[c]->tree.leaves : nullptr;
-        p.lde_stride[c] = c < n_commits ? commits[c]->tree.es : 0;
-    }
-    p.log_N = db + rate_bits;
+    TRY(x_pow_tables(ctx, w_size, size, xtab));
+    p.log_N = db + c0->rate_bits;
     p.degree_bits = db;
     p.qd_bits = qd_bits;
     p.prog = (const gl_vp_instr*)dprog.get();
@@ -2474,20 +2529,40 @@ int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits
     p.n_field = canon((u64)1 << db);
     for (uint32_t j = 0; j < GL_VP_MAX_QD; j++) p.zh[j] = p.zh_inv[j] = 0;
     zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
-    p.out = out_coeffs;
+    p.out = out;
     p.flag = (unsigned int*)dflag.get();
-    k_plonk_quotient<<<(unsigned)((size + 127) / 128), 128, 0, ctx->stream>>>(p);
+    p.row0 = (size_t)c0->shard_index << log_M;
+    p.shard_log = sl;
+    p.next_in_shard = next_in_shard;
+    k_plonk_quotient<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p);
     CKL(ctx);
-    // .coset_ifft(F::coset_shift()) of every challenge's values (prover.rs:811-814)
-    TRY(ntt_natural(ctx, out_coeffs, size, out_coeffs, size, (int)size_log, n_alphas, true, MULTIPLICATIVE_GROUP_GENERATOR));
-    // trim_to_len(quotient_degree) (prover.rs:327-331): the rest must vanish
-    const size_t keep = ((size_t)quotient_degree_factor) << db;
-    if (keep < size) {
-        k_any_nonzero<<<dim3((unsigned)((size - keep + 255) / 256), n_alphas), 256, 0, ctx->stream>>>(out_coeffs, size, keep,
-                                                                                               size - keep, (unsigned int*)dflag.get());
-        CKL(ctx);
-    }
-    return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
+    return GL_OK;
+}
+int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                      uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                      uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
+    uint32_t qd_bits = 0, next_mask = 0;
+    TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
+                             quotient_degree_factor, out_coeffs, true, &qd_bits, &next_mask));
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf dflag(ctx);
+    TRY(flag_alloc(ctx, dflag));
+    TRY(plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
+                              qd_bits, next_mask, out_coeffs, dflag));
+    return quotient_coeffs(ctx, out_coeffs, commits[0]->degree_log, n_alphas, quotient_degree_factor, dflag);
+}
+int gl_plonk_quotient_shard(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                            uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                            uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_values) {
+    uint32_t qd_bits = 0, next_mask = 0;
+    TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
+                             quotient_degree_factor, out_values, false, &qd_bits, &next_mask));
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf dflag(ctx);
+    TRY(flag_alloc(ctx, dflag));
+    TRY(plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
+                              qd_bits, next_mask, out_values, dflag));
+    return flag_status(ctx, dflag, {INVERT_ZERO});
 }
 
 void gl_poseidon_permute_host(uint64_t state[12]) {

@@ -6,9 +6,12 @@ Merkle-cap entries (2^cap_height x 32 bytes in total) -- and PipelinedCommitter 
 No LDE data ever crosses NVLink: shard g of G evaluates every column on its own coset
 (g_shift * w_N^{bitrev(g)}) <w_{N/G}>, hashes its leaves and reduces its own cap subtrees.
 
-prove_stark proves one STARK on the ranks of a group with these shards: besides the caps, only the quotient's values on
-each rank's shard of the quotient coset (quotient_polys_sharded) and the FRI query openings (prove_openings_sharded)
-cross ranks."""
+prove_stark proves one STARK, and prove_plonk one plonky2 circuit, on the ranks of a group with these shards: besides
+the caps, only the quotient's values on each rank's shard of the quotient coset (quotient_polys_sharded,
+plonk_quotient_polys_sharded) and the FRI query openings (prove_openings_sharded) cross ranks. Both provers take a
+`placement` ((g, G), group) -- None on one device -- and build their commitments with shard_of / shard_kwargs / full_cap."""
+import ctypes as C
+
 import numpy as np
 
 from .hash import MerkleCap
@@ -135,32 +138,47 @@ def all_gather_tensor(t, group=None):
     return out
 
 
-def quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, group=None, auxiliary_polys_commitment=None,
-                           lookup_challenges=None, ctl_vars=None):
-    """stark.compute_quotient_polys when the trace (and auxiliary) commitments are this rank's row-block shard: each rank
-    evaluates C(x)/Z_H(x) on its shard of the quotient coset (gl_stark_quotient_shard), the ranks all-gather the values,
-    and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same torch
-    tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
+def shard_of(placement):
+    """(g, G) of a prover's placement ((g, G), group): this rank's row block of every commitment; (0, 1) on one device
+    (placement None)."""
+    return (0, 1) if placement is None else placement[0]
+
+
+def shard_kwargs(placement):
+    """The keyword arguments that build a commitment on the placement (none on one device)."""
+    return dict(shard=shard_of(placement)) if shard_of(placement)[1] > 1 else {}
+
+
+def full_cap(commitment, placement):
+    """The commitment's Merkle cap; for a row-block shard, every rank's cap entries all-gathered."""
+    if shard_of(placement)[1] == 1:
+        return commitment.merkle_tree.cap
+    group = placement[1]
+    return gather_cap(commitment.merkle_tree.cap, group, device=_comm_device(group, commitment.ctx))
+
+
+def _comm_device(group, ctx):
+    """Where `group`'s collectives take their tensors: the context's GPU under NCCL, the host otherwise."""
+    import torch.distributed as dist
+
+    return "cuda:%d" % ctx.device if dist.get_backend(group) == "nccl" else None
+
+
+def _quotient_from_shards(ctx, run_shard, n_alphas, degree_bits, quotient_degree_factor, num_shards, group):
+    """The steps both sharded quotients share. run_shard(local) writes this rank's shard values into `local`, an
+    (n_alphas, size / G) int64 CUDA tensor, through its C entry point. Then every rank learns whether any shard failed,
+    the ranks all-gather the values, and every rank interpolates the whole quotient (gl_stark_quotient_from_shards).
+    Collective. A failure on one rank raises on every rank: its own exception there, NativeError elsewhere."""
     import torch
 
     from . import _native as N
-    from .stark import quotient_program
 
-    qdf = stark.quotient_degree_factor()
-    if qdf == 0:
-        return None
-    b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
-                                     ctl_vars)
-    ctx, G = trace_commitment.ctx, trace_commitment.num_shards
-    size = (1 << trace_commitment.degree_log) << (qdf - 1).bit_length()
+    size = (1 << degree_bits) << (quotient_degree_factor - 1).bit_length()
     dev = "cuda:%d" % ctx.device
-    local = torch.empty((len(al), size // G), dtype=torch.int64, device=dev)
-    aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
+    local = torch.empty((n_alphas, size // num_shards), dtype=torch.int64, device=dev)
     failure = None
     try:
-        N.check(N.lib().gl_stark_quotient_shard(ctx.h, trace_commitment.h, aux_h, b.program(), len(b.instrs),
-                                                N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
-                                                N.vp(local.data_ptr())), ctx.h)
+        run_shard(local)
     except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
         failure = e
     failed = all_gather_tensor(torch.tensor([int(failure is not None)], dtype=torch.int64, device=dev), group)
@@ -169,22 +187,79 @@ def quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, group
     if int(failed.sum()):
         raise N.NativeError("the quotient failed on rank %d" % int(torch.nonzero(failed.view(-1))[0]))
     values = all_gather_tensor(local, group)
-    out = torch.empty((len(al), size), dtype=torch.int64, device=dev)
-    N.check(N.lib().gl_stark_quotient_from_shards(ctx.h, N.vp(values.data_ptr()), G, len(al),
-                                                  trace_commitment.degree_log, qdf, N.vp(out.data_ptr())), ctx.h)
+    out = torch.empty((n_alphas, size), dtype=torch.int64, device=dev)
+    N.check(N.lib().gl_stark_quotient_from_shards(ctx.h, N.vp(values.data_ptr()), num_shards, n_alphas, degree_bits,
+                                                  quotient_degree_factor, N.vp(out.data_ptr())), ctx.h)
     ctx.synchronize()
     return out
+
+
+def quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, group=None, auxiliary_polys_commitment=None,
+                           lookup_challenges=None, ctl_vars=None):
+    """stark.compute_quotient_polys when the trace (and auxiliary) commitments are this rank's row-block shard: each rank
+    evaluates C(x)/Z_H(x) on its shard of the quotient coset (gl_stark_quotient_shard), the ranks all-gather the values,
+    and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same torch
+    tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
+    from . import _native as N
+    from .stark import quotient_program
+
+    qdf = stark.quotient_degree_factor()
+    if qdf == 0:
+        return None
+    b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
+                                     ctl_vars)
+    ctx = trace_commitment.ctx
+    aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
+
+    def run_shard(local):
+        N.check(N.lib().gl_stark_quotient_shard(ctx.h, trace_commitment.h, aux_h, b.program(), len(b.instrs),
+                                                N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
+                                                N.vp(local.data_ptr())), ctx.h)
+
+    return _quotient_from_shards(ctx, run_shard, len(al), trace_commitment.degree_log, qdf, trace_commitment.num_shards,
+                                 group)
+
+
+def plonk_quotient_polys_sharded(common_data, constants_sigmas_commitment, public_inputs_hash, wires_commitment,
+                                 zs_partial_products_commitment, betas, gammas, alphas, deltas=(), group=None):
+    """plonk.compute_quotient_polys when the three commitments are this rank's row-block shard: each rank evaluates the
+    vanishing polynomial over Z_H on its shard of the quotient coset (gl_plonk_quotient_shard), the ranks all-gather the
+    values, and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same
+    torch tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
+    from . import _native as N
+    from .plonk import quotient_program
+
+    commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
+    prog, consts, al = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas)
+    ctx = wires_commitment.ctx
+    handles = (C.c_void_p * 3)(*[c.h for c in commits])
+    qdf = common_data.quotient_degree_factor
+
+    def run_shard(local):
+        N.check(N.lib().gl_plonk_quotient_shard(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts),
+                                                N.np_ptr(al), len(al), common_data.num_vanishing_terms(), qdf,
+                                                N.vp(local.data_ptr())), ctx.h)
+
+    return _quotient_from_shards(ctx, run_shard, len(al), common_data.degree_bits, qdf, wires_commitment.num_shards,
+                                 group)
+
+
+def _check_world(what, cap_height, world):
+    """The world-size refusals of prove_stark and prove_plonk: the same on every rank."""
+    from . import _native as N
+
+    if world < 1 or world & (world - 1):
+        raise N.ShapeError("%s needs a power-of-two number of ranks, got %d" % (what, world))
+    if world > 1 << cap_height:
+        raise N.ShapeError("%d ranks exceed the %d cap entries of a commitment (cap_height %d)"
+                           % (world, 1 << cap_height, cap_height))
 
 
 def check_prove_stark(stark, config, world):
     """prove_stark's refusals, raised identically on every rank before any device work or collective."""
     from . import _native as N
 
-    if world < 1 or world & (world - 1):
-        raise N.ShapeError("prove_stark needs a power-of-two number of ranks, got %d" % world)
-    if world > 1 << config.fri_config.cap_height:
-        raise N.ShapeError("%d ranks exceed the %d cap entries of a commitment (cap_height %d)"
-                           % (world, 1 << config.fri_config.cap_height, config.fri_config.cap_height))
+    _check_world("prove_stark", config.fri_config.cap_height, world)
     if stark.requires_ctls():
         raise N.ShapeError("prove_stark proves one STARK without cross-table lookups; see "
                            "cross_table_lookup.prove_with_ctls")
@@ -212,6 +287,74 @@ def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circui
         ctx = N.default_context(torch.cuda.current_device())
     placement = ((dist.get_rank(group), world), group) if world > 1 else None
     return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement)
+
+
+def _check_constants_sigmas_shard(prover_data, rank, world):
+    from . import _native as N
+
+    cs = prover_data.constants_sigmas_commitment
+    if (cs.shard_index, cs.num_shards) != (rank, world):
+        raise N.ShapeError("the constants/sigmas commitment is shard %d of %d; rank %d of %d needs shard %d of %d "
+                           "(PolynomialBatch.from_values(..., shard=(rank, world)))"
+                           % (cs.shard_index, cs.num_shards, rank, world, rank, world))
+
+
+def check_prove_plonk(prover_data, common_data, world, rank=0):
+    """prove_plonk's refusals on rank `rank` of `world`: a world size that is not a power of two or exceeds
+    2^cap_height (the same on every rank), and a constants/sigmas commitment that is not this rank's row-block shard
+    (which can differ between ranks; prove_plonk exchanges that outcome so that every rank refuses)."""
+    _check_world("prove_plonk", common_data.config.cap_height, world)
+    _check_constants_sigmas_shard(prover_data, rank, world)
+
+
+def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=None, *, salt_keys=None):
+    """plonk.prove_with_witness on the ranks of a torch.distributed group (the default group if None): rank g commits
+    row block g of the wires, Z / partial-product (+ lookup) and quotient LDEs, evaluates the quotient on its shard of
+    the quotient coset and answers the FRI queries that land in its rows. The Z's, partial products and lookup columns
+    (over all n rows), the openings (from the replicated coefficients) and the transcript are computed on every rank.
+    Collective: every rank passes the same full witness and returns the same ProofWithPublicInputs, whose bytes equal
+    prove_with_witness's on one device. prover_data.constants_sigmas_commitment must be this rank's row-block shard
+    (rank, world), built at circuit build with PolynomialBatch.from_values(..., shard=(rank, world)).
+
+    Refusals (ShapeError, on every rank, before the proof's device work): a world size that is not a power of two or
+    above 2^cap_height; a constants/sigmas commitment of another shard index or count on any rank. Without an
+    initialised process group, or with one rank, this is prove_with_witness. ctx: this rank's context (default: the
+    current CUDA device's).
+
+    Zero knowledge: salt_keys (three 32-byte keys, equal on every rank) give the bytes of
+    prove_with_witness(..., salt_keys=salt_keys), since a keyed shard holds the unsharded commitment's salted leaves. With
+    None ("fresh" keys) each rank draws its own key for its own rows, without a collective: a leaf's salt is only ever
+    read by the rank that owns the leaf (open_sharded), so the proof is valid and hiding, but no single-device run
+    reproduces it."""
+    import torch
+    import torch.distributed as dist
+
+    from . import _native as N
+    from . import plonk as P
+
+    world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    rank = dist.get_rank(group) if world > 1 else 0
+    _check_world("prove_plonk", common_data.config.cap_height, world)
+    refusal = None
+    try:
+        _check_constants_sigmas_shard(prover_data, rank, world)
+    except N.ShapeError as e:
+        refusal = e
+    if world == 1 and refusal is not None:
+        raise refusal
+    if ctx is None:
+        ctx = N.default_context(torch.cuda.current_device())
+    if world > 1:
+        # the shard check may fail on some ranks only: every rank learns the outcome before a collective could wait
+        flag = torch.tensor([int(refusal is not None)], dtype=torch.int64, device=_comm_device(group, ctx) or "cpu")
+        refused = all_gather_tensor(flag, group).view(-1)
+        if refusal is not None:
+            raise refusal
+        if int(refused.sum()):
+            raise N.ShapeError("rank %d's constants/sigmas commitment is not its row-block shard"
+                               % int(torch.nonzero(refused)[0]))
+    placement = ((rank, world), group) if world > 1 else None
+    return P._prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys)
 
 
 def chunk_layout(num_polys, world, chunk_cols=64):

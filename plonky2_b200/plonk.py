@@ -19,6 +19,7 @@ import re
 import numpy as np
 
 from . import _native as N
+from . import distributed
 from . import field as F
 from .polynomial_batch import SALT_SIZE, PolynomialBatch
 
@@ -1435,11 +1436,28 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
     stay where they are; nothing but the program and the challenges crosses PCIe."""
     import torch
 
+    commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
+    prog, consts, al = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas)
+    nc = common_data.config.num_challenges
+    qdf = common_data.quotient_degree_factor
+    size = (1 << common_data.degree_bits) << (qdf - 1).bit_length()
+    ctx = wires_commitment.ctx
+    out = torch.empty((nc, size), dtype=torch.int64, device="cuda:%d" % ctx.device)
+    handles = (C.c_void_p * 3)(*[c.h for c in commits])
+    N.check(N.lib().gl_plonk_quotient(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts), N.np_ptr(al), nc,
+                                      common_data.num_vanishing_terms(), qdf, N.vp(out.data_ptr())), ctx.h)
+    ctx.synchronize()
+    return out
+
+
+def quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas=()):
+    """What gl_plonk_quotient and gl_plonk_quotient_shard take besides the three commitments (constants / sigmas, wires,
+    Z / partial products [+ lookups]): the compiled vanishing program, its constants and the alphas, as arrays. Raises
+    ShapeError for wrong challenge counts or commitments of the wrong width or degree."""
     cfg = common_data.config
     nc = cfg.num_challenges
     if not (len(betas) == len(gammas) == len(alphas) == nc) or len(public_inputs_hash) != 4:
         raise N.ShapeError("expected %d betas, gammas, alphas and a 4-element public_inputs_hash" % nc)
-    commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
     n_luts = len(common_data.luts)
     if len(deltas) != (NUM_COINS_LOOKUP * nc if n_luts else 0):
         raise N.ShapeError("expected %d lookup challenges (deltas)" % (NUM_COINS_LOOKUP * nc if n_luts else 0))
@@ -1452,27 +1470,18 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
     b = common_data.vanishing_program()
     prog, _ = b.compile()
     consts = program_constants(common_data, b, public_inputs_hash, betas, gammas, deltas)
-    al = np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
-    qdf = common_data.quotient_degree_factor
-    size = (1 << common_data.degree_bits) << (qdf - 1).bit_length()
-    ctx = wires_commitment.ctx
-    out = torch.empty((nc, size), dtype=torch.int64, device="cuda:%d" % ctx.device)
-    handles = (C.c_void_p * 3)(*[c.h for c in commits])
-    N.check(N.lib().gl_plonk_quotient(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts), N.np_ptr(al), nc,
-                                      common_data.num_vanishing_terms(), qdf, N.vp(out.data_ptr())), ctx.h)
-    ctx.synchronize()
-    return out
+    return prog, consts, np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
 
 
-def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None):
+def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None, shard=(0, 1)):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients (trim_to_len(quotient_degree) was checked by the kernel call), all
     chunks committed with from_coeffs -- straight from the device tensor compute_quotient_polys returned. With blinding
-    the salt is drawn on the device from salt_key (PolynomialBatch._from_device)."""
+    the salt is drawn on the device from salt_key (PolynomialBatch._from_device). shard=(g, G): row block g of G only."""
     cfg = common_data.config
     return PolynomialBatch._from_coeff_chunks(quotient_polys, common_data.quotient_degree_factor,
                                               common_data.degree_bits, cfg.rate_bits, cfg.cap_height, ctx,
-                                              blinding=blinding, salt_key=salt_key)
+                                              blinding=blinding, salt_key=salt_key, shard=shard)
 
 
 # ------------------------------------------------------------------ prove (plonk/prover.rs:113-360)
@@ -1668,6 +1677,16 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
     The salt is drawn on the device: salt_keys = three 32-byte keys (wires, Z's, quotient) give a reproducible proof;
     None draws a fresh key from the OS CSPRNG per commitment. The blinding rows of the circuit (blinding_counts) are part
     of the witness, which the caller generates."""
+    return _prove(prover_data, common_data, wires, public_inputs, ctx, None, salt_keys)
+
+
+def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys=None):
+    """prove_with_witness on a placement ((g, G), group) of distributed.prove_plonk (None: one device). With G > 1 this
+    rank holds row block g of the wires, Z / partial-product (+ lookup) and quotient commitments, and
+    prover_data.constants_sigmas_commitment is that shard too: the caps are all-gathered before they are observed, the
+    quotient is evaluated shard by shard and all-gathered (distributed.plonk_quotient_polys_sharded), and FRI routes the
+    query openings between the ranks (distributed.prove_openings_sharded). The Z's, partial products and lookup columns,
+    the openings and the transcript run on every rank, so every rank returns the same proof."""
     from .challenger import Challenger
     from .fri import prove_openings
     from .hash import PoseidonHash
@@ -1690,14 +1709,17 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
     # keyword arguments of the three salted commitments (none without zero knowledge)
     salted = [dict(salt_key=salt_keys[i] if salt_keys is not None else "fresh") if zk else {} for i in range(3)]
     public_inputs_hash = [int(x) for x in PoseidonHash.hash_no_pad(np.array(public_inputs, dtype=np.uint64), ctx)]
-    wires_commitment = PolynomialBatch.from_values(wires, cfg.rate_bits, zk, cfg.cap_height, ctx=ctx, **salted[0])
+    on = distributed.shard_kwargs(placement)
+    sharded = distributed.shard_of(placement)[1] > 1
+    wires_commitment = PolynomialBatch.from_values(wires, cfg.rate_bits, zk, cfg.cap_height, ctx=ctx, **salted[0], **on)
     commitments = [wires_commitment]
     try:
         challenger = Challenger()
         prover_data.fri_params.observe(challenger)                     # observe the FRI config
         challenger.observe_hash(prover_data.circuit_digest)            # observe the instance
         challenger.observe_hash(public_inputs_hash)
-        challenger.observe_cap(wires_commitment.merkle_tree.cap)
+        wires_cap = distributed.full_cap(wires_commitment, placement)
+        challenger.observe_cap(wires_cap)
         betas = challenger.get_n_challenges(nc)
         gammas = challenger.get_n_challenges(nc)
         deltas = (betas + gammas + challenger.get_n_challenges(NUM_COINS_LOOKUP * nc - 2 * nc)) if has_lookup else []
@@ -1714,22 +1736,30 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
                 pps += list(out[:-1])
             lookup_polys = compute_all_lookup_polys(wires, nr, cfg.max_quotient_degree_factor, deltas, cd.lookup_rows, nc, ctx)
             zs_commitment = PolynomialBatch.from_values(np.concatenate([np.stack(zs + pps), lookup_polys]), cfg.rate_bits,
-                                                        zk, cfg.cap_height, ctx=ctx, **salted[1])
+                                                        zk, cfg.cap_height, ctx=ctx, **salted[1], **on)
         else:
             wires_dev, sigmas_dev = _to_device(wires[:nr], ctx), _to_device(prover_data.sigmas, ctx)
             zs_commitment = commit_zs_partial_products(wires_dev, sigmas_dev, cd.k_is, betas, gammas,
                                                        cd.quotient_degree_factor, cfg.rate_bits, cfg.cap_height, ctx,
-                                                       **(dict(blinding=True, **salted[1]) if zk else {}))
+                                                       **(dict(blinding=True, **salted[1]) if zk else {}), **on)
         commitments.append(zs_commitment)
-        challenger.observe_cap(zs_commitment.merkle_tree.cap)
+        zs_cap = distributed.full_cap(zs_commitment, placement)
+        challenger.observe_cap(zs_cap)
         alphas = challenger.get_n_challenges(nc)
         cs = prover_data.constants_sigmas_commitment
-        quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas, gammas,
-                                                alphas, deltas)
+        if sharded:
+            quotient_polys = distributed.plonk_quotient_polys_sharded(cd, cs, public_inputs_hash, wires_commitment,
+                                                                      zs_commitment, betas, gammas, alphas, deltas,
+                                                                      placement[1])
+        else:
+            quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas,
+                                                    gammas, alphas, deltas)
         quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx,
-                                                    **(dict(blinding=True, **salted[2]) if zk else {}))
+                                                    **(dict(blinding=True, **salted[2]) if zk else {}), **on)
         commitments.append(quotient_commitment)
-        challenger.observe_cap(quotient_commitment.merkle_tree.cap)
+        del quotient_polys
+        quotient_cap = distributed.full_cap(quotient_commitment, placement)
+        challenger.observe_cap(quotient_cap)
         zeta = challenger.get_extension_challenge()
         g = F.primitive_root_of_unity(cd.degree_bits)
         if F.ext_pow(zeta, 1 << cd.degree_bits) == (1, 0):
@@ -1741,10 +1771,13 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
                                   lookup_range=range(n_zs_pp, n_zs_pp + nc * cd.num_lookup_polys))
         for batch in openings.to_fri_openings():                       # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
-        opening_proof = prove_openings(get_fri_instance(cd, zeta), [cs, wires_commitment, zs_commitment, quotient_commitment],
-                                       challenger, prover_data.fri_params)
-        proof = Proof(wires_commitment.merkle_tree.cap, zs_commitment.merkle_tree.cap, quotient_commitment.merkle_tree.cap,
-                      openings, opening_proof)
+        oracles = [cs, wires_commitment, zs_commitment, quotient_commitment]
+        if sharded:
+            opening_proof = distributed.prove_openings_sharded(get_fri_instance(cd, zeta), oracles, challenger,
+                                                               prover_data.fri_params, placement[1])
+        else:
+            opening_proof = prove_openings(get_fri_instance(cd, zeta), oracles, challenger, prover_data.fri_params)
+        proof = Proof(wires_cap, zs_cap, quotient_cap, openings, opening_proof)
         return ProofWithPublicInputs(proof, public_inputs)
     finally:
         for c in commitments:

@@ -14,6 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _native as N
+from . import distributed as D
 from . import field as F
 from .fri import starky_standard_fast_fri_config
 from .polynomial_batch import PolynomialBatch
@@ -678,43 +679,16 @@ def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx
     if stark.uses_lookups():
         check_lookup_shapes(stark)
         trace = _device_trace(trace, ctx)
-    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx, **_on(placement))
+    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx, **D.shard_kwargs(placement))
     try:
         challenger = Challenger()
         challenger.observe_elements(public_inputs)
         config.observe(challenger)
-        challenger.observe_cap(_full_cap(trace_commitment, placement))
+        challenger.observe_cap(D.full_cap(trace_commitment, placement))
         return prove_with_commitment(stark, config, trace, trace_commitment, None, None, challenger, public_inputs,
                                      params, ctx=ctx, placement=placement)
     finally:
         trace_commitment.close()
-
-
-def _shard(placement):
-    """(g, G) of a placement: this rank's row block of every commitment."""
-    return (0, 1) if placement is None else placement[0]
-
-
-def _on(placement):
-    """The keyword arguments that build a commitment on the placement (none on one device)."""
-    return dict(shard=_shard(placement)) if _shard(placement)[1] > 1 else {}
-
-
-def _full_cap(commitment, placement):
-    """The commitment's Merkle cap; for a row-block shard, every rank's cap entries all-gathered."""
-    if _shard(placement)[1] == 1:
-        return commitment.merkle_tree.cap
-    from .distributed import gather_cap
-
-    group = placement[1]
-    return gather_cap(commitment.merkle_tree.cap, group, device=_comm_device(group, commitment.ctx))
-
-
-def _comm_device(group, ctx):
-    """Where `group`'s collectives take their tensors: the context's GPU under NCCL, the host otherwise."""
-    import torch.distributed as dist
-
-    return "cuda:%d" % ctx.device if dist.get_backend(group) == "nccl" else None
 
 
 def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_challenges, challenger, public_inputs,
@@ -736,7 +710,7 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
     from .lookup import get_grand_product_challenge_set
 
     ctx = ctx or N.default_context()
-    shard = _shard(placement)
+    shard = D.shard_of(placement)
     degree_bits = params.degree_bits
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     uses_lookups = stark.uses_lookups()
@@ -763,12 +737,13 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         elif uses_lookups:
             auxiliary = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
         if uses_lookups or ctl_data is not None:
-            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx, **_on(placement))
+            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx,
+                                                    **D.shard_kwargs(placement))
             commitments.append(aux_commitment)
             del auxiliary
             if ctl_data is not None:
                 ctl_data.auxiliary = None
-            aux_cap = _full_cap(aux_commitment, placement)
+            aux_cap = D.full_cap(aux_commitment, placement)
             challenger.observe_cap(aux_cap)
             quotient_args["auxiliary_polys_commitment"] = aux_commitment
         num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
@@ -785,10 +760,10 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         quotient_commitment = None
         if quotient_polys is not None:
             quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx,
-                                                        **_on(placement))
+                                                        **D.shard_kwargs(placement))
             commitments.append(quotient_commitment)
             del quotient_polys
-            quotient_cap = _full_cap(quotient_commitment, placement)
+            quotient_cap = D.full_cap(quotient_commitment, placement)
             challenger.observe_cap(quotient_cap)
         zeta = challenger.get_extension_challenge()
         if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
@@ -808,7 +783,7 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         else:
             opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
                                            params.final_poly_coeff_len, params.max_num_query_steps)
-        proof = StarkProof(_full_cap(trace_commitment, placement),
+        proof = StarkProof(D.full_cap(trace_commitment, placement),
                            quotient_cap if quotient_commitment is not None else None,
                            openings, opening_proof,
                            aux_cap if aux_commitment is not None else None)

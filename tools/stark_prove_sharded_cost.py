@@ -39,7 +39,7 @@ def _timed_phases(ctx):
 
     times = {}
     # one rank takes stark.prove's path: compute_quotient_polys and prove_openings stand for the sharded steps
-    patches = [(stark_mod, "_commit_trace", "trace_commitment"), (stark_mod, "_full_cap", "cap_gathers"),
+    patches = [(stark_mod, "_commit_trace", "trace_commitment"), (dist_mod, "full_cap", "cap_gathers"),
                (stark_mod, "_bind_constraints", "binding_step"), (dist_mod, "quotient_polys_sharded", "quotient"),
                (stark_mod, "compute_quotient_polys", "quotient"),
                (stark_mod, "commit_quotient_polys", "quotient_commitment"), (proof_mod, "eval_commitments", "openings"),
