@@ -401,8 +401,9 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
             dev_traces.append(dt)
             commitments.append(S._commit_trace(dt, rate_bits, cap_height, ctx))
         challenger = Challenger()
-        for c in commitments:
-            challenger.observe_cap(c.merkle_tree.cap)
+        caps = [c.merkle_tree.cap for c in commitments]
+        for cap in caps:
+            challenger.observe_cap(cap)
         ctl_challenges = get_grand_product_challenge_set(challenger, config.num_challenges)
         nls = [s.num_lookup_helper_columns(config) if s.uses_lookups() else 0 for s in starks]
         ctl_data = cross_table_lookup_data([t if s.requires_ctls() else None for s, t in zip(starks, dev_traces)],
@@ -411,8 +412,8 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
         for i, s in enumerate(starks):
             challenger.observe_elements(public_inputs[i])
             config.observe(challenger)
-            proofs.append(S.prove_with_commitment(s, config, dev_traces[i], commitments[i], ctl_data[i], ctl_challenges,
-                                                  challenger, public_inputs[i], params[i], ctx=ctx))
+            proofs.append(S.prove_with_commitment(s, config, dev_traces[i], commitments[i], caps[i], ctl_data[i],
+                                                  ctl_challenges, challenger, public_inputs[i], params[i], ctx=ctx))
             ctl_data[i] = None
         return MultiStarkProof(proofs)
     finally:

@@ -12,6 +12,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
 #include <map>
 #include <memory>
@@ -2037,6 +2038,19 @@ static uint32_t quotient_degree_bits(uint32_t quotient_degree_factor) {
     while (((size_t)1 << qd_bits) < quotient_degree_factor) qd_bits++;
     return qd_bits;
 }
+// The checks both quotients end with, on commitments of degree 2^db and rate rate_bits in 2^sl shards: the quotient
+// degree against the rate and max_qd, the shard count against the quotient coset. Sets *qd_bits_out.
+static int quotient_shape_check(gl_ctx* ctx, uint32_t db, uint32_t rate_bits, uint32_t sl,
+                                uint32_t quotient_degree_factor, uint32_t max_qd, uint32_t* qd_bits_out) {
+    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
+    if (qd_bits > rate_bits)
+        return set_err(ctx, GL_ERR_UNSUPPORTED, "Having constraints of degree higher than the rate is not supported yet.");
+    if ((1u << qd_bits) > max_qd) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
+    if (sl > db + qd_bits)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", 1u << sl, db + qd_bits);
+    *qd_bits_out = qd_bits;
+    return GL_OK;
+}
 // The checks of gl_stark_quotient[_aux] (whole = true: both LDEs whole on this device) and gl_stark_quotient_shard
 // (whole = false: the trace and the auxiliary commitment are shards of the same index and count). Sets *qd_bits.
 static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
@@ -2059,13 +2073,8 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
             return set_err(ctx, GL_ERR_BAD_SHAPE, "the auxiliary commitment's degree or rate differs from the trace's");
         if (!aux->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the auxiliary commitment");
     }
-    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
-    if (qd_bits > trace->rate_bits)
-        return set_err(ctx, GL_ERR_UNSUPPORTED, "Having constraints of degree higher than the rate is not supported yet.");
-    if ((1u << qd_bits) > GL_STARK_MAX_QD) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
-    if (trace->shard_log > trace->degree_log + qd_bits)
-        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", 1u << trace->shard_log,
-                       trace->degree_log + qd_bits);
+    TRY(quotient_shape_check(ctx, trace->degree_log, trace->rate_bits, trace->shard_log, quotient_degree_factor,
+                             GL_STARK_MAX_QD, qd_bits_out));
     for (uint32_t k = 0; k < n_instr; k++) {  // validate once on the host: the kernel trusts the program
         const gl_stark_instr in = program[k];
         bool ok = true;
@@ -2079,54 +2088,72 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
         }
         if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "constraint program: bad instruction %u", k);
     }
-    *qd_bits_out = qd_bits;
     return GL_OK;
 }
-// The values of commitment c's polynomials (its replicated coefficients) on the coset shift*<w_M>, M = 2^log_M, in leaf
-// order, column k at buf + k*M: a shard's quotient-coset values when its commitment's leaves are another coset
-static int commit_coset_values(gl_ctx* ctx, const gl_commit* c, uint32_t log_M, u64 shift, DevBuf& buf) {
-    const size_t M = (size_t)1 << log_M;
-    TRY(buf.alloc((size_t)c->B * M));
-    return coset_lde_columns(ctx, c->coeffs, c->B, c->degree_log, log_M, shift, buf.get(), M);
+// The part of the quotient coset g*<w_size> (size = 2^(degree_log + qd_bits)) that a commitment's shard evaluates: shard
+// g of G = 2^sl owns the M = size / G points g*w_size^r*<w_M>, r = the sl-bit reversal of g (the whole coset for an
+// unsharded commitment)
+struct QuotientCoset {
+    uint32_t size_log, log_M;
+    size_t size, M, r;
+    u64 w_size, shift;
+    // The local values are read in place when the shard's coset is its commitment's -- always on one device (the
+    // LDE's first `size` leaves), and on every shard when the quotient coset is the LDE coset. Else the LDE onto it.
+    bool local_in_place;
+    // The next row, point i + 2^qd_bits, lies in the same shard when G divides 2^qd_bits: local point k + 2^qd_bits / G.
+    // Else the values on the coset times w_n.
+    bool next_in_shard;
+};
+static QuotientCoset quotient_coset(const gl_commit* c, uint32_t qd_bits) {
+    QuotientCoset q;
+    const uint32_t sl = c->shard_log;
+    q.size_log = c->degree_log + qd_bits;
+    q.log_M = q.size_log - sl;
+    q.size = (size_t)1 << q.size_log;
+    q.M = (size_t)1 << q.log_M;
+    q.r = bitrev32(c->shard_index, sl);
+    q.w_size = root_of_unity(q.size_log);
+    q.shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(q.w_size, q.r));
+    q.local_in_place = sl == 0 || qd_bits == c->rate_bits;
+    q.next_in_shard = sl <= qd_bits;
+    return q;
+}
+// Where a quotient kernel reads a commitment's values: column k at p + k*stride, leaf order
+struct ColumnsView {
+    const u64* p = nullptr;
+    size_t stride = 0;
+};
+// Commitment c's values on the coset q (*local) and, when want_next, at the next row (*next): local values in place
+// or the LDE of its replicated coefficients onto the coset, in lbuf; the next row from the local values when it lies
+// in the shard, else the LDE onto the coset times w_n, in nbuf
+static int quotient_views(gl_ctx* ctx, const QuotientCoset& q, const gl_commit* c, bool want_next, DevBuf& lbuf,
+                          DevBuf& nbuf, ColumnsView* local, ColumnsView* next) {
+    auto values_on = [&](u64 shift, DevBuf& buf, ColumnsView* v) -> int {
+        TRY(buf.alloc((size_t)c->B * q.M));
+        TRY(coset_lde_columns(ctx, c->coeffs, c->B, c->degree_log, q.log_M, shift, buf.get(), q.M));
+        *v = {buf.get(), q.M};
+        return GL_OK;
+    };
+    if (q.local_in_place) *local = {c->tree.leaves, c->tree.es};
+    else TRY(values_on(q.shift, lbuf, local));
+    if (!want_next) return GL_OK;
+    if (q.next_in_shard) *next = *local;
+    else TRY(values_on(mul(q.shift, root_of_unity(c->degree_log)), nbuf, next));
+    return GL_OK;
 }
 // C(x)/Z_H(x) on the trace handle's shard of the quotient coset (the whole coset for an unsharded handle): M values per
 // challenge in local natural order, at out + a*M. Division by zero sets bit 1 of dflag.
 static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
                                  uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                                  uint32_t n_alphas, uint32_t qd_bits, uint64_t* out, const DevBuf& dflag) {
-    const uint32_t db = trace->degree_log, size_log = db + qd_bits, sl = trace->shard_log, log_M = size_log - sl;
-    const size_t size = (size_t)1 << size_log, M = (size_t)1 << log_M;
-    const size_t r = bitrev32(trace->shard_index, sl);
-    const u64 w_size = root_of_unity(size_log);
-    const u64 shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(w_size, r));  // this shard's coset g*w_size^r*<w_M>
-    // The local values: in place when the shard's coset is its commitment's -- always on one device (the LDE's first
-    // `size` leaves), and on every shard when the quotient coset is the LDE coset. Else the LDE onto the coset.
-    const bool local_in_place = sl == 0 || qd_bits == trace->rate_bits;
-    // The next row, point i + 2^qd_bits, lies in the same shard when G divides 2^qd_bits: local point k + 2^qd_bits / G.
-    // Else the values on the coset times w_n.
-    const bool next_in_local = sl <= qd_bits;
+    const uint32_t db = trace->degree_log, sl = trace->shard_log;
+    const QuotientCoset q = quotient_coset(trace, qd_bits);
     DevBuf dprog(ctx), dconst(ctx), xtab(ctx), tl(ctx), tn(ctx), al(ctx), an(ctx);
-    struct View {
-        const u64* p;
-        size_t stride;
-    };
-    auto values_on = [&](gl_commit* c, u64 s, DevBuf& buf, View* v) -> int {
-        TRY(commit_coset_values(ctx, c, log_M, s, buf));
-        *v = {buf.get(), M};
-        return GL_OK;
-    };
-    auto views = [&](gl_commit* c, DevBuf& lbuf, DevBuf& nbuf, View* vl, View* vn) -> int {
-        if (local_in_place) *vl = {c->tree.leaves, c->tree.es};
-        else TRY(values_on(c, shift, lbuf, vl));
-        if (next_in_local) *vn = *vl;
-        else TRY(values_on(c, mul(shift, root_of_unity(db)), nbuf, vn));
-        return GL_OK;
-    };
-    View trl, trn, axl = {nullptr, 0}, axn = {nullptr, 0};
-    TRY(views(trace, tl, tn, &trl, &trn));
-    if (aux) TRY(views(aux, al, an, &axl, &axn));
+    ColumnsView trl, trn, axl, axn;
+    TRY(quotient_views(ctx, q, trace, true, tl, tn, &trl, &trn));
+    if (aux) TRY(quotient_views(ctx, q, aux, true, al, an, &axl, &axn));
     TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_stark_instr), consts, n_consts, dprog, dconst));
-    TRY(x_pow_tables(ctx, w_size, size, xtab));
+    TRY(x_pow_tables(ctx, q.w_size, q.size, xtab));
     StarkQuotientParams p;
     p.loc = trl.p;
     p.loc_stride = trl.stride;
@@ -2136,10 +2163,10 @@ static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, 
     p.aux_loc_stride = axl.stride;
     p.aux_nxt = axn.p;
     p.aux_nxt_stride = axn.stride;
-    p.log_M = log_M;
+    p.log_M = q.log_M;
     p.shard_log = sl;
-    p.r = r;
-    p.next_off = next_in_local ? ((size_t)1 << (qd_bits - sl)) : 0;
+    p.r = q.r;
+    p.next_off = q.next_in_shard ? ((size_t)1 << (qd_bits - sl)) : 0;
     p.degree_bits = db;
     p.qd_bits = qd_bits;
     p.prog = (const gl_stark_instr*)dprog.get();
@@ -2148,14 +2175,14 @@ static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, 
     p.n_alphas = n_alphas;
     for (uint32_t a = 0; a < GL_STARK_MAX_ALPHAS; a++) p.alphas[a] = a < n_alphas ? canon(alphas[a]) : 0;
     p.xhi = xtab.get();
-    p.xlo = xtab.get() + x_pow_table_len(size);
+    p.xlo = xtab.get() + x_pow_table_len(q.size);
     p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
     p.last = gl::inv(root_of_unity(db));
     p.n_field = canon((u64)1 << db);
     zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
     p.out = out;
     p.flag = (unsigned int*)dflag.get();
-    k_stark_quotient<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p);
+    k_stark_quotient<<<(unsigned)((q.M + 127) / 128), 128, 0, ctx->stream>>>(p);
     CKL(ctx);
     return GL_OK;
 }
@@ -2176,45 +2203,49 @@ static int quotient_coeffs(gl_ctx* ctx, uint64_t* coeffs, uint32_t degree_bits, 
     }
     return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
 }
-// gl_stark_quotient and gl_stark_quotient_aux (aux = NULL: the program may not read auxiliary columns)
-static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
-                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
-                          uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
-    uint32_t qd_bits = 0;
-    TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor,
-                             out_coeffs, true, &qd_bits));
+// What every quotient entry point runs after its checks, on its context's device: values(dflag) writes the values on
+// this device's shard of the quotient coset to `out`; then, for the whole coset, the coefficients in place
+// (quotient_coeffs), else the flags alone
+static int run_quotient(gl_ctx* ctx, bool whole, uint64_t* out, uint32_t degree_bits, uint32_t n_alphas,
+                        uint32_t quotient_degree_factor, const std::function<int(const DevBuf&)>& values) {
     CK(ctx, cudaSetDevice(ctx->device));
     DevBuf dflag(ctx);
     TRY(flag_alloc(ctx, dflag));
-    TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out_coeffs,
-                              dflag));
-    return quotient_coeffs(ctx, out_coeffs, trace->degree_log, n_alphas, quotient_degree_factor, dflag);
+    TRY(values(dflag));
+    if (!whole) return flag_status(ctx, dflag, {INVERT_ZERO});
+    return quotient_coeffs(ctx, out, degree_bits, n_alphas, quotient_degree_factor, dflag);
+}
+// gl_stark_quotient and gl_stark_quotient_aux (whole; aux = NULL: the program may not read auxiliary columns), and
+// gl_stark_quotient_shard (!whole: the values on the shard's part of the coset)
+static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                          const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
+                          uint32_t quotient_degree_factor, uint64_t* out, bool whole) {
+    uint32_t qd_bits = 0;
+    TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor, out,
+                             whole, &qd_bits));
+    return run_quotient(ctx, whole, out, trace->degree_log, n_alphas, quotient_degree_factor, [&](const DevBuf& dflag) {
+        return stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out,
+                                     dflag);
+    });
 }
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
                       const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
                       uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
     return stark_quotient(ctx, trace, nullptr, program, n_instr, consts, n_consts, alphas, n_alphas,
-                          quotient_degree_factor, out_coeffs);
+                          quotient_degree_factor, out_coeffs, true);
 }
 int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
                           const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
                           uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
     if (!aux) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     return stark_quotient(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, quotient_degree_factor,
-                          out_coeffs);
+                          out_coeffs, true);
 }
 int gl_stark_quotient_shard(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                             uint32_t n_alphas, uint32_t quotient_degree_factor, uint64_t* out_values) {
-    uint32_t qd_bits = 0;
-    TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor,
-                             out_values, false, &qd_bits));
-    CK(ctx, cudaSetDevice(ctx->device));
-    DevBuf dflag(ctx);
-    TRY(flag_alloc(ctx, dflag));
-    TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out_values,
-                              dflag));
-    return flag_status(ctx, dflag, {INVERT_ZERO});
+    return stark_quotient(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, quotient_degree_factor,
+                          out_values, false);
 }
 int gl_stark_quotient_from_shards(gl_ctx* ctx, const uint64_t* values, uint32_t num_shards, uint32_t n_alphas,
                                   uint32_t degree_bits, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
@@ -2431,15 +2462,10 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
         if (commits[c]->degree_log != commits[0]->degree_log || commits[c]->rate_bits != commits[0]->rate_bits)
             return set_err(ctx, GL_ERR_BAD_SHAPE, "commitments of different degree or rate");
     }
-    const uint32_t db = commits[0]->degree_log, rate_bits = commits[0]->rate_bits, sl = commits[0]->shard_log;
-    const uint32_t qd_bits = quotient_degree_bits(quotient_degree_factor);
-    if (qd_bits > rate_bits)
-        return set_err(ctx, GL_ERR_UNSUPPORTED, "Having constraints of degree higher than the rate is not supported yet.");
-    if ((1u << qd_bits) > GL_VP_MAX_QD) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient degree factor too large");
-    if (sl > db + qd_bits)
-        return set_err(ctx, GL_ERR_BAD_SHAPE, "%u shards of a quotient coset of 2^%u points", 1u << sl, db + qd_bits);
+    TRY(quotient_shape_check(ctx, commits[0]->degree_log, commits[0]->rate_bits, commits[0]->shard_log,
+                             quotient_degree_factor, GL_VP_MAX_QD, qd_bits_out));
     // a shard whose quotient coset is not its LDE coset reads values computed from the coefficients: no salt columns
-    const bool in_place = sl == 0 || qd_bits == rate_bits;
+    const bool in_place = quotient_coset(commits[0], *qd_bits_out).local_in_place;
     uint32_t next_mask = 0;
     {  // validate once on the host: the kernel trusts the program (operands in range, no register read before it is written)
         bool written[GL_VP_MAX_REGS] = {false};
@@ -2463,7 +2489,6 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
             if (in.op != GL_VP_TERM) written[in.dst] = true;
         }
     }
-    *qd_bits_out = qd_bits;
     *next_mask_out = next_mask;
     return GL_OK;
 }
@@ -2474,35 +2499,19 @@ static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_
                                  uint32_t n_alphas, uint32_t n_terms, uint32_t qd_bits, uint32_t next_mask, uint64_t* out,
                                  const DevBuf& dflag) {
     const gl_commit* c0 = commits[0];
-    const uint32_t db = c0->degree_log, size_log = db + qd_bits, sl = c0->shard_log, log_M = size_log - sl;
-    const size_t size = (size_t)1 << size_log, M = (size_t)1 << log_M;
-    const u64 w_size = root_of_unity(size_log);
-    // this shard's coset g*w_size^r*<w_M>, r = the sl-bit reversal of the shard index
-    const u64 shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(w_size, bitrev32(c0->shard_index, sl)));
-    // The local values: in place when the shard's coset is its commitments' -- always on one device (the LDE's first
-    // `size` leaves), and on every shard when the quotient coset is the LDE coset. Else the LDE onto the coset.
-    const bool local_in_place = sl == 0 || qd_bits == c0->rate_bits;
-    // The next row, point i + 2^qd_bits, lies in the same shard when G divides 2^qd_bits. Else the values on the coset
-    // times w_n, for the commitments the program reads there.
-    const bool next_in_shard = sl <= qd_bits;
+    const uint32_t db = c0->degree_log;
+    const QuotientCoset q = quotient_coset(c0, qd_bits);
     VanishingParams p;
-    std::vector<DevBuf> bufs;
-    bufs.reserve(2 * GL_VP_MAX_COMMITS);
+    std::vector<DevBuf> bufs;  // per commitment: its values on the coset, and at the next row
+    for (uint32_t k = 0; k < 2 * n_commits; k++) bufs.emplace_back(ctx);
     for (uint32_t c = 0; c < GL_VP_MAX_COMMITS; c++) {
-        p.lde[c] = c < n_commits && local_in_place ? commits[c]->tree.leaves : nullptr;
-        p.lde_stride[c] = c < n_commits && local_in_place ? commits[c]->tree.es : 0;
-        if (c < n_commits && !local_in_place) {
-            bufs.emplace_back(ctx);
-            TRY(commit_coset_values(ctx, commits[c], log_M, shift, bufs.back()));
-            p.lde[c] = bufs.back().get();
-            p.lde_stride[c] = M;
-        }
-        if (c < n_commits && !next_in_shard && ((next_mask >> c) & 1)) {
-            bufs.emplace_back(ctx);
-            TRY(commit_coset_values(ctx, commits[c], log_M, mul(shift, root_of_unity(db)), bufs.back()));
-            p.nxt[c] = bufs.back().get();
-            p.nxt_stride[c] = M;
-        }
+        ColumnsView loc, nxt;  // only the next rows the program reads
+        if (c < n_commits)
+            TRY(quotient_views(ctx, q, commits[c], (next_mask >> c) & 1, bufs[2 * c], bufs[2 * c + 1], &loc, &nxt));
+        p.lde[c] = loc.p;
+        p.lde_stride[c] = loc.stride;
+        p.nxt[c] = nxt.p;
+        p.nxt_stride[c] = nxt.stride;
     }
     DevBuf dprog(ctx), dconst(ctx), dapow(ctx), xtab(ctx);
     TRY(upload_program(ctx, program, (size_t)n_instr * sizeof(gl_vp_instr), consts, n_consts, dprog, dconst));
@@ -2513,7 +2522,7 @@ static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_
     }
     TRY(dapow.alloc(apow.size()));
     TRY(h2d(ctx, dapow.get(), apow.data(), apow.size()));
-    TRY(x_pow_tables(ctx, w_size, size, xtab));
+    TRY(x_pow_tables(ctx, q.w_size, q.size, xtab));
     p.log_N = db + c0->rate_bits;
     p.degree_bits = db;
     p.qd_bits = qd_bits;
@@ -2524,45 +2533,43 @@ static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_
     p.n_alphas = n_alphas;
     p.n_terms = n_terms;
     p.xhi = xtab.get();
-    p.xlo = xtab.get() + x_pow_table_len(size);
+    p.xlo = xtab.get() + x_pow_table_len(q.size);
     p.shift = MULTIPLICATIVE_GROUP_GENERATOR;
     p.n_field = canon((u64)1 << db);
     for (uint32_t j = 0; j < GL_VP_MAX_QD; j++) p.zh[j] = p.zh_inv[j] = 0;
     zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
     p.out = out;
     p.flag = (unsigned int*)dflag.get();
-    p.row0 = (size_t)c0->shard_index << log_M;
-    p.shard_log = sl;
-    p.next_in_shard = next_in_shard;
-    k_plonk_quotient<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p);
+    p.row0 = (size_t)c0->shard_index << q.log_M;
+    p.shard_log = c0->shard_log;
+    p.next_in_shard = q.next_in_shard;
+    k_plonk_quotient<<<(unsigned)((q.M + 127) / 128), 128, 0, ctx->stream>>>(p);
     CKL(ctx);
     return GL_OK;
+}
+// gl_plonk_quotient (whole) and gl_plonk_quotient_shard (!whole: the values on the shard's part of the coset)
+static int plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                          uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
+                          uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out, bool whole) {
+    uint32_t qd_bits = 0, next_mask = 0;
+    TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
+                             quotient_degree_factor, out, whole, &qd_bits, &next_mask));
+    return run_quotient(ctx, whole, out, commits[0]->degree_log, n_alphas, quotient_degree_factor, [&](const DevBuf& dflag) {
+        return plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas,
+                                     n_terms, qd_bits, next_mask, out, dflag);
+    });
 }
 int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                       uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                       uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
-    uint32_t qd_bits = 0, next_mask = 0;
-    TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
-                             quotient_degree_factor, out_coeffs, true, &qd_bits, &next_mask));
-    CK(ctx, cudaSetDevice(ctx->device));
-    DevBuf dflag(ctx);
-    TRY(flag_alloc(ctx, dflag));
-    TRY(plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
-                              qd_bits, next_mask, out_coeffs, dflag));
-    return quotient_coeffs(ctx, out_coeffs, commits[0]->degree_log, n_alphas, quotient_degree_factor, dflag);
+    return plonk_quotient(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
+                          quotient_degree_factor, out_coeffs, true);
 }
 int gl_plonk_quotient_shard(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                             uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_values) {
-    uint32_t qd_bits = 0, next_mask = 0;
-    TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
-                             quotient_degree_factor, out_values, false, &qd_bits, &next_mask));
-    CK(ctx, cudaSetDevice(ctx->device));
-    DevBuf dflag(ctx);
-    TRY(flag_alloc(ctx, dflag));
-    TRY(plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
-                              qd_bits, next_mask, out_values, dflag));
-    return flag_status(ctx, dflag, {INVERT_ZERO});
+    return plonk_quotient(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
+                          quotient_degree_factor, out_values, false);
 }
 
 void gl_poseidon_permute_host(uint64_t state[12]) {

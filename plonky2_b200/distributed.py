@@ -7,10 +7,11 @@ No LDE data ever crosses NVLink: shard g of G evaluates every column on its own 
 (g_shift * w_N^{bitrev(g)}) <w_{N/G}>, hashes its leaves and reduces its own cap subtrees.
 
 prove_stark proves one STARK, and prove_plonk one plonky2 circuit, on the ranks of a group with these shards: besides
-the caps, only the quotient's values on each rank's shard of the quotient coset (quotient_polys_sharded,
-plonk_quotient_polys_sharded) and the FRI query openings (prove_openings_sharded) cross ranks. Both provers take a
-`placement` ((g, G), group) -- None on one device -- and build their commitments with shard_of / shard_kwargs / full_cap."""
-import ctypes as C
+the caps, only the quotient's values on each rank's shard of the quotient coset (Placement.quotient_from_shards) and
+the FRI query openings (Placement.open_many) cross ranks. Both provers take a Placement -- Placement() on one device --
+and never ask themselves whether there is more than one rank. prove_openings_sharded is fri.prove_openings on the
+oracles' own shards, for a caller that commits the shards itself."""
+from dataclasses import dataclass
 
 import numpy as np
 
@@ -59,67 +60,127 @@ def gather_cap(local_cap, group=None, device=None):
     return MerkleCap(full.copy())
 
 
-def open_sharded(batch, leaf_indices, group=None):
-    """MerkleTree::get + prove (merkle_tree.rs:226-237) for GLOBAL leaf indices of a row-block sharded
-    PolynomialBatch: every rank opens the indices it owns on its own GPU (local index, local cap subtree --
-    the sibling path is the same as in the single-device tree) and the ranks all-gather the results.
-    Collective: every rank must call it with the same indices. Returns (leaves (q, W), paths (q, L, 4))."""
-    import torch.distributed as dist
+@dataclass(frozen=True)
+class Placement:
+    """Where a prover's commitments live: row block `shard_index` of `num_shards` of every commitment, one block per rank
+    of the torch.distributed `group`. Placement() is one device. The provers build every commitment with
+    `commit_kwargs`, observe `cap`, and run the quotient and FRI with `step_kwargs` (fri.prove_openings opens its
+    queries with `open_many`); the two compute_quotient_polys pick their C entry point by num_shards and, with several
+    ranks, gather the quotient with `quotient_from_shards`. Nothing else in the provers tests whether there is more
+    than one rank. On one device both keyword sets are empty, so every call a prover makes is the plain single-device
+    call."""
+    shard_index: int = 0
+    num_shards: int = 1
+    group: object = None
 
-    idx = [int(i) for i in leaf_indices]
-    G = batch.num_shards
-    mine = [(k, owner_of_leaf(i, batch.lde_size, G)[1]) for k, i in enumerate(idx)
-            if owner_of_leaf(i, batch.lde_size, G)[0] == batch.shard_index]
-    lv, pt = batch.merkle_tree.open_many([loc for _, loc in mine])
-    part = [(k, lv[j], pt[j]) for j, (k, _) in enumerate(mine)]
-    if G == 1 or not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
-        parts = [part]
-    else:
-        parts = [None] * dist.get_world_size(group)
-        dist.all_gather_object(parts, part, group=group)
-    layers = batch.degree_log + batch.rate_bits - batch.cap_height
-    leaves = np.empty((len(idx), batch.leaf_width), dtype=np.uint64)
-    paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
-    seen = 0
-    for p in parts:
-        for k, l, q in p:
-            leaves[k], paths[k] = l, q
-            seen += 1
-    if seen != len(idx):
-        raise RuntimeError("sharded opening: %d of %d indices were served" % (seen, len(idx)))
-    return leaves, paths
+    @property
+    def shard(self):
+        """(g, G): the shard= of every commitment on this placement; (0, 1) builds the unsharded commitment."""
+        return self.shard_index, self.num_shards
+
+    @property
+    def commit_kwargs(self):
+        """The keyword arguments that build a commitment on this placement: shard=(g, G), or none on one device, whose
+        default is the unsharded commitment."""
+        return {} if self.num_shards == 1 else dict(shard=self.shard)
+
+    @property
+    def step_kwargs(self):
+        """The keyword arguments that run compute_quotient_polys or fri.prove_openings on this placement: placement=self,
+        or none on one device, their default."""
+        return {} if self.num_shards == 1 else dict(placement=self)
+
+    def cap(self, commitment):
+        """The commitment's full Merkle cap: its own on one device, every rank's cap entries all-gathered otherwise."""
+        if self.num_shards == 1:
+            return commitment.merkle_tree.cap
+        return gather_cap(commitment.merkle_tree.cap, self.group, device=_comm_device(self.group, commitment.ctx))
+
+    def open_many(self, batch, leaf_indices):
+        """MerkleTree::get + prove (merkle_tree.rs:226-237) for GLOBAL leaf indices of `batch`. Returns (leaves (q, W),
+        paths (q, L, 4)). On one device the tree opens them itself. With several ranks every rank opens the indices it
+        owns on its own GPU (local index, local cap subtree -- the sibling path is the same as in the single-device tree)
+        and the ranks all-gather the results: every rank must call it with the same indices."""
+        if self.num_shards == 1:
+            return batch.merkle_tree.open_many(leaf_indices)
+        import torch.distributed as dist
+
+        idx = [int(i) for i in leaf_indices]
+        G = self.num_shards
+        mine = [(k, owner_of_leaf(i, batch.lde_size, G)[1]) for k, i in enumerate(idx)
+                if owner_of_leaf(i, batch.lde_size, G)[0] == self.shard_index]
+        lv, pt = batch.merkle_tree.open_many([loc for _, loc in mine])
+        part = [(k, lv[j], pt[j]) for j, (k, _) in enumerate(mine)]
+        if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(self.group) == 1:
+            parts = [part]
+        else:
+            parts = [None] * dist.get_world_size(self.group)
+            dist.all_gather_object(parts, part, group=self.group)
+        layers = batch.degree_log + batch.rate_bits - batch.cap_height
+        leaves = np.empty((len(idx), batch.leaf_width), dtype=np.uint64)
+        paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
+        seen = 0
+        for p in parts:
+            for k, l, q in p:
+                leaves[k], paths[k] = l, q
+                seen += 1
+        if seen != len(idx):
+            raise RuntimeError("sharded opening: %d of %d indices were served" % (seen, len(idx)))
+        return leaves, paths
+
+    def quotient_from_shards(self, ctx, run_shard, n_alphas, degree_bits, quotient_degree_factor):
+        """The quotient's coefficients from the ranks' shards of its values. run_shard(local) writes this rank's values on
+        its shard of the quotient coset into `local`, an (n_alphas, size / G) int64 CUDA tensor, through its C entry
+        point. Then the ranks all-gather the values and every rank interpolates the whole quotient
+        (gl_stark_quotient_from_shards). Collective. Returns the same (n_alphas, size) tensor on every rank. A failure on
+        one rank raises on every rank: its own exception there, NativeError elsewhere."""
+        import torch
+
+        from . import _native as N
+
+        size = (1 << degree_bits) << (quotient_degree_factor - 1).bit_length()
+        dev = "cuda:%d" % ctx.device
+        local = torch.empty((n_alphas, size // self.num_shards), dtype=torch.int64, device=dev)
+        failure = None
+        try:
+            run_shard(local)
+        except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
+            failure = e
+        self._agree_on_failure(failure, ctx, N.NativeError, "the quotient failed on rank %d")
+        values = all_gather_tensor(local, self.group)
+        out = torch.empty((n_alphas, size), dtype=torch.int64, device=dev)
+        N.check(N.lib().gl_stark_quotient_from_shards(ctx.h, N.vp(values.data_ptr()), self.num_shards, n_alphas,
+                                                      degree_bits, quotient_degree_factor, N.vp(out.data_ptr())), ctx.h)
+        ctx.synchronize()
+        return out
+
+    def _agree_on_failure(self, failure, ctx, error, message):
+        """Every rank learns whether any rank failed. `failure` (an exception, or None) is raised on its own rank, and
+        error(message % the first failed rank) on every other rank when one failed. Collective with several ranks: call
+        it before any collective that a failed rank would skip, so that no rank waits for one that has raised."""
+        if self.num_shards > 1:
+            import torch
+
+            flag = torch.tensor([int(failure is not None)], dtype=torch.int64,
+                                device=_comm_device(self.group, ctx) or "cpu")
+            failed = all_gather_tensor(flag, self.group).view(-1)
+        if failure is not None:
+            raise failure
+        if self.num_shards > 1 and int(failed.sum()):
+            raise error(message % int(torch.nonzero(failed)[0]))
 
 
 def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None, final_poly_coeff_len=None,
                            max_num_query_steps=None):
-    """prove_openings (oracle.rs:176-237) when the initial oracles are row-block sharded over the ranks.
-    Coefficients are replicated (every rank ran the iNTT), so every rank runs the (small, single-column) FRI
-    commit phase and the transcript redundantly and deterministically; only the initial-tree openings cross
-    ranks. The returned FriProof is identical on every rank and byte-identical to the single-device proof.
-    The caller must already have observed the FULL caps (gather_cap) in `challenger`. final_poly_coeff_len /
-    max_num_query_steps: as in fri.prove_openings (a verifier circuit's shape)."""
-    from . import fri as F
+    """fri.prove_openings when the initial oracles are this rank's row-block shards of `group`: the Placement of the
+    oracles' shard, whose open_many routes the query openings between the ranks. Collective; the caller must already
+    have observed the full caps (gather_cap) in `challenger`. Returns the same FriProof on every rank, byte-identical to
+    the single-device proof."""
+    from .fri import prove_openings
 
-    alpha = challenger.get_extension_challenge()
-    state = F._begin(instance, oracles, alpha, fri_params)
-    try:
-        caps, final_coeffs = F.fri_committed_trees(state, challenger, fri_params, final_poly_coeff_len,
-                                                   max_num_query_steps)
-        pow_witness = F.fri_proof_of_work(challenger, fri_params.config, state.ctx)
-        n = fri_params.lde_size()
-
-        class _Routed:  # quacks like PolynomialBatch for fri_prover_query_rounds
-            def __init__(self, b):
-                self.merkle_tree = self
-                self._b = b
-
-            def open_many(self, indices):
-                return open_sharded(self._b, indices, group)
-
-        rounds, _ = F.fri_prover_query_rounds([_Routed(o) for o in oracles], state, challenger, n, fri_params)
-        return F.FriProof(caps, rounds, final_coeffs, pow_witness)
-    finally:
-        state.close()
+    placement = Placement(oracles[0].shard_index, oracles[0].num_shards, group)
+    return prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len, max_num_query_steps,
+                          placement=placement)
 
 
 def all_gather_tensor(t, group=None):
@@ -138,25 +199,6 @@ def all_gather_tensor(t, group=None):
     return out
 
 
-def shard_of(placement):
-    """(g, G) of a prover's placement ((g, G), group): this rank's row block of every commitment; (0, 1) on one device
-    (placement None)."""
-    return (0, 1) if placement is None else placement[0]
-
-
-def shard_kwargs(placement):
-    """The keyword arguments that build a commitment on the placement (none on one device)."""
-    return dict(shard=shard_of(placement)) if shard_of(placement)[1] > 1 else {}
-
-
-def full_cap(commitment, placement):
-    """The commitment's Merkle cap; for a row-block shard, every rank's cap entries all-gathered."""
-    if shard_of(placement)[1] == 1:
-        return commitment.merkle_tree.cap
-    group = placement[1]
-    return gather_cap(commitment.merkle_tree.cap, group, device=_comm_device(group, commitment.ctx))
-
-
 def _comm_device(group, ctx):
     """Where `group`'s collectives take their tensors: the context's GPU under NCCL, the host otherwise."""
     import torch.distributed as dist
@@ -164,84 +206,24 @@ def _comm_device(group, ctx):
     return "cuda:%d" % ctx.device if dist.get_backend(group) == "nccl" else None
 
 
-def _quotient_from_shards(ctx, run_shard, n_alphas, degree_bits, quotient_degree_factor, num_shards, group):
-    """The steps both sharded quotients share. run_shard(local) writes this rank's shard values into `local`, an
-    (n_alphas, size / G) int64 CUDA tensor, through its C entry point. Then every rank learns whether any shard failed,
-    the ranks all-gather the values, and every rank interpolates the whole quotient (gl_stark_quotient_from_shards).
-    Collective. A failure on one rank raises on every rank: its own exception there, NativeError elsewhere."""
+def _world_size(group):
+    """The number of ranks in `group`: 1 without an initialised process group."""
+    import torch.distributed as dist
+
+    return dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+
+
+def _placement(group, ctx):
+    """This rank's Placement in `group` (Placement() with one rank or without an initialised process group), and its
+    context: `ctx`, or the current CUDA device's when None."""
     import torch
+    import torch.distributed as dist
 
     from . import _native as N
 
-    size = (1 << degree_bits) << (quotient_degree_factor - 1).bit_length()
-    dev = "cuda:%d" % ctx.device
-    local = torch.empty((n_alphas, size // num_shards), dtype=torch.int64, device=dev)
-    failure = None
-    try:
-        run_shard(local)
-    except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
-        failure = e
-    failed = all_gather_tensor(torch.tensor([int(failure is not None)], dtype=torch.int64, device=dev), group)
-    if failure is not None:
-        raise failure
-    if int(failed.sum()):
-        raise N.NativeError("the quotient failed on rank %d" % int(torch.nonzero(failed.view(-1))[0]))
-    values = all_gather_tensor(local, group)
-    out = torch.empty((n_alphas, size), dtype=torch.int64, device=dev)
-    N.check(N.lib().gl_stark_quotient_from_shards(ctx.h, N.vp(values.data_ptr()), num_shards, n_alphas, degree_bits,
-                                                  quotient_degree_factor, N.vp(out.data_ptr())), ctx.h)
-    ctx.synchronize()
-    return out
-
-
-def quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, group=None, auxiliary_polys_commitment=None,
-                           lookup_challenges=None, ctl_vars=None):
-    """stark.compute_quotient_polys when the trace (and auxiliary) commitments are this rank's row-block shard: each rank
-    evaluates C(x)/Z_H(x) on its shard of the quotient coset (gl_stark_quotient_shard), the ranks all-gather the values,
-    and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same torch
-    tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
-    from . import _native as N
-    from .stark import quotient_program
-
-    qdf = stark.quotient_degree_factor()
-    if qdf == 0:
-        return None
-    b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
-                                     ctl_vars)
-    ctx = trace_commitment.ctx
-    aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
-
-    def run_shard(local):
-        N.check(N.lib().gl_stark_quotient_shard(ctx.h, trace_commitment.h, aux_h, b.program(), len(b.instrs),
-                                                N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
-                                                N.vp(local.data_ptr())), ctx.h)
-
-    return _quotient_from_shards(ctx, run_shard, len(al), trace_commitment.degree_log, qdf, trace_commitment.num_shards,
-                                 group)
-
-
-def plonk_quotient_polys_sharded(common_data, constants_sigmas_commitment, public_inputs_hash, wires_commitment,
-                                 zs_partial_products_commitment, betas, gammas, alphas, deltas=(), group=None):
-    """plonk.compute_quotient_polys when the three commitments are this rank's row-block shard: each rank evaluates the
-    vanishing polynomial over Z_H on its shard of the quotient coset (gl_plonk_quotient_shard), the ranks all-gather the
-    values, and every rank interpolates the whole quotient (gl_stark_quotient_from_shards). Collective. Returns the same
-    torch tensor on every rank, equal to compute_quotient_polys's; a failure on any rank raises on every rank."""
-    from . import _native as N
-    from .plonk import quotient_program
-
-    commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
-    prog, consts, al = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas)
-    ctx = wires_commitment.ctx
-    handles = (C.c_void_p * 3)(*[c.h for c in commits])
-    qdf = common_data.quotient_degree_factor
-
-    def run_shard(local):
-        N.check(N.lib().gl_plonk_quotient_shard(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts),
-                                                N.np_ptr(al), len(al), common_data.num_vanishing_terms(), qdf,
-                                                N.vp(local.data_ptr())), ctx.h)
-
-    return _quotient_from_shards(ctx, run_shard, len(al), common_data.degree_bits, qdf, wires_commitment.num_shards,
-                                 group)
+    world = _world_size(group)
+    placement = Placement(dist.get_rank(group), world, group) if world > 1 else Placement()
+    return placement, ctx if ctx is not None else N.default_context(torch.cuda.current_device())
 
 
 def _check_world(what, cap_height, world):
@@ -274,18 +256,10 @@ def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circui
     of at most 2^cap_height, and the Stark must not take part in cross-table lookups (ShapeError otherwise, on every
     rank). Without an initialised process group, or with one rank, this is stark.prove. ctx: this rank's context
     (default: the current CUDA device's)."""
-    import torch.distributed as dist
-
-    from . import _native as N
     from . import stark as S
 
-    world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
-    check_prove_stark(stark, config, world)
-    if ctx is None:
-        import torch
-
-        ctx = N.default_context(torch.cuda.current_device())
-    placement = ((dist.get_rank(group), world), group) if world > 1 else None
+    check_prove_stark(stark, config, _world_size(group))
+    placement, ctx = _placement(group, ctx)
     return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement)
 
 
@@ -324,36 +298,27 @@ def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=
     Zero knowledge: salt_keys (three 32-byte keys, equal on every rank) give the bytes of
     prove_with_witness(..., salt_keys=salt_keys), since a keyed shard holds the unsharded commitment's salted leaves. With
     None ("fresh" keys) each rank draws its own key for its own rows, without a collective: a leaf's salt is only ever
-    read by the rank that owns the leaf (open_sharded), so the proof is valid and hiding, but no single-device run
+    read by the rank that owns the leaf (Placement.open_many), so the proof is valid and hiding, but no single-device run
     reproduces it."""
-    import torch
     import torch.distributed as dist
 
     from . import _native as N
     from . import plonk as P
 
-    world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    world = _world_size(group)
     rank = dist.get_rank(group) if world > 1 else 0
     _check_world("prove_plonk", common_data.config.cap_height, world)
     refusal = None
     try:
         _check_constants_sigmas_shard(prover_data, rank, world)
     except N.ShapeError as e:
+        if world == 1:
+            raise
         refusal = e
-    if world == 1 and refusal is not None:
-        raise refusal
-    if ctx is None:
-        ctx = N.default_context(torch.cuda.current_device())
-    if world > 1:
-        # the shard check may fail on some ranks only: every rank learns the outcome before a collective could wait
-        flag = torch.tensor([int(refusal is not None)], dtype=torch.int64, device=_comm_device(group, ctx) or "cpu")
-        refused = all_gather_tensor(flag, group).view(-1)
-        if refusal is not None:
-            raise refusal
-        if int(refused.sum()):
-            raise N.ShapeError("rank %d's constants/sigmas commitment is not its row-block shard"
-                               % int(torch.nonzero(refused)[0]))
-    placement = ((rank, world), group) if world > 1 else None
+    placement, ctx = _placement(group, ctx)
+    # the shard check may fail on some ranks only: every rank learns the outcome before a collective could wait
+    placement._agree_on_failure(refusal, ctx, N.ShapeError,
+                                "rank %d's constants/sigmas commitment is not its row-block shard")
     return P._prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys)
 
 

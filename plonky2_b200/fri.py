@@ -11,6 +11,7 @@ from typing import List, Optional, Tuple
 import numpy as np
 
 from . import _native as N
+from .distributed import Placement
 from .field import ORDER
 from .hash import NUM_HASH_OUT_ELTS, MerkleCap
 
@@ -526,13 +527,14 @@ def fri_proof_of_work(challenger, config, ctx=None):
     return pow_witness
 
 
-def fri_prover_query_rounds(oracles, state, challenger, n, fri_params):
-    """fri_prover_query_rounds / fri_prover_query_round (prover.rs:204-258), batched per tree."""
+def fri_prover_query_rounds(oracles, state, challenger, n, fri_params, placement=Placement()):
+    """fri_prover_query_rounds / fri_prover_query_round (prover.rs:204-258), batched per tree. The initial trees are
+    opened on their placement (Placement.open_many)."""
     L, ctx = N.lib(), state.ctx
     nq = fri_params.config.num_query_rounds
     x_indices = [c % n for c in challenger.get_n_challenges(nq)]
     idx = np.array(x_indices, dtype=np.uint64)
-    initial = [o.merkle_tree.open_many(idx) for o in oracles]
+    initial = [placement.open_many(o, idx) for o in oracles]
     steps = []
     cur = idx.copy()
     log_cur = fri_params.lde_bits()
@@ -556,8 +558,12 @@ def fri_prover_query_rounds(oracles, state, challenger, n, fri_params):
 
 
 def prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len=None,
-                   max_num_query_steps=None, taps=None):
-    """PolynomialBatch::prove_openings -> fri_proof (oracle.rs:176-237, prover.rs:24-70)."""
+                   max_num_query_steps=None, taps=None, placement=Placement()):
+    """PolynomialBatch::prove_openings -> fri_proof (oracle.rs:176-237, prover.rs:24-70). placement: where the initial
+    oracles live. With row-block shards over several ranks, the coefficients are replicated, so every rank runs the
+    (small, single-column) FRI commit phase and the transcript redundantly and deterministically; only the initial-tree
+    openings cross ranks, and the returned FriProof is the same on every rank and byte-identical to the single-device
+    proof. The caller must already have observed the full caps (Placement.cap) in `challenger`."""
     alpha = challenger.get_extension_challenge()
     state = _begin(instance, oracles, alpha, fri_params)
     try:
@@ -570,7 +576,7 @@ def prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_l
                                                  max_num_query_steps)
         pow_witness = fri_proof_of_work(challenger, fri_params.config, state.ctx)
         n = fri_params.lde_size()
-        rounds, x_indices = fri_prover_query_rounds(oracles, state, challenger, n, fri_params)
+        rounds, x_indices = fri_prover_query_rounds(oracles, state, challenger, n, fri_params, placement)
         if taps is not None:
             taps["pow_witness"] = pow_witness
             taps["query_indices"] = x_indices

@@ -1430,20 +1430,31 @@ def program_constants(common_data, b, public_inputs_hash, betas, gammas, deltas=
 
 
 def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inputs_hash, wires_commitment,
-                           zs_partial_products_commitment, betas, gammas, alphas, deltas=()):
+                           zs_partial_products_commitment, betas, gammas, alphas, deltas=(),
+                           placement=distributed.Placement()):
     """compute_quotient_polys (plonk/prover.rs:609-815) on the device: a torch int64 CUDA tensor (num_challenges, size) of
     quotient-polynomial coefficients, size = n << log2_ceil(quotient_degree_factor). The three PolynomialBatch handles
-    stay where they are; nothing but the program and the challenges crosses PCIe."""
+    stay where they are; nothing but the program and the challenges crosses PCIe. On a placement of several ranks the
+    commitments are this rank's row-block shards: each rank evaluates the vanishing polynomial over Z_H on its shard of
+    the quotient coset (gl_plonk_quotient_shard), and every rank gets the same quotient
+    (Placement.quotient_from_shards; collective, a failure on any rank raises on every rank)."""
     import torch
 
     commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
     prog, consts, al = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas)
     nc = common_data.config.num_challenges
     qdf = common_data.quotient_degree_factor
-    size = (1 << common_data.degree_bits) << (qdf - 1).bit_length()
     ctx = wires_commitment.ctx
-    out = torch.empty((nc, size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     handles = (C.c_void_p * 3)(*[c.h for c in commits])
+    if placement.num_shards > 1:
+        def run_shard(local):
+            N.check(N.lib().gl_plonk_quotient_shard(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts),
+                                                    N.np_ptr(al), nc, common_data.num_vanishing_terms(), qdf,
+                                                    N.vp(local.data_ptr())), ctx.h)
+
+        return placement.quotient_from_shards(ctx, run_shard, nc, common_data.degree_bits, qdf)
+    size = (1 << common_data.degree_bits) << (qdf - 1).bit_length()
+    out = torch.empty((nc, size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     N.check(N.lib().gl_plonk_quotient(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts), N.np_ptr(al), nc,
                                       common_data.num_vanishing_terms(), qdf, N.vp(out.data_ptr())), ctx.h)
     ctx.synchronize()
@@ -1677,16 +1688,15 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
     The salt is drawn on the device: salt_keys = three 32-byte keys (wires, Z's, quotient) give a reproducible proof;
     None draws a fresh key from the OS CSPRNG per commitment. The blinding rows of the circuit (blinding_counts) are part
     of the witness, which the caller generates."""
-    return _prove(prover_data, common_data, wires, public_inputs, ctx, None, salt_keys)
+    return _prove(prover_data, common_data, wires, public_inputs, ctx, distributed.Placement(), salt_keys)
 
 
 def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys=None):
-    """prove_with_witness on a placement ((g, G), group) of distributed.prove_plonk (None: one device). With G > 1 this
-    rank holds row block g of the wires, Z / partial-product (+ lookup) and quotient commitments, and
-    prover_data.constants_sigmas_commitment is that shard too: the caps are all-gathered before they are observed, the
-    quotient is evaluated shard by shard and all-gathered (distributed.plonk_quotient_polys_sharded), and FRI routes the
-    query openings between the ranks (distributed.prove_openings_sharded). The Z's, partial products and lookup columns,
-    the openings and the transcript run on every rank, so every rank returns the same proof."""
+    """prove_with_witness on a distributed.Placement. With G > 1 ranks this one holds row block g of the wires,
+    Z / partial-product (+ lookup) and quotient commitments, and prover_data.constants_sigmas_commitment is that shard
+    too: the caps are all-gathered before they are observed, the quotient is evaluated shard by shard and all-gathered,
+    and FRI routes the query openings between the ranks. The Z's, partial products and lookup columns, the openings and
+    the transcript run on every rank, so every rank returns the same proof."""
     from .challenger import Challenger
     from .fri import prove_openings
     from .hash import PoseidonHash
@@ -1709,8 +1719,7 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
     # keyword arguments of the three salted commitments (none without zero knowledge)
     salted = [dict(salt_key=salt_keys[i] if salt_keys is not None else "fresh") if zk else {} for i in range(3)]
     public_inputs_hash = [int(x) for x in PoseidonHash.hash_no_pad(np.array(public_inputs, dtype=np.uint64), ctx)]
-    on = distributed.shard_kwargs(placement)
-    sharded = distributed.shard_of(placement)[1] > 1
+    on = placement.commit_kwargs
     wires_commitment = PolynomialBatch.from_values(wires, cfg.rate_bits, zk, cfg.cap_height, ctx=ctx, **salted[0], **on)
     commitments = [wires_commitment]
     try:
@@ -1718,7 +1727,7 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
         prover_data.fri_params.observe(challenger)                     # observe the FRI config
         challenger.observe_hash(prover_data.circuit_digest)            # observe the instance
         challenger.observe_hash(public_inputs_hash)
-        wires_cap = distributed.full_cap(wires_commitment, placement)
+        wires_cap = placement.cap(wires_commitment)
         challenger.observe_cap(wires_cap)
         betas = challenger.get_n_challenges(nc)
         gammas = challenger.get_n_challenges(nc)
@@ -1743,22 +1752,17 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
                                                        cd.quotient_degree_factor, cfg.rate_bits, cfg.cap_height, ctx,
                                                        **(dict(blinding=True, **salted[1]) if zk else {}), **on)
         commitments.append(zs_commitment)
-        zs_cap = distributed.full_cap(zs_commitment, placement)
+        zs_cap = placement.cap(zs_commitment)
         challenger.observe_cap(zs_cap)
         alphas = challenger.get_n_challenges(nc)
         cs = prover_data.constants_sigmas_commitment
-        if sharded:
-            quotient_polys = distributed.plonk_quotient_polys_sharded(cd, cs, public_inputs_hash, wires_commitment,
-                                                                      zs_commitment, betas, gammas, alphas, deltas,
-                                                                      placement[1])
-        else:
-            quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas,
-                                                    gammas, alphas, deltas)
+        quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas,
+                                                gammas, alphas, deltas, **placement.step_kwargs)
         quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx,
                                                     **(dict(blinding=True, **salted[2]) if zk else {}), **on)
         commitments.append(quotient_commitment)
         del quotient_polys
-        quotient_cap = distributed.full_cap(quotient_commitment, placement)
+        quotient_cap = placement.cap(quotient_commitment)
         challenger.observe_cap(quotient_cap)
         zeta = challenger.get_extension_challenge()
         g = F.primitive_root_of_unity(cd.degree_bits)
@@ -1772,11 +1776,8 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
         for batch in openings.to_fri_openings():                       # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         oracles = [cs, wires_commitment, zs_commitment, quotient_commitment]
-        if sharded:
-            opening_proof = distributed.prove_openings_sharded(get_fri_instance(cd, zeta), oracles, challenger,
-                                                               prover_data.fri_params, placement[1])
-        else:
-            opening_proof = prove_openings(get_fri_instance(cd, zeta), oracles, challenger, prover_data.fri_params)
+        opening_proof = prove_openings(get_fri_instance(cd, zeta), oracles, challenger, prover_data.fri_params,
+                                       **placement.step_kwargs)
         proof = Proof(wires_cap, zs_cap, quotient_cap, openings, opening_proof)
         return ProofWithPublicInputs(proof, public_inputs)
     finally:

@@ -8,7 +8,7 @@ on the host (the constraint-binding step of the prover, and any verifier). `prov
 cross_table_lookup.prove_with_ctls (several) both run prove_with_commitment, which strings the device steps together in
 the reference's order with the transcript on the host; the lookup helper columns are written on the device by
 gl_stark_lookup_helpers, the CTL helper and Z columns by gl_stark_ctl_helpers. distributed.prove_stark runs the same
-prove_with_commitment on row-block shards over several GPUs (its `placement`)."""
+prove_with_commitment on row-block shards over several GPUs (its distributed.Placement)."""
 import ctypes as C
 
 import numpy as np
@@ -253,13 +253,15 @@ class FibonacciStark(Stark):
 
 
 def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxiliary_polys_commitment=None,
-                           lookup_challenges=None, ctl_vars=None):
+                           lookup_challenges=None, ctl_vars=None, placement=D.Placement()):
     """compute_quotient_polys (prover.rs:488-668) on the device. Returns a torch int64 CUDA tensor (num_challenges, size)
     of quotient-polynomial coefficients, size = n << log2_ceil(quotient_degree_factor), or None if the Stark has no
     quotient. Raises if the vanishing polynomial is not divisible by Z_H. A Stark with lookups also needs the auxiliary
     commitment (its LDE is read in place, like the trace's) and the lookup challenges; one with CTLs the auxiliary
     commitment and ctl_vars (CtlCheckVars of its CTL data's shape; their challenges are bound like the public
-    inputs)."""
+    inputs). On a placement of several ranks the commitments are this rank's row-block shards: each rank evaluates
+    C(x)/Z_H(x) on its shard of the quotient coset (gl_stark_quotient_shard), and every rank gets the same quotient
+    (Placement.quotient_from_shards; collective, a failure on any rank raises on every rank)."""
     import torch
 
     qdf = stark.quotient_degree_factor()
@@ -267,11 +269,19 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
         return None
     b, consts, al = quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment, lookup_challenges,
                                      ctl_vars)
-    qd_bits = (qdf - 1).bit_length()
-    size = (1 << trace_commitment.degree_log) << qd_bits
     ctx = trace_commitment.ctx
-    out = torch.empty((len(al), size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     prog = b.program()
+    if placement.num_shards > 1:
+        aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
+
+        def run_shard(local):
+            N.check(N.lib().gl_stark_quotient_shard(ctx.h, trace_commitment.h, aux_h, prog, len(b.instrs),
+                                                    N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
+                                                    N.vp(local.data_ptr())), ctx.h)
+
+        return placement.quotient_from_shards(ctx, run_shard, len(al), trace_commitment.degree_log, qdf)
+    size = (1 << trace_commitment.degree_log) << (qdf - 1).bit_length()
+    out = torch.empty((len(al), size), dtype=torch.int64, device="cuda:%d" % ctx.device)
     if stark.uses_lookups() or ctl_vars is not None:
         N.check(N.lib().gl_stark_quotient_aux(ctx.h, trace_commitment.h, auxiliary_polys_commitment.h, prog,
                                               len(b.instrs), N.np_ptr(consts), len(consts), N.np_ptr(al), len(al), qdf,
@@ -665,11 +675,11 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     verifier circuit made for another degree (ConstantArityBits only); the transcript then observes the zero caps and
     coefficients that verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment
     is released on every exit path."""
-    return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, None)
+    return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, D.Placement())
 
 
 def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement):
-    """prove on the placement of prove_with_commitment (None: one device)."""
+    """prove on a distributed.Placement (see prove_with_commitment)."""
     from .challenger import Challenger
 
     ctx = ctx or N.default_context()
@@ -679,38 +689,37 @@ def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx
     if stark.uses_lookups():
         check_lookup_shapes(stark)
         trace = _device_trace(trace, ctx)
-    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx, **D.shard_kwargs(placement))
+    trace_commitment = _commit_trace(trace, rate_bits, cap_height, ctx, **placement.commit_kwargs)
     try:
         challenger = Challenger()
         challenger.observe_elements(public_inputs)
         config.observe(challenger)
-        challenger.observe_cap(D.full_cap(trace_commitment, placement))
-        return prove_with_commitment(stark, config, trace, trace_commitment, None, None, challenger, public_inputs,
-                                     params, ctx=ctx, placement=placement)
+        trace_cap = placement.cap(trace_commitment)
+        challenger.observe_cap(trace_cap)
+        return prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, None, None, challenger,
+                                     public_inputs, params, ctx=ctx, placement=placement)
     finally:
         trace_commitment.close()
 
 
-def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_challenges, challenger, public_inputs,
-                          params, ctx=None, placement=None):
+def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl_data, ctl_challenges, challenger,
+                          public_inputs, params, ctx=None, placement=D.Placement()):
     """prove_with_commitment (starky/src/prover.rs:125-484): one table's proof from its committed trace, on a challenger
-    that has already observed what precedes it (the config among them). Every array-sized step runs on the device
-    (lookup helper columns and the auxiliary commitment, quotient from the LDEs in place, quotient commitment, openings,
-    FRI); the transcript and the constraint-binding step run on the host. With ctl_challenges the lookups use their
+    that has already observed what precedes it (the config and trace_cap, the trace's full cap, among them). Every
+    array-sized step runs on the device (lookup helper columns and the auxiliary commitment, quotient from the LDEs in
+    place, quotient commitment, openings, FRI); the transcript and the constraint-binding step run on the host. With ctl_challenges the lookups use their
     betas (prover.rs:165-168). With ctl_data (cross_table_lookup.CtlData, its CTL columns already in its auxiliary
     buffer) the auxiliary oracle is [lookup helpers | CTL helpers | CTL Zs], the CTL constraints join the quotient and
     the openings carry ctl_zs_first. trace: the values the lookup helper columns read (a CUDA tensor when the Stark has
-    lookups). params: _check_prove_shapes's. placement=((g, G), group) proves on the G ranks of the torch.distributed
-    group, this one holding row block g of every commitment (trace_commitment too): the caps are all-gathered before
-    they are observed, the quotient is evaluated shard by shard and all-gathered (distributed.quotient_polys_sharded),
-    and FRI routes the query openings between the ranks (distributed.prove_openings_sharded). Everything else runs
-    redundantly on every rank, so every rank returns the same proof. None: one device. Every commitment made here is
+    lookups). params: _check_prove_shapes's. placement: a distributed.Placement of G ranks proves on them, this one
+    holding row block g of every commitment (trace_commitment too): the caps are all-gathered before they are observed,
+    the quotient is evaluated shard by shard and all-gathered, and FRI routes the query openings between the ranks.
+    Everything else runs redundantly on every rank, so every rank returns the same proof. Every commitment made here is
     released on every exit path; the trace commitment stays the caller's."""
     from .fri import prove_openings
     from .lookup import get_grand_product_challenge_set
 
     ctx = ctx or N.default_context()
-    shard = D.shard_of(placement)
     degree_bits = params.degree_bits
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     uses_lookups = stark.uses_lookups()
@@ -737,33 +746,27 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         elif uses_lookups:
             auxiliary = compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx)
         if uses_lookups or ctl_data is not None:
-            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx,
-                                                    **D.shard_kwargs(placement))
+            aux_commitment = commit_auxiliary_polys(auxiliary, rate_bits, cap_height, ctx, **placement.commit_kwargs)
             commitments.append(aux_commitment)
             del auxiliary
             if ctl_data is not None:
                 ctl_data.auxiliary = None
-            aux_cap = D.full_cap(aux_commitment, placement)
+            aux_cap = placement.cap(aux_commitment)
             challenger.observe_cap(aux_cap)
             quotient_args["auxiliary_polys_commitment"] = aux_commitment
         num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
         num_ctl_helpers, num_ctl_zs = sum(num_ctl_polys), len(num_ctl_polys)
         alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
                                    lookup_challenges, ctl_vars, nl + num_ctl_helpers + num_ctl_zs if ctl_vars else None)
-        if shard[1] > 1:
-            from .distributed import quotient_polys_sharded
-
-            quotient_polys = quotient_polys_sharded(stark, trace_commitment, public_inputs, alphas, placement[1],
-                                                    **quotient_args)
-        else:
-            quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **quotient_args)
+        quotient_polys = compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, **quotient_args,
+                                                **placement.step_kwargs)
         quotient_commitment = None
         if quotient_polys is not None:
             quotient_commitment = commit_quotient_polys(stark, quotient_polys, degree_bits, rate_bits, cap_height, ctx,
-                                                        **D.shard_kwargs(placement))
+                                                        **placement.commit_kwargs)
             commitments.append(quotient_commitment)
             del quotient_polys
-            quotient_cap = D.full_cap(quotient_commitment, placement)
+            quotient_cap = placement.cap(quotient_commitment)
             challenger.observe_cap(quotient_cap)
         zeta = challenger.get_extension_challenge()
         if F.ext_pow(zeta, 1 << degree_bits) == (1, 0):
@@ -774,16 +777,9 @@ def prove_with_commitment(stark, config, trace, trace_commitment, ctl_data, ctl_
         for batch in openings.to_fri_openings():                        # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         instance = stark.fri_instance(zeta, g, config, num_ctl_helpers, num_ctl_zs)
-        if shard[1] > 1:
-            from .distributed import prove_openings_sharded
-
-            opening_proof = prove_openings_sharded(instance, [trace_commitment] + commitments, challenger,
-                                                   params.fri_params, placement[1], params.final_poly_coeff_len,
-                                                   params.max_num_query_steps)
-        else:
-            opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
-                                           params.final_poly_coeff_len, params.max_num_query_steps)
-        proof = StarkProof(D.full_cap(trace_commitment, placement),
+        opening_proof = prove_openings(instance, [trace_commitment] + commitments, challenger, params.fri_params,
+                                       params.final_poly_coeff_len, params.max_num_query_steps, **placement.step_kwargs)
+        proof = StarkProof(trace_cap,
                            quotient_cap if quotient_commitment is not None else None,
                            openings, opening_proof,
                            aux_cap if aux_commitment is not None else None)

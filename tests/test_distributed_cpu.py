@@ -80,12 +80,15 @@ def test_shard_ranges():
     assert np.array_equal(D.gather_cap(cap).hashes, cap)
 
 
-def test_open_sharded_routing_single_process():
-    """Routing logic of open_sharded with a fake local batch (no GPU): owned indices are opened locally with
-    the local index; an index owned by another shard makes the single-process call fail loudly."""
+def test_placement_open_many_routing_single_process():
+    """Routing logic of Placement.open_many with a fake local batch (no GPU, no process group): owned indices are
+    opened locally with the local index; an index owned by another shard makes the single-process call fail loudly.
+    On one device (Placement()) the tree opens the indices itself and the cap is the commitment's own."""
     from plonky2_b200 import distributed as D
 
     class FakeTree:
+        cap = np.arange(8, dtype=np.uint64).reshape(2, 4)
+
         def open_many(self, idx):
             idx = list(idx)
             return (np.array([[100 + i, 7] for i in idx], dtype=np.uint64).reshape(len(idx), 2),
@@ -96,10 +99,53 @@ def test_open_sharded_routing_single_process():
         degree_log, rate_bits, cap_height = 5, 1, 3
         merkle_tree = FakeTree()
 
-    lv, pt = D.open_sharded(FakeBatch(), [32, 63])   # both owned by shard 1 -> local 0 and 31
+    shard = D.Placement(1, 2)
+    lv, pt = shard.open_many(FakeBatch(), [32, 63])   # both owned by shard 1 -> local 0 and 31
     assert lv[:, 0].tolist() == [100, 131] and pt.shape == (2, 3, 4)
     with pytest.raises(RuntimeError):
-        D.open_sharded(FakeBatch(), [5])             # owned by shard 0, nobody serves it here
+        shard.open_many(FakeBatch(), [5])             # owned by shard 0, nobody serves it here
+    one = D.Placement()
+    assert one.shard == (0, 1)
+    lv, pt = one.open_many(FakeBatch(), [5, 32])      # the tree's own indices
+    assert lv[:, 0].tolist() == [105, 132] and pt.shape == (2, 3, 4)
+    assert one.cap(FakeBatch()) is FakeBatch.merkle_tree.cap
+
+
+def _failure_worker(rank, world, port, q):
+    sys.path.insert(0, ROOT)
+    import torch.distributed as dist
+
+    from plonky2_b200 import distributed as D
+
+    dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%d" % port, rank=rank, world_size=world)
+    try:
+        placement = D.Placement(rank, world, None)
+        try:
+            placement._agree_on_failure(ValueError("rank 1's own failure") if rank == 1 else None, None, RuntimeError,
+                                        "rank %d failed")
+            q.put((rank, None))
+        except Exception as e:
+            q.put((rank, "%s: %s" % (type(e).__name__, e)))
+    finally:
+        dist.destroy_process_group()
+
+
+def test_failure_on_one_rank_raises_on_every_rank():
+    """Placement._agree_on_failure over two gloo ranks, rank 1 failing: rank 1 raises its own exception, rank 0 the
+    agreed error naming rank 1, and neither waits for the other."""
+    import torch.multiprocessing as mp
+
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    port = _free_port()
+    procs = [ctx.Process(target=_failure_worker, args=(r, 2, port, q)) for r in range(2)]
+    for p in procs:
+        p.start()
+    res = sorted(q.get(timeout=180) for _ in procs)
+    for p in procs:
+        p.join(timeout=60)
+        assert p.exitcode == 0
+    assert res == [(0, "RuntimeError: rank 1 failed"), (1, "ValueError: rank 1's own failure")]
 
 
 @pytest.mark.parametrize("num_polys,world", [(234, 8), (234, 4), (234, 2), (64, 8), (5, 4), (3, 8), (16, 1), (300, 2)])

@@ -38,12 +38,10 @@ def _timed_phases(ctx):
     import plonky2_b200.stark as stark_mod
 
     times = {}
-    # one rank takes stark.prove's path: compute_quotient_polys and prove_openings stand for the sharded steps
-    patches = [(stark_mod, "_commit_trace", "trace_commitment"), (dist_mod, "full_cap", "cap_gathers"),
-               (stark_mod, "_bind_constraints", "binding_step"), (dist_mod, "quotient_polys_sharded", "quotient"),
-               (stark_mod, "compute_quotient_polys", "quotient"),
+    patches = [(stark_mod, "_commit_trace", "trace_commitment"), (dist_mod.Placement, "cap", "cap_gathers"),
+               (stark_mod, "_bind_constraints", "binding_step"), (stark_mod, "compute_quotient_polys", "quotient"),
                (stark_mod, "commit_quotient_polys", "quotient_commitment"), (proof_mod, "eval_commitments", "openings"),
-               (dist_mod, "prove_openings_sharded", "fri"), (fri_mod, "prove_openings", "fri")]
+               (fri_mod, "prove_openings", "fri")]
     saved = []
     for mod, name, label in patches:
         fn = getattr(mod, name)
