@@ -199,6 +199,25 @@ int gl_partial_products_and_zs(gl_ctx* ctx, const uint64_t* wires, const uint64_
                                uint32_t log_n, uint32_t num_routed, uint64_t beta, uint64_t gamma, uint32_t degree,
                                uint64_t* out, int mem);
 
+/* The sigma polynomials of a circuit (CircuitBuilder::sigma_vecs, plonky2/src/plonk/circuit_builder.rs:993-1028, with
+ * WirePartition::get_sigma_polys, plonk/permutation_argument.rs:113-157) on the device. pairs = n_pairs copy constraints,
+ * 2 * n_pairs target indices in Target::index numbering (iop/target.rs:55-60): wire (row, col) -> row * num_wires + col,
+ * virtual target i -> n * num_wires + i, n = 2^degree_bits, num_targets = n * num_wires + num_virtual_targets.
+ * out = num_routed_wires columns of n values (column c at out + c * n): row r of column c holds k_is[c'] * w_n^r', where
+ * (r', c') is the routed wire after (r, c) in its partition set, in ascending row-major order r * num_routed_wires + c,
+ * wrapping around to the set's first wire; a wire alone in its set maps to itself. Virtual targets and non-routed
+ * wires take part in the partition (they may join sets) but get no sigma. k_is = num_routed_wires host words.
+ * The sets are the connected components of the pairs: one lock-free union-find launch (each edge retries only while a
+ * root it links moves, at most num_targets times) and one path compression, then a stable radix sort of the routed
+ * wires by component and a gather: 8 kernel launches of this library and the sort's, with no host round trip after the check of
+ * device-resident pairs.
+ * Errors (GL_ERR_BAD_SHAPE, before any device work for host pairs, from a device flag for device pairs): a target index
+ * >= num_targets; a wire endpoint of column >= num_routed_wires (CircuitBuilder::connect asserts routability,
+ * circuit_builder.rs:516-528); num_targets >= 2^32; num_routed_wires > num_wires or 0. */
+int gl_sigma_polys(gl_ctx* ctx, const uint64_t* pairs, size_t n_pairs, int pairs_mem, uint32_t num_wires,
+                   uint32_t num_routed_wires, uint32_t degree_bits, uint64_t num_virtual_targets, const uint64_t* k_is,
+                   uint64_t* out, int out_mem);
+
 /* compute_lookup_polys (plonky2/src/plonk/prover.rs:458-577) for ONE challenge set deltas = (A, B, alpha, delta): the RE
  * polynomial followed by the num_partial_lookups partial Sum/LDC polynomials, as value columns of n = 2^log_n rows:
  * out = (num_partial_lookups + 1) columns of n words (column-major), num_partial_lookups =

@@ -7,6 +7,7 @@
 //   fri_committed_trees / fri_proof_of_work   plonky2/src/fri/prover.rs:84-202    -> gl_fri_commit_round/fold/pow
 // There is no CPU fallback anywhere in this file: every compute entry point launches kernels.
 #include <cooperative_groups.h>
+#include <cub/device/device_radix_sort.cuh>
 #include <cuda_runtime.h>
 
 #include <cstdarg>
@@ -32,6 +33,7 @@
 #include "gl_ctl.cuh"
 #include "gl_ntt.cuh"
 #include "gl_poseidon.cuh"
+#include "gl_sigma.cuh"
 #include "gl_vanishing.cuh"
 
 using namespace gl;
@@ -1506,6 +1508,95 @@ static int upload_program(gl_ctx* ctx, const void* prog, size_t prog_bytes, cons
 }
 
 // =====================================================================================
+// sigma polynomials (CircuitBuilder::sigma_vecs, plonk/circuit_builder.rs:993-1028; index code in gl_sigma.cuh)
+// =====================================================================================
+// Blocks of 256 threads for a grid-stride loop over `count` items
+static unsigned sigma_blocks(size_t count) {
+    const size_t b = (count + 255) / 256;
+    return (unsigned)(b == 0 ? 1 : b < (1u << 20) ? b : (1u << 20));
+}
+#define SIGMA_FOR(i, count) \
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (count); i += (size_t)gridDim.x * blockDim.x)
+
+// The copy constraints' endpoints, checked (flag bits SIGMA_OUT_OF_RANGE / SIGMA_NOT_ROUTED) and narrowed to u32
+__global__ void __launch_bounds__(256) k_sigma_edges(const u64* pairs, size_t count, SigmaShape s, uint32_t* edges,
+                                                     unsigned int* flag) {
+    SIGMA_FOR(i, count) {
+        const uint32_t bad = sigma_check_target(pairs[i], s);
+        if (bad) atomicOr(flag, bad);
+        edges[i] = bad ? 0 : (uint32_t)pairs[i];
+    }
+}
+__global__ void __launch_bounds__(256) k_cc_init(uint32_t* L, size_t count) {
+    SIGMA_FOR(i, count) L[i] = (uint32_t)i;
+}
+// Forest::find on labels that point to a smaller index (a root points to itself), halving the path it walks. Other
+// threads shorten or extend the same paths concurrently; every value any thread stores is an ancestor of the node.
+__device__ __forceinline__ uint32_t cc_find(uint32_t* L, uint32_t x) {
+    volatile uint32_t* V = L;
+    uint32_t cur = V[x];
+    if (cur == x) return x;
+    uint32_t prev = x, next;
+    while (cur > (next = V[cur])) {
+        V[prev] = next;
+        prev = cur;
+        cur = next;
+    }
+    return cur;
+}
+// Forest::merge of every copy constraint at once, lock-free (the hooking of ECL-CC, Jaiganesh and Burtscher 2018): the
+// larger of the two roots is linked below the smaller with a compare-and-swap. A failed swap means that root has just
+// been linked elsewhere, and the thread retries from its new parent. Each retry lowers the larger of the two indices,
+// so one edge takes at most num_targets attempts, and no thread ever waits for another. One launch merges everything.
+__global__ void __launch_bounds__(256) k_cc_hook(const uint32_t* edges, size_t n_pairs, uint32_t* L) {
+    SIGMA_FOR(e, n_pairs) {
+        uint32_t a = cc_find(L, edges[2 * e]), b = cc_find(L, edges[2 * e + 1]);
+        while (a != b) {
+            const uint32_t hi = a > b ? a : b, lo = a > b ? b : a;
+            const uint32_t old = atomicCAS(L + hi, hi, lo);
+            if (old == hi) break;
+            a = old;
+            b = lo;
+        }
+    }
+}
+// Forest::compress_paths: every label becomes its root (the component's smallest target index)
+__global__ void __launch_bounds__(256) k_cc_compress(uint32_t* L, size_t count) {
+    SIGMA_FOR(i, count) {
+        uint32_t x = L[i];
+        while (L[x] != x) x = L[x];
+        L[i] = x;
+    }
+}
+// Forest::wire_partition's walk: key = the component of routed wire i, value = i
+__global__ void __launch_bounds__(256) k_sigma_keys(const uint32_t* L, SigmaShape s, size_t count, uint32_t* keys,
+                                                    uint32_t* vals) {
+    SIGMA_FOR(i, count) {
+        keys[i] = L[sigma_target(i, s)];
+        vals[i] = (uint32_t)i;
+    }
+}
+__global__ void __launch_bounds__(256) k_sigma_heads(const uint32_t* keys, size_t count, uint32_t* heads) {
+    SIGMA_FOR(p, count) if (sigma_is_head(keys, p)) heads[keys[p]] = (uint32_t)p;
+}
+struct SigmaFill {
+    const uint32_t *keys, *vals, *heads;  // sorted keys and values; heads[label] = the segment's first position
+    size_t count;
+    SigmaShape s;
+    const u64* k_is;
+    const u64 *xhi, *xlo;                 // w_n^r = xhi[r >> 12] * xlo[r & 4095]
+    u64* out;
+};
+// get_sigma_map + get_sigma_polys: sorted position p's wire gets k_is[col'] * w_n^row' of its successor (row', col')
+__global__ void __launch_bounds__(256) k_sigma_fill(SigmaFill f) {
+    SIGMA_FOR(p, f.count) {
+        const uint32_t j = sigma_successor(f.keys, f.vals, f.heads, f.count, p);
+        const uint32_t row = j / f.s.num_routed, col = j % f.s.num_routed;
+        f.out[sigma_out_index(f.vals[p], f.s)] = canon(mul(f.k_is[col], mul(f.xhi[row >> 12], f.xlo[row & 4095])));
+    }
+}
+
+// =====================================================================================
 // C ABI
 // =====================================================================================
 extern "C" {
@@ -2029,6 +2120,89 @@ int gl_lookup_polys(gl_ctx* ctx, const uint64_t* wires, uint32_t log_n, uint32_t
     }
     TRY(flag_status(ctx, dflag, {INVERT_ZERO}));
     if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, (size_t)(P + 1) * n));
+    return GL_OK;
+}
+
+static int sigma_refusal(gl_ctx* ctx, uint32_t bad, const char* where) {
+    if (bad & SIGMA_OUT_OF_RANGE)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "copy constraint %s: a target index >= num_targets", where);
+    return set_err(ctx, GL_ERR_BAD_SHAPE, "copy constraint %s: a wire of column >= num_routed_wires is not routable",
+                   where);
+}
+
+int gl_sigma_polys(gl_ctx* ctx, const uint64_t* pairs, size_t n_pairs, int pairs_mem, uint32_t num_wires,
+                   uint32_t num_routed_wires, uint32_t degree_bits, uint64_t num_virtual_targets, const uint64_t* k_is,
+                   uint64_t* out, int out_mem) {
+    // the shape and the host pairs are checked before the context is looked at: no refusal touches the device
+    if (!k_is || !out || (n_pairs && !pairs)) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (num_routed_wires == 0 || num_routed_wires > num_wires)
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "need 0 < num_routed_wires (%u) <= num_wires (%u)", num_routed_wires,
+                       num_wires);
+    const u64 T = degree_bits < 32 ? ((u64)num_wires << degree_bits) + num_virtual_targets : ~0ull;
+    if (degree_bits >= 32 || num_virtual_targets >= (1ull << 32) || T >= (1ull << 32))
+        return set_err(ctx, GL_ERR_BAD_SHAPE, "num_wires * 2^degree_bits + num_virtual_targets must be below 2^32");
+    const SigmaShape s{num_wires, num_routed_wires, degree_bits, T};
+    if (pairs_mem == GL_MEM_HOST)
+        for (size_t i = 0; i < 2 * n_pairs; i++)
+            if (uint32_t bad = sigma_check_target(pairs[i], s)) {
+                char where[64];
+                snprintf(where, sizeof(where), "%zu (endpoint %llu)", i / 2, (unsigned long long)pairs[i]);
+                return sigma_refusal(ctx, bad, where);
+            }
+    if (!ctx) return set_err(nullptr, GL_ERR_BAD_ARG, "null context");
+    CK(ctx, cudaSetDevice(ctx->device));
+    const size_t n = (size_t)1 << degree_bits, count = n * num_routed_wires;
+    DevBuf dout_stage(ctx), labels(ctx), dpairs(ctx), edges(ctx), dflag(ctx), keys(ctx), vals(ctx), temp(ctx), dk(ctx),
+        xtab(ctx);
+    u64* dout;
+    TRY(device_out(out, count, out_mem, dout_stage, &dout));
+    TRY(labels.alloc((T + 1) / 2));  // u32 arrays live in u64-word buffers
+    uint32_t* L = (uint32_t*)labels.get();
+    k_cc_init<<<sigma_blocks(T), 256, 0, ctx->stream>>>(L, T);
+    CKL(ctx);
+    if (n_pairs) {
+        u64* pp;
+        TRY(device_in(ctx, pairs, 2 * n_pairs, pairs_mem, dpairs, &pp));
+        TRY(edges.alloc(n_pairs));
+        uint32_t* E = (uint32_t*)edges.get();
+        TRY(flag_alloc(ctx, dflag));
+        k_sigma_edges<<<sigma_blocks(2 * n_pairs), 256, 0, ctx->stream>>>(pp, 2 * n_pairs, s, E,
+                                                                          (unsigned int*)dflag.get());
+        CKL(ctx);
+        u64 bad = 0;  // the one host read of the call before the sort: device-resident pairs are checked here
+        TRY(d2h(ctx, &bad, dflag.get(), 1));
+        if (bad) return sigma_refusal(ctx, (uint32_t)bad, "in device memory");
+        dpairs.reset();
+        k_cc_hook<<<sigma_blocks(n_pairs), 256, 0, ctx->stream>>>(E, n_pairs, L);
+        CKL(ctx);
+        edges.reset();
+        k_cc_compress<<<sigma_blocks(T), 256, 0, ctx->stream>>>(L, T);
+        CKL(ctx);
+    }
+    TRY(keys.alloc(count));  // keys in, keys out: 2 x count u32
+    TRY(vals.alloc(count));
+    uint32_t *kin = (uint32_t*)keys.get(), *kout = kin + count, *vin = (uint32_t*)vals.get(), *vout = vin + count;
+    k_sigma_keys<<<sigma_blocks(count), 256, 0, ctx->stream>>>(L, s, count, kin, vin);
+    CKL(ctx);
+    int end_bit = 1;  // the labels are target indices < T
+    while (end_bit < 32 && ((T - 1) >> end_bit)) end_bit++;
+    size_t temp_bytes = 0;
+    CK(ctx, cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, kin, kout, vin, vout, count, 0, end_bit, ctx->stream));
+    TRY(temp.alloc((temp_bytes + 7) / 8));
+    CK(ctx, cub::DeviceRadixSort::SortPairs(temp.get(), temp_bytes, kin, kout, vin, vout, count, 0, end_bit,
+                                            ctx->stream));
+    CKL(ctx);
+    temp.reset();
+    // the labels are no longer read: their array becomes heads[label]
+    k_sigma_heads<<<sigma_blocks(count), 256, 0, ctx->stream>>>(kout, count, L);
+    CKL(ctx);
+    TRY(dk.alloc(num_routed_wires));
+    TRY(h2d(ctx, dk.get(), k_is, num_routed_wires));
+    TRY(x_pow_tables(ctx, root_of_unity(degree_bits), n, xtab));
+    const SigmaFill f{kout, vout, L, count, s, dk.get(), xtab.get(), xtab.get() + x_pow_table_len(n), dout};
+    k_sigma_fill<<<sigma_blocks(count), 256, 0, ctx->stream>>>(f);
+    CKL(ctx);
+    if (out_mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, count));
     return GL_OK;
 }
 

@@ -322,6 +322,23 @@ def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=
     return P._prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys)
 
 
+def build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets=0, luts=(), lookup_rows=(),
+                       domain_separator=(), group=None, ctx=None):
+    """plonk.build_circuit_data on the ranks of a torch.distributed group (the default group if None): every rank
+    computes the sigma polynomials (replicated, they are prove_plonk's input) and commits row block `rank` of the
+    constants/sigmas LDE; the ranks all-gather the cap entries for the digest. Collective: every rank passes the same
+    circuit and returns the CircuitData prove_plonk needs -- prover_only.constants_sigmas_commitment is this rank's
+    shard (rank, world) -- with the digest and verifier_only cap of the single-device build. The world size must be a
+    power of two of at most 2^cap_height (ShapeError on every rank). Without an initialised process group, or with one
+    rank, this is plonk.build_circuit_data. ctx: this rank's context (default: the current CUDA device's)."""
+    from . import plonk as P
+
+    _check_world("build_circuit_data", config.cap_height, _world_size(group))
+    placement, ctx = _placement(group, ctx)
+    return P._build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets, luts, lookup_rows,
+                                 domain_separator, ctx, placement)
+
+
 def chunk_layout(num_polys, world, chunk_cols=64):
     """Column layout of the pipelined multi-GPU commitment: K chunks of Wc = pc*world consecutive columns; inside
     chunk c rank r transforms columns [c*Wc + r*pc, c*Wc + (r+1)*pc) (clipped to num_polys). Returns (pc, Wc, K)."""

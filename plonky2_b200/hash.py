@@ -103,13 +103,22 @@ class PoseidonHash:
         return np.array(perm.squeeze()[:NUM_HASH_OUT_ELTS], dtype=np.uint64)
 
     @staticmethod
-    def hash_pad(inputs, ctx=None):
-        """pad10*1 then hash_no_pad (config.rs:50-59)."""
+    def _pad(inputs):
+        """The pad10*1 rule of hash_pad (config.rs:50-59)."""
         padded = [int(x) for x in inputs] + [1]
         while (len(padded) + 1) % SPONGE_RATE != 0:
             padded.append(0)
-        padded.append(1)
-        return PoseidonHash.hash_no_pad(np.array(padded, dtype=np.uint64), ctx)
+        return padded + [1]
+
+    @staticmethod
+    def hash_pad(inputs, ctx=None):
+        """pad10*1 then hash_no_pad (config.rs:50-59)."""
+        return PoseidonHash.hash_no_pad(np.array(PoseidonHash._pad(inputs), dtype=np.uint64), ctx)
+
+    @staticmethod
+    def hash_pad_host(inputs):
+        """hash_pad on the HOST permutation."""
+        return PoseidonHash.hash_no_pad_host(PoseidonHash._pad(inputs))
 
     @staticmethod
     def two_to_one_many(pairs, ctx=None):

@@ -7,9 +7,10 @@ The reference evaluates, for every point of the quotient coset, each gate's cons
 terms L_0(x)(Z(x) - 1) and the partial-product checks of the permutation argument, and combines them with powers of
 alpha. Here that walk is done ONCE per circuit, symbolically: gates implement eval_unfiltered over expression handles,
 `vanishing_program` records the whole vanishing polynomial as a register program, and gl_plonk_quotient interprets it
-for all points on the GPU, reading the three commitments' LDEs in place. Circuit construction itself (CircuitBuilder,
-witness generation) stays with the caller; `CommonCircuitData.from_gate_instances` restates only what the quotient
-needs from `CircuitBuilder::build` (gate order, selector polynomials, constant columns, k_is, counts).
+for all points on the GPU, reading the three commitments' LDEs in place. Placing a circuit (CircuitBuilder's gates,
+targets and generators, witness generation) stays with the caller; from the placed circuit, `blind_and_pad` and
+`build_circuit_data` restate the rest of `CircuitBuilder::build` (gate order, selector polynomials, constant columns,
+k_is, counts, the sigma polynomials on the device, the constants/sigmas commitment, the circuit digest).
 Lookup circuits carry the extra terms of `check_lookup_constraints` (the RE / Sum / LDC checks over the lookup selectors)."""
 import ctypes as C
 import heapq
@@ -1503,6 +1504,144 @@ class ProverOnlyCircuitData:
     def __init__(self, constants_sigmas_commitment, sigmas, circuit_digest, fri_params):
         self.constants_sigmas_commitment, self.sigmas = constants_sigmas_commitment, sigmas
         self.circuit_digest, self.fri_params = [int(x) for x in circuit_digest], fri_params
+
+
+class VerifierOnlyCircuitData:
+    """VerifierOnlyCircuitData (plonk/circuit_data.rs:372-380): the constants/sigmas Merkle cap and the circuit digest."""
+
+    def __init__(self, constants_sigmas_cap, circuit_digest):
+        self.constants_sigmas_cap, self.circuit_digest = constants_sigmas_cap, [int(x) for x in circuit_digest]
+
+
+class CircuitData:
+    """CircuitData (plonk/circuit_data.rs:150-160) as build_circuit_data returns it."""
+
+    def __init__(self, common, prover_only, verifier_only):
+        self.common, self.prover_only, self.verifier_only = common, prover_only, verifier_only
+
+
+# ------------------------------------------------------------------ circuit build (plonk/circuit_builder.rs:911-1321)
+def blind_and_pad(config, fri_config, instances):
+    """CircuitBuilder::blind_and_pad (plonk/circuit_builder.rs:911-968) on the gate instances [(gate, constants)] the
+    builder holds once every gate is placed. With config.zero_knowledge it appends the rows blinding_counts asks for:
+    regular_poly_openings NoopGate rows, whose every wire the witness fills with a random value, then z_openings pairs
+    of NoopGate rows, whose two rows carry one random value per routed wire. Then NoopGate rows pad to a power of two.
+    Returns (instances, regular_rows, z_pairs): regular_rows a range of rows, z_pairs a list of (row_1, row_2).
+
+    The reference ties a pair's two rows with generate_copy (a CopyGenerator of witness generation,
+    circuit_builder.rs:507-510), not with connect, so the pairs add no copy constraint and their sigmas stay the
+    identity; the copy constraints are unchanged."""
+    out = list(instances)
+    regular_rows, z_pairs = range(len(out), len(out)), []
+    if config.zero_knowledge:
+        regular, z_openings = blinding_counts(config, fri_config, len(out))
+        regular_rows = range(len(out), len(out) + regular)
+        out += [(NoopGate(), [])] * regular
+        for _ in range(z_openings):
+            z_pairs.append((len(out), len(out) + 1))
+            out += [(NoopGate(), [])] * 2
+    out += [(NoopGate(), [])] * ((1 << max(0, len(out) - 1).bit_length()) - len(out))
+    return out, regular_rows, z_pairs
+
+
+def target_indices(copy_constraints, num_wires, degree_bits):
+    """Copy constraints in the degree-independent encoding -- wire (row, col) -> row * num_wires + col, virtual target
+    i -> -(i + 1) -- as an (E, 2) uint64 array of Target::index values (iop/target.rs:55-60): virtual target i becomes
+    n * num_wires + i. A wire index past the last row is refused (it would alias a virtual target)."""
+    pairs = np.asarray(copy_constraints, dtype=np.int64).reshape(-1, 2)
+    wires = num_wires << degree_bits
+    if (pairs >= wires).any():
+        raise N.ShapeError("copy constraint wire index %d is past the last of the %d rows"
+                           % (int(pairs.max()), 1 << degree_bits))
+    return np.ascontiguousarray(np.where(pairs >= 0, pairs, wires - 1 - pairs), dtype=np.uint64)
+
+
+def sigma_polys(config, degree_bits, pairs, num_virtual_targets=0, ctx=None):
+    """The sigma polynomials' values (CircuitBuilder::sigma_vecs, plonk/circuit_builder.rs:993-1028) on the device:
+    gl_sigma_polys. pairs: the copy constraints' Target::index values, an (E, 2) host array or a CUDA int64 tensor on
+    the context's device. Returns a (num_routed_wires, n) int64 CUDA tensor: row c is sigma column c."""
+    import torch
+
+    ctx = ctx or N.default_context()
+    nr, n = config.num_routed_wires, 1 << degree_bits
+    k_is = np.array(get_unique_coset_shifts(nr), dtype=np.uint64)
+    if isinstance(pairs, torch.Tensor):
+        host, n_pairs, ptr, mem = None, pairs.numel() // 2, N.vp(pairs.data_ptr()), N.MEM_DEVICE
+    else:
+        host = np.ascontiguousarray(pairs, dtype=np.uint64).reshape(-1, 2)
+        n_pairs, mem = len(host), N.MEM_HOST
+        ptr = N.np_ptr(host) if n_pairs else None
+    out = torch.empty((nr, n), dtype=torch.int64, device="cuda:%d" % ctx.device)
+    torch.cuda.synchronize(out.device)
+    N.check(N.lib().gl_sigma_polys(ctx.h, ptr, n_pairs, mem, config.num_wires, nr, degree_bits, int(num_virtual_targets),
+                                   N.np_ptr(k_is), N.vp(out.data_ptr()), N.MEM_DEVICE), ctx.h)
+    ctx.synchronize()  # the tensor goes to torch, whose stream is not the context's
+    return out
+
+
+def commit_constants_sigmas(common_data, constant_vecs, sigmas, ctx=None, shard=(0, 1)):
+    """The constants/sigmas commitment (circuit_builder.rs:1177-1188, never blinded): the constant columns (host), then
+    the sigma columns read in place from the device tensor sigma_polys returned. shard=(g, G): row block g of G."""
+    cfg = common_data.config
+    ctx = ctx or N.default_context()
+    consts = np.ascontiguousarray(np.stack(constant_vecs), dtype=np.uint64)
+    n = 1 << common_data.degree_bits
+
+    def add_columns(h):
+        N.check(N.lib().gl_commit_add_columns(h, 0, len(consts), N.np_ptr(consts), n, N.COLS_VALUES, N.MEM_HOST), ctx.h)
+        N.check(N.lib().gl_commit_add_columns(h, len(consts), cfg.num_routed_wires, N.vp(sigmas.data_ptr()), n,
+                                              N.COLS_VALUES, N.MEM_DEVICE), ctx.h)
+
+    return PolynomialBatch._from_device(ctx, len(consts) + cfg.num_routed_wires, common_data.degree_bits, cfg.rate_bits,
+                                        cfg.cap_height, add_columns, shard=shard)
+
+
+def circuit_digest(constants_sigmas_cap, domain_separator, degree_bits):
+    """The circuit digest (circuit_builder.rs:1252-1264): hash_no_pad(cap.flatten() || hash_pad(domain_separator) ||
+    [degree_bits]), on the host permutation."""
+    from .hash import PoseidonHash
+
+    cap = getattr(constants_sigmas_cap, "hashes", constants_sigmas_cap)
+    separator = PoseidonHash.hash_pad_host([int(x) % F.ORDER for x in domain_separator])
+    parts = [int(x) for x in np.asarray(cap, dtype=np.uint64).reshape(-1)] + [int(x) for x in separator] + [degree_bits]
+    return [int(x) for x in PoseidonHash.hash_no_pad_host(parts)]
+
+
+def build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets=0, luts=(), lookup_rows=(),
+                       domain_separator=(), ctx=None):
+    """CircuitBuilder::build_with_options(true) (plonk/circuit_builder.rs:1061-1321) from the placed circuit on one
+    device: `instances` already through blind_and_pad, the copy constraints as an (E, 2) array in target_indices'
+    encoding, num_virtual_targets virtual targets. Returns CircuitData(common, prover_only, verifier_only), equal to the
+    reference's: the sigma polynomials and the constants/sigmas commitment are computed on the device, the digest
+    from the cap. prover_only.sigmas is the host (num_routed_wires, n) array prove_with_witness reads.
+    distributed.build_circuit_data builds the same data with the commitment sharded over ranks."""
+    return _build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets, luts, lookup_rows,
+                               domain_separator, ctx, distributed.Placement())
+
+
+def _build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets, luts, lookup_rows,
+                        domain_separator, ctx, placement):
+    """build_circuit_data on a distributed.Placement: the constants/sigmas commitment is this rank's row block, its cap
+    the gathered full cap. The sigmas are computed on every rank."""
+    degree_bits = F.log2_strict(len(instances))
+    pairs = target_indices(copy_constraints, config.num_wires, degree_bits)
+    fri_params = fri_config.fri_params(degree_bits, config.zero_knowledge)
+    if fri_params.total_arities() > degree_bits + fri_config.rate_bits - fri_config.cap_height:
+        raise N.ShapeError("FRI total reduction arity is too large.")
+    common, constant_vecs = CommonCircuitData.from_gate_instances(config, instances, luts, lookup_rows)
+    ctx = ctx or N.default_context()
+    sigmas = sigma_polys(config, degree_bits, pairs, num_virtual_targets, ctx)
+    commitment = commit_constants_sigmas(common, constant_vecs, sigmas, ctx, **placement.commit_kwargs)
+    try:
+        host_sigmas = sigmas.cpu().numpy().view(np.uint64)
+        del sigmas
+        cap = placement.cap(commitment)
+        digest = circuit_digest(cap, domain_separator, degree_bits)
+    except Exception:
+        commitment.close()
+        raise
+    return CircuitData(common, ProverOnlyCircuitData(commitment, host_sigmas, digest, fri_params),
+                       VerifierOnlyCircuitData(cap, digest))
 
 
 def _le_words(arr):
