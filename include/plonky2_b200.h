@@ -173,6 +173,15 @@ int gl_commit_eval_ext(gl_commit* c, const uint64_t point[2], uint64_t* out);
  * D2H (mem = GL_MEM_HOST) or none (GL_MEM_DEVICE). Coefficients never leave the device. */
 int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals,
                 const uint64_t* points, size_t n_points, uint64_t* out, int mem);
+/* gl_openings split between G = num_shards callers (plonky2/src/plonk/proof.rs:313-351,
+ * starky/src/proof.rs:221-265): same arguments and output layout, but every request's value is shard g's partial sum
+ * sum_{k in B_g(n_c)} c_k * z^k (canonical F_{p^2}), B_g(n) = [floor(g*n/G), floor((g+1)*n/G)) with n_c the commitment's
+ * own coefficient count. The G blocks tile [0, n_c) (empty ones give 0 when n_c < G), so the G outputs summed mod p
+ * are gl_openings' output bit for bit; gl_openings is shard (0, 1). Each caller reads its whole (replicated)
+ * coefficient matrix. GL_ERR_BAD_ARG for num_shards == 0 or shard_index >= num_shards, before any launch. */
+int gl_openings_shard(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals,
+                      const uint64_t* points, size_t n_points, uint32_t shard_index, uint32_t num_shards, uint64_t* out,
+                      int mem);
 /* device views (valid until destroy; for device-resident pipelines such as quotient evaluation).
  * The LDE is kept COLUMN-MAJOR on the device: the value of polynomial (or salt column) k at leaf j -- the LDE row
  * reverse_bits(j), oracle.rs:142-147 -- is at lde[k * col_stride + j]; col_stride = number of local leaves. The

@@ -371,19 +371,12 @@ class MultiStarkProof:
         return dict(ctl_challenges=ctl_challenges, stark_challenges=out)
 
 
-def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None):
-    """A multi-STARK proof with cross-table lookups: every table's trace commitment, every trace cap observed in table
-    order, the CTL challenge set (get_ctl_data), every table's CTL helper and Z columns on the device
-    (cross_table_lookup_data at the system's largest constraint degree), then table by table on the same challenger its
-    public inputs, the config and prove_with_commitment with its CTL data -- the order the reference's verifier-side
-    replay accepts. traces: per table (COLUMNS, n) host columns or a torch CUDA tensor, read on the device once. Raises
-    ShapeError before any device work for every shape the reference cannot prove or verify (check_ctl_shapes).
-    Returns a MultiStarkProof."""
-    from .challenger import Challenger
-    from .lookup import get_grand_product_challenge_set
+def check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs):
+    """prove_with_ctls's refusals, before any device work: trace and public-input counts, every table's
+    stark.prove checks, check_ctl_shapes and check_lookup_shapes. Returns (each table's ProveParams,
+    max_constraint_degree)."""
     from . import stark as S
 
-    ctx = ctx or N.default_context()
     if len(traces) != len(starks):
         raise N.ShapeError("expected %d traces, got %d" % (len(starks), len(traces)))
     if len(public_inputs) != len(starks):
@@ -392,6 +385,32 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     max_degree = check_ctl_shapes(starks, cross_table_lookups, config.num_challenges)
     for s in starks:
         S.check_lookup_shapes(s)
+    return params, max_degree
+
+
+def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None):
+    """A multi-STARK proof with cross-table lookups: every table's trace commitment, every trace cap observed in table
+    order, the CTL challenge set (get_ctl_data), every table's CTL helper and Z columns on the device
+    (cross_table_lookup_data at the system's largest constraint degree), then table by table on the same challenger its
+    public inputs, the config and prove_with_commitment with its CTL data -- the order the reference's verifier-side
+    replay accepts. traces: per table (COLUMNS, n) host columns or a torch CUDA tensor, read on the device once. Raises
+    ShapeError before any device work for every shape the reference cannot prove or verify (check_prove_shapes).
+    Returns a MultiStarkProof. distributed.prove_with_ctls proves the same system across several GPUs."""
+    from .distributed import Placement
+
+    return _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, Placement())
+
+
+def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement):
+    """prove_with_ctls on a distributed.Placement: every trace is committed with placement.commit_kwargs and observed
+    as placement.cap, and each table runs prove_with_commitment on the placement. The CTL helper and Z columns are
+    computed from the full traces on every rank."""
+    from .challenger import Challenger
+    from .lookup import get_grand_product_challenge_set
+    from . import stark as S
+
+    ctx = ctx or N.default_context()
+    params, max_degree = check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs)
     public_inputs = [[int(v) % F.ORDER for v in p] for p in public_inputs]
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     dev_traces, commitments = [], []
@@ -399,9 +418,9 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
         for s, t in zip(starks, traces):
             dt = S._device_trace(t, ctx) if (s.requires_ctls() or s.uses_lookups()) else t
             dev_traces.append(dt)
-            commitments.append(S._commit_trace(dt, rate_bits, cap_height, ctx))
+            commitments.append(S._commit_trace(dt, rate_bits, cap_height, ctx, **placement.commit_kwargs))
         challenger = Challenger()
-        caps = [c.merkle_tree.cap for c in commitments]
+        caps = [placement.cap(c) for c in commitments]
         for cap in caps:
             challenger.observe_cap(cap)
         ctl_challenges = get_grand_product_challenge_set(challenger, config.num_challenges)
@@ -413,7 +432,8 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
             challenger.observe_elements(public_inputs[i])
             config.observe(challenger)
             proofs.append(S.prove_with_commitment(s, config, dev_traces[i], commitments[i], caps[i], ctl_data[i],
-                                                  ctl_challenges, challenger, public_inputs[i], params[i], ctx=ctx))
+                                                  ctl_challenges, challenger, public_inputs[i], params[i], ctx=ctx,
+                                                  placement=placement))
             ctl_data[i] = None
         return MultiStarkProof(proofs)
     finally:

@@ -1972,9 +1972,12 @@ int gl_commit_eval_ext(gl_commit* c, const uint64_t point[2], uint64_t* out) {
 }
 // OpeningSet::new / StarkOpeningSet::new (plonk/proof.rs:313-351, starky/src/proof.rs:221-260) in ONE call: every
 // polynomial of commits[i] evaluated at points[point_index[i]], results concatenated in request order, one D2H.
-int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals, const uint64_t* points,
-                size_t n_points, uint64_t* out, int mem) {
-    if (!ctx || !commits || !point_index || !points || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+// Shard g of G sums only the coefficients k in [g*n_c/G, (g+1)*n_c/G) of each commitment (n_c its own coefficient
+// count): a pointer offset into the coefficients and the z^k table plus a length, so shard (0, 1) is the whole sum with
+// the same launches. The power table is built whole on every shard; it is a small part of the work.
+static int openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals,
+                    const uint64_t* points, size_t n_points, uint32_t shard_index, uint32_t num_shards, uint64_t* out,
+                    int mem) {
     if (n_evals == 0) return GL_OK;
     CK(ctx, cudaSetDevice(ctx->device));
     uint32_t max_log = 0;
@@ -2008,7 +2011,8 @@ int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_in
             const gl_commit* c = commits[i];
             if (point_index[i] == p) {
                 const size_t nc = (size_t)1 << c->degree_log;
-                k_eval_ext<<<c->B, 256, 0, ctx->stream>>>(c->coeffs, nc, nc, zt.get(), dout + 2 * off);
+                const size_t lo = shard_index * nc / num_shards, hi = (shard_index + 1) * nc / num_shards;
+                k_eval_ext<<<c->B, 256, 0, ctx->stream>>>(c->coeffs + lo, nc, hi - lo, zt.get() + 2 * lo, dout + 2 * off);
                 CKL(ctx);
             }
             off += c->B;
@@ -2016,6 +2020,19 @@ int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_in
     }
     if (mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, 2 * total));
     return GL_OK;
+}
+int gl_openings(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals, const uint64_t* points,
+                size_t n_points, uint64_t* out, int mem) {
+    if (!ctx || !commits || !point_index || !points || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    return openings(ctx, commits, point_index, n_evals, points, n_points, 0, 1, out, mem);
+}
+int gl_openings_shard(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* point_index, size_t n_evals,
+                      const uint64_t* points, size_t n_points, uint32_t shard_index, uint32_t num_shards, uint64_t* out,
+                      int mem) {
+    if (!ctx || !commits || !point_index || !points || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    if (num_shards == 0 || shard_index >= num_shards)
+        return set_err(ctx, GL_ERR_BAD_ARG, "shard %u of %u", shard_index, num_shards);
+    return openings(ctx, commits, point_index, n_evals, points, n_points, shard_index, num_shards, out, mem);
 }
 const uint64_t* gl_commit_dev_lde(const gl_commit* c, size_t* col_stride) {
     if (col_stride) *col_stride = c->tree.es;

@@ -6,11 +6,12 @@ Merkle-cap entries (2^cap_height x 32 bytes in total) -- and PipelinedCommitter 
 No LDE data ever crosses NVLink: shard g of G evaluates every column on its own coset
 (g_shift * w_N^{bitrev(g)}) <w_{N/G}>, hashes its leaves and reduces its own cap subtrees.
 
-prove_stark proves one STARK, and prove_plonk one plonky2 circuit, on the ranks of a group with these shards: besides
-the caps, only the quotient's values on each rank's shard of the quotient coset (Placement.quotient_from_shards) and
-the FRI query openings (Placement.open_many) cross ranks. Both provers take a Placement -- Placement() on one device --
-and never ask themselves whether there is more than one rank. prove_openings_sharded is fri.prove_openings on the
-oracles' own shards, for a caller that commits the shards itself."""
+prove_stark proves one STARK, prove_with_ctls a multi-STARK system with cross-table lookups, and prove_plonk one
+plonky2 circuit, on the ranks of a group with these shards: besides the caps, only the quotient's values on each rank's
+shard of the quotient coset (Placement.quotient_from_shards), the partial sums of the openings over each rank's block
+of coefficients (Placement.openings_from_shards) and the FRI query openings (Placement.open_many) cross ranks. The
+provers take a Placement -- Placement() on one device -- and never ask themselves whether there is more than one rank.
+prove_openings_sharded is fri.prove_openings on the oracles' own shards, for a caller that commits the shards itself."""
 from dataclasses import dataclass
 
 import numpy as np
@@ -64,11 +65,11 @@ def gather_cap(local_cap, group=None, device=None):
 class Placement:
     """Where a prover's commitments live: row block `shard_index` of `num_shards` of every commitment, one block per rank
     of the torch.distributed `group`. Placement() is one device. The provers build every commitment with
-    `commit_kwargs`, observe `cap`, and run the quotient and FRI with `step_kwargs` (fri.prove_openings opens its
-    queries with `open_many`); the two compute_quotient_polys pick their C entry point by num_shards and, with several
-    ranks, gather the quotient with `quotient_from_shards`. Nothing else in the provers tests whether there is more
-    than one rank. On one device both keyword sets are empty, so every call a prover makes is the plain single-device
-    call."""
+    `commit_kwargs`, observe `cap`, and run the quotient, the openings and FRI with `step_kwargs` (fri.prove_openings
+    opens its queries with `open_many`); the two compute_quotient_polys and proof.eval_commitments pick their C entry
+    point by num_shards and, with several ranks, gather the quotient with `quotient_from_shards` and the openings with
+    `openings_from_shards`. Nothing else in the provers tests whether there is more than one rank. On one device both
+    keyword sets are empty, so every call a prover makes is the plain single-device call."""
     shard_index: int = 0
     num_shards: int = 1
     group: object = None
@@ -86,8 +87,8 @@ class Placement:
 
     @property
     def step_kwargs(self):
-        """The keyword arguments that run compute_quotient_polys or fri.prove_openings on this placement: placement=self,
-        or none on one device, their default."""
+        """The keyword arguments that run compute_quotient_polys, OpeningSet.new / StarkOpeningSet.new or
+        fri.prove_openings on this placement: placement=self, or none on one device, their default."""
         return {} if self.num_shards == 1 else dict(placement=self)
 
     def cap(self, commitment):
@@ -154,6 +155,31 @@ class Placement:
         ctx.synchronize()
         return out
 
+    def openings_from_shards(self, ctx, run_shard, total):
+        """The openings (total, 2) from the ranks' partial sums. run_shard(partial) writes this rank's partial sums of
+        the `total` polynomials into `partial`, a (total, 2) uint64 host array, through gl_openings_shard. Then the ranks
+        all-gather the partials (16 bytes per polynomial) and every rank adds them up mod p in rank order. Collective.
+        Returns the same canonical array on every rank. A failure on one rank raises on every rank: its own exception
+        there, NativeError elsewhere."""
+        import torch
+
+        from . import _native as N
+
+        partial = np.zeros((total, 2), dtype=np.uint64)
+        failure = None
+        try:
+            run_shard(partial)
+        except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
+            failure = e
+        self._agree_on_failure(failure, ctx, N.NativeError, "the openings failed on rank %d")
+        t = torch.from_numpy(partial.view(np.int64))
+        dev = _comm_device(self.group, ctx)
+        parts = all_gather_tensor(t.to(dev) if dev else t, self.group).cpu().numpy().view(np.uint64)
+        out = parts[0].copy()
+        for p in parts[1:]:
+            out = _add_mod_p(out, p)
+        return out
+
     def _agree_on_failure(self, failure, ctx, error, message):
         """Every rank learns whether any rank failed. `failure` (an exception, or None) is raised on its own rank, and
         error(message % the first failed rank) on every other rank when one failed. Collective with several ranks: call
@@ -168,6 +194,17 @@ class Placement:
             raise failure
         if self.num_shards > 1 and int(failed.sum()):
             raise error(message % int(torch.nonzero(failed)[0]))
+
+
+def _add_mod_p(a, b):
+    """a + b mod p elementwise for canonical uint64 arrays: the wrapped sum minus p (mod 2^64) when the sum is p or
+    more, which its wrapping past 2^64 also signals."""
+    from .field import ORDER
+
+    s = a + b
+    over = (s < a) | (s >= np.uint64(ORDER))
+    s[over] -= np.uint64(ORDER)
+    return s
 
 
 def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None, final_poly_coeff_len=None,
@@ -249,8 +286,9 @@ def check_prove_stark(stark, config, world):
 
 def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circuit_fri_params=None, ctx=None):
     """stark.prove on the ranks of a torch.distributed group (the default group if None): rank g commits row block g
-    of the trace, auxiliary and quotient LDEs, evaluates the quotient on its shard of the quotient coset and answers the
-    FRI queries that land in its rows; the coefficients, openings and transcript are computed on every rank.
+    of the trace, auxiliary and quotient LDEs, evaluates the quotient on its shard of the quotient coset, sums block g
+    of the coefficients into the openings and answers the FRI queries that land in its rows; the coefficients and the
+    transcript are computed on every rank.
     Collective: every rank passes the same full trace (host columns or a torch CUDA tensor) and returns the same
     StarkProofWithPublicInputs, equal to what stark.prove returns on one device. The world size must be a power of two
     of at most 2^cap_height, and the Stark must not take part in cross-table lookups (ShapeError otherwise, on every
@@ -261,6 +299,39 @@ def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circui
     check_prove_stark(stark, config, _world_size(group))
     placement, ctx = _placement(group, ctx)
     return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement)
+
+
+def check_prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, world):
+    """prove_with_ctls's refusals, raised identically on every rank before any device work or collective: everything
+    cross_table_lookup.prove_with_ctls refuses; a world size that is not a power of two or exceeds 2^cap_height; a
+    table whose quotient coset (n << log2_ceil(quotient_degree_factor) points) has fewer points than there are ranks,
+    which a small table has when its quotient degree bits are fewer than rate_bits."""
+    from . import _native as N
+    from . import cross_table_lookup as X
+
+    params, _ = X.check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs)
+    _check_world("prove_with_ctls", config.fri_config.cap_height, world)
+    for i, (s, p) in enumerate(zip(starks, params)):
+        qdf = s.quotient_degree_factor()
+        size = (1 << p.degree_bits) << max(qdf - 1, 0).bit_length()
+        if qdf and size < world:
+            raise N.ShapeError("table %d's quotient coset has %d points, fewer than the %d ranks" % (i, size, world))
+
+
+def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, group=None, ctx=None):
+    """cross_table_lookup.prove_with_ctls on the ranks of a torch.distributed group (the default group if None): rank g
+    commits row block g of every table's trace, auxiliary and quotient LDEs, evaluates each quotient on its shard of
+    the quotient coset, sums block g of the coefficients into the openings and answers the FRI queries that land in its
+    rows. The CTL and lookup helper and Z columns (from the full traces), the coefficients and the one challenger
+    chained through the tables run on every rank. Collective: every rank passes the same full traces (host columns or
+    torch CUDA tensors) and returns the same MultiStarkProof, field for field prove_with_ctls's on one device.
+    Refusals: check_prove_with_ctls (ShapeError on every rank). Without an initialised process group, or with one rank,
+    this is prove_with_ctls. ctx: this rank's context (default: the current CUDA device's)."""
+    from . import cross_table_lookup as X
+
+    check_prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, _world_size(group))
+    placement, ctx = _placement(group, ctx)
+    return X._prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement)
 
 
 def _check_constants_sigmas_shard(prover_data, rank, world):
@@ -284,8 +355,9 @@ def check_prove_plonk(prover_data, common_data, world, rank=0):
 def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=None, *, salt_keys=None):
     """plonk.prove_with_witness on the ranks of a torch.distributed group (the default group if None): rank g commits
     row block g of the wires, Z / partial-product (+ lookup) and quotient LDEs, evaluates the quotient on its shard of
-    the quotient coset and answers the FRI queries that land in its rows. The Z's, partial products and lookup columns
-    (over all n rows), the openings (from the replicated coefficients) and the transcript are computed on every rank.
+    the quotient coset, sums block g of the replicated coefficients into the openings and answers the FRI queries that
+    land in its rows. The Z's, partial products and lookup columns (over all n rows) and the transcript are computed on
+    every rank.
     Collective: every rank passes the same full witness and returns the same ProofWithPublicInputs, whose bytes equal
     prove_with_witness's on one device. prover_data.constants_sigmas_commitment must be this rank's row-block shard
     (rank, world), built at circuit build with PolynomialBatch.from_values(..., shard=(rank, world)).

@@ -1834,8 +1834,9 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
     """prove_with_witness on a distributed.Placement. With G > 1 ranks this one holds row block g of the wires,
     Z / partial-product (+ lookup) and quotient commitments, and prover_data.constants_sigmas_commitment is that shard
     too: the caps are all-gathered before they are observed, the quotient is evaluated shard by shard and all-gathered,
-    and FRI routes the query openings between the ranks. The Z's, partial products and lookup columns, the openings and
-    the transcript run on every rank, so every rank returns the same proof."""
+    each rank sums its block of the coefficients into the openings and the ranks add up the partial sums, and FRI routes
+    the query openings between the ranks. The Z's, partial products and lookup columns and the transcript run on every
+    rank, so every rank returns the same proof."""
     from .challenger import Challenger
     from .fri import prove_openings
     from .hash import PoseidonHash
@@ -1911,7 +1912,8 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
         openings = OpeningSet.new(zeta, g, cs, wires_commitment, zs_commitment, quotient_commitment,
                                   constants_range=cd.constants_range(), sigmas_range=cd.sigmas_range(), zs_range=cd.zs_range(),
                                   partial_products_range=cd.partial_products_range(),
-                                  lookup_range=range(n_zs_pp, n_zs_pp + nc * cd.num_lookup_polys))
+                                  lookup_range=range(n_zs_pp, n_zs_pp + nc * cd.num_lookup_polys),
+                                  **placement.step_kwargs)
         for batch in openings.to_fri_openings():                       # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         oracles = [cs, wires_commitment, zs_commitment, quotient_commitment]

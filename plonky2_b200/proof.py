@@ -8,11 +8,14 @@ import numpy as np
 
 from . import _native as N
 from . import field as F
+from .distributed import Placement
 
 
-def eval_commitments(requests):
+def eval_commitments(requests, placement=Placement()):
     """requests: [(PolynomialBatch, point)], point in F_{p^2} as (c0, c1). Returns a list of (num_polys, 2) uint64 arrays
-    (eval_commitment, proof.rs:323-328), all from one gl_openings call."""
+    (eval_commitment, proof.rs:323-328), all from one gl_openings call. On a placement of G ranks the coefficients are
+    the same on every rank: rank g sums its block of each polynomial's coefficients (gl_openings_shard) and the ranks
+    add up the partial sums (Placement.openings_from_shards), so every rank returns the same arrays. Collective then."""
     if not requests:
         return []
     ctx = requests[0][0].ctx
@@ -26,9 +29,17 @@ def eval_commitments(requests):
     pidx = np.array(idx, dtype=np.uint32)
     points = np.array(pts, dtype=np.uint64).reshape(-1)
     total = sum(b.num_polys for b, _ in requests)
-    out = np.empty((total, 2), dtype=np.uint64)
-    N.check(N.lib().gl_openings(ctx.h, handles, pidx.ctypes.data_as(N.u32p), len(requests), N.np_ptr(points), len(pts),
-                                N.np_ptr(out), N.MEM_HOST), ctx.h)
+    if placement.num_shards == 1:
+        out = np.empty((total, 2), dtype=np.uint64)
+        N.check(N.lib().gl_openings(ctx.h, handles, pidx.ctypes.data_as(N.u32p), len(requests), N.np_ptr(points),
+                                    len(pts), N.np_ptr(out), N.MEM_HOST), ctx.h)
+    else:
+        def run_shard(partial):
+            N.check(N.lib().gl_openings_shard(ctx.h, handles, pidx.ctypes.data_as(N.u32p), len(requests),
+                                              N.np_ptr(points), len(pts), placement.shard_index, placement.num_shards,
+                                              N.np_ptr(partial), N.MEM_HOST), ctx.h)
+
+        out = placement.openings_from_shards(ctx, run_shard, total)
     res, off = [], 0
     for b, _ in requests:
         res.append(out[off:off + b.num_polys].copy())
@@ -51,13 +62,16 @@ class OpeningSet:
 
     @classmethod
     def new(cls, zeta, g, constants_sigmas_commitment, wires_commitment, zs_partial_products_lookup_commitment,
-            quotient_polys_commitment, constants_range, sigmas_range, zs_range, partial_products_range, lookup_range):
+            quotient_polys_commitment, constants_range, sigmas_range, zs_range, partial_products_range, lookup_range,
+            placement=Placement()):
         """OpeningSet::new (proof.rs:313-351). The *_range arguments are the CommonCircuitData ranges
-        (circuit_data.rs constants_range() ... lookup_range()) as Python ranges/slices."""
+        (circuit_data.rs constants_range() ... lookup_range()) as Python ranges/slices. placement: see
+        eval_commitments."""
         g_zeta = F.ext_mul((int(g[0]), int(g[1])) if isinstance(g, (tuple, list, np.ndarray)) else (int(g), 0), zeta)
         cs, zs, zs_next, quot, wires = eval_commitments([
             (constants_sigmas_commitment, zeta), (zs_partial_products_lookup_commitment, zeta),
-            (zs_partial_products_lookup_commitment, g_zeta), (quotient_polys_commitment, zeta), (wires_commitment, zeta)])
+            (zs_partial_products_lookup_commitment, g_zeta), (quotient_polys_commitment, zeta), (wires_commitment, zeta)],
+            **placement.step_kwargs)
 
         def take(a, r):
             return a[r.start:r.stop] if isinstance(r, (range, slice)) else a[list(r)]
@@ -90,10 +104,10 @@ class StarkOpeningSet:
 
     @classmethod
     def new(cls, zeta, g, trace_commitment, auxiliary_polys_commitment=None, quotient_commitment=None,
-            num_ctl_zs_first=None):
+            num_ctl_zs_first=None, placement=Placement()):
         """StarkOpeningSet::new (starky/src/proof.rs:221-265): trace (and auxiliary) polynomials at zeta and g*zeta,
         quotient polynomials at zeta; with num_ctl_zs_first = (first, count), the auxiliary polynomials first ..
-        first + count (the CTL Zs) at 1."""
+        first + count (the CTL Zs) at 1. placement: see eval_commitments."""
         g_zeta = F.ext_mul((int(g), 0), zeta)
         req = [(trace_commitment, zeta), (trace_commitment, g_zeta)]
         if auxiliary_polys_commitment is not None:
@@ -102,7 +116,7 @@ class StarkOpeningSet:
             req.append((quotient_commitment, zeta))
         if num_ctl_zs_first is not None:
             req.append((auxiliary_polys_commitment, (1, 0)))
-        res = eval_commitments(req)
+        res = eval_commitments(req, **placement.step_kwargs)
         k = 2
         aux = aux_next = quot = first = None
         if auxiliary_polys_commitment is not None:

@@ -713,7 +713,8 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
     the openings carry ctl_zs_first. trace: the values the lookup helper columns read (a CUDA tensor when the Stark has
     lookups). params: _check_prove_shapes's. placement: a distributed.Placement of G ranks proves on them, this one
     holding row block g of every commitment (trace_commitment too): the caps are all-gathered before they are observed,
-    the quotient is evaluated shard by shard and all-gathered, and FRI routes the query openings between the ranks.
+    the quotient is evaluated shard by shard and all-gathered, the openings are summed over each rank's block of the
+    coefficients and added up, and FRI routes the query openings between the ranks.
     Everything else runs redundantly on every rank, so every rank returns the same proof. Every commitment made here is
     released on every exit path; the trace commitment stays the caller's."""
     from .fri import prove_openings
@@ -773,7 +774,8 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
             raise N.NativeError("Opening point is in the subgroup.")
         g = F.primitive_root_of_unity(degree_bits)
         ctl_first = dict(num_ctl_zs_first=(nl + num_ctl_helpers, num_ctl_zs)) if stark.requires_ctls() else {}
-        openings = StarkOpeningSet.new(zeta, g, trace_commitment, aux_commitment, quotient_commitment, **ctl_first)
+        openings = StarkOpeningSet.new(zeta, g, trace_commitment, aux_commitment, quotient_commitment, **ctl_first,
+                                       **placement.step_kwargs)
         for batch in openings.to_fri_openings():                        # Challenger::observe_openings
             challenger.observe_elements(batch.reshape(-1))
         instance = stark.fri_instance(zeta, g, config, num_ctl_helpers, num_ctl_zs)
