@@ -2,7 +2,7 @@
 tests/test_stark_ctl.py (its CPU table also has a logUp lookup) from host columns and from torch device traces, and for
 a variant whose memory table has a logUp lookup of its own, every rank's MultiStarkProof equals
 cross_table_lookup.prove_with_ctls's on its own device, table by table -- caps, openings, ctl_zs_first, FRI bytes and
-proof-of-work witness -- and rank 0 has the restated verifier (tests/stark_ctl_twin.py) accept it. Too many ranks for
+proof-of-work witness -- and rank 0 has the restated verifier (tests/stark_twin.py) accept it. Too many ranks for
 the cap and a wrong trace count are refused on every rank. With fewer GPUs than ranks all ranks share GPU 0 and
 exchange through gloo, since NCCL refuses two ranks on one device. Launched by tests/test_stark_ctl_sharded.py, or by
 hand:
@@ -100,10 +100,10 @@ def main():
             pass
     if rank == 0:
         import oracle_lib
-        import stark_ctl_twin as CT
+        import stark_twin as T
 
         for name, st, cfg, cl, proof in proofs:
-            verdict = CT.verify(oracle_lib, st, cfg, cl, proof)
+            verdict = T.verify_with_ctls(oracle_lib, st, cfg, cl, proof)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
     everyone = [None] * world

@@ -1,10 +1,10 @@
 """distributed.prove_stark across ranks (run under torchrun, one rank per GPU): for FibonacciStark and the lookup
 RangeCheckStark of tests/test_stark_lookups.py at 2^12 - 2^14 rows in standard_fast_config, from host columns and from
 a torch device trace, every rank's proof equals stark.prove's on its own device -- caps, openings, FRI bytes and
-proof-of-work witness -- and rank 0 has the restated verifiers (tests/stark_twin.py, tests/stark_lookup_twin.py) accept
-it; a verifier circuit's FRI shape passes through; too many ranks for the cap and a Stark with CTLs are refused on every
-rank. With fewer GPUs than ranks all ranks share GPU 0 and exchange through gloo, since NCCL refuses two ranks on one
-device. Launched by tests/test_gpu_stark_sharded.py, or by hand:
+proof-of-work witness -- and rank 0 has the restated verifier (tests/stark_twin.py) accept it; a verifier circuit's
+FRI shape passes through; too many ranks for the cap and a Stark with CTLs are refused on every rank. With fewer GPUs
+than ranks all ranks share GPU 0 and exchange through gloo, since NCCL refuses two ranks on one device. Launched by
+tests/test_gpu_stark_sharded.py, or by hand:
   python -m torch.distributed.run --standalone --nproc-per-node 2 tests/mgpu_stark_check.py
 """
 import os
@@ -102,11 +102,10 @@ def main():
             pass
     if rank == 0:
         import oracle_lib
-        import stark_lookup_twin as LT
         import stark_twin as T
 
         for name, stark, proof in proofs:
-            verdict = (LT if stark.uses_lookups() else T).verify(oracle_lib, stark, config, proof)
+            verdict = T.verify(oracle_lib, stark, config, proof)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
     everyone = [None] * world

@@ -31,7 +31,6 @@ import numpy as np
 import pytest
 
 import gl_numpy as G
-import stark_lookup_twin as LT
 import stark_twin as T
 from conftest import EDGE, P, synth
 from plonky2_b200 import _native as N
@@ -316,7 +315,7 @@ def test_identities_reject_a_wrong_column():
     """The identity checks fail on a helper or Z column with one word changed, at the first and last rows."""
     stark, trace = RangeCheckStark(), range_check_trace(8)
     challenges = [int(v) for v in synth(0xE10, (2,))]
-    aux, _ = LT.aux_columns(stark, trace, challenges)
+    aux, _ = T.aux_columns(stark, trace, challenges)
     check_lookup_columns(stark, trace, challenges, aux, honest=True)
     for col, row in [(0, 0), (2, 255), (3, 17), (4, 255), (9, 1)]:
         bad = aux.copy()
@@ -372,7 +371,7 @@ def test_edge_operand_lookup_columns_on_host(logup_emu):
     f = _lookup_values(stark, trace)
     assert _hits([G.add(f, np.uint64(g)) for g in challenges]) == (True, True)
     assert not np.isin(trace[SEL], [0, 1]).all()
-    want, wraps = LT.aux_columns(stark, trace, challenges)
+    want, wraps = T.aux_columns(stark, trace, challenges)
     rc, got = _emu_helpers(logup_emu, stark, trace, challenges)
     assert rc == 0 and np.array_equal(got, want)
     check_lookup_columns(stark, trace, challenges, want, honest=False)
@@ -451,7 +450,7 @@ def test_device_lookup_columns_satisfy_the_identities(pb, case):
     assert got.shape == (stark._helper_columns_per_challenge() * len(challenges), 1 << log_n)
     check_lookup_columns(stark, trace, challenges, got, honest)
     if kind == "edge":
-        assert np.array_equal(got, LT.aux_columns(stark, trace, challenges)[0])
+        assert np.array_equal(got, T.aux_columns(stark, trace, challenges)[0])
 
 
 CTL_CASES = ["wide_22_d3_c4", "wide_22_d4_c1", "system_22_d3_c4", "system_22_d3_c1", "wide_24_d3_c1",
@@ -739,12 +738,12 @@ def replay_challenges(oracle, stark, config, proof, lookups):
     pairs = betas = None
     num_aux = 0
     if lookups:
-        pairs = LT._draw_lookup_challenges(ch, config.num_challenges)
+        pairs = T._draw_lookup_challenges(ch, config.num_challenges)
         betas = [bt for bt, _ in pairs]
         ch.observe_cap(p.auxiliary_polys_cap.hashes)
         num_aux = len(p.openings.auxiliary_polys)
-    alphas = LT.bind_constraints(ch, stark, list(proof.public_inputs), config.num_challenges, degree_bits, betas,
-                                 num_aux)
+    alphas = T.bind_constraints(ch, stark, list(proof.public_inputs), config.num_challenges, degree_bits, betas,
+                                num_aux)
     ch.observe_cap(p.quotient_polys_cap.hashes)
     return pairs, alphas, ch.get_extension_challenge()
 
@@ -790,12 +789,12 @@ def test_prove_range_check_2_20_from_a_torch_trace(pb, oracle):
     stark, config = RangeCheckStark(), S.StarkConfig.standard_fast_config()
     trace = range_check_trace(20, seed=20)
     proof = S.prove(stark, config, _to_device(trace), [0])
-    assert LT.verify(oracle, stark, config, proof) is None
+    assert T.verify(oracle, stark, config, proof) is None
     _check_replay(oracle, stark, config, proof, True)
-    assert LT.verify(oracle, stark, config, _opening_changed(proof, "auxiliary_polys")) is not None
-    assert LT.verify(oracle, stark, config, _fri_byte_changed(proof)) is not None
+    assert T.verify(oracle, stark, config, _opening_changed(proof, "auxiliary_polys")) is not None
+    assert T.verify(oracle, stark, config, _fri_byte_changed(proof)) is not None
     trace[MA, 5] += np.uint64(1)
-    assert LT.verify(oracle, stark, config, S.prove(stark, config, _to_device(trace), [0])) == (
+    assert T.verify(oracle, stark, config, S.prove(stark, config, _to_device(trace), [0])) == (
         "Mismatch between evaluation and opening of quotient polynomial")
 
 
@@ -924,15 +923,14 @@ def test_equal_height_system_traces_satisfy_the_ctls():
 def test_prove_with_ctls_2_18(pb, oracle):
     """The three-table system at 2^18 rows per table: accepted by the restated verifier; with one looking tuple moved
     where its filter is on, every table still proves and the cross-table check rejects."""
-    import stark_ctl_twin as CT
     from test_stark_ctl import MG, MR, system
 
     starks, config, ctls = system()
     traces, pis = system_traces_equal_heights(18)
     X.check_ctls(traces, ctls)
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis)
-    assert CT.verify(oracle, starks, config, ctls, mp) is None
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
     on = int(np.nonzero(traces[1][MG])[0][0])
     traces[1][MR, on] += np.uint64(1)
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis)
-    assert CT.verify(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."

@@ -8,7 +8,7 @@ The test system has three tables of different heights, all with num_challenges =
   the looked table of CTL 1.
 - LookedTable (2^6 rows, degree 3) is CTL 0's looked table and looks into CTL 1.
 
-CPU: the restatement (tests/stark_ctl_twin.py) pinned by the CTL invariant and every column identity; the CTL terms of
+CPU: the restatement (tests/stark_twin.py) pinned by the CTL invariant and every column identity; the CTL terms of
 eval_vanishing_poly against hand-written formulas; the device row arithmetic run on the host (tests/emu/ctl_emu.cpp)
 against the restatement; prove_with_ctls's host logic with the oracle standing in for the device calls (field-for-field
 equal to the twin, accepted by the restated verifier, its transcript replayed by MultiStarkProof.get_challenges,
@@ -24,8 +24,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import stark_ctl_twin as CT
-import stark_lookup_twin as LT
+import stark_twin as T
 from conftest import P, synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import cross_table_lookup as X
@@ -152,7 +151,7 @@ def test_ctl_invariant_pins_the_restatement():
     traces, _ = system_traces()
     check_ctls(traces, ctls)
     pairs = _pairs(0xA00)
-    data = CT.cross_table_lookup_data(traces, ctls, pairs, 3)
+    data = T.cross_table_lookup_data(traces, ctls, pairs, 3)
     assert [len(d) for d in data] == [2, 4, 4]
     firsts = [[int(z["z"][0]) for z in d] for d in data]
     # CTL 0: table 0 (group), table 1, looked table 2; CTL 1: table 2 looking, table 1 looked
@@ -170,12 +169,12 @@ def test_ctl_invariant_pins_the_restatement():
                 row = sum(h, np.zeros(len(zz), dtype=object)) % P
                 for k, hk in enumerate(h):      # chunk k of two entries: h * c0 * c1 = f0 c1 + f1 c0
                     ents = list(zip(z["columns"], z["filter"]))[2 * k:2 * k + 2]
-                    cs = [CT.combine_rows(cols, tr, beta, gamma) for cols, _ in ents]
-                    fs = [LT.filter_eval_table(f, tr) for _, f in ents]
+                    cs = [T.combine_rows(cols, tr, beta, gamma) for cols, _ in ents]
+                    fs = [T.filter_eval_table(f, tr) for _, f in ents]
                     assert all(v % P == 0 for v in (hk * cs[0] * cs[1] - fs[0] * cs[1] - fs[1] * cs[0]))
             else:
-                c0 = CT.combine_rows(z["columns"][0], tr, beta, gamma)
-                row = LT._inv_each(c0) * LT.filter_eval_table(z["filter"][0], tr) % P
+                c0 = T.combine_rows(z["columns"][0], tr, beta, gamma)
+                row = T._inv_each(c0) * T.filter_eval_table(z["filter"][0], tr) % P
             assert zz[-1] == row[-1]
             assert all((zz[:-1] - zz[1:] - row[:-1]) % P == 0)
     # a tuple moved where its filter is on breaks the check and the sums; one moved where it is off does not
@@ -184,13 +183,13 @@ def test_ctl_invariant_pins_the_restatement():
     bad[1][MR, on] += np.uint64(1)
     with pytest.raises(ValueError, match="Cross-table lookup 0"):
         check_ctls(bad, ctls)
-    d = CT.cross_table_lookup_data(bad, ctls, pairs, 3)
+    d = T.cross_table_lookup_data(bad, ctls, pairs, 3)
     assert all((int(d[0][c]["z"][0]) + int(d[1][c]["z"][0])) % P != int(d[2][c]["z"][0]) for c in range(2))
     off = [t.copy() for t in traces]
     o = int(np.nonzero(off[1][MG] == 0)[0][0])
     off[1][MR, o] += np.uint64(1)
     check_ctls(off, ctls)
-    d = CT.cross_table_lookup_data(off, ctls, pairs, 3)
+    d = T.cross_table_lookup_data(off, ctls, pairs, 3)
     assert all((int(d[0][c]["z"][0]) + int(d[1][c]["z"][0])) % P == int(d[2][c]["z"][0]) for c in range(2))
     # extra looking values: a looked row nobody looks up
     extra = [t.copy() for t in traces]
@@ -281,7 +280,7 @@ def emu_lib(tmp_path_factory):
 
 def _groups_and_aux(traces, ctls, t, pairs, degree):
     groups = X.table_groups(ctls, t)
-    want = CT.ctl_aux(CT.cross_table_lookup_data(traces, ctls, pairs, degree)[t], traces[t].shape[1])
+    want = T.ctl_aux(T.cross_table_lookup_data(traces, ctls, pairs, degree)[t], traces[t].shape[1])
     return groups, want
 
 
@@ -344,7 +343,7 @@ def _cpu_ctl_backends(monkeypatch, oracle, calls):
 
     def lookup_helpers(stark_, trace, challenges, ctx_, out=None):
         calls.append(("helpers", [int(c) for c in challenges]))
-        cols = LT.aux_columns(stark_, np.asarray(trace), challenges)[0]
+        cols = T.aux_columns(stark_, np.asarray(trace), challenges)[0]
         if out is None:
             return cols
         out[...] = cols
@@ -357,7 +356,7 @@ def _cpu_ctl_backends(monkeypatch, oracle, calls):
 
     def quotient(stark_, tc, pis, alphas, auxiliary_polys_commitment=None, lookup_challenges=None, ctl_vars=None):
         aux = auxiliary_polys_commitment.o.coeffs if auxiliary_polys_commitment is not None else None
-        return CT.host_quotient(oracle, stark_, tc.o.coeffs, aux, pis, alphas, lookup_challenges or [], ctl_vars or [])
+        return T.host_quotient(oracle, stark_, tc.o.coeffs, pis, alphas, aux, lookup_challenges or [], ctl_vars or [])
 
     import plonky2_b200.fri as fri_mod
 
@@ -386,7 +385,7 @@ def _restated_table_aux(trace, groups, pairs, degree):
         for pr in pairs:
             for c, entries in groups:
                 if c == i:
-                    cols = CT.partial_sums(trace, [(t.columns, t.filter) for t in entries], pr, degree)
+                    cols = T.partial_sums(trace, [(t.columns, t.filter) for t in entries], pr, degree)
                     helpers += cols[:-1]
                     zs.append(cols[-1])
     return np.stack(helpers + zs)
@@ -418,12 +417,12 @@ def _tampered(mp, what):
 def test_prove_with_ctls_host_logic_with_cpu_backends(oracle, monkeypatch):
     starks, config, ctls = system()
     traces, pis = system_traces()
-    twin = CT.twin_prove(oracle, starks, config, traces, ctls, pis)
+    twin = T.twin_prove_with_ctls(oracle, starks, config, traces, ctls, pis)
     calls = []
     logs, ctx = _cpu_ctl_backends(monkeypatch, oracle, calls)
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis, ctx=ctx)
     _same_as_twin(mp, twin)
-    assert CT.verify(oracle, starks, config, ctls, mp) is None
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
     betas = [b for b, _ in twin["ctl_challenges"]]
     assert [c for c in calls if isinstance(c, tuple) and c[0] == "helpers"] == [("helpers", betas)]
     assert [c for c in calls if isinstance(c, tuple) and c[0] == "ctl"] == [("ctl", 1), ("ctl", 2), ("ctl", 2)]
@@ -436,8 +435,8 @@ def test_prove_with_ctls_host_logic_with_cpu_backends(oracle, monkeypatch):
     replay_draws = [v for kind, v in logs[1] if kind == "challenge"]
     assert replay_draws[:len(prover_draws)] == prover_draws
     for what in ("ctl_zs_first", "ctl_z_opening", "swapped"):
-        assert CT.verify(oracle, starks, config, ctls, _tampered(mp, what)) is not None, what
-    assert CT.verify(oracle, starks, config, ctls, _tampered(mp, "ctl_zs_first")).startswith("table 2")
+        assert T.verify_with_ctls(oracle, starks, config, ctls, _tampered(mp, what)) is not None, what
+    assert T.verify_with_ctls(oracle, starks, config, ctls, _tampered(mp, "ctl_zs_first")).startswith("table 2")
 
 
 class _Deg1(MemTable):
@@ -569,9 +568,9 @@ def test_prove_with_ctls_on_device_equals_cpu_twin(pb, oracle, source):
     arg = traces if source == "host" else [_to_device(t) for t in traces]
     torch.cuda.synchronize()
     mp = X.prove_with_ctls(starks, config, arg, ctls, pis)
-    twin = CT.twin_prove(oracle, starks, config, traces, ctls, pis)
+    twin = T.twin_prove_with_ctls(oracle, starks, config, traces, ctls, pis)
     _same_as_twin(mp, twin)
-    assert CT.verify(oracle, starks, config, ctls, mp) is None
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
     ch = mp.get_challenges(starks, config, ctls)
     assert [(c.beta, c.gamma) for c in ch["ctl_challenges"]] == twin["ctl_challenges"]
     for got, t in zip(ch["stark_challenges"], twin["tables"]):
@@ -589,7 +588,7 @@ def test_mismatched_system_proves_and_the_ctl_check_rejects(pb, oracle):
     with pytest.raises(ValueError):
         check_ctls(traces, ctls)
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis)
-    assert CT.verify(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."
 
 
 @pytest.mark.gpu
@@ -604,8 +603,8 @@ def test_extra_looking_sums(pb, oracle):
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis)
     ch = mp.get_challenges(starks, config, ctls)["ctl_challenges"]
     sums = [(pow((row[0] + c.beta * row[1] + c.gamma) % P, P - 2, P)) for c in ch]
-    assert CT.verify(oracle, starks, config, ctls, mp, {0: sums}) is None
-    assert CT.verify(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp, {0: sums}) is None
+    assert T.verify_with_ctls(oracle, starks, config, ctls, mp) == "Cross-table lookup 0 verification failed."
 
 
 @pytest.mark.gpu

@@ -8,7 +8,7 @@ looking columns (chunks of 2 + 1), one of them a linear combination with a next-
 product filter; the generator writes the frequencies and puts out-of-range values wherever a filter is off.
 
 CPU: eval_vanishing_poly's lookup terms against hand-written formulas; the device row arithmetic run on the host
-(tests/emu/logup_emu.cpp) bit-exact against the restatement of lookup_helper_columns (tests/stark_lookup_twin.py),
+(tests/emu/logup_emu.cpp) bit-exact against the restatement of lookup_helper_columns (tests/stark_twin.py),
 wrap-around next-row terms included; the logUp invariant pinning that restatement; prove's host logic with the oracle
 standing in for the device calls (accepted by the restated verifier, field-for-field equal to the CPU twin, transcript
 replayed by get_challenges, tampering rejected); every shape error.
@@ -24,7 +24,6 @@ import subprocess
 import numpy as np
 import pytest
 
-import stark_lookup_twin as LT
 import stark_twin as T
 from conftest import P, synth
 from plonky2_b200 import _native as N
@@ -288,7 +287,7 @@ def test_helper_rows_on_host_match_restatement(emu_lib, case):
         assert trace[SEL, -1] == 1 and trace[SEL2, -1] == 1
     challenges = [int(v) for v in synth(0x900, (2,))]
     rc, got = _emu_helpers(emu_lib, stark, trace, challenges)
-    want, wraps = LT.aux_columns(stark, trace, challenges)
+    want, wraps = T.aux_columns(stark, trace, challenges)
     assert rc == 0 and np.array_equal(got, want)
     assert wraps == [0] * len(wraps)
     if not case.startswith("permutation"):
@@ -313,7 +312,7 @@ def test_next_row_terms_on_host_match_restatement(emu_lib):
     trace = synth(0x940, (7, 64))
     challenges = [int(v) for v in synth(0x941, (2,))]
     rc, got = _emu_helpers(emu_lib, stark, trace, challenges)
-    want, _ = LT.aux_columns(stark, trace, challenges)
+    want, _ = T.aux_columns(stark, trace, challenges)
     assert rc == 0 and np.array_equal(got, want)
     # a next-row term read at row r belongs to row r - 1: the table and frequencies enter Z's step from row r - 1 to
     # r, so Z first differs at row r; the filter enters h at row r - 1 (row 0: at the last row, the wrap)
@@ -321,7 +320,7 @@ def test_next_row_terms_on_host_match_restatement(emu_lib):
         moved = trace.copy()
         moved[col, row] = (moved[col, row] + np.uint64(1)) % np.uint64(P)
         rc, got_moved = _emu_helpers(emu_lib, stark, moved, challenges)
-        assert rc == 0 and np.array_equal(got_moved, LT.aux_columns(stark, moved, challenges)[0])
+        assert rc == 0 and np.array_equal(got_moved, T.aux_columns(stark, moved, challenges)[0])
         for a in aux_cols:
             assert np.array_equal(got_moved[a, :first], got[a, :first]), col
             assert got_moved[a, first] != got[a, first], col
@@ -331,12 +330,12 @@ def test_logup_invariant_pins_the_restatement():
     """Z closes to 0 at the wrap exactly when the frequencies match the filtered looked multiset."""
     challenges = [int(v) for v in synth(0x910, (2,))]
     for stark, trace in [(_perm_case(5)[0], _perm_case(5)[2]), (RangeCheckStark(), RangeCheckStark.generate_trace(6))]:
-        _, wraps = LT.aux_columns(stark, trace, challenges)
+        _, wraps = T.aux_columns(stark, trace, challenges)
         assert wraps == [0] * len(wraps)
         bad = trace.copy()
         fcol = 2 if isinstance(stark, PermutationStark) else MB
         bad[fcol, 1] += np.uint64(1)
-        _, wraps = LT.aux_columns(stark, bad, challenges)
+        _, wraps = T.aux_columns(stark, bad, challenges)
         assert all(w != 0 for w in wraps[-len(challenges):])
     # a looked value moved where its filter is off does not matter; where it is on, it does
     trace = RangeCheckStark.generate_trace(6)
@@ -344,9 +343,9 @@ def test_logup_invariant_pins_the_restatement():
     on = int(np.nonzero(trace[SEL] == 1)[0][0])
     moved = trace.copy()
     moved[A0, off] = np.uint64(12345678901)
-    assert LT.aux_columns(RangeCheckStark(), moved, challenges)[1] == [0] * 4
+    assert T.aux_columns(RangeCheckStark(), moved, challenges)[1] == [0] * 4
     moved[A0, on] = np.uint64(12345678901)
-    assert LT.aux_columns(RangeCheckStark(), moved, challenges)[1][:2] != [0, 0]
+    assert T.aux_columns(RangeCheckStark(), moved, challenges)[1][:2] != [0, 0]
 
 
 def _cpu_lookup_backends(monkeypatch, oracle, stark, calls):
@@ -356,11 +355,11 @@ def _cpu_lookup_backends(monkeypatch, oracle, stark, calls):
 
     def helpers(stark_, trace, challenges, ctx_):
         calls.append(("helpers", [int(c) for c in challenges]))
-        return LT.aux_columns(stark_, np.asarray(trace), challenges)[0]
+        return T.aux_columns(stark_, np.asarray(trace), challenges)[0]
 
     def quotient(stark_, tc, pis, alphas, auxiliary_polys_commitment=None, lookup_challenges=None):
-        return LT.host_quotient(oracle, stark_, tc.o.coeffs, auxiliary_polys_commitment.o.coeffs, pis, alphas,
-                                lookup_challenges)
+        return T.host_quotient(oracle, stark_, tc.o.coeffs, pis, alphas, auxiliary_polys_commitment.o.coeffs,
+                               lookup_challenges)
 
     monkeypatch.setattr(S, "_device_trace", lambda trace, ctx_: np.asarray(trace))
     monkeypatch.setattr(S, "compute_lookup_helper_columns", helpers)
@@ -403,13 +402,13 @@ def _tampered(proof, what):
 @pytest.mark.parametrize("case", ["permutation", "range_check"])
 def test_prove_host_logic_with_cpu_backends(oracle, monkeypatch, case):
     stark, config, trace, pi = _perm_case(5) if case == "permutation" else _range_case(5)
-    twin = LT.twin_prove(oracle, stark, config, trace, pi)
+    twin = T.twin_prove(oracle, stark, config, trace, pi)
     calls = []
     logs, ctx = _cpu_lookup_backends(monkeypatch, oracle, stark, calls)
     proof = S.prove(stark, config, trace, pi, ctx=ctx)
     assert calls.count("close") == (2 if case == "permutation" else 3)
     _same_as_twin(proof, twin)
-    assert LT.verify(oracle, stark, config, proof) is None
+    assert T.verify(oracle, stark, config, proof) is None
     nq = stark.num_quotient_polys(config)
     assert len(proof.proof.opening_proof.query_round_proofs[0].initial_trees_proof.evals_proofs) == (3 if nq else 2)
     helpers = [c for c in calls if isinstance(c, tuple) and c[0] == "helpers"]
@@ -421,8 +420,8 @@ def test_prove_host_logic_with_cpu_backends(oracle, monkeypatch, case):
     assert [(c.beta, c.gamma) for c in ch["lookup_challenge_set"]] == twin["lookup_challenge_set"]
     assert ch["stark_alphas"] == twin["alphas"] and ch["stark_zeta"] == twin["zeta"]
     for what in ["aux_opening", "aux_next_opening", "aux_cap", "dropped_aux_cap"]:
-        assert LT.verify(oracle, stark, config, _tampered(proof, what)) is not None, what
-    assert LT.verify(oracle, stark, config, _tampered(proof, "dropped")) == "Missing auxiliary_polys_cap"
+        assert T.verify(oracle, stark, config, _tampered(proof, what)) is not None, what
+    assert T.verify(oracle, stark, config, _tampered(proof, "dropped")) == "Missing auxiliary_polys_cap"
     with pytest.raises(N.ShapeError, match="Missing auxiliary_polys_cap"):
         _tampered(proof, "dropped").get_challenges(stark, config)
 
@@ -501,7 +500,7 @@ def test_device_helper_columns_equal_restatement(pb, case):
     dev = _to_device(trace)
     torch.cuda.synchronize()
     got = S.compute_lookup_helper_columns(stark, dev, challenges, pb.default_context()).cpu().numpy().view(np.uint64)
-    want, wraps = LT.aux_columns(stark, trace, challenges)
+    want, wraps = T.aux_columns(stark, trace, challenges)
     assert np.array_equal(got, want)
     if case.startswith("range"):
         assert wraps == [0] * 4
@@ -525,9 +524,9 @@ def test_prove_on_device_equals_cpu_twin(pb, oracle, name, source):
         arg = _to_device(trace)
         torch.cuda.synchronize()
     proof = S.prove(stark, config, arg, pi)
-    twin = LT.twin_prove(oracle, stark, config, trace, pi)
+    twin = T.twin_prove(oracle, stark, config, trace, pi)
     _same_as_twin(proof, twin)
-    assert LT.verify(oracle, stark, config, proof) is None
+    assert T.verify(oracle, stark, config, proof) is None
     ch = proof.get_challenges(stark, config)
     assert [(c.beta, c.gamma) for c in ch["lookup_challenge_set"]] == twin["lookup_challenge_set"]
     assert ch["stark_alphas"] == twin["alphas"] and ch["stark_zeta"] == twin["zeta"]
@@ -540,11 +539,11 @@ def test_prove_on_device_with_a_wrong_frequency(pb, oracle):
     restated verifier rejects it at zeta. At degree 4 (three chunks) prove raises "Quotient has failed"."""
     stark, config, trace, pi = _range_case(10)
     trace[MA, 5] += np.uint64(1)
-    assert LT.verify(oracle, stark, config, S.prove(stark, config, trace, pi)) == (
+    assert T.verify(oracle, stark, config, S.prove(stark, config, trace, pi)) == (
         "Mismatch between evaluation and opening of quotient polynomial")
     stark4, config4 = RangeCheckStark4(), T_config_rate2()
     trace = RangeCheckStark.generate_trace(10, count_combination=False)
-    assert LT.verify(oracle, stark4, config4, S.prove(stark4, config4, trace, pi)) is None
+    assert T.verify(oracle, stark4, config4, S.prove(stark4, config4, trace, pi)) is None
     trace[MA, 5] += np.uint64(1)
     with pytest.raises(pb.NativeError, match="Quotient has failed"):
         S.prove(stark4, config4, trace, pi)

@@ -6,7 +6,7 @@ columns behind sparse boolean selectors.
 Prints one JSON line: the GPU's name and power limit, the median of --reps full proofs after --warmup (each ends in a
 device synchronise), one proof's per-phase times (trace commitments, CTL helper columns, auxiliary commitments,
 constraint-binding steps, quotients, quotient commitments, openings, FRI; measured in a separate run with a synchronise
-after each phase, summed over the tables), and whether the restated verifier of tests/stark_ctl_twin.py accepts.
+after each phase, summed over the tables), and whether the restated verifier of tests/stark_twin.py accepts.
 
 Usage: python tools/stark_ctl_cost.py [--log-n 22] [--reps 3] [--warmup 1]"""
 import argparse
@@ -122,7 +122,7 @@ def main():
     args = ap.parse_args()
 
     import oracle_lib
-    import stark_ctl_twin as CT
+    import stark_twin as T
     import torch
 
     import plonky2_b200 as pb
@@ -144,7 +144,7 @@ def main():
         proof = prove_with_ctls(starks, config, traces, ctls, pis, ctx=ctx)
         ctx.synchronize()
         ms.append((time.perf_counter() - t0) * 1e3)
-    accepted = CT.verify(oracle_lib, starks, config, ctls, proof) is None
+    accepted = T.verify_with_ctls(oracle_lib, starks, config, ctls, proof) is None
     phases = phase_times(starks, config, traces, ctls, ctx)
     out = {"gpu": gpu_info(),
            "workload": "prove_with_ctls: 3 tables of 2^%d x 6, 2^%d x 3, 2^%d x 3 columns, one CTL (2 + 1 looking "

@@ -5,7 +5,7 @@ StarkConfig.standard_fast_config (rate 1/2, so constraint degree 3: chunks of tw
 Prints one JSON line: the GPU's name and power limit, the median of --reps full proofs after --warmup (each ends in a
 device synchronise), one proof's per-phase times (trace commitment, lookup helper columns, auxiliary commitment,
 constraint-binding step, quotient, quotient commitment, openings, FRI; measured in a separate run with a synchronise
-after each phase), and whether the restated verifier of tests/stark_lookup_twin.py accepts the proof.
+after each phase), and whether the restated verifier of tests/stark_twin.py accepts the proof.
 
 Usage: python tools/stark_lookup_cost.py [--log-n 22] [--reps 3] [--warmup 1]"""
 import argparse
@@ -124,7 +124,7 @@ def main():
     args = ap.parse_args()
 
     import oracle_lib
-    import stark_lookup_twin as LT
+    import stark_twin as T
     import torch
 
     import plonky2_b200 as pb
@@ -144,7 +144,7 @@ def main():
         proof = S.prove(stark, config, trace, [], ctx=ctx)
         ctx.synchronize()
         ms.append((time.perf_counter() - t0) * 1e3)
-    accepted = LT.verify(oracle_lib, stark, config, proof) is None
+    accepted = T.verify(oracle_lib, stark, config, proof) is None
     phases = phase_times(stark, config, trace, ctx)
     out = {"gpu": gpu_info(),
            "workload": "starky prove with logUp: RangeCheckStark, %d limb columns (%d filtered) in a 2^%d table, "
