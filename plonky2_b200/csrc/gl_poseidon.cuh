@@ -29,7 +29,8 @@
 // sum is < 2^53, so doubles are exact. Define GL_MDS_INT to force the integer (IMAD.WIDE) formulation.
 // Other measured alternatives kept as switches: GL_PARTIAL_FAST (integer rounds everywhere),
 // GL_CVT_MAGIC (2^52 magic-number conversions on the FP64 pipe everywhere), GL_SBOX_I2F (I2F in the S-box),
-// GL_SBOX_SQR4 (four-product squarings in the S-box); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT,
+// GL_SBOX_SQR4 (four-product squarings in the S-box), GL_PAIR_RENORM_F64 (the partial-round pair's former form:
+// two separate rank-one updates, renormalisation on the FP64 pipe); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT,
 // GL_REDUCE_V1. tools/variants/ ranks them with one GPU call.
 #if !defined(GL_MDS_INT) && !defined(GL_MDS_FP64)
 #define GL_MDS_FP64 1
@@ -81,6 +82,15 @@ struct PoseidonTables {
     // pan_f64[pair] = cA_0 split WITHOUT bias (the bias is added at the conversion).
     double pks_f64[11][24];
     double pan_f64[11][2];
+    // The default pair (poseidon_partial_rounds_f64) holds lanes 1..11 SHIFTED: y = x - d[pair] (mod p) with d[0] = 0,
+    // d[pair + 1] = C*C*d[pair] + k2[pair] on lanes 1..11 (d_0 = 0 always), so that a pair adds no constant to them
+    // and only these few constants are read inside the loop:
+    // pk0_f64[pair] = lane 0's constant e0 = (C*C*d + k2)_0 + bias, halved: the seed of both row-0 accumulators of
+    // circ12_f64 (the halves cancel in out[6]); pad_f64[pair] = cA_0 + (M*d)_0 in 32-bit halves, no bias;
+    // pdf_f64 = d[11] + bias on lanes 1..11 ([2(i-1)] low half, [2(i-1)+1] high half), added once after the last pair.
+    double pk0_f64[11][2];
+    double pad_f64[11][2];
+    double pdf_f64[22];
 };
 
 #if defined(__CUDACC__)
@@ -125,27 +135,57 @@ inline const PoseidonTables& host_poseidon_tables() {
         for (int i = 0; i < 12; i++)
             for (int j = 0; j < 12; j++)
                 M[i][j] = GL_POSEIDON_MDS_CIRC[(j - i + 12) % 12] + ((i == 0 && j == 0) ? GL_POSEIDON_MDS_DIAG[0] : 0);
+        const unsigned __int128 PP = (unsigned __int128)0xFFFFFFFF00000001ULL;
+        uint64_t CC[12][12];  // C*C, C = M without its diagonal
+        for (int i = 0; i < 12; i++)
+            for (int j = 0; j < 12; j++) {
+                CC[i][j] = 0;
+                for (int t = 0; t < 12; t++) CC[i][j] += GL_POSEIDON_MDS_CIRC[(t - i + 12) % 12] * GL_POSEIDON_MDS_CIRC[(j - t + 12) % 12];
+            }
+        uint64_t d[12] = {0};  // the shift of lanes 1..11 going into pair pr
         for (int pr = 0; pr < 11; pr++) {
             const uint64_t* cA = &x.rc[12 * (5 + 2 * pr)];      // constants after round A = 2*pr
             const uint64_t* cB = &x.rc[12 * (5 + 2 * pr + 1)];  // constants after round B = 2*pr + 1
             x.pan_f64[pr][0] = (double)(uint32_t)cA[0];
             x.pan_f64[pr][1] = (double)(uint32_t)(cA[0] >> 32);
             double k2[12][2];
+            uint64_t k2r[12];
             for (int i = 0; i < 12; i++) {
                 unsigned __int128 k = cB[i];
                 for (int t = 0; t < 12; t++) k += (unsigned __int128)M[i][t] * cA[t];
-                const unsigned __int128 PP = (unsigned __int128)0xFFFFFFFF00000001ULL;
                 if (i == 0) k += 8 * (PP - cA[0] % PP);  // - 8*cA_0 on lane 0
                 const uint64_t kr = (uint64_t)(k % PP);
+                k2r[i] = kr;
                 const bool biased = (i == 0) || (pr == 10);
                 k2[i][0] = (double)(uint32_t)kr + (biased ? bl : 0.0);
                 k2[i][1] = (double)(uint32_t)(kr >> 32) + (biased ? bh : 0.0);
+            }
+            {
+                unsigned __int128 a = cA[0];
+                for (int t = 0; t < 12; t++) a += (unsigned __int128)M[0][t] * d[t];
+                const uint64_t ar = (uint64_t)(a % PP);
+                x.pad_f64[pr][0] = (double)(uint32_t)ar;
+                x.pad_f64[pr][1] = (double)(uint32_t)(ar >> 32);
+                uint64_t e[12];
+                for (int i = 0; i < 12; i++) {
+                    unsigned __int128 v = k2r[i];
+                    for (int t = 0; t < 12; t++) v += (unsigned __int128)CC[i][t] * d[t];
+                    e[i] = (uint64_t)(v % PP);
+                }
+                x.pk0_f64[pr][0] = ((double)(uint32_t)e[0] + bl) * 0.5;
+                x.pk0_f64[pr][1] = ((double)(uint32_t)(e[0] >> 32) + bh) * 0.5;
+                d[0] = 0;
+                for (int i = 1; i < 12; i++) d[i] = e[i];
             }
             for (int q = 0; q < 6; q++)
                 for (int l = 0; l < 2; l++) {
                     x.pks_f64[pr][12 * l + q] = (k2[q][l] + k2[q + 6][l]) * 0.5;
                     x.pks_f64[pr][12 * l + 6 + q] = (k2[q][l] - k2[q + 6][l]) * 0.5;
                 }
+        }
+        for (int i = 1; i < 12; i++) {
+            x.pdf_f64[2 * (i - 1)] = (double)(uint32_t)d[i] + bl;
+            x.pdf_f64[2 * (i - 1) + 1] = (double)(uint32_t)(d[i] >> 32) + bh;
         }
         return x;
     }();
@@ -240,6 +280,34 @@ GL_HD double u32_magic_f64(uint32_t x) {
     return __hiloint2double(0x43300000, (int)x);
 #else
     const uint64_t b = 0x4330000000000000ULL | x;
+    double d;
+    __builtin_memcpy(&d, &b, 8);
+    return d;
+#endif
+}
+// The words of a double's bit pattern, and a double from a bit pattern (register moves on the device).
+GL_HD uint32_t f64_lo_word(double x) {
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__double2loint(x);
+#else
+    uint64_t b;
+    __builtin_memcpy(&b, &x, 8);
+    return (uint32_t)b;
+#endif
+}
+GL_HD uint32_t f64_hi_word(double x) {
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__double2hiint(x);
+#else
+    uint64_t b;
+    __builtin_memcpy(&b, &x, 8);
+    return (uint32_t)(b >> 32);
+#endif
+}
+GL_HD double f64_from_bits(uint64_t b) {
+#if defined(__CUDA_ARCH__)
+    return __longlong_as_double((long long)b);
+#else
     double d;
     __builtin_memcpy(&d, &b, 8);
     return d;
@@ -488,19 +556,89 @@ GL_HD void poseidon_partial_rounds_noconst(uint64_t s[12]) {
 //     a  = (M x~)_0 + cA_0                                                        (12 DFMAs per limb)
 //     x' = Q x~ + a^7 * M[:,0] + k,   Q = M diag(0,1..1) M,  k = M diag(0,1..1) cA + cB
 //        = C*C*x~ + 8*x~0*C[:,0] + (a^7 - a)*M[:,0] + 8*a*e0 + k2,   k2 = M*cA + cB - 8*cA_0*e0
-// so that the split-circulant form (circ12_f64) applies to C*C: 135 FP64 operations per limb instead of 2 x 144.
-// All matrix entries are compile-time literals (DFMA immediates); k2 and cA_0 come from PoseidonTables::pks_f64 /
-// pan_f64.
-// Exactness: limbs are integers. After a renormalisation |L|, |H| <= 2^31 + 2^18; the row sums of Q are
-// <= 264^2 (those of C*C are 256^2), lane 0 enters with |L| < 2^33 (sbox7_f64), so a pair stays < 2^49 < 2^53; then lanes 1..11 are
-// renormalised ON THE FP64 PIPE (round to a multiple of 2^32 with the 1.5*2^84 trick; 2^64 = 2^32 - 1 moves the
-// carry of H into L) -- 9 FP64 ops per lane per pair. Limbs that are converted to integers (lane 0 twice per
-// pair, all lanes after the last pair) can be negative, so their constants carry a bias (bl, bh) = 0 (mod p) of
-// 2^50 and f64_pair_to_u64 sees non-negative integers < 2^51 (tests/emu/poseidon_f64_emu.cpp tracks the bound).
+// so that the split-circulant form (circ12_f64) applies to C*C, and with M[:,0] = C[:,0] + 8*e0 the three rank-one
+// terms are one: 8*x~0*C[:,0] + (a^7 - a)*M[:,0] + 8*a*e0 = (8*x~0 + a^7 - a)*C[:,0] + 8*a^7*e0
+// (partial_pair_limbs): 96 + 15 FP64 operations per limb (-DGL_PAIR_RENORM_F64: 96 + 26, the terms one by one).
+// All matrix entries are compile-time literals (DFMA immediates). The constants k2 would cost 24 constant loads
+// indexed by the pair counter per pair, so lanes 1..11 are held shifted, y = x - d[pair] (mod p), with
+// d[pair + 1] = C*C*d[pair] + k2 chosen on the host so that a pair adds nothing to them: only lane 0's constant and
+// a's (PoseidonTables::pk0_f64 / pad_f64) are read per pair, and d[11] once after the last pair (pdf_f64).
+// Under GL_PAIR_RENORM_F64 the pair reads k2 and cA_0 from pks_f64 / pan_f64.
+// Exactness: limbs are integers. After a renormalisation -2^18 < L, H < 2^32 + 2^18 (partial_pair_renorm;
+// |L|, |H| <= 2^31 + 2^18 under GL_PAIR_RENORM_F64); the row sums of Q are <= 264^2 (those of C*C are 256^2),
+// lane 0 enters with |L| < 2^33.6, 0 <= H < 2^33 (sbox7_f64), so an unbiased lane of a pair stays < 2^49 < 2^53 and
+// the sums of halves inside circ12_f64 below 2^52; then lanes 1..11 are renormalised: X + 1.5*2^52 exposes
+// X = r + 2^32*q in its bit pattern, and 2^64 = 2^32 - 1 folds the high limb's q back (5 ALU + 4 FP64
+// instructions per lane; under GL_PAIR_RENORM_F64 9 FP64 operations that round to multiples of 2^32 with
+// 1.5*2^84). Limbs that are converted to integers (lane 0 twice per pair, all lanes after the last pair) can be
+// negative, so their constants carry a bias (bl, bh) = 0 (mod p) of 2^50 and f64_pair_to_u64 sees non-negative
+// integers < 2^51 (tests/emu/poseidon_f64_emu.cpp tracks the bound).
 // Versus the "fast" integer form (23 64x64 products + 12 reductions per round, all on the integer pipes that
 // bound this kernel): no init matrix, ~90 integer instructions per round instead of ~520.
 // In: s after full round 4's MDS + first partial constant layer (original constants). Out: s after the last
 // partial round's MDS + the 5th full round's constant layer.
+// One limb vector of a pair: v <- C*C*v + k + (rank-one terms), with x0 = v[0] = x~0's limb, z = a^7's, a = a's.
+// k: the constants in seed form (GL_PAIR_RENORM_F64, a row of pks_f64), else lane 0's halved constant only
+// (pk0_f64: the shifted lanes 1..11 get none).
+GL_HD void partial_pair_limbs(double v[12], const double* k, double z, double a) {
+    const double x0 = v[0];
+    double n[12];
+#if defined(GL_PAIR_RENORM_F64)
+    circ12_f64<MdsCirc2>(v, k, n);
+#else
+    const double seed[12] = {k[0], 0, 0, 0, 0, 0, k[0], 0, 0, 0, 0, 0};  // out[0] = 2*k[0], out[6] = 0
+    circ12_f64<MdsCirc2>(v, seed, n);
+#endif
+#if defined(GL_PAIR_RENORM_F64)
+    const double za = z - a;
+#pragma unroll
+    for (int i = 0; i < 12; i++) {
+        n[i] = f64_fma(x0, 8.0 * MdsCirc::c(12 - i), n[i]);  // 8 * x~0 * C[:,0]
+        n[i] = f64_fma(za, (double)mds_entry(i, 0), n[i]);   // (a^7 - a) * M[:,0]
+    }
+    n[0] = f64_fma(a, 8.0, n[0]);
+#else
+    // 8*x~0*C[:,0] + (a^7 - a)*M[:,0] + 8*a*e0 = (8*x~0 + a^7 - a)*C[:,0] + 8*a^7*e0   (M[:,0] = C[:,0] + 8*e0)
+    const double w = f64_fma(x0, 8.0, z - a);
+#pragma unroll
+    for (int i = 0; i < 12; i++) n[i] = f64_fma(w, MdsCirc::c(12 - i), n[i]);
+    n[0] = f64_fma(z, 8.0, n[0]);
+#endif
+#pragma unroll
+    for (int i = 0; i < 12; i++) {
+        v[i] = n[i];
+        GL_F64_TRACK(n[i]);
+    }
+}
+// Renormalise a lane between pairs: integers |L|, |H| < 2^49 -> L', H' with L' + 2^32*H' = L + 2^32*H (mod p).
+GL_HD void partial_pair_renorm(double& L, double& H) {
+#if defined(GL_PAIR_RENORM_F64)
+    // on the FP64 pipe: round H to a multiple of 2^32 (x + 1.5*2^84 - 1.5*2^84), move that carry into L with
+    // 2^64 = 2^32 - 1, round L the same way and move its carry into H: |L'|, |H'| <= 2^31 + 2^18, 9 FP64 operations
+    const double C84 = 29014219670751100192948224.0;  // 1.5 * 2^84: x + C84 is rounded to a multiple of 2^32
+    const double I32 = 2.3283064365386962890625e-10;  // 2^-32
+    const double th = (H + C84) - C84;
+    const double hlo = H - th;
+    const double l2 = f64_fma(th, -I32, L);
+    const double tl = (l2 + C84) - C84;
+    L = l2 - tl;
+    H = f64_fma(tl, I32, f64_fma(th, I32, hlo));
+#else
+    // through the integer pipes: X + 1.5*2^52 (exact, |X| < 2^51) has the bit pattern hX : rX = 0x43380000 + qX : rX
+    // with X = rX + 2^32*qX, 0 <= rX < 2^32, |qX| <= 2^17. With 2^64 = 2^32 - 1 the value is
+    // (rL - qH) + 2^32*(rH + qL + qH). Both limbs are assembled as 2^52-offset bit patterns by a three-input add
+    // and its carry (IADD3, IADD3.X and for H' a LOP3 that ORs in the exponent, on the ALU pipe, nearly idle here),
+    // and one DADD each removes the offset: 4 FP64 and 5 ALU instructions instead of 9 FP64 ones,
+    // -2^18 < L', H' < 2^32 + 2^18.
+    const double tL = L + 6755399441055744.0, tH = H + 6755399441055744.0;  // + 1.5 * 2^52
+    const uint32_t rL = f64_lo_word(tL), hL = f64_hi_word(tL), rH = f64_lo_word(tH), hH = f64_hi_word(tH);
+    // 2^52 + 2^32 + rL - (qH + 2^19)  and  2^52 + rH + (qL + qH + 0x86700000)
+    const uint64_t yl = (0x4330000143300000ULL + rL) - hH;
+    const uint64_t yh = 0x4330000000000000ULL + rH + hL + hH;
+    L = f64_from_bits(yl) - 4503603921813504.0;  // 2^52 + 2^32 - 2^19
+    H = f64_from_bits(yh) - 4503601882857472.0;  // 2^52 + 0x86700000
+#endif
+}
 GL_HD void poseidon_partial_rounds_f64(uint64_t s[12]) {
     const PoseidonTables& T = GL_POS;
     double L[12], H[12];
@@ -514,7 +652,11 @@ GL_HD void poseidon_partial_rounds_f64(uint64_t s[12]) {
     for (int rp = 0; rp < 11; rp++) {
         sbox7_f64(s0, L[0], H[0]);  // x~0 = x0^7: signed low limb, |L[0]| < 2^33
         // a = (M x~)_0 + cA_0 (no bias in the limbs; the bias (bl, bh) = 0 (mod p) is added for the conversion only)
+#if defined(GL_PAIR_RENORM_F64)
         double aL = T.pan_f64[rp][0], aH = T.pan_f64[rp][1];
+#else
+        double aL = T.pad_f64[rp][0], aH = T.pad_f64[rp][1];  // + (M d)_0: lanes 1..11 hold x - d
+#endif
 #pragma unroll
         for (int j = 0; j < 12; j++) {
             aL = f64_fma(L[j], (double)mds_entry(0, j), aL);
@@ -522,55 +664,30 @@ GL_HD void poseidon_partial_rounds_f64(uint64_t s[12]) {
         }
         double zL, zH;
         sbox7_f64(f64_pair_to_u64(aL + (1125899906842624.0 + 262144.0), aH + (1125899906842624.0 - 524288.0)), zL, zH);
-        zL -= aL;  // z0 - a
-        zH -= aH;
+#if defined(GL_PAIR_RENORM_F64)
         const double* k = T.pks_f64[rp];
-        {
-            double n[12];
-            circ12_f64<MdsCirc2>(L, k, n);
-#pragma unroll
-            for (int i = 0; i < 12; i++) {
-                n[i] = f64_fma(L[0], 8.0 * MdsCirc::c(12 - i), n[i]);        // 8 * x~0 * C[:,0]
-                n[i] = f64_fma(zL, (double)mds_entry(i, 0), n[i]);           // (a^7 - a) * M[:,0]
-            }
-            n[0] = f64_fma(aL, 8.0, n[0]);
-#pragma unroll
-            for (int i = 0; i < 12; i++) {
-                L[i] = n[i];
-                GL_F64_TRACK(n[i]);
-            }
-        }
-        {
-            double n[12];
-            circ12_f64<MdsCirc2>(H, k + 12, n);
-#pragma unroll
-            for (int i = 0; i < 12; i++) {
-                n[i] = f64_fma(H[0], 8.0 * MdsCirc::c(12 - i), n[i]);
-                n[i] = f64_fma(zH, (double)mds_entry(i, 0), n[i]);
-            }
-            n[0] = f64_fma(aH, 8.0, n[0]);
-#pragma unroll
-            for (int i = 0; i < 12; i++) {
-                H[i] = n[i];
-                GL_F64_TRACK(n[i]);
-            }
-        }
+        partial_pair_limbs(L, k, zL, aL);
+        partial_pair_limbs(H, k + 12, zH, aH);
+#else
+        partial_pair_limbs(L, &T.pk0_f64[rp][0], zL, aL);
+        partial_pair_limbs(H, &T.pk0_f64[rp][1], zH, aH);
+#endif
         s0 = f64_pair_to_u64(L[0], H[0]);
         if (rp != 10) {
-            const double C84 = 29014219670751100192948224.0;  // 1.5 * 2^84: x + C84 is rounded to a multiple of 2^32
-            const double I32 = 2.3283064365386962890625e-10;  // 2^-32
 #pragma unroll
-            for (int i = 1; i < 12; i++) {
-                const double th = (H[i] + C84) - C84;
-                const double hlo = H[i] - th;
-                const double l2 = f64_fma(th, -I32, L[i]);
-                const double tl = (l2 + C84) - C84;
-                L[i] = l2 - tl;
-                H[i] = f64_fma(tl, I32, f64_fma(th, I32, hlo));
-            }
+            for (int i = 1; i < 12; i++) partial_pair_renorm(L[i], H[i]);
         }
     }
     s[0] = s0;
+#if !defined(GL_PAIR_RENORM_F64)
+#pragma unroll
+    for (int i = 1; i < 12; i++) {  // x = y + d[11], plus the conversion bias
+        L[i] += T.pdf_f64[2 * (i - 1)];
+        H[i] += T.pdf_f64[2 * (i - 1) + 1];
+        GL_F64_TRACK(L[i]);
+        GL_F64_TRACK(H[i]);
+    }
+#endif
 #pragma unroll
     for (int i = 1; i < 12; i++) s[i] = f64_pair_to_u64(L[i], H[i]);
 }

@@ -27,6 +27,7 @@ VARIANTS = {
     "minb5": ["-DGL_HASH_MINB=5"],
     "sboxsqr4": ["-DGL_SBOX_SQR4"],
     "sboxi2f": ["-DGL_SBOX_I2F"],
+    "pairf64": ["-DGL_PAIR_RENORM_F64"],
     "parent": ["-DGL_HASH_MINB=5", "-DGL_SBOX_SQR4", "-DGL_SBOX_I2F"],
 }
 

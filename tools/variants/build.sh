@@ -14,6 +14,7 @@ v mulx -DGL_MUL_EXPLICIT
 v sqr3 -DGL_SQR_3WIDE
 v sboxsqr4 -DGL_SBOX_SQR4
 v sboxi2f -DGL_SBOX_I2F
+v pairf64 -DGL_PAIR_RENORM_F64                          # the partial-round pair before the ALU renormalisation
 v parent -DGL_SBOX_SQR4 -DGL_SBOX_I2F -DVB_MINB=5      # the S-box and budget before the spill-free change
 v parentb4 -DGL_SBOX_SQR4 -DGL_SBOX_I2F                # that S-box at the shipped budget
 v redv1 -DGL_REDUCE_V1
