@@ -23,10 +23,8 @@ from plonky2_b200 import plonk  # noqa: E402
 def main():
     import numpy as np
 
-    import zk_circuits as ZC
-    from test_circuit_data import instances_of, pairs_from_sigmas
-    from test_plonk_sharded import LOOKUP_64, _fri_cfg, _small_circuit
-    from test_zk_commit_and_prove import KEYS
+    from plonk_circuits import (KEYS, LOOKUP_64, instances_of, pairs_from_sigmas, quick_fri_config, shape_circuit,
+                                zk_circuit)
 
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     shared = torch.cuda.device_count() < world
@@ -40,15 +38,15 @@ def main():
     failures = []
 
     zk_cfg = plonk.standard_recursion_zk_config()
-    zk_c, _ = ZC.zk_circuit(plonk, zk_cfg, _fri_cfg(zk_cfg))
-    zk_rows, _, zk_pairs = plonk.blind_and_pad(zk_cfg, _fri_cfg(zk_cfg), instances_of(zk_c)[:14])
-    lookup = _small_circuit(LOOKUP_64, public_inputs=[2, 7, 1, 8])
+    zk_c, _ = zk_circuit(plonk, zk_cfg, quick_fri_config(zk_cfg))
+    zk_rows, _, zk_pairs = plonk.blind_and_pad(zk_cfg, quick_fri_config(zk_cfg), instances_of(zk_c)[:14])
+    lookup = shape_circuit(LOOKUP_64, 4, public_inputs=[2, 7, 1, 8])
     cases = [("lookups", lookup, instances_of(lookup), pairs_from_sigmas(lookup), {}),
              ("zk_keys", zk_c, zk_rows, pairs_from_sigmas(zk_c, [r for p in zk_pairs for r in p]),
               dict(salt_keys=KEYS))]
     for name, c, rows, pairs, kw in cases:
         cd = c.common
-        args = (c.config, _fri_cfg(c.config), rows, pairs, 0, cd.luts, c.lookup_rows, [9])
+        args = (c.config, quick_fri_config(c.config), rows, pairs, 0, cd.luts, c.lookup_rows, [9])
         whole = plonk.build_circuit_data(*args, ctx=ctx)
         mine = D.build_circuit_data(*args, ctx=ctx)
         try:

@@ -1,11 +1,11 @@
 """distributed.prove_plonk across ranks (run under torchrun, one rank per GPU): for a circuit without lookups (the device
 Z path), one with every gate type and a lookup table (the host Z path), LargeCircuit at 2^13 gates in the standard
 recursion config, and a zero-knowledge circuit with explicit salt keys, every rank's proof bytes equal
-prove_with_witness's on its own device, and rank 0 has the restated verifiers (tests/plonk_circuits.oracle_verify, and
-tests/zk_circuits.oracle_verify_zk for zero knowledge) accept them; a zero-knowledge proof with fresh keys is accepted
-too. Too many ranks for the cap and a constants/sigmas commitment of the wrong shard -- on one rank only -- are refused
-on every rank. With fewer GPUs than ranks all ranks share GPU 0 and exchange through gloo, since NCCL refuses two ranks on
-one device. Launched by tests/test_plonk_sharded.py, or by hand:
+prove_with_witness's on its own device, and rank 0 has the restated verifier (tests/plonk_circuits.oracle_verify, with
+and without zero knowledge) accept them; a zero-knowledge proof with fresh keys is accepted too. Too many ranks for the
+cap and a constants/sigmas commitment of the wrong shard -- on one rank only -- are refused on every rank. With fewer GPUs
+than ranks all ranks share GPU 0 and exchange through gloo, since NCCL refuses two ranks on one device. Launched by
+tests/test_plonk_sharded.py, or by hand:
   python -m torch.distributed.run --standalone --nproc-per-node 2 tests/mgpu_plonk_check.py
 """
 import os
@@ -26,22 +26,11 @@ from plonky2_b200 import plonk  # noqa: E402
 DIGEST = [11, 22, 33, 44]
 
 
-def parts_of(data, c, fri_params, cs_cap):
-    """What the restated verifier reads, from the proof bytes."""
-    proof = plonk.ProofWithPublicInputs.from_bytes(data, c.common, fri_params)
-    p, o = proof.proof, proof.proof.openings
-    keys = ("constants", "plonk_sigmas", "wires", "plonk_zs", "plonk_zs_next", "partial_products", "quotient_polys",
-            "lookup_zs", "lookup_zs_next")
-    return dict(constants_sigmas_cap=cs_cap, wires_cap=p.wires_cap.hashes, zs_cap=p.plonk_zs_partial_products_cap.hashes,
-                quotient_cap=p.quotient_polys_cap.hashes, openings={k: getattr(o, k) for k in keys},
-                fri_bytes=p.opening_proof.to_bytes(), public_inputs=list(proof.public_inputs))
-
-
 def main():
-    import zk_circuits as ZC
-    from test_gpu_plonk_large import _circuit as large_circuit
-    from test_plonk_sharded import LOOKUP_64, RECURSION_5, _fri_cfg, _small_circuit
-    from test_zk_commit_and_prove import KEYS
+    import oracle_lib
+    import plonk_circuits as PC
+    import plonk_large as PL
+    from plonk_circuits import KEYS, LOOKUP_64, RECURSION_5, quick_fri_config, shape_circuit
 
     from plonky2_b200.fri import standard_recursion_fri_config
 
@@ -57,16 +46,16 @@ def main():
     failures = []
 
     zk_cfg = plonk.standard_recursion_zk_config()
-    zk_c, _ = ZC.zk_circuit(plonk, zk_cfg, _fri_cfg(zk_cfg))
-    cases = [("no_lookups", _small_circuit(RECURSION_5, public_inputs=[3, 1, 4, 1, 5]), None, {}),
-             ("lookups", _small_circuit(LOOKUP_64, public_inputs=[2, 7, 1, 8]), None, {}),
-             ("large_2_13", large_circuit(13, luts="range16", public_inputs=[3, 1, 4, 1, 5, 9, 2, 6]),
+    zk_c, _ = PC.zk_circuit(plonk, zk_cfg, quick_fri_config(zk_cfg))
+    cases = [("no_lookups", shape_circuit(RECURSION_5, 4, public_inputs=[3, 1, 4, 1, 5]), None, {}),
+             ("lookups", shape_circuit(LOOKUP_64, 4, public_inputs=[2, 7, 1, 8]), None, {}),
+             ("large_2_13", PL.large_circuit(13, luts="range16", public_inputs=[3, 1, 4, 1, 5, 9, 2, 6]),
               standard_recursion_fri_config(), {}),
              ("zk_keys", zk_c, None, dict(salt_keys=KEYS))]
     verified = []
     for name, c, fri_cfg, kw in cases:
         cfg, cd = c.config, c.common
-        fri_cfg = fri_cfg or _fri_cfg(cfg)
+        fri_cfg = fri_cfg or quick_fri_config(cfg)
         zk = cfg.zero_knowledge
         fri_params = fri_cfg.fri_params(cd.degree_bits, zk)
         whole = pb.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height, ctx=ctx)
@@ -90,8 +79,8 @@ def main():
     # refusals on every rank: too many ranks for the cap; a constants/sigmas commitment of the wrong shard on rank 0 only
     c = cases[0][1]
     cfg, cd = c.config, c.common
-    fri_params = _fri_cfg(cfg).fri_params(cd.degree_bits, False)
-    tiny = _small_circuit((12, 8, 4, 2, 4), cap_height=0)
+    fri_params = quick_fri_config(cfg).fri_params(cd.degree_bits, False)
+    tiny = shape_circuit((12, 8, 4, 2, 4), 0)
     cs_tiny = pb.PolynomialBatch.from_values(tiny.constants_sigmas, 2, False, 0, ctx=ctx)
     wrong = pb.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height, ctx=ctx,
                                            shard=((rank + 1) % world if rank == 0 else rank, world))
@@ -110,15 +99,9 @@ def main():
         wrong.close()
 
     if rank == 0:
-        import oracle_lib
-        import plonk_circuits as PC
-
         for name, c, fri_cfg, fri_params, data, cs_cap in verified:
-            parts = parts_of(data, c, fri_params, cs_cap)
-            if c.config.zero_knowledge:
-                verdict = ZC.oracle_verify_zk(plonk, c, DIGEST, fri_cfg, parts)
-            else:
-                verdict = PC.oracle_verify(oracle_lib, plonk, c, DIGEST, fri_cfg, parts)
+            parts = PC.parts_of(plonk.ProofWithPublicInputs.from_bytes(data, c.common, fri_params), cs_cap)
+            verdict = PC.oracle_verify(oracle_lib, plonk, c, DIGEST, fri_cfg, parts)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
     everyone = [None] * world

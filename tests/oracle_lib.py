@@ -386,6 +386,44 @@ class Challenger:
             self.h = None
 
 
+def log_transcripts(monkeypatch):
+    """Make every Challenger the product creates log what it observes and draws, for replay(). Returns the list that
+    gets one log per Challenger made."""
+    import plonky2_b200.challenger as challenger_mod
+
+    logs = []
+
+    class LoggingChallenger(challenger_mod.Challenger):
+        def __init__(self):
+            super().__init__()
+            self.log = []
+            logs.append(self.log)
+
+        def observe_element(self, element):
+            self.log.append(("observe", int(element)))
+            super().observe_element(element)
+
+        def get_challenge(self):
+            v = super().get_challenge()
+            self.log.append(("challenge", v))
+            return v
+
+    monkeypatch.setattr(challenger_mod, "Challenger", LoggingChallenger)
+    return logs
+
+
+def replay(log):
+    """An oracle Challenger that continues the product's transcript: it observes what the product observed and draws
+    each challenge the product drew, asserting that the two are equal."""
+    ch = Challenger()
+    for kind, v in log:
+        if kind == "observe":
+            ch.observe_element(v)
+        else:
+            assert ch.get_challenge() == v
+    return ch
+
+
 def make_params(rate_bits, cap_height, pow_bits, num_queries, arity_bits):
     p = FriParams()
     p.rate_bits, p.cap_height = rate_bits, cap_height

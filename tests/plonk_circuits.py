@@ -1,13 +1,72 @@
 """Test infrastructure: a Fibonacci-style plonky2 circuit built by hand (the CircuitBuilder is out of scope): gate
 instances, a witness that satisfies every gate, copy constraints and the sigma polynomials they induce
-(WirePartition::get_sigma_polys, plonky2/src/plonk/permutation_argument.rs:113-157). Used by the CPU pins and the GPU
-parity test of the plonky2 quotient."""
+(WirePartition::get_sigma_polys, plonky2/src/plonk/permutation_argument.rs:113-157); its zero-knowledge layout
+(zk_circuit); the CPU twin of plonky2's prover and a restated verifier, with and without zero knowledge (oracle_prove,
+oracle_verify, parts_of); and the oracle standing in for prove_with_witness's device calls (cpu_backends). Used by the
+CPU pins and the GPU parity tests of the plonky2 quotient and proofs."""
 import numpy as np
 
+import gl_numpy as gn
 import oracle_lib as OL
 
 P = 0xFFFFFFFF00000001
 G = 14293326489335486720   # MULTIPLICATIVE_GROUP_GENERATOR
+KEYS = [bytes([k]) * 32 for k in (0x11, 0x22, 0x33)]   # salt keys of the wires, Z and quotient commitments
+# every gate type FibonacciCircuit can add a row of (extra=), besides its arithmetic and Poseidon rows
+OTHER_GATES = ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "BaseSumGate4", "ReducingGate",
+               "ReducingExtensionGate", "PoseidonMdsGate", "RandomAccessGate", "ExponentiationGate",
+               "CosetInterpolationGate")
+# shape_circuit's shapes: (num_wires, num_routed_wires, max_quotient_degree_factor, rate_bits, degree_bits[,
+# poseidon_rows[, other gates[, lookups]]])
+SHAPES = [
+    (12, 8, 4, 2, 4),     # two selector groups, partial-product chunks of 4
+    (13, 8, 3, 2, 4),     # quotient_degree_factor 3: coset of 4n points, the top n coefficients must vanish
+    (24, 16, 8, 3, 3),    # one selector for all gates, chunks of 8
+    (135, 80, 8, 3, 5),   # CircuitConfig::standard_recursion_config
+    (135, 80, 8, 3, 5, 9),  # ... with nine PoseidonGate rows (a hash chain): two selector groups, 123 gate constraints
+    (135, 80, 8, 3, 5, 4, OTHER_GATES),   # ... and a row of every other gate type built so far: three selector groups
+    # ... plus a lookup table of 30 entries on two LookupTableGate rows and 80 lookups on two LookupGate rows
+    (135, 80, 8, 3, 5, 4, OTHER_GATES, True),
+]
+RECURSION_5 = SHAPES[3]                              # standard_recursion_config, 32 gates
+LOOKUP_64 = (135, 80, 8, 3, 6, 4, OTHER_GATES, True)  # every gate type and a lookup table on 64 gates
+
+
+def shape_circuit(shape, cap_height, num_challenges=2, **kw):
+    """The FibonacciCircuit of a shape tuple, with a cap of 2^cap_height entries."""
+    from plonky2_b200 import plonk
+
+    nw, nr, qdf, rate_bits, degree_bits = shape[:5]
+    for k, name in ((5, "poseidon_rows"), (6, "extra"), (7, "lookups")):
+        if len(shape) > k:
+            kw.setdefault(name, shape[k])
+    cfg = plonk.CircuitConfig(num_wires=nw, num_routed_wires=nr, max_quotient_degree_factor=qdf, rate_bits=rate_bits,
+                              cap_height=cap_height, num_challenges=num_challenges)
+    return FibonacciCircuit(plonk, cfg, degree_bits, seed=nw + qdf + len(shape), **kw)
+
+
+def quick_fri_config(config):
+    """standard_recursion_config's FRI shape with fewer queries and grinding bits, so that the CPU twin stays quick."""
+    from plonky2_b200.fri import FriConfig
+
+    return FriConfig(rate_bits=config.rate_bits, cap_height=config.cap_height, proof_of_work_bits=6,
+                     reduction_strategy=("ConstantArityBits", 2, 2), num_query_rounds=6)
+
+
+def challenges(seed, c):
+    """(betas, gammas, alphas, deltas) of a circuit: deltas only with lookups."""
+    from conftest import synth
+
+    nc = c.config.num_challenges
+    v = [int(x) for x in synth(seed, (7 * nc,))]
+    return v[:nc], v[nc:2 * nc], v[2 * nc:3 * nc], (v[3 * nc:] if c.common.luts else [])
+
+
+def salts(c):
+    """The salt arrays (4 x N, chacha_ref's restatement) of KEYS at the circuit's LDE size."""
+    import chacha_ref as R
+
+    return [R.salt_array(k, c.n << c.config.rate_bits) for k in KEYS]
 
 
 def root_of_unity(bits):
@@ -417,6 +476,72 @@ class FibonacciCircuit:
         return np.stack(zs + pps + lk)
 
 
+def zk_circuit(plonk, config, fri_config, seed=7, arithmetic_rows=12, poseidon_rows=0, extra=(), lookups=False,
+               public_inputs=(3, 1, 4, 1, 5)):
+    """A FibonacciCircuit with the blinding rows of CircuitBuilder::blind (plonk/circuit_builder.rs:911-970) that
+    blinding_counts asks for -- regular_rows NoopGate rows with random values on every wire, then z_pairs pairs of
+    NoopGate rows with one random value per routed wire in both rows of the pair and a copy constraint between them --
+    padded with NoopGate rows to a power of two (CircuitBuilder::blind_and_pad). Returns (circuit, (regular_rows,
+    z_pairs))."""
+    num_gates = 2 + arithmetic_rows + poseidon_rows + len(extra) + (4 if lookups else 0)
+    regular, z_pairs = plonk.blinding_counts(config, fri_config, num_gates)
+    degree_bits = (num_gates + regular + 2 * z_pairs).bit_length()   # at least one padding row after the blinding
+    c = FibonacciCircuit(plonk, config, degree_bits, seed=seed, arithmetic_rows=arithmetic_rows,
+                         poseidon_rows=poseidon_rows, extra=extra, lookups=lookups, public_inputs=list(public_inputs))
+    # FibonacciCircuit fills the NoopGate rows after the gates with random wires, each wire alone in its copy set: the
+    # regular blinding rows as they are. Each Z pair gets one value per routed wire and the 2-cycle sigma of its set.
+    omega = root_of_unity(degree_bits)
+    k_is = c.common.k_is
+    for q in range(z_pairs):
+        r1 = num_gates + regular + 2 * q
+        r2 = r1 + 1
+        for w in range(config.num_routed_wires):
+            assert int(c.sigmas[w, r1]) == k_is[w] * pow(omega, r1, P) % P   # not copied anywhere yet
+            c.wires[w, r2] = c.wires[w, r1]
+            c.sigmas[w, r1] = k_is[w] * pow(omega, r2, P) % P
+            c.sigmas[w, r2] = k_is[w] * pow(omega, r1, P) % P
+    c.constants_sigmas = np.concatenate([np.stack(c.constant_vecs), c.sigmas])
+    return c, (regular, z_pairs)
+
+
+def instances_of(c):
+    """The gate instances [(gate, constants)] of a test circuit, read back from its selector and constant columns."""
+    from plonky2_b200 import plonk
+
+    cd = c.common
+    info = cd.selectors_info
+    nsel = info.num_selectors()
+    consts = c.constant_vecs[nsel + cd.num_lookup_selectors:]
+    out = []
+    for row in range(c.n):
+        vals = [int(c.constant_vecs[s][row]) for s in range(nsel)]
+        i = vals[0] if nsel == 1 else next(v for v in vals if v != plonk.UNUSED_SELECTOR)
+        g = cd.gates[i]
+        out.append((g, [int(k[row]) for k in consts[:g.num_constants()]]))
+    return out
+
+
+def pairs_from_sigmas(c, skip_rows=()):
+    """Copy constraints (Target::index) reproducing a test circuit's cycles: each wire paired with its sigma successor.
+    Rows in skip_rows are left out."""
+    cfg = c.config
+    nw, nr, n = cfg.num_wires, cfg.num_routed_wires, c.n
+    k_is = c.common.k_is
+    subgroup = gn.powers(root_of_unity(c.common.degree_bits), n)
+    where = {}
+    for col in range(nr):
+        for row, v in enumerate(gn.mul(np.full(n, k_is[col], dtype=np.uint64), subgroup).tolist()):
+            where[v] = (row, col)
+    skip = set(skip_rows)
+    pairs = []
+    for col in range(nr):
+        for row in range(n):
+            r, cc = where[int(c.sigmas[col, row])]
+            if (r, cc) != (row, col) and row not in skip:
+                pairs.append((row * nw + col, r * nw + cc))
+    return np.array(pairs, dtype=np.int64).reshape(-1, 2)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # The whole prover and verifier of plonky2 for these circuits, on the CPU, from the oracle's restatements:
 # prove_with_partition_witness (plonk/prover.rs:132-360) and verify_with_challenges (plonk/verifier.rs:40-120).
@@ -584,39 +709,51 @@ def fri_batches(cd, zeta):
     return [(zeta, all_polys), (zeta_next, [(2, i) for i in range(nc)] + lookup)], [n_pre, cfg.num_wires, n_zs_pp + n_lookup, n_quot]
 
 
-def observe_fri_params(ch, fri_cfg, degree_bits, arity_bits):
-    """FriParams::observe (fri/mod.rs:73-79,145-157) for a ConstantArityBits strategy, hiding = false."""
+def observe_fri_params(ch, fri_cfg, degree_bits, arity_bits, hiding):
+    """FriParams::observe (fri/mod.rs:73-79,145-157) for a ConstantArityBits strategy."""
     ch.observe_elements([fri_cfg.rate_bits, fri_cfg.cap_height, fri_cfg.proof_of_work_bits])
     ch.observe_elements([1, fri_cfg.reduction_strategy[1], fri_cfg.reduction_strategy[2]])
     ch.observe_element(fri_cfg.num_query_rounds)
-    ch.observe_elements([0, degree_bits] + list(arity_bits))
+    ch.observe_elements([int(hiding), degree_bits] + list(arity_bits))
 
 
-def oracle_prove(oracle, c, circuit_digest, fri_cfg, public_inputs, taps=False):
+def salt_widths(widths):
+    """Leaf widths of the four plonky2 oracles with hiding: constants / sigmas unsalted, the others + SALT_SIZE."""
+    return [w + (4 if k else 0) for k, w in enumerate(widths)]
+
+
+def oracle_prove(oracle, c, circuit_digest, fri_cfg, public_inputs, taps=False, *, salts=None):
     """prove_with_partition_witness with the oracle's pieces. Returns (proof bytes = write_proof_with_public_inputs,
-    parts) where parts carries what the verifier reads from the proof."""
+    parts) where parts carries what the verifier reads from the proof. With c.config.zero_knowledge (FriParams.hiding)
+    salts are the (4 x N) salt arrays of the wires, Z and quotient commitments; the constants / sigmas commitment is
+    never salted. Without zero knowledge there are no salts."""
     cd, cfg = c.common, c.config
     nc, nr, n = cfg.num_challenges, cfg.num_routed_wires, c.n
-    arity_bits = fri_cfg.fri_params(cd.degree_bits, False).reduction_arity_bits
+    hiding = cfg.zero_knowledge
+    if (salts is not None) != hiding:
+        raise ValueError("salts are required with zero knowledge and refused without")
+    salt_wires, salt_zs, salt_quotient = salts if hiding else (None, None, None)
+    arity_bits = fri_cfg.fri_params(cd.degree_bits, hiding).reduction_arity_bits
     public_inputs_hash = [int(x) for x in oracle.hash_no_pad(np.array(public_inputs, dtype=np.uint64))]
     assert public_inputs_hash == c.public_inputs_hash
     cs = oracle.Commit(c.constants_sigmas, cfg.rate_bits, cfg.cap_height)
-    wc = oracle.Commit(c.wires, cfg.rate_bits, cfg.cap_height)
+    wc = oracle.Commit(c.wires, cfg.rate_bits, cfg.cap_height, salt=salt_wires)
     ch = oracle.Challenger()
-    observe_fri_params(ch, fri_cfg, cd.degree_bits, arity_bits)
+    observe_fri_params(ch, fri_cfg, cd.degree_bits, arity_bits, hiding)
     ch.observe_elements(circuit_digest)
     ch.observe_elements(public_inputs_hash)
     ch.observe_cap(wc.cap)
     betas, gammas = ch.get_n_challenges(nc), ch.get_n_challenges(nc)
     deltas = (betas + gammas + ch.get_n_challenges(2 * nc)) if cd.luts else []
-    zc = oracle.Commit(c.oracle_zs_partial_products(oracle, betas, gammas, deltas), cfg.rate_bits, cfg.cap_height)
+    zc = oracle.Commit(c.oracle_zs_partial_products(oracle, betas, gammas, deltas), cfg.rate_bits, cfg.cap_height,
+                       salt=salt_zs)
     ch.observe_cap(zc.cap)
     alphas = ch.get_n_challenges(nc)
     q = oracle.plonk_quotient(c.oracle_circuit(), cs, wc, zc, public_inputs_hash, betas, gammas, alphas, deltas)
     qdf = cd.quotient_degree_factor
     assert not q[:, qdf * n:].any(), "Quotient has failed, the vanishing polynomial is not divisible by Z_H"
     chunks = np.concatenate([q[i, :qdf * n].reshape(qdf, n) for i in range(nc)])
-    qc = oracle.Commit(chunks, cfg.rate_bits, cfg.cap_height, is_coeffs=True)
+    qc = oracle.Commit(chunks, cfg.rate_bits, cfg.cap_height, salt=salt_quotient, is_coeffs=True)
     ch.observe_cap(qc.cap)
     zeta = ch.get_extension_challenge()
     batches, num_polys = fri_batches(cd, zeta)
@@ -658,14 +795,17 @@ def oracle_prove(oracle, c, circuit_digest, fri_cfg, public_inputs, taps=False):
 
 def oracle_verify(oracle, plonk, c, circuit_digest, fri_cfg, parts):
     """verify (plonk/verifier.rs:20-120): get_challenges (plonk/get_challenges.rs:26-90) replayed on a fresh transcript,
-    eval_vanishing_poly at zeta in F_{p^2} (vanishing_at), the quotient identity, then verify_fri_proof (the oracle's). Returns None or the reason of the rejection."""
+    eval_vanishing_poly at zeta in F_{p^2} (vanishing_at), the quotient identity, then verify_fri_proof (the oracle's).
+    With c.config.zero_knowledge (FriParams.hiding) the salted oracles' leaves are SALT_SIZE wider, and the FRI check
+    strips the salt (fri/verifier.rs fri_combine_initial). Returns None or the reason of the rejection."""
     cd, cfg = c.common, c.config
     nc = cfg.num_challenges
     o = parts["openings"]
-    arity_bits = fri_cfg.fri_params(cd.degree_bits, False).reduction_arity_bits
+    hiding = cfg.zero_knowledge
+    arity_bits = fri_cfg.fri_params(cd.degree_bits, hiding).reduction_arity_bits
     public_inputs_hash = [int(x) for x in oracle.hash_no_pad(np.array(parts["public_inputs"], dtype=np.uint64))]
     ch = oracle.Challenger()
-    observe_fri_params(ch, fri_cfg, cd.degree_bits, arity_bits)
+    observe_fri_params(ch, fri_cfg, cd.degree_bits, arity_bits, hiding)
     ch.observe_elements(circuit_digest)
     ch.observe_elements(public_inputs_hash)
     ch.observe_cap(parts["wires_cap"])
@@ -697,6 +837,122 @@ def oracle_verify(oracle, plonk, c, circuit_digest, fri_cfg, parts):
     batches, num_polys = fri_batches(cd, zeta)
     params = oracle.make_params(cfg.rate_bits, cfg.cap_height, fri_cfg.proof_of_work_bits, fri_cfg.num_query_rounds, arity_bits)
     rc = oracle.verify_fri_proof([parts["constants_sigmas_cap"], parts["wires_cap"], parts["zs_cap"], parts["quotient_cap"]],
-                                 num_polys, num_polys, batches, np.concatenate([zeta_batch.reshape(-1), next_batch.reshape(-1)]),
+                                 num_polys, salt_widths(num_polys) if hiding else num_polys, batches,
+                                 np.concatenate([zeta_batch.reshape(-1), next_batch.reshape(-1)]),
                                  cd.degree_bits, ch, params, parts["fri_bytes"])
     return None if rc == 0 else "FRI proof rejected (rc=%d)" % rc
+
+
+OPENING_KEYS = ("constants", "plonk_sigmas", "wires", "plonk_zs", "plonk_zs_next", "partial_products", "quotient_polys",
+                "lookup_zs", "lookup_zs_next")
+
+
+def parts_of(proof, constants_sigmas_cap):
+    """What oracle_verify reads, from a ProofWithPublicInputs and the circuit's constants / sigmas cap."""
+    p, o = proof.proof, proof.proof.openings
+    return dict(constants_sigmas_cap=constants_sigmas_cap, wires_cap=p.wires_cap.hashes,
+                zs_cap=p.plonk_zs_partial_products_cap.hashes, quotient_cap=p.quotient_polys_cap.hashes,
+                openings={k: getattr(o, k) for k in OPENING_KEYS}, fri_bytes=p.opening_proof.to_bytes(),
+                public_inputs=list(proof.public_inputs))
+
+
+def cpu_backends(monkeypatch, oracle, c, fri_cfg, salt_keys=None):
+    """Stand the oracle's pieces in for plonk.prove_with_witness's device calls on circuit c: commitments, Z / partial
+    products, lookup columns, quotient, evaluations, the public-input hash and prove_openings, which replays the
+    product's transcript into the oracle's Challenger. With salt_keys every salted commitment takes
+    chacha_ref.salt_array(key, N) of its key. Returns (the context stand-in, the transcript logs, the salt keys used in
+    order). The patched plonk.PolynomialBatch.from_values makes the constants / sigmas commitment."""
+    import chacha_ref as R
+
+    import plonky2_b200.fri as fri_mod
+    import plonky2_b200.hash as hash_mod
+    import plonky2_b200.proof as proof_mod
+    import plonky2_b200.prover as prover_mod
+    from plonky2_b200 import plonk
+
+    cfg, cd = c.config, c.common
+    N = c.n << cfg.rate_bits
+    used = []
+
+    def salt(blinding, salt_key):
+        if not blinding:
+            assert salt_key is None
+            return None
+        assert salt_keys is not None and salt_key in salt_keys
+        used.append(salt_key)
+        return R.salt_array(salt_key, N)
+
+    class Cap:
+        def __init__(self, hashes):
+            self.hashes = hashes
+
+    class Tree:
+        def __init__(self, commit):
+            self.cap = Cap(commit.cap)
+
+    class Batch:   # a PolynomialBatch whose device work is done by the oracle
+        def __init__(self, commit):
+            self.o, self.merkle_tree, self.num_polys, self.degree_log = commit, Tree(commit), commit.B, commit.log_n
+            self.ctx = ctx
+
+        @classmethod
+        def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None, salt_key=None):
+            return cls(oracle.Commit(values, rate_bits, cap_height, salt=salt(blinding, salt_key)))
+
+        def close(self):
+            pass
+
+    class Ctx:
+        device, h = 0, None
+
+    ctx = Ctx()
+
+    def commit_zs(wires_dev, sigmas_dev, k_is, betas, gammas, degree, rate_bits, cap_height, ctx=None, blinding=False,
+                  salt_key=None):
+        assert np.array_equal(wires_dev, c.wires[:cfg.num_routed_wires]) and np.array_equal(sigmas_dev, c.sigmas)
+        return Batch(oracle.Commit(c.oracle_zs_partial_products(oracle, betas, gammas), rate_bits, cap_height,
+                                   salt=salt(blinding, salt_key)))
+
+    def quotient(cd_, cs, pih, w, z, betas, gammas, alphas, deltas=()):
+        return oracle.plonk_quotient(c.oracle_circuit(), cs.o, w.o, z.o, pih, betas, gammas, alphas, deltas)
+
+    def commit_quotient(cd_, q, ctx=None, blinding=False, salt_key=None):
+        qdf, n = cd.quotient_degree_factor, c.n
+        chunks = np.concatenate([q[i, :qdf * n].reshape(qdf, n) for i in range(q.shape[0])])
+        return Batch(oracle.Commit(chunks, cfg.rate_bits, cfg.cap_height, salt=salt(blinding, salt_key),
+                                   is_coeffs=True))
+
+    def evals(requests):
+        return [np.array([oracle.eval_poly_base_at_ext(p, z) for p in b.o.coeffs], dtype=np.uint64).reshape(-1, 2)
+                for b, z in requests]
+
+    class FriBytes:
+        def __init__(self, b):
+            self.b = b
+
+        def to_bytes(self):
+            return self.b
+
+    def prove_openings(instance, oracles, challenger, fri_params):
+        assert [o.blinding for o in instance.oracles] == [False] + [salt_keys is not None] * 3
+        assert [o.num_polys for o in instance.oracles] == [b.num_polys for b in oracles]
+        batches = [(b.point, [(p.oracle_index, p.polynomial_index) for p in b.polynomials]) for b in instance.batches]
+        params = oracle.make_params(cfg.rate_bits, cfg.cap_height, fri_cfg.proof_of_work_bits, fri_cfg.num_query_rounds,
+                                    fri_params.reduction_arity_bits)
+        return FriBytes(oracle.prove_openings([b.o for b in oracles], batches, oracle.replay(challenger.log), params))
+
+    logs = oracle.log_transcripts(monkeypatch)
+    monkeypatch.setattr(plonk, "PolynomialBatch", Batch)
+    monkeypatch.setattr(plonk, "_to_device", lambda columns, ctx: np.ascontiguousarray(columns, dtype=np.uint64))
+    monkeypatch.setattr(plonk, "compute_quotient_polys", quotient)
+    monkeypatch.setattr(plonk, "commit_quotient_polys", commit_quotient)
+    monkeypatch.setattr(prover_mod, "commit_zs_partial_products", commit_zs)
+    monkeypatch.setattr(prover_mod, "wires_permutation_partial_products_and_zs",
+                        lambda w, s, k, beta, gamma, degree, ctx=None: oracle.partial_products_and_zs(w, s, k, beta, gamma, degree))
+    monkeypatch.setattr(prover_mod, "compute_all_lookup_polys",
+                        lambda w, nr, qdf, deltas, rows, nc, ctx=None: np.concatenate(
+                            [oracle.lookup_polys(w, nr, qdf, deltas[4 * k:4 * k + 4], rows) for k in range(nc)]))
+    monkeypatch.setattr(proof_mod, "eval_commitments", evals)
+    monkeypatch.setattr(fri_mod, "prove_openings", prove_openings)
+    monkeypatch.setattr(hash_mod.PoseidonHash, "hash_no_pad", staticmethod(lambda x, ctx=None: oracle.hash_no_pad(x)))
+    return ctx, logs, used

@@ -22,8 +22,8 @@ import oracle_lib as OL
 import plonk_circuits as PC
 
 P = PC.P
-EXTRA = ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "BaseSumGate4", "ReducingGate",
-         "ReducingExtensionGate", "PoseidonMdsGate", "RandomAccessGate", "ExponentiationGate", "CosetInterpolationGate")
+QDF3_EXTRA = ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "ReducingGate", "ReducingExtensionGate",
+              "PoseidonMdsGate")   # the gate types of degree < 4, which fit quotient_degree_factor 3
 
 
 def range_table(bits=16):
@@ -40,8 +40,8 @@ class LargeCircuit:
     """luts: a list of (table, number of LookupGate rows). break_arith: an arithmetic row at which one operation's out
     is off by one (the vanishing polynomial is then not divisible by Z_H)."""
 
-    def __init__(self, plonk, config, degree_bits, seed=1, poseidon_rows=8, extra=EXTRA, luts=(), public_inputs=None,
-                 break_arith=None):
+    def __init__(self, plonk, config, degree_bits, seed=1, poseidon_rows=8, extra=PC.OTHER_GATES, luts=(),
+                 public_inputs=None, break_arith=None):
         rng = np.random.default_rng(seed)
         n = 1 << degree_bits
         self.config, self.n = config, n
@@ -162,6 +162,22 @@ class LargeCircuit:
 
     oracle_circuit = PC.FibonacciCircuit.oracle_circuit
     oracle_zs_partial_products = PC.FibonacciCircuit.oracle_zs_partial_products
+
+
+def large_circuit(degree_bits, qdf=8, rate_bits=3, nc=2, cap_height=4, luts="small", **kw):
+    """A LargeCircuit of the standard recursion config's wires with the given quotient degree factor, rate, number of
+    challenges and cap height. luts: None, "small" (two small tables) or "range16" (the 2^16-entry range table and a
+    small table)."""
+    from plonky2_b200 import plonk
+
+    tables = {None: [], "small": [(small_table(), 2), ([(7 * e + 2, e) for e in range(41)], 1)],
+              "range16": [(range_table(), 64), (small_table(), 2)]}[luts]
+    if qdf == 3:
+        kw.setdefault("extra", QDF3_EXTRA)
+        kw.setdefault("poseidon_rows", 0)
+    config = plonk.CircuitConfig(max_quotient_degree_factor=qdf, rate_bits=rate_bits, num_challenges=nc,
+                                 cap_height=cap_height)
+    return LargeCircuit(plonk, config, degree_bits, seed=degree_bits + 10 * nc + qdf, luts=tables, **kw)
 
 
 def sigma_values(k_is, num_routed_wires, n, degree_bits, cycles):

@@ -5,7 +5,7 @@ CPU: a literal restatement of Forest + wire_partition + get_sigma_map (plonk/per
 insertion-ordered sets) against a vectorised one (scipy connected components + stable argsort) on small random
 circuits with virtual targets bridging sets, duplicate pairs and self-pairs; the header's index code run on the host
 (tests/emu/sigma_emu.cpp) against the restatement; the digest against the oracle's Poseidon; blind_and_pad against
-tests/zk_circuits.zk_circuit; every refusal of gl_sigma_polys raised before the context is used.
+tests/plonk_circuits.zk_circuit; every refusal of gl_sigma_polys raised before the context is used.
 
 GPU (-m gpu): gl_sigma_polys bit-equal to the restatement on every FibonacciCircuit shape, LargeCircuit at 2^18 gates,
 no constraints, one set of every routed wire, a 2^22-edge descending chain, random graphs joined by virtual targets,
@@ -26,6 +26,7 @@ import gl_numpy as gn
 import oracle_lib as OL
 import plonk_circuits as PC
 from conftest import synth
+from plonk_circuits import instances_of, pairs_from_sigmas
 from plonky2_b200 import _native as N
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -126,43 +127,6 @@ def random_pairs(rng, num_wires, num_routed, degree_bits, num_virtual, count):
     return pairs
 
 
-def pairs_from_sigmas(c, skip_rows=()):
-    """Copy constraints (Target::index) reproducing a test circuit's cycles: each wire paired with its sigma successor.
-    Rows in skip_rows are left out."""
-    cfg = c.config
-    nw, nr, n = cfg.num_wires, cfg.num_routed_wires, c.n
-    k_is = c.common.k_is
-    subgroup = gn.powers(PC.root_of_unity(c.common.degree_bits), n)
-    where = {}
-    for col in range(nr):
-        for row, v in enumerate(gn.mul(np.full(n, k_is[col], dtype=np.uint64), subgroup).tolist()):
-            where[v] = (row, col)
-    skip = set(skip_rows)
-    pairs = []
-    for col in range(nr):
-        for row in range(n):
-            r, cc = where[int(c.sigmas[col, row])]
-            if (r, cc) != (row, col) and row not in skip:
-                pairs.append((row * nw + col, r * nw + cc))
-    return np.array(pairs, dtype=np.int64).reshape(-1, 2)
-
-
-def instances_of(c):
-    """The gate instances [(gate, constants)] of a test circuit, read back from its selector and constant columns."""
-    plonk = _plonk()
-    cd = c.common
-    info = cd.selectors_info
-    nsel = info.num_selectors()
-    consts = c.constant_vecs[nsel + cd.num_lookup_selectors:]
-    out = []
-    for row in range(c.n):
-        vals = [int(c.constant_vecs[s][row]) for s in range(nsel)]
-        i = vals[0] if nsel == 1 else next(v for v in vals if v != plonk.UNUSED_SELECTOR)
-        g = cd.gates[i]
-        out.append((g, [int(k[row]) for k in consts[:g.num_constants()]]))
-    return out
-
-
 # ----------------------------------------------------------------------------------------------------------- CPU
 @pytest.mark.parametrize("seed", range(6))
 def test_restatements_agree_on_random_circuits(seed):
@@ -239,19 +203,11 @@ def test_circuit_digest_restated_with_the_oracle(separator):
     assert plonk.circuit_digest(cap, separator, 3) != plonk.circuit_digest(cap, separator + [0], 3)
 
 
-def _zk_fri_cfg(cfg):
-    from test_plonk_sharded import _fri_cfg
-
-    return _fri_cfg(cfg)
-
-
 def test_blind_and_pad_is_the_zk_test_circuit_layout():
-    import zk_circuits as ZC
-
     plonk = _plonk()
     cfg = plonk.standard_recursion_zk_config()
-    fri_cfg = _zk_fri_cfg(cfg)
-    c, (regular, z_pairs) = ZC.zk_circuit(plonk, cfg, fri_cfg)
+    fri_cfg = PC.quick_fri_config(cfg)
+    c, (regular, z_pairs) = PC.zk_circuit(plonk, cfg, fri_cfg)
     rows = instances_of(c)
     num_gates = 2 + 12
     out, regular_rows, pairs = plonk.blind_and_pad(cfg, fri_cfg, rows[:num_gates])
@@ -347,11 +303,9 @@ def _want(cfg, db, pairs, nv=0, literal=False):
 
 @pytest.mark.gpu
 def test_sigmas_of_every_fibonacci_shape(pb):
-    import test_plonk_quotient as TQ
-
-    for shape in TQ.SHAPES:
+    for shape in PC.SHAPES:
         for kw in ({}, dict(break_copy=True)):
-            c = TQ._circuit(shape, **kw)
+            c = PC.shape_circuit(shape, cap_height=1, **kw)
             cfg, db = c.config, c.common.degree_bits
             pairs = pairs_from_sigmas(c)
             want = _want(cfg, db, pairs, literal=True)
@@ -436,12 +390,10 @@ def _fib(plonk, public_inputs=None, **kw):
 
 @pytest.mark.gpu
 def test_constants_sigmas_commitment_and_shards(pb):
-    from test_plonk_sharded import _fri_cfg
-
     plonk = _plonk()
     c = _fib(plonk)
     cfg = c.config
-    fri_cfg = _fri_cfg(cfg)
+    fri_cfg = PC.quick_fri_config(cfg)
     data = plonk.build_circuit_data(cfg, fri_cfg, instances_of(c), pairs_from_sigmas(c))
     cs = data.prover_only.constants_sigmas_commitment
     ref = pb.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height)
@@ -472,26 +424,18 @@ def test_constants_sigmas_commitment_and_shards(pb):
         ref.close()
 
 
-def _parts(proof, cs_cap):
-    from test_zk_commit_and_prove import _parts as parts
-
-    return parts(_plonk(), proof, cs_cap, None)
-
-
 @pytest.mark.gpu
 def test_build_then_prove_is_accepted(pb):
-    from test_plonk_sharded import _fri_cfg
-
     plonk = _plonk()
     c = _fib(plonk, public_inputs=[3, 1, 4, 1, 5], extra=("RandomAccessGate",), lookups=True)
     cfg = c.config
-    fri_cfg = _fri_cfg(cfg)
+    fri_cfg = PC.quick_fri_config(cfg)
     data = plonk.build_circuit_data(cfg, fri_cfg, instances_of(c), pairs_from_sigmas(c), luts=c.common.luts,
                                     lookup_rows=c.lookup_rows, domain_separator=[7, 8])
     try:
         digest = data.verifier_only.circuit_digest
         proof = plonk.prove_with_witness(data.prover_only, data.common, c.wires, c.public_inputs)
-        parts = _parts(proof, data.verifier_only.constants_sigmas_cap.hashes)
+        parts = PC.parts_of(proof, data.verifier_only.constants_sigmas_cap.hashes)
         assert PC.oracle_verify(OL, plonk, c, digest, fri_cfg, parts) is None
         assert PC.oracle_verify(OL, plonk, c, [digest[0] ^ 1] + digest[1:], fri_cfg, parts) is not None
         other = plonk.circuit_digest(data.verifier_only.constants_sigmas_cap, [], c.common.degree_bits)
@@ -502,12 +446,10 @@ def test_build_then_prove_is_accepted(pb):
 
 @pytest.mark.gpu
 def test_zero_knowledge_build_then_prove_is_accepted(pb):
-    import zk_circuits as ZC
-
     plonk = _plonk()
     cfg = plonk.standard_recursion_zk_config()
-    fri_cfg = _zk_fri_cfg(cfg)
-    c, (regular, z_pairs) = ZC.zk_circuit(plonk, cfg, fri_cfg)
+    fri_cfg = PC.quick_fri_config(cfg)
+    c, (regular, z_pairs) = PC.zk_circuit(plonk, cfg, fri_cfg)
     num_gates = 2 + 12
     instances, _, pairs_rows = plonk.blind_and_pad(cfg, fri_cfg, instances_of(c)[:num_gates])
     skip = [r for pr in pairs_rows for r in pr]
@@ -519,10 +461,10 @@ def test_zero_knowledge_build_then_prove_is_accepted(pb):
         r1 = pairs_rows[0][0]
         assert int(data.prover_only.sigmas[5, r1]) == k_is[5] * pow(w, r1, PC.P) % PC.P
         proof = plonk.prove_with_witness(data.prover_only, data.common, c.wires, c.public_inputs)
-        parts = _parts(proof, data.verifier_only.constants_sigmas_cap.hashes)
+        parts = PC.parts_of(proof, data.verifier_only.constants_sigmas_cap.hashes)
         digest = data.verifier_only.circuit_digest
-        assert ZC.oracle_verify_zk(plonk, c, digest, fri_cfg, parts) is None
-        assert ZC.oracle_verify_zk(plonk, c, [digest[0] ^ 1] + digest[1:], fri_cfg, parts) is not None
+        assert PC.oracle_verify(OL, plonk, c, digest, fri_cfg, parts) is None
+        assert PC.oracle_verify(OL, plonk, c, [digest[0] ^ 1] + digest[1:], fri_cfg, parts) is not None
     finally:
         data.prover_only.constants_sigmas_commitment.close()
 

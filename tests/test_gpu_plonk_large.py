@@ -26,36 +26,12 @@ import plonk_large as PL
 from conftest import synth
 
 G = 14293326489335486720   # F::coset_shift()
-QDF3_EXTRA = ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "ReducingGate", "ReducingExtensionGate",
-              "PoseidonMdsGate")   # the gate types of degree < 4, which fit quotient_degree_factor 3
 
 
 def _plonk():
     from plonky2_b200 import plonk
 
     return plonk
-
-
-def _config(qdf=8, rate_bits=3, nc=2, cap_height=4):
-    return _plonk().CircuitConfig(max_quotient_degree_factor=qdf, rate_bits=rate_bits, num_challenges=nc,
-                                  cap_height=cap_height)
-
-
-def _circuit(degree_bits, qdf=8, rate_bits=3, nc=2, cap_height=4, luts="small", **kw):
-    """luts: None, "small" (two small tables) or "range16" (the 2^16-entry range table and a small table)."""
-    tables = {None: [], "small": [(PL.small_table(), 2), ([(7 * e + 2, e) for e in range(41)], 1)],
-              "range16": [(PL.range_table(), 64), (PL.small_table(), 2)]}[luts]
-    if qdf == 3:
-        kw.setdefault("extra", QDF3_EXTRA)
-        kw.setdefault("poseidon_rows", 0)
-    return PL.LargeCircuit(_plonk(), _config(qdf, rate_bits, nc, cap_height), degree_bits, seed=degree_bits + 10 * nc + qdf,
-                           luts=tables, **kw)
-
-
-def _challenges(seed, c):
-    nc = c.config.num_challenges
-    v = [int(x) for x in synth(seed, (7 * nc,))]
-    return v[:nc], v[nc:2 * nc], v[2 * nc:3 * nc], (v[3 * nc:] if c.common.luts else [])
 
 
 def _points(seed):
@@ -84,8 +60,8 @@ def _identity_failures(oracle, c, cs_coeffs, w_coeffs, z_coeffs, chunks, ch, poi
 def test_builder_passes_the_verifier_identity(oracle, degree_bits, luts, nc):
     """The builder's circuits are satisfied: the oracle's quotient has no coefficients past qdf * n and meets the
     verifier's identity at two points of F_p and two of F_{p^2}."""
-    c = _circuit(degree_bits, nc=nc, cap_height=1, luts=luts)
-    ch = _challenges(0x6100 + degree_bits, c)
+    c = PL.large_circuit(degree_bits, nc=nc, cap_height=1, luts=luts)
+    ch = PC.challenges(0x6100 + degree_bits, c)
     cfg = c.config
     cs, w = oracle.Commit(c.constants_sigmas, cfg.rate_bits, 1), oracle.Commit(c.wires, cfg.rate_bits, 1)
     z = oracle.Commit(c.oracle_zs_partial_products(oracle, *ch[:2], ch[3]), cfg.rate_bits, 1)
@@ -96,8 +72,8 @@ def test_builder_passes_the_verifier_identity(oracle, degree_bits, luts, nc):
 
 def test_builder_at_quotient_degree_factor_3(oracle):
     """qdf 3 with lookups: the coset has 4n points and the top n quotient coefficients vanish."""
-    c = _circuit(8, qdf=3, cap_height=1)
-    ch = _challenges(0x6120, c)
+    c = PL.large_circuit(8, qdf=3, cap_height=1)
+    ch = PC.challenges(0x6120, c)
     cfg = c.config
     cs, w = oracle.Commit(c.constants_sigmas, cfg.rate_bits, 1), oracle.Commit(c.wires, cfg.rate_bits, 1)
     z = oracle.Commit(c.oracle_zs_partial_products(oracle, *ch[:2], ch[3]), cfg.rate_bits, 1)
@@ -109,7 +85,7 @@ def test_builder_at_quotient_degree_factor_3(oracle):
 def test_vectorised_sigmas_equal_the_loop_form():
     """sigma_values equals get_sigma_map written out wire by wire (as tests/plonk_circuits.FibonacciCircuit does) on the
     same partition; every cycle is a true cycle of distinct routed wires."""
-    c = _circuit(8, cap_height=1)
+    c = PL.large_circuit(8, cap_height=1)
     nr, n = c.config.num_routed_wires, c.n
     neighbor = {}
     for members in c.partition():
@@ -135,8 +111,8 @@ def test_vectorised_sigmas_equal_the_loop_form():
 def test_identity_rejects_a_wrong_column(oracle, change):
     """The identity accepts the oracle's quotient at 2^8 gates and rejects it after one change: one coset value of the
     quotient before the coset iNTT, one partial-product value, or one RE (lookup) value."""
-    c = _circuit(8, cap_height=1)
-    ch = _challenges(0x6130, c)
+    c = PL.large_circuit(8, cap_height=1)
+    ch = PC.challenges(0x6130, c)
     cfg, cd = c.config, c.common
     cs, w = oracle.Commit(c.constants_sigmas, cfg.rate_bits, 1), oracle.Commit(c.wires, cfg.rate_bits, 1)
     zv = c.oracle_zs_partial_products(oracle, *ch[:2], ch[3])
@@ -213,7 +189,7 @@ def _check_quotient_against_oracle(pb, oracle, c, seed):
     from plonky2_b200 import plonk
 
     cfg = c.config
-    ch = _challenges(seed, c)
+    ch = PC.challenges(seed, c)
     ocs, ow = oracle.Commit(c.constants_sigmas, cfg.rate_bits, cfg.cap_height), oracle.Commit(c.wires, cfg.rate_bits, cfg.cap_height)
     oz = oracle.Commit(c.oracle_zs_partial_products(oracle, *ch[:2], ch[3]), cfg.rate_bits, cfg.cap_height)
     want = oracle.plonk_quotient(c.oracle_circuit(), ocs, ow, oz, c.public_inputs_hash, *ch)
@@ -258,13 +234,7 @@ def _prove(pb, c, digest, wires=None):
     finally:
         cs.close()
     proof = plonk.ProofWithPublicInputs.from_bytes(data, cd, fri_params)
-    p, o = proof.proof, proof.proof.openings
-    keys = ("constants", "plonk_sigmas", "wires", "plonk_zs", "plonk_zs_next", "partial_products", "quotient_polys",
-            "lookup_zs", "lookup_zs_next")
-    parts = dict(constants_sigmas_cap=cs_cap, wires_cap=p.wires_cap.hashes, zs_cap=p.plonk_zs_partial_products_cap.hashes,
-                 quotient_cap=p.quotient_polys_cap.hashes, openings={k: getattr(o, k) for k in keys},
-                 fri_bytes=p.opening_proof.to_bytes(), public_inputs=proof.public_inputs)
-    return data, parts
+    return data, PC.parts_of(proof, cs_cap)
 
 
 def _verify(oracle, c, digest, parts):
@@ -280,7 +250,7 @@ def test_a_recursion_circuit_2_13_is_bit_exact(pb, oracle):
     """Case a: the standard recursion config (135 wires, 80 routed, qdf 8, rate 3) at 2^13 gates with every gate type,
     Poseidon rows, the 2^16-entry range table and a small table. The quotient over its 2^16-point coset equals the
     oracle's bit for bit, and prove_with_witness gives the CPU prover's bytes, which the restated verifier accepts."""
-    c = _circuit(13, luts="range16", public_inputs=PUBLIC_INPUTS)
+    c = PL.large_circuit(13, luts="range16", public_inputs=PUBLIC_INPUTS)
     _check_quotient_against_oracle(pb, oracle, c, 0x6200)
     want, _ = PC.oracle_prove(oracle, c, DIGEST, _fri_cfg(c), c.public_inputs)
     got, parts = _prove(pb, c, DIGEST)
@@ -293,7 +263,7 @@ def test_a_recursion_circuit_2_13_is_bit_exact(pb, oracle):
 def test_quotient_with_a_coset_smaller_than_the_lde(pb, oracle, qdf, rate_bits):
     """Case b: step = 2^(rate_bits - qd_bits) = 4 (qdf 8 at rate 5) and 2 (qdf 3 at rate 3, with the trim check): the
     local and next-row leaves are bitrev over the coset's size. Bit-exact against the oracle, and the quotient cap."""
-    _check_quotient_against_oracle(pb, oracle, _circuit(13, qdf=qdf, rate_bits=rate_bits), 0x6210 + qdf)
+    _check_quotient_against_oracle(pb, oracle, PL.large_circuit(13, qdf=qdf, rate_bits=rate_bits), 0x6210 + qdf)
 
 
 class _PeakDeviceMemory:
@@ -328,7 +298,7 @@ def _check_identity_on_device(pb, oracle, c, seed):
 
     cfg, cd = c.config, c.common
     nr, nc = cfg.num_routed_wires, cfg.num_challenges
-    ch = _challenges(seed, c)
+    ch = PC.challenges(seed, c)
     cs, w, z, zv = _device_commitments(pb, c, ch)
     try:
         nprod = cd.num_partial_products
@@ -352,7 +322,7 @@ def _check_identity_on_device(pb, oracle, c, seed):
 @pytest.mark.parametrize("degree_bits,nc", [(16, 4), (18, 2)])
 def test_quotient_identity_at_2_16_and_2_18(pb, oracle, degree_bits, nc):
     """Case c: the standard config at 2^16 and 2^18 gates (cosets of 2^19 and 2^21 points), both lookup tables."""
-    c = _circuit(degree_bits, nc=nc, luts="range16")
+    c = PL.large_circuit(degree_bits, nc=nc, luts="range16")
     with _PeakDeviceMemory() as mem:
         _check_identity_on_device(pb, oracle, c, 0x6220 + degree_bits)
     print("\n2^%d gates, %d challenges: peak device memory %.2f GiB (%.2f GiB in use before)"
@@ -367,11 +337,11 @@ def test_lookups_and_proof_2_16(pb, oracle):
     after tampering with an opening, the public inputs, one wire of a looking pair, or one table multiplicity."""
     from plonky2_b200.prover import compute_all_lookup_polys
 
-    c = _circuit(16, luts="range16", public_inputs=PUBLIC_INPUTS)
+    c = PL.large_circuit(16, luts="range16", public_inputs=PUBLIC_INPUTS)
     cfg, cd = c.config, c.common
     nr, nc = cfg.num_routed_wires, cfg.num_challenges
     assert c.lookup_rows[0][2] - c.lookup_rows[0][1] + 1 == 2521
-    deltas = _challenges(0x6230, c)[3]
+    deltas = PC.challenges(0x6230, c)[3]
     got = compute_all_lookup_polys(c.wires, nr, cfg.max_quotient_degree_factor, deltas, c.lookup_rows, nc)
     npoly = cd.num_lookup_polys
     for k in range(nc):
@@ -405,10 +375,10 @@ def test_a_bad_witness_past_row_4096_is_rejected(pb, oracle, qdf):
     rejects it."""
     from plonky2_b200 import NativeError
 
-    c = _circuit(13, qdf=qdf, break_arith=5000, public_inputs=PUBLIC_INPUTS)
+    c = PL.large_circuit(13, qdf=qdf, break_arith=5000, public_inputs=PUBLIC_INPUTS)
     assert c.broken_row > 4096
     if qdf == 3:
-        ch = _challenges(0x6240, c)
+        ch = PC.challenges(0x6240, c)
         cs, w, z, _ = _device_commitments(pb, c, ch)
         try:
             with pytest.raises((NativeError, ValueError), match="Quotient has failed"):
@@ -426,6 +396,6 @@ def test_a_bad_witness_past_row_4096_is_rejected(pb, oracle, qdf):
 def test_recursion_circuit_2_20(pb, oracle):
     """Case f: the standard config at 2^20 gates: the verifier identity of the device quotient, and the device proof
     accepted by the restated verifier."""
-    c = _circuit(20, luts="range16", public_inputs=PUBLIC_INPUTS)
+    c = PL.large_circuit(20, luts="range16", public_inputs=PUBLIC_INPUTS)
     _check_identity_on_device(pb, oracle, c, 0x6250)
     assert _verify(oracle, c, DIGEST, _prove(pb, c, DIGEST)[1]) is None

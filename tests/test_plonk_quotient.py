@@ -20,27 +20,13 @@ import subprocess
 import numpy as np
 import pytest
 
+import plonk_circuits as PC
 from conftest import P, synth
+from plonk_circuits import LOOKUP_64, SHAPES
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P_ = int(P)
-
-# (num_wires, num_routed_wires, max_quotient_degree_factor, rate_bits, degree_bits)
-SHAPES = [
-    (12, 8, 4, 2, 4),     # two selector groups, partial-product chunks of 4
-    (13, 8, 3, 2, 4),     # quotient_degree_factor 3: coset of 4n points, the top n coefficients must vanish
-    (24, 16, 8, 3, 3),    # one selector for all gates, chunks of 8
-    (135, 80, 8, 3, 5),   # CircuitConfig::standard_recursion_config
-    (135, 80, 8, 3, 5, 9),  # ... with nine PoseidonGate rows (a hash chain): two selector groups, 123 gate constraints
-    # ... and a row of every other gate type built so far: three selector groups
-    (135, 80, 8, 3, 5, 4, ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "BaseSumGate4", "ReducingGate",
-                           "ReducingExtensionGate", "PoseidonMdsGate", "RandomAccessGate", "ExponentiationGate",
-                           "CosetInterpolationGate")),
-]
-NUM_EXTRA = len(SHAPES[5][6])
-# ... plus a lookup table of 30 entries on two LookupTableGate rows and 80 lookups on two LookupGate rows
-SHAPES.append(SHAPES[5] + (True,))
-LOOKUP_SHAPE_64 = SHAPES[6][:4] + (6,) + SHAPES[6][5:]     # the same circuit on 64 rows (the GPU cases use this one)
+NUM_EXTRA = len(PC.OTHER_GATES)
 
 
 def _plonk():
@@ -50,19 +36,7 @@ def _plonk():
 
 
 def _circuit(shape, **kw):
-    import plonk_circuits as PC
-
-    plonk = _plonk()
-    nw, nr, qdf, rate_bits, degree_bits = shape[:5]
-    if len(shape) > 5:
-        kw.setdefault("poseidon_rows", shape[5])
-    if len(shape) > 6:
-        kw.setdefault("extra", shape[6])
-    if len(shape) > 7:
-        kw.setdefault("lookups", shape[7])
-    cfg = plonk.CircuitConfig(num_wires=nw, num_routed_wires=nr, max_quotient_degree_factor=qdf, rate_bits=rate_bits,
-                              cap_height=1, num_challenges=kw.pop("num_challenges", 2))
-    return PC.FibonacciCircuit(plonk, cfg, degree_bits, seed=nw + qdf + len(shape), **kw)
+    return PC.shape_circuit(shape, cap_height=1, **kw)
 
 
 def _challenges(seed, nc):
@@ -92,8 +66,6 @@ def _ev(coeffs, x):
 
 def _vanishing_at(c, cs, w, z, zeta, betas, gammas, alphas, deltas=()):
     """eval_vanishing_poly (vanishing_poly.rs:29-164) at a base-field point, from the committed polynomials."""
-    import plonk_circuits as PC
-
     cd = c.common
     g = PC.root_of_unity(cd.degree_bits)
     o = PC.openings_at(cd, cs.coeffs, w.coeffs, z.coeffs, (zeta, 0), (zeta * g % P_, 0), lambda p, x: (_ev(p, x[0]), 0))
@@ -217,7 +189,7 @@ def _emu_quotient(L, oracle, c, cs, w, z, betas, gammas, alphas, deltas):
     return np.stack([oracle.coset_ifft(v, 14293326489335486720) for v in vals])   # .coset_ifft(F::coset_shift())
 
 
-@pytest.mark.parametrize("shape", SHAPES + [LOOKUP_SHAPE_64, (135, 80, 8, 3, 6, 20), (135, 80, 8, 3, 7)])
+@pytest.mark.parametrize("shape", SHAPES + [LOOKUP_64, (135, 80, 8, 3, 6, 20), (135, 80, 8, 3, 7)])
 def test_vanishing_program_through_the_kernel_source_on_host_matches_oracle(oracle, emu_lib, shape):
     c = _circuit(shape)
     nc = c.config.num_challenges
@@ -247,8 +219,6 @@ def test_coset_interpolation_row_holds_the_true_interpolant():
     """The CosetInterpolationGate row's evaluation_value is the Lagrange interpolant of its 16 F_{p^2} values on the coset
     shift*H at the evaluation point (computed here directly from the definition) -- so the barycentric recurrences the
     gate constrains (and the oracle restates) compute what the reference's gate is documented to compute."""
-    import plonk_circuits as PC
-
     plonk = _plonk()
     c = _circuit(SHAPES[5])
     info = [i for i in c.extra_info if i][0]
@@ -297,7 +267,7 @@ def pb():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("shape", [SHAPES[0], SHAPES[1], (135, 80, 8, 3, 7), (135, 80, 8, 3, 6, 20), SHAPES[5], LOOKUP_SHAPE_64])
+@pytest.mark.parametrize("shape", [SHAPES[0], SHAPES[1], (135, 80, 8, 3, 7), (135, 80, 8, 3, 6, 20), SHAPES[5], LOOKUP_64])
 def test_plonk_quotient_on_device_matches_oracle(pb, oracle, shape):
     """The prover's third phase without leaving the device (plonk/prover.rs:220-352): wires + constants_sigmas
     commitments -> Z / partial products commitment (device) -> quotient polynomials (device, LDEs read in place) ->
@@ -371,15 +341,7 @@ def test_plonk_quotient_of_a_bad_witness_is_rejected(pb):
 
 
 # ----------------------------------------------------------------------------- the whole proof
-def _fri_cfg(c):
-    from plonky2_b200.fri import FriConfig
-
-    # standard_recursion_config's FRI shape with fewer queries / grinding bits so that the CPU twin stays quick
-    return FriConfig(rate_bits=c.config.rate_bits, cap_height=c.config.cap_height, proof_of_work_bits=6,
-                     reduction_strategy=("ConstantArityBits", 2, 2), num_query_rounds=6)
-
-
-PROOF_SHAPES = [SHAPES[0], SHAPES[3], LOOKUP_SHAPE_64]
+PROOF_SHAPES = [SHAPES[0], SHAPES[3], LOOKUP_64]
 
 
 @pytest.mark.parametrize("shape", PROOF_SHAPES)
@@ -387,12 +349,10 @@ def test_whole_proof_is_accepted_by_the_restated_verifier(oracle, shape):
     """prove (plonk/prover.rs:132-360) assembled from the oracle's restatements produces a ProofWithPublicInputs that
     verify (plonk/verifier.rs:20-120) accepts: transcript replay, the vanishing-polynomial identity at zeta in F_{p^2},
     the FRI opening proof; and rejects after tampering with an opening or with the public inputs."""
-    import plonk_circuits as PC
-
     plonk = _plonk()
     c = _circuit(shape, public_inputs=[3, 1, 4, 1, 5])
     digest = [int(x) for x in synth(0x590, (4,))]
-    fri_cfg = _fri_cfg(c)
+    fri_cfg = PC.quick_fri_config(c.config)
     proof_bytes, parts = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs)
     assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, parts) is None
     bad = dict(parts, openings=dict(parts["openings"]))
@@ -411,113 +371,15 @@ def test_prove_host_logic_with_cpu_backends(oracle, shape, monkeypatch):
     serialisation -- run on the CPU by standing the oracle's pieces in for the device calls (commitments, Z / partial
     products, lookup columns, quotient, evaluations, prove_openings): the bytes must equal the CPU twin's. The device calls
     themselves are compared with the same oracle pieces one by one in the `-m gpu` tests."""
-    import plonk_circuits as PC
-
-    import plonky2_b200.fri as fri_mod
-    import plonky2_b200.hash as hash_mod
-    import plonky2_b200.proof as proof_mod
-    import plonky2_b200.prover as prover_mod
     from plonky2_b200 import plonk
 
     c = _circuit(shape, public_inputs=[3, 1, 4, 1, 5])
     cfg, cd = c.config, c.common
     digest = [int(x) for x in synth(0x590, (4,))]
-    fri_cfg = _fri_cfg(c)
+    fri_cfg = PC.quick_fri_config(cfg)
     want, _ = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs)
-
-    class Cap:
-        def __init__(self, hashes):
-            self.hashes = hashes
-
-    class Tree:
-        def __init__(self, commit):
-            self.cap = Cap(commit.cap)
-
-    class Batch:   # a PolynomialBatch whose device work is done by the oracle
-        def __init__(self, commit):
-            self.o, self.merkle_tree, self.num_polys, self.degree_log = commit, Tree(commit), commit.B, commit.log_n
-            self.ctx = ctx
-
-        @classmethod
-        def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None):
-            assert not blinding
-            return cls(oracle.Commit(values, rate_bits, cap_height))
-
-        def close(self):
-            pass
-
-    class Ctx:
-        device, h = 0, None
-
-    ctx = Ctx()
-
-    def commit_zs(wires_dev, sigmas_dev, k_is, betas, gammas, degree, rate_bits, cap_height, ctx=None):
-        assert np.array_equal(wires_dev, c.wires[:cfg.num_routed_wires]) and np.array_equal(sigmas_dev, c.sigmas)
-        return Batch(oracle.Commit(c.oracle_zs_partial_products(oracle, betas, gammas), rate_bits, cap_height))
-
-    def quotient(cd_, cs, pih, w, z, betas, gammas, alphas, deltas=()):
-        return oracle.plonk_quotient(c.oracle_circuit(), cs.o, w.o, z.o, pih, betas, gammas, alphas, deltas)
-
-    def commit_quotient(cd_, q, ctx=None):
-        qdf, n = cd.quotient_degree_factor, c.n
-        chunks = np.concatenate([q[i, :qdf * n].reshape(qdf, n) for i in range(q.shape[0])])
-        return Batch(oracle.Commit(chunks, cfg.rate_bits, cfg.cap_height, is_coeffs=True))
-
-    def evals(requests):
-        return [np.array([oracle.eval_poly_base_at_ext(p, z) for p in b.o.coeffs], dtype=np.uint64).reshape(-1, 2)
-                for b, z in requests]
-
-    class FriBytes:
-        def __init__(self, b):
-            self.b = b
-
-        def to_bytes(self):
-            return self.b
-
-    import plonky2_b200.challenger as challenger_mod
-
-    class LoggingChallenger(challenger_mod.Challenger):   # the product's host transcript, with a log to replay
-        def __init__(self):
-            super().__init__()
-            self.log = []
-
-        def observe_element(self, element):
-            self.log.append(("observe", int(element)))
-            super().observe_element(element)
-
-        def get_challenge(self):
-            v = super().get_challenge()
-            self.log.append(("challenge", v))
-            return v
-
-    def prove_openings(instance, oracles, challenger, fri_params):
-        och = oracle.Challenger()     # continue the product transcript inside the oracle's prover: replay it
-        for kind, v in challenger.log:
-            if kind == "observe":
-                och.observe_element(v)
-            else:
-                assert och.get_challenge() == v
-        batches = [(b.point, [(p.oracle_index, p.polynomial_index) for p in b.polynomials]) for b in instance.batches]
-        assert [o.num_polys for o in instance.oracles] == [b.num_polys for b in oracles]
-        params = oracle.make_params(cfg.rate_bits, cfg.cap_height, fri_cfg.proof_of_work_bits, fri_cfg.num_query_rounds,
-                                    fri_params.reduction_arity_bits)
-        return FriBytes(oracle.prove_openings([b.o for b in oracles], batches, och, params))
-
-    monkeypatch.setattr(challenger_mod, "Challenger", LoggingChallenger)
-    monkeypatch.setattr(plonk, "PolynomialBatch", Batch)
-    monkeypatch.setattr(plonk, "_to_device", lambda columns, ctx: np.ascontiguousarray(columns, dtype=np.uint64))
-    monkeypatch.setattr(plonk, "compute_quotient_polys", quotient)
-    monkeypatch.setattr(plonk, "commit_quotient_polys", commit_quotient)
-    monkeypatch.setattr(prover_mod, "commit_zs_partial_products", commit_zs)
-    monkeypatch.setattr(prover_mod, "wires_permutation_partial_products_and_zs",
-                        lambda w, s, k, beta, gamma, degree, ctx=None: oracle.partial_products_and_zs(w, s, k, beta, gamma, degree))
-    monkeypatch.setattr(prover_mod, "compute_all_lookup_polys",
-                        lambda w, nr, qdf, deltas, rows, nc, ctx=None: np.concatenate(
-                            [oracle.lookup_polys(w, nr, qdf, deltas[4 * k:4 * k + 4], rows) for k in range(nc)]))
-    monkeypatch.setattr(proof_mod, "eval_commitments", evals)
-    monkeypatch.setattr(fri_mod, "prove_openings", prove_openings)
-    monkeypatch.setattr(hash_mod.PoseidonHash, "hash_no_pad", staticmethod(lambda x, ctx=None: oracle.hash_no_pad(x)))
-    cs = Batch(oracle.Commit(c.constants_sigmas, cfg.rate_bits, cfg.cap_height))
+    ctx, _, _ = PC.cpu_backends(monkeypatch, oracle, c, fri_cfg)
+    cs = plonk.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height)
     prover_data = plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_cfg.fri_params(cd.degree_bits, False))
     proof = plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs, ctx=ctx)
     assert proof.to_bytes() == want
@@ -529,14 +391,12 @@ def test_prove_on_device_is_byte_identical_to_the_cpu_prover(pb, oracle, shape):
     """plonk.prove_with_witness: wires commitment, Z / partial products (+ lookups), quotient, openings and FRI on the
     device, the transcript on the host -- write_proof_with_public_inputs equals the CPU twin's bytes, which the restated
     verifier accepts."""
-    import plonk_circuits as PC
-
     from plonky2_b200 import plonk
 
     c = _circuit(shape, public_inputs=[3, 1, 4, 1, 5])
     cfg, cd = c.config, c.common
     digest = [int(x) for x in synth(0x590, (4,))]
-    fri_cfg = _fri_cfg(c)
+    fri_cfg = PC.quick_fri_config(c.config)
     want, parts = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs)
     assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, parts) is None
     cs = pb.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height)
@@ -551,12 +411,10 @@ def test_proof_bytes_round_trip_challenges_and_compression(oracle, shape):
     """read_proof_with_public_inputs / write_... round trip on the CPU prover's bytes; get_challenges replayed by the
     product's host code gives the prover's own query indices and grinding witness; Proof::compress shrinks the proof and
     keeps one initial-tree proof per distinct index."""
-    import plonk_circuits as PC
-
     plonk = _plonk()
     c = _circuit(shape, public_inputs=[3, 1, 4, 1, 5])
     digest = [int(x) for x in synth(0x590, (4,))]
-    fri_cfg = _fri_cfg(c)
+    fri_cfg = PC.quick_fri_config(c.config)
     fri_params = fri_cfg.fri_params(c.common.degree_bits, False)
     data, parts = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs, taps=True)
     proof = plonk.ProofWithPublicInputs.from_bytes(data, c.common, fri_params)
@@ -597,8 +455,6 @@ def test_low_degree_like_the_reference_gate_tests(oracle, k):
     constraints applied to random witness polynomials of degree < 32 are polynomials of degree <= 31 * gate.degree()
     (the value the selector grouping relies on) and there are num_constraints() of them. Beyond the reference: the bound
     is attained, so no gate over-declares its degree."""
-    import plonk_circuits as PC
-
     gate = _all_gates()[k]
     WITNESS_SIZE = 32
     rate_bits = gate.degree().bit_length()            # log2_ceil(degree + 1)

@@ -25,7 +25,10 @@ import sys
 import numpy as np
 import pytest
 
+import plonk_circuits as PC
+import plonk_large as PL
 from conftest import synth
+from plonk_circuits import LOOKUP_64, RECURSION_5
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 
@@ -41,32 +44,8 @@ def _plonk():
 
 
 def _small_circuit(shape, cap_height=4, **kw):
-    """tests/test_plonk_quotient.py's circuits (FibonacciCircuit) with a cap of 2^cap_height entries, enough for 16
-    shards. shape: (num_wires, num_routed_wires, max_quotient_degree_factor, rate_bits, degree_bits[, poseidon_rows[,
-    extra gates[, lookups]]])."""
-    import plonk_circuits as PC
-
-    plonk = _plonk()
-    nw, nr, qdf, rate_bits, degree_bits = shape[:5]
-    for k, name in ((5, "poseidon_rows"), (6, "extra"), (7, "lookups")):
-        if len(shape) > k:
-            kw.setdefault(name, shape[k])
-    cfg = plonk.CircuitConfig(num_wires=nw, num_routed_wires=nr, max_quotient_degree_factor=qdf, rate_bits=rate_bits,
-                              cap_height=cap_height)
-    return PC.FibonacciCircuit(plonk, cfg, degree_bits, seed=nw + qdf + len(shape), **kw)
-
-
-ALL_GATES = ("ArithmeticExtensionGate", "MulExtensionGate", "BaseSumGate", "BaseSumGate4", "ReducingGate",
-             "ReducingExtensionGate", "PoseidonMdsGate", "RandomAccessGate", "ExponentiationGate",
-             "CosetInterpolationGate")
-RECURSION_5 = (135, 80, 8, 3, 5)                                   # standard_recursion_config, 32 gates
-LOOKUP_64 = (135, 80, 8, 3, 6, 4, ALL_GATES, True)                 # every gate type, a lookup table, 64 gates
-
-
-def _challenges(seed, c):
-    nc = c.config.num_challenges
-    v = [int(x) for x in synth(seed, (7 * nc,))]
-    return v[:nc], v[nc:2 * nc], v[2 * nc:3 * nc], (v[3 * nc:] if c.common.luts else [])
+    """A FibonacciCircuit with a cap of 2^cap_height entries, enough for 16 shards."""
+    return PC.shape_circuit(shape, cap_height, **kw)
 
 
 # ----------------------------------------------------------------------------------------------------------- CPU
@@ -144,7 +123,7 @@ def test_shard_addressing_through_the_kernel_source_on_host(oracle, emu_libs, sh
     c = _small_circuit(shape)
     cfg, cd = c.config, c.common
     nc, rate_bits, db = cfg.num_challenges, cfg.rate_bits, cd.degree_bits
-    betas, gammas, alphas, deltas = _challenges(0x7A0 + shape[3] + shape[4], c)
+    betas, gammas, alphas, deltas = PC.challenges(0x7A0 + shape[3] + shape[4], c)
     commits = [oracle.Commit(v, rate_bits, 1) for v in
                (c.constants_sigmas, c.wires, c.oracle_zs_partial_products(oracle, betas, gammas, deltas))]
     b = cd.vanishing_program()
@@ -253,7 +232,7 @@ def _check_sharded_against_whole(pb, c, seed, shard_counts):
     plonk = _plonk()
     ctx = pb.default_context()
     cd = c.common
-    ch = _challenges(seed, c)
+    ch = PC.challenges(seed, c)
     betas, gammas, alphas, deltas = ch
     zv = _z_columns(c, ch)
     whole = _commitments(pb, c, zv)
@@ -283,9 +262,7 @@ def _check_sharded_against_whole(pb, c, seed, shard_counts):
 
 
 def _large(degree_bits, qdf=8, rate_bits=3, **kw):
-    from test_gpu_plonk_large import _circuit
-
-    return _circuit(degree_bits, qdf=qdf, rate_bits=rate_bits, luts="range16", **kw)
+    return PL.large_circuit(degree_bits, qdf=qdf, rate_bits=rate_bits, luts="range16", **kw)
 
 
 @pytest.mark.gpu
@@ -321,7 +298,7 @@ def test_entry_point_errors(pb):
     L = N.lib()
     c = _small_circuit(LOOKUP_64)
     cd = c.common
-    ch = _challenges(0x7E0, c)
+    ch = PC.challenges(0x7E0, c)
     betas, gammas, alphas, deltas = ch
     zv = _z_columns(c, ch)
     base = _commitments(pb, c, zv, (0, 2))
@@ -357,7 +334,7 @@ def test_entry_point_errors(pb):
     # quotient degree factor 3 on a coset of 4n points: the top n coefficients must vanish
     c3 = _large(13, 3, 3, break_arith=5000)
     cd3 = c3.common
-    ch3 = _challenges(0x7E1, c3)
+    ch3 = PC.challenges(0x7E1, c3)
     zv3 = _z_columns(c3, ch3)
     G, size = 4, c3.n << 2
     values = torch.empty((G, 2, size // G), dtype=torch.int64, device="cuda")
@@ -377,14 +354,6 @@ def test_entry_point_errors(pb):
     assert b"Quotient has failed" in L.gl_last_error(ctx.h)
 
 
-def _fri_cfg(config):
-    from plonky2_b200.fri import FriConfig
-
-    # standard_recursion_config's FRI shape with fewer queries and grinding bits, as tests/test_plonk_quotient.py
-    return FriConfig(rate_bits=config.rate_bits, cap_height=config.cap_height, proof_of_work_bits=6,
-                     reduction_strategy=("ConstantArityBits", 2, 2), num_query_rounds=6)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("zk", [False, True])
 def test_prove_plonk_on_one_rank_is_prove_with_witness(pb, zk):
@@ -392,18 +361,16 @@ def test_prove_plonk_on_one_rank_is_prove_with_witness(pb, zk):
     plonk = _plonk()
     digest = [int(x) for x in synth(0x7F0, (4,))]
     if zk:
-        import zk_circuits as ZC
-        from test_zk_commit_and_prove import KEYS
-
         cfg = plonk.standard_recursion_zk_config()
-        c, _ = ZC.zk_circuit(plonk, cfg, _fri_cfg(cfg))
-        kw = dict(salt_keys=KEYS)
+        c, _ = PC.zk_circuit(plonk, cfg, PC.quick_fri_config(cfg))
+        kw = dict(salt_keys=PC.KEYS)
     else:
         c, kw = _small_circuit(LOOKUP_64, public_inputs=[3, 1, 4, 1, 5]), {}
     cd = c.common
     cs = pb.PolynomialBatch.from_values(c.constants_sigmas, c.config.rate_bits, False, c.config.cap_height)
     try:
-        prover_data = plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, _fri_cfg(c.config).fri_params(cd.degree_bits, zk))
+        fri_params = PC.quick_fri_config(c.config).fri_params(cd.degree_bits, zk)
+        prover_data = plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_params)
         want = plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs, **kw).to_bytes()
         got = D.prove_plonk(prover_data, cd, c.wires, c.public_inputs, **kw).to_bytes()
     finally:

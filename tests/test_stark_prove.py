@@ -154,9 +154,8 @@ def test_host_quotient_matches_oracle(oracle):
 
 
 def _cpu_backends(monkeypatch, oracle, stark, calls):
-    """Replace prove's device calls by the oracle: commitments, quotient, openings, FRI. Returns the list of
-    LoggingChallenger logs (one per Challenger made)."""
-    import plonky2_b200.challenger as challenger_mod
+    """Replace prove's device calls by the oracle: commitments, quotient, openings, FRI. Returns the list of transcript
+    logs (one per Challenger made)."""
     import plonky2_b200.fri as fri_mod
     import plonky2_b200.proof as proof_mod
     from plonky2_b200.fri import FriProof
@@ -180,34 +179,12 @@ def _cpu_backends(monkeypatch, oracle, stark, calls):
         def close(self):
             calls.append("close")
 
-    logs = []
-
-    class LoggingChallenger(challenger_mod.Challenger):
-        def __init__(self):
-            super().__init__()
-            self.log = []
-            logs.append(self.log)
-
-        def observe_element(self, element):
-            self.log.append(("observe", int(element)))
-            super().observe_element(element)
-
-        def get_challenge(self):
-            v = super().get_challenge()
-            self.log.append(("challenge", v))
-            return v
-
     def commit_quotient(stark_, q, degree_bits, rate_bits, cap_height, ctx=None):
         return Batch(oracle.Commit(T.quotient_chunks(stark_, q, 1 << degree_bits), rate_bits, cap_height, is_coeffs=True))
 
     def prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len=None, max_num_query_steps=None):
         calls.append(("prove_openings", final_poly_coeff_len, max_num_query_steps))
-        och = oracle.Challenger()
-        for kind, v in challenger.log:
-            if kind == "observe":
-                och.observe_element(v)
-            else:
-                assert och.get_challenge() == v
+        och = oracle.replay(challenger.log)
         batches = [(b.point, [(p.oracle_index, p.polynomial_index) for p in b.polynomials]) for b in instance.batches]
         f = fri_params.config
         params = oracle.make_params(f.rate_bits, f.cap_height, f.proof_of_work_bits, f.num_query_rounds,
@@ -219,7 +196,7 @@ def _cpu_backends(monkeypatch, oracle, stark, calls):
     class Ctx:
         device, h = 0, None
 
-    monkeypatch.setattr(challenger_mod, "Challenger", LoggingChallenger)
+    logs = oracle.log_transcripts(monkeypatch)
     monkeypatch.setattr(S, "PolynomialBatch", Batch)
     monkeypatch.setattr(S, "compute_quotient_polys", lambda stark_, tc, pis, alphas: T.quotient(oracle, stark_, tc.o, pis, alphas))
     monkeypatch.setattr(S, "commit_quotient_polys", commit_quotient)

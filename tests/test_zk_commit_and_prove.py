@@ -16,24 +16,17 @@ import numpy as np
 import pytest
 
 import chacha_ref as R
+import plonk_circuits as PC
 from conftest import synth
+from plonk_circuits import KEYS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KEYS = [bytes([k]) * 32 for k in (0x11, 0x22, 0x33)]
 
 
 def _plonk():
     from plonky2_b200 import plonk
 
     return plonk
-
-
-def _fri_cfg(cap_height):
-    from plonky2_b200.fri import FriConfig
-
-    # standard_recursion_config's FRI shape with fewer queries / grinding bits so that the CPU twin stays quick
-    return FriConfig(rate_bits=3, cap_height=cap_height, proof_of_work_bits=6,
-                     reduction_strategy=("ConstantArityBits", 2, 2), num_query_rounds=6)
 
 
 # name -> (PoseidonGate rows, other gate rows, lookups)
@@ -44,18 +37,12 @@ ZK_SHAPES = {"plain": (0, (), False), "poseidon": (9, (), False),
 def _zk_circuit(name):
     """A circuit of standard_recursion_zk_config with the blinding rows blinding_counts asks for, padded to a power of
     two like CircuitBuilder::blind_and_pad."""
-    import zk_circuits as ZC
-
     plonk = _plonk()
     cfg = plonk.standard_recursion_zk_config()
     poseidon_rows, extra, lookups = ZK_SHAPES[name]
-    c, _ = ZC.zk_circuit(plonk, cfg, _fri_cfg(cfg.cap_height), poseidon_rows=poseidon_rows, extra=extra, lookups=lookups)
+    c, _ = PC.zk_circuit(plonk, cfg, PC.quick_fri_config(cfg), poseidon_rows=poseidon_rows, extra=extra,
+                         lookups=lookups)
     return c
-
-
-def _salts(c):
-    N = c.n << c.config.rate_bits
-    return [R.salt_array(k, N) for k in KEYS]
 
 
 # ----------------------------------------------------------------------------------------------------------- CPU
@@ -68,8 +55,8 @@ def test_blinding_counts_restate_the_reference():
     # 2^12 and 2^13 are too small; at 2^14 the arities are [4, 4, 4] and the final polynomial has 4 coefficients:
     # 28 * (1 + 2 * 45 + 2 * 4) = 2772 FRI openings
     assert plonk.blinding_counts(cfg, fri, 4000) == (2774, 2776)
-    # _fri_cfg at 2^10: arities [2, 2, 2, 2], 4 final coefficients: 6 * (1 + 2 * 12 + 2 * 4) = 198
-    assert plonk.blinding_counts(cfg, _fri_cfg(4), 20) == (200, 202)
+    # quick_fri_config at 2^10: arities [2, 2, 2, 2], 4 final coefficients: 6 * (1 + 2 * 12 + 2 * 4) = 198
+    assert plonk.blinding_counts(cfg, PC.quick_fri_config(cfg), 20) == (200, 202)
 
 
 def test_zk_fri_instance_and_proof_widths():
@@ -81,135 +68,26 @@ def test_zk_fri_instance_and_proof_widths():
     assert not any(o.blinding for o in plonk.get_fri_instance(c.common, (5, 7)).oracles)
 
 
-def _zk_twin(c, digest, fri_cfg):
-    import zk_circuits as ZC
-
-    return ZC.oracle_prove_zk(c, digest, fri_cfg, _salts(c))
-
-
-def _verify(plonk, c, digest, fri_cfg, parts):
-    import zk_circuits as ZC
-
-    return ZC.oracle_verify_zk(plonk, c, digest, fri_cfg, parts)
-
-
 @pytest.mark.parametrize("name", list(ZK_SHAPES))
 def test_zk_prove_host_logic_with_cpu_backends(oracle, name, monkeypatch):
     """prove_with_witness with config.zero_knowledge, its device calls answered by the oracle with the restated salt of
-    each key: equal bytes to the salted CPU twin, accepted by the restated verifier; the bytes read back, and
-    get_challenges replays the prover's transcript."""
-    import plonky2_b200.challenger as challenger_mod
-    import plonky2_b200.fri as fri_mod
-    import plonky2_b200.hash as hash_mod
-    import plonky2_b200.proof as proof_mod
-    import plonky2_b200.prover as prover_mod
-
+    each key: equal bytes to the salted CPU twin, accepted by the restated verifier, which rejects them when the circuit
+    does not say zero knowledge; the bytes read back, and get_challenges replays the prover's transcript."""
     plonk = _plonk()
     c = _zk_circuit(name)
     cfg, cd = c.config, c.common
     digest = [int(x) for x in synth(0x590, (4,))]
-    fri_cfg = _fri_cfg(cfg.cap_height)
-    want, parts = _zk_twin(c, digest, fri_cfg)
-    assert _verify(plonk, c, digest, fri_cfg, parts) is None
-    N = c.n << cfg.rate_bits
-    used = []
-
-    class Cap:
-        def __init__(self, hashes):
-            self.hashes = hashes
-
-    class Tree:
-        def __init__(self, commit):
-            self.cap = Cap(commit.cap)
-
-    class Batch:   # a PolynomialBatch whose device work is done by the oracle, salted from the key's restatement
-        def __init__(self, commit):
-            self.o, self.merkle_tree, self.num_polys, self.degree_log = commit, Tree(commit), commit.B, commit.log_n
-
-        @classmethod
-        def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None, salt_key=None):
-            assert blinding and salt_key in KEYS
-            used.append(salt_key)
-            return cls(oracle.Commit(values, rate_bits, cap_height, salt=R.salt_array(salt_key, N)))
-
-        def close(self):
-            pass
-
-    class Ctx:
-        device, h = 0, None
-
-    def commit_zs(wires_dev, sigmas_dev, k_is, betas, gammas, degree, rate_bits, cap_height, ctx=None, blinding=False,
-                  salt_key=None):
-        assert blinding and salt_key in KEYS
-        used.append(salt_key)
-        return Batch(oracle.Commit(c.oracle_zs_partial_products(oracle, betas, gammas), rate_bits, cap_height,
-                                   salt=R.salt_array(salt_key, N)))
-
-    def commit_quotient(cd_, q, ctx=None, blinding=False, salt_key=None):
-        assert blinding and salt_key in KEYS
-        used.append(salt_key)
-        qdf, n = cd.quotient_degree_factor, c.n
-        chunks = np.concatenate([q[i, :qdf * n].reshape(qdf, n) for i in range(q.shape[0])])
-        return Batch(oracle.Commit(chunks, cfg.rate_bits, cfg.cap_height, is_coeffs=True, salt=R.salt_array(salt_key, N)))
-
-    class FriBytes:
-        def __init__(self, b):
-            self.b = b
-
-        def to_bytes(self):
-            return self.b
-
-    class LoggingChallenger(challenger_mod.Challenger):
-        def __init__(self):
-            super().__init__()
-            self.log = []
-            logs.append(self.log)
-
-        def observe_element(self, element):
-            self.log.append(("observe", int(element)))
-            super().observe_element(element)
-
-        def get_challenge(self):
-            v = super().get_challenge()
-            self.log.append(("challenge", v))
-            return v
-
-    logs = []
-
-    def prove_openings(instance, oracles, challenger, fri_params):
-        assert [o.blinding for o in instance.oracles] == [False, True, True, True]
-        och = oracle.Challenger()
-        for kind, v in challenger.log:
-            if kind == "observe":
-                och.observe_element(v)
-            else:
-                assert och.get_challenge() == v
-        batches = [(b.point, [(p.oracle_index, p.polynomial_index) for p in b.polynomials]) for b in instance.batches]
-        params = oracle.make_params(cfg.rate_bits, cfg.cap_height, fri_cfg.proof_of_work_bits, fri_cfg.num_query_rounds,
-                                    fri_params.reduction_arity_bits)
-        return FriBytes(oracle.prove_openings([b.o for b in oracles], batches, och, params))
-
-    monkeypatch.setattr(challenger_mod, "Challenger", LoggingChallenger)
-    monkeypatch.setattr(plonk, "PolynomialBatch", Batch)
-    monkeypatch.setattr(plonk, "_to_device", lambda columns, ctx: np.ascontiguousarray(columns, dtype=np.uint64))
-    monkeypatch.setattr(plonk, "compute_quotient_polys", lambda cd_, cs, pih, w, z, betas, gammas, alphas, deltas=():
-                        oracle.plonk_quotient(c.oracle_circuit(), cs.o, w.o, z.o, pih, betas, gammas, alphas, deltas))
-    monkeypatch.setattr(plonk, "commit_quotient_polys", commit_quotient)
-    monkeypatch.setattr(prover_mod, "commit_zs_partial_products", commit_zs)
-    monkeypatch.setattr(prover_mod, "wires_permutation_partial_products_and_zs",
-                        lambda w, s, k, beta, gamma, degree, ctx=None: oracle.partial_products_and_zs(w, s, k, beta, gamma, degree))
-    monkeypatch.setattr(prover_mod, "compute_all_lookup_polys",
-                        lambda w, nr, qdf, deltas, rows, nc, ctx=None: np.concatenate(
-                            [oracle.lookup_polys(w, nr, qdf, deltas[4 * k:4 * k + 4], rows) for k in range(nc)]))
-    monkeypatch.setattr(proof_mod, "eval_commitments", lambda requests: [
-        np.array([oracle.eval_poly_base_at_ext(p, z) for p in b.o.coeffs], dtype=np.uint64).reshape(-1, 2)
-        for b, z in requests])
-    monkeypatch.setattr(fri_mod, "prove_openings", prove_openings)
-    monkeypatch.setattr(hash_mod.PoseidonHash, "hash_no_pad", staticmethod(lambda x, ctx=None: oracle.hash_no_pad(x)))
-    cs = Batch(oracle.Commit(c.constants_sigmas, cfg.rate_bits, cfg.cap_height))
+    fri_cfg = PC.quick_fri_config(cfg)
+    want, parts = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs, salts=PC.salts(c))
+    assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, parts) is None
+    cfg.zero_knowledge = False       # no hiding in the transcript and unsalted leaf widths: the same proof is rejected
+    assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, parts) is not None
+    cfg.zero_knowledge = True
+    ctx, logs, used = PC.cpu_backends(monkeypatch, oracle, c, fri_cfg, salt_keys=KEYS)
+    cs = plonk.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height)
     fri_params = fri_cfg.fri_params(cd.degree_bits, True)
     prover_data = plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_params)
-    proof = plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs, ctx=Ctx(), salt_keys=KEYS)
+    proof = plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs, ctx=ctx, salt_keys=KEYS)
     data = proof.to_bytes()
     assert data == want and used == KEYS
     # the proof format: salted initial-tree leaves, round trip, transcript replay, compression
@@ -226,7 +104,7 @@ def test_zk_prove_host_logic_with_cpu_backends(oracle, name, monkeypatch):
     # a proof whose parameters do not say hiding is refused before any work
     with pytest.raises(plonk.N.ShapeError):
         plonk.prove_with_witness(plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_cfg.fri_params(cd.degree_bits, False)),
-                                 cd, c.wires, c.public_inputs, ctx=Ctx(), salt_keys=KEYS)
+                                 cd, c.wires, c.public_inputs, ctx=ctx, salt_keys=KEYS)
 
 
 # ----------------------------------------------------------------------------------------------------------- GPU
@@ -382,17 +260,6 @@ def test_fresh_keys_and_abi_errors(pb):
         pb.PolynomialBatch.from_values(vals, 2, False, 2, salt_key=KEYS[0])
 
 
-def _parts(plonk, proof, cs_cap, c):
-    """What the restated verifier reads, from a parsed proof."""
-    p, o = proof.proof, proof.proof.openings
-    return dict(constants_sigmas_cap=cs_cap, wires_cap=p.wires_cap.hashes, zs_cap=p.plonk_zs_partial_products_cap.hashes,
-                quotient_cap=p.quotient_polys_cap.hashes, fri_bytes=p.opening_proof.to_bytes(),
-                public_inputs=list(proof.public_inputs),
-                openings=dict(constants=o.constants, plonk_sigmas=o.plonk_sigmas, wires=o.wires, plonk_zs=o.plonk_zs,
-                              plonk_zs_next=o.plonk_zs_next, partial_products=o.partial_products,
-                              quotient_polys=o.quotient_polys, lookup_zs=o.lookup_zs, lookup_zs_next=o.lookup_zs_next))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(ZK_SHAPES))
 def test_zk_proof_on_device(pb, oracle, name):
@@ -403,26 +270,26 @@ def test_zk_proof_on_device(pb, oracle, name):
     c = _zk_circuit(name)
     cfg, cd = c.config, c.common
     digest = [int(x) for x in synth(0x591, (4,))]
-    fri_cfg = _fri_cfg(cfg.cap_height)
+    fri_cfg = PC.quick_fri_config(cfg)
     fri_params = fri_cfg.fri_params(cd.degree_bits, True)
-    want, _ = _zk_twin(c, digest, fri_cfg)
+    want, _ = PC.oracle_prove(oracle, c, digest, fri_cfg, c.public_inputs, salts=PC.salts(c))
     cs = pb.PolynomialBatch.from_values(c.constants_sigmas, cfg.rate_bits, False, cfg.cap_height)
     cs_cap = cs.merkle_tree.cap.hashes
     prover_data = plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_params)
     data = plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs, salt_keys=KEYS).to_bytes()
     assert data == want
     proof = plonk.ProofWithPublicInputs.from_bytes(data, cd, fri_params)
-    assert _verify(plonk, c, digest, fri_cfg, _parts(plonk, proof, cs_cap, c)) is None
+    assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, PC.parts_of(proof, cs_cap)) is None
     for oracle_index, word, mask in ((1, -1, 1), (2, -2, 1 << 40), (3, 0, 0xFF)):   # salt words, a polynomial word
         bad = plonk.ProofWithPublicInputs.from_bytes(data, cd, fri_params)
         leaf = bad.proof.opening_proof.query_round_proofs[1].initial_trees_proof.evals_proofs[oracle_index][0]
         leaf[word] ^= np.uint64(mask)
         assert bad.to_bytes() != data
-        assert _verify(plonk, c, digest, fri_cfg, _parts(plonk, bad, cs_cap, c)) is not None
+        assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, PC.parts_of(bad, cs_cap)) is not None
     fresh = [plonk.prove_with_witness(prover_data, cd, c.wires, c.public_inputs) for _ in range(2)]
     assert fresh[0].to_bytes() != fresh[1].to_bytes()
     for f in fresh:
-        assert _verify(plonk, c, digest, fri_cfg, _parts(plonk, f, cs_cap, c)) is None
+        assert PC.oracle_verify(oracle, plonk, c, digest, fri_cfg, PC.parts_of(f, cs_cap)) is None
     with pytest.raises(pb.ShapeError):
         plonk.prove_with_witness(plonk.ProverOnlyCircuitData(cs, c.sigmas, digest, fri_cfg.fri_params(cd.degree_bits, False)),
                                  cd, c.wires, c.public_inputs, salt_keys=KEYS)
