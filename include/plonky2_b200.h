@@ -141,6 +141,12 @@ int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem);
  * array salt[s * N + i] = element (s, i). key = 32 bytes, or NULL: the library draws a fresh key from the OS CSPRNG
  * (getrandom(2)) for this commitment and forgets it (the reference's OsRng salt, oracle.rs:133-137). */
 int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]);
+/* gl_commit_finish for a later stage of a batch Merkle tree (plonky2/src/hash/batch_merkle_tree.rs:84-110), begun with
+ * blinding = 0: the tree is built over the leaves `prefix_j || row_j` of width W + 4, where prefix is a DEVICE array of
+ * N_local x 4 words (row j at prefix + 4j, e.g. the previous stage's gl_commit_dev_cap) and row j is leaf j of this
+ * handle's LDE, hashed in place. The handle keeps its own copy of the prefix. gl_commit_open then returns the prefixed
+ * leaves (W + 4 words); gl_commit_leaves, gl_commit_get_lde_values and gl_commit_dev_lde still return the LDE alone. */
+int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix);
 int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_shards);
 void gl_commit_destroy(gl_commit* c);
 /* shape queries */
@@ -188,6 +194,9 @@ int gl_openings_shard(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* po
  * reference's row-major MerkleTree.leaves is what gl_commit_leaves / gl_commit_open return. */
 const uint64_t* gl_commit_dev_lde(const gl_commit* c, size_t* col_stride);
 const uint64_t* gl_commit_dev_coeffs(const gl_commit* c);
+/* the (local) Merkle cap on the device, 4 x 2^(cap_height - log2 num_shards) words: the prefix of the next stage of a
+ * batch Merkle tree (gl_commit_finish_prefixed). NULL before the commitment is finished. */
+const uint64_t* gl_commit_dev_cap(const gl_commit* c);
 
 /* ---- random field elements (F::rand, field/src/goldilocks_field.rs:61-67) ------------------------------------------ */
 /* out[j] = element (column, first + j) of the keystream of `key` (32 bytes), j < count: uniform canonical field elements,

@@ -31,6 +31,7 @@ EXPORTS = [
     "gl_merkle_cap", "gl_merkle_digests", "gl_merkle_open", "gl_fri_begin", "gl_fri_begin_values", "gl_fri_values_local", "gl_fri_begin_from_coeffs",
     "gl_fri_destroy", "gl_fri_coeffs", "gl_fri_commit_round", "gl_fri_commit_round_sharded", "gl_fri_mix", "gl_fri_fold", "gl_fri_final_poly",
     "gl_fri_open", "gl_fri_num_rounds", "gl_fri_pow", "gl_commit_finish_keyed", "gl_random_field_elements",
+    "gl_commit_finish_prefixed", "gl_commit_dev_cap",
 ]
 
 
@@ -78,6 +79,7 @@ def lib():
     L.gl_commit_add_columns.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_size_t, C.c_int, C.c_int]
     L.gl_commit_finish.argtypes = [vp, vp, C.c_int]
     L.gl_commit_finish_keyed.argtypes = [vp, C.c_char_p]
+    L.gl_commit_finish_prefixed.argtypes = [vp, vp]
     L.gl_random_field_elements.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint64, C.c_size_t, vp, C.c_int]
     L.gl_commit_create.argtypes = [vp, vp, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp,
                                    C.c_int, C.c_int, C.POINTER(vp)]
@@ -122,6 +124,8 @@ def lib():
     L.gl_commit_dev_lde.restype = vp
     L.gl_commit_dev_coeffs.argtypes = [vp]
     L.gl_commit_dev_coeffs.restype = vp
+    L.gl_commit_dev_cap.argtypes = [vp]
+    L.gl_commit_dev_cap.restype = vp
     L.gl_partial_products_and_zs.argtypes = [vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                              C.c_uint32, vp, C.c_int]
     L.gl_poseidon_permute_host.argtypes = [vp]

@@ -2,68 +2,85 @@
 polynomials of several degrees -- one BatchMerkleTree over the degree groups' LDE rows -- and one FRI proof for all of
 them, the lower-degree instances being mixed into the folded codeword when it reaches their length. SURVEY 8(f) row 4.
 
-Device path: every degree group is a PolynomialBatch (coefficients and LDE stay on the device); the batch tree's first
-stage IS the tallest group's own Merkle tree built to the height of the next group, later stages hash `previous cap ||
-group rows`; every instance's composed polynomial comes from gl_fri_begin, and the rounds are fri.fri_committed_trees
-with the lower-degree instances mixed in at their LDE sizes."""
+Device path: every degree group is a PolynomialBatch (coefficients and LDE stay on the device) whose own Merkle tree IS
+its stage of the batch tree: the tallest group's tree is built to the height of the next group, and every later group's
+tree hashes `previous stage's cap digest j || LDE row j` (gl_commit_finish_prefixed), reading the LDE in place and the
+previous cap from device memory. Row-block sharded (shard=(g, G)): rank g holds rows [g*N_k/G, (g+1)*N_k/G) of every
+group k; the local cap of its stage k-1 has exactly N_k/G entries, the prefixes of its own rows, so every stage is
+rank-local and only the last stage's cap entries cross ranks (distributed.Placement.cap). Every instance's composed
+polynomial comes from gl_fri_begin on the (replicated) coefficients, and the rounds are fri.fri_committed_trees with the
+lower-degree instances mixed in at their LDE sizes."""
 import numpy as np
 
 from . import _native as N
 from . import fri as F
-from .batch_merkle_tree import _stage_chain
+from .distributed import Placement, _check_world
 from .field import log2_strict
 from .hash import NUM_HASH_OUT_ELTS, MerkleProof
 from .polynomial_batch import PolynomialBatch
 
 
 class BatchFriOracle:
-    """BatchFriOracle<F, C, D> (batch_fri/oracle.rs:30-40)."""
+    """BatchFriOracle<F, C, D> (batch_fri/oracle.rs:30-40); groups[k] is the degree group k and stage k of the batch
+    tree. On a shard, leaf indices (values, open_many) are local to this rank's rows of the tallest group."""
 
     def __init__(self, groups, degree_bits, rate_bits, cap_height, group_of_poly, ctx):
         self.groups, self.degree_bits, self.rate_bits, self.cap_height = groups, degree_bits, rate_bits, cap_height
         self.group_of_poly, self.ctx = group_of_poly, ctx   # polynomial index -> (group, index inside the group)
         self.blinding = False
-        heights = [d + rate_bits for d in degree_bits]
-        self.leaf_heights = heights
-        # stage 0 is the tallest group's own tree, built with cap height = next stage's height; the later groups' rows
-        # are read back as their stage is built
-        rows = (g.merkle_tree.get_rows(0, 1 << h) for g, h in zip(groups[1:], heights[1:]))
-        self.stages, self.cap = _stage_chain(groups[0].merkle_tree, rows, heights, cap_height, ctx)
+        self.leaf_heights = [d + rate_bits for d in degree_bits]
+        self.shard_index, self.num_shards = groups[0].shard_index, groups[0].num_shards
+        self.lde_size = 1 << self.leaf_heights[0]      # leaves of the tallest group (all shards)
+        self.leaf_width = sum(g.num_polys for g in groups)
+
+    @property
+    def stages(self):
+        """The batch tree's stages: stage k is group k's own commitment."""
+        return self.groups
+
+    @property
+    def cap(self):
+        """The batch tree's cap: the last stage's (on a shard, this rank's cap entries)."""
+        return self.groups[-1].merkle_tree.cap
 
     @classmethod
-    def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None):
-        """from_values (oracle.rs:45-68): values = list of 1-D arrays, lengths non-increasing powers of two."""
-        return cls._build(values, rate_bits, blinding, cap_height, False, ctx)
+    def from_values(cls, values, rate_bits, blinding, cap_height, ctx=None, shard=(0, 1)):
+        """from_values (oracle.rs:45-68): values = list of 1-D arrays, lengths non-increasing powers of two.
+        shard=(g, G): this rank's row block of every group, as in PolynomialBatch.from_values."""
+        return cls._build(values, rate_bits, blinding, cap_height, False, ctx, shard)
 
     @classmethod
-    def from_coeffs(cls, polynomials, rate_bits, blinding, cap_height, ctx=None):
-        """from_coeffs (oracle.rs:71-131)."""
-        return cls._build(polynomials, rate_bits, blinding, cap_height, True, ctx)
+    def from_coeffs(cls, polynomials, rate_bits, blinding, cap_height, ctx=None, shard=(0, 1)):
+        """from_coeffs (oracle.rs:71-131); shard as in from_values."""
+        return cls._build(polynomials, rate_bits, blinding, cap_height, True, ctx, shard)
 
     @classmethod
-    def _build(cls, polys, rate_bits, blinding, cap_height, is_coeffs, ctx):
+    def _build(cls, polys, rate_bits, blinding, cap_height, is_coeffs, ctx, shard):
         if blinding:
             raise NotImplementedError("blinding batch oracles are not supported")
-        ctx = ctx or N.default_context()
+        shard = (int(shard[0]), int(shard[1]))
+        _check_world("BatchFriOracle", cap_height, shard[1])
         polys = [np.ascontiguousarray(p, dtype=np.uint64).reshape(-1) for p in polys]
         bits = [log2_strict(len(p)) for p in polys]
         if any(a < b for a, b in zip(bits, bits[1:])):
             raise N.ShapeError("polynomials must be sorted by degree, largest first")   # oracle.rs:83
-        groups, degree_bits, group_of_poly = [], [], []
-        start = 0
-        for i, d in enumerate(bits):
-            if i == len(bits) - 1 or d > bits[i + 1]:
-                cols = np.stack(polys[start:i + 1])
-                nxt_bits = bits[i + 1] if i + 1 < len(bits) else None
-                # stage 0 is built straight to the next group's height; later groups only need their LDE rows
-                h = (nxt_bits + rate_bits if nxt_bits is not None else cap_height) if not groups else 0
-                make = PolynomialBatch.from_coeffs if is_coeffs else PolynomialBatch.from_values
-                groups.append(make(cols, rate_bits, False, h, ctx=ctx))
-                group_of_poly += [(len(groups) - 1, j) for j in range(i + 1 - start)]
-                degree_bits.append(d)
-                start = i + 1
-        if cap_height > degree_bits[-1] + rate_bits:
-            raise N.ShapeError("cap_height=%d should be at most last_leaves_cap_height=%d" % (cap_height, degree_bits[-1] + rate_bits))
+        if cap_height > bits[-1] + rate_bits:
+            raise N.ShapeError("cap_height=%d should be at most last_leaves_cap_height=%d" % (cap_height, bits[-1] + rate_bits))
+        ctx = ctx or N.default_context()
+        degree_bits = sorted(set(bits), reverse=True)
+        group_of_poly = [(degree_bits.index(d), bits[:i].count(d)) for i, d in enumerate(bits)]
+        groups = []
+        try:
+            for k, d in enumerate(degree_bits):
+                cols = np.stack([p for p, b in zip(polys, bits) if b == d])
+                # stage k is built to the next group's height, the last one to cap_height
+                h = degree_bits[k + 1] + rate_bits if k + 1 < len(degree_bits) else cap_height
+                groups.append(PolynomialBatch._create(cols, rate_bits, False, h, is_coeffs, None, ctx, shard,
+                                                      prefix=groups[-1] if groups else None))
+        except Exception:
+            for g in groups:
+                g.close()
+            raise
         return cls(groups, degree_bits, rate_bits, cap_height, group_of_poly, ctx)
 
     @property
@@ -71,7 +88,7 @@ class BatchFriOracle:
         return [self.groups[g].polynomials[j] for g, j in self.group_of_poly]
 
     def values(self, leaf_index):
-        """BatchMerkleTree::values (batch_merkle_tree.rs:154-164)."""
+        """BatchMerkleTree::values (batch_merkle_tree.rs:154-164): the row of every group above leaf_index."""
         h0 = self.leaf_heights[0]
         return [g.merkle_tree.get_rows(leaf_index >> (h0 - hk), 1)[0] for g, hk in zip(self.groups, self.leaf_heights)]
 
@@ -89,7 +106,7 @@ class BatchFriOracle:
         per index, `open_batch` siblings (q, L, 4))."""
         idx = np.asarray(indices, dtype=np.uint64)
         h0 = self.leaf_heights[0]
-        opened = [st.open_many(idx >> np.uint64(h0 - hk)) for st, hk in zip(self.stages, self.leaf_heights)]
+        opened = [g.merkle_tree.open_many(idx >> np.uint64(h0 - hk)) for g, hk in zip(self.groups, self.leaf_heights)]
         # a later stage's leaf is `previous cap digest || the group's row`
         rows = [lv if k == 0 else lv[:, NUM_HASH_OUT_ELTS:] for k, (lv, _) in enumerate(opened)]
         return np.concatenate(rows, axis=1), np.concatenate([pt for _, pt in opened], axis=1)
@@ -101,13 +118,15 @@ class BatchFriOracle:
     def close(self):
         for g in self.groups:
             g.close()
-        for t in self.stages[1:]:
-            t.close()
 
 
-def batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params):
+def batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params, placement=Placement()):
     """BatchFriOracle::prove_openings + batch_fri_proof (oracle.rs:124-183, prover.rs:30-147). instances[i] opens the
-    polynomials of degree 2^degree_bits[i]; polynomial indices are indices into each oracle's full polynomial list."""
+    polynomials of degree 2^degree_bits[i]; polynomial indices are indices into each oracle's full polynomial list.
+    placement: where the oracles live, as in fri.prove_openings. With row-block shards over several ranks every rank runs
+    the composition, the (replicated) round trees, the mixes and the transcript on the replicated coefficients; only the
+    initial-tree openings cross ranks (Placement.open_many), and the proof is the same on every rank and byte-identical to
+    the single-device proof. The caller must already have observed the full caps (Placement.cap) in `challenger`."""
     assert len(degree_bits) == len(instances)
     ctx = oracles[0].ctx
     alpha = challenger.get_extension_challenge()
@@ -135,7 +154,7 @@ def batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params
         mixes = [(db + rate_bits, st) for db, st in zip(degree_bits[1:], states[1:])]
         caps, final = F.fri_committed_trees(states[0], challenger, params[0], mixes=mixes)
         pow_witness = F.fri_proof_of_work(challenger, fri_params.config, ctx)
-        rounds, _ = F.fri_prover_query_rounds(oracles, states[0], challenger, params[0].lde_size(), params[0])
+        rounds, _ = F.fri_prover_query_rounds(oracles, states[0], challenger, params[0].lde_size(), params[0], placement)
         return F.FriProof(caps, rounds, final, pow_witness)
     finally:
         for st in states:

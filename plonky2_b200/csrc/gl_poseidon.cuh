@@ -770,4 +770,25 @@ GL_HD void hash_or_noop_strided(const uint64_t* in, size_t stride, uint32_t W, u
     for (int i = 0; i < 4; i++) out[i] = canon(s[i]);
 }
 
+// hash_or_noop of the leaf `prefix[0..4) || in[k * stride], k < W` (a later stage of a batch Merkle tree,
+// batch_merkle_tree.rs:84-96: the previous stage's cap digest, then the row). W + 4 > 4 words: always hashed.
+template <bool SYNC = false>
+GL_HD void hash_prefixed_strided(const uint64_t* prefix, const uint64_t* in, size_t stride, uint32_t W,
+                                 uint64_t out[4]) {
+    uint64_t s[12];
+#pragma unroll
+    for (int i = 0; i < 4; i++) s[i] = prefix[i];
+#pragma unroll
+    for (uint32_t i = 0; i < 8; i++) s[4 + i] = (i < 4 && i < W) ? in[(size_t)i * stride] : 0;
+    poseidon_permute_t<SYNC>(s);
+    for (uint32_t off = 4; off < W; off += 8) {
+#pragma unroll
+        for (uint32_t i = 0; i < 8; i++)
+            if (off + i < W) s[i] = in[(size_t)(off + i) * stride];
+        poseidon_permute_t<SYNC>(s);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) out[i] = canon(s[i]);
+}
+
 }  // namespace gl

@@ -319,6 +319,29 @@ __global__ void __launch_bounds__(HASH_CTA, HASH_MINB) k_leaf_hash(TreeView t) {
     dst[2] = h[2];
     dst[3] = h[3];
 }
+// k_leaf_hash over the leaves `prefix[4j .. 4j + 4) || row j` (a later stage of a batch Merkle tree): prefix is
+// row-major, N x 4 words, the previous stage's cap
+__global__ void __launch_bounds__(HASH_CTA, HASH_MINB) k_leaf_hash_prefixed(TreeView t, const u64* prefix) {
+    size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = j < t.N;
+    if (!live) j = t.N - 1;
+    u64 h[4];
+    hash_prefixed_strided<true>(prefix + 4 * j, t.leaves + j * t.ls, t.es, t.W, h);
+    if (!live) return;
+    u64* dst;
+    const uint32_t sub_log = t.log_n - t.cap_height;
+    if (sub_log == 0) {
+        dst = t.cap + 4 * j;
+    } else {
+        const size_t L = (size_t)1 << sub_log;
+        const size_t c = j >> sub_log, q = j & (L - 1);
+        dst = t.digests + 4 * (c * 2 * (L - 1) + digest_pos(q, 0));
+    }
+    dst[0] = h[0];
+    dst[1] = h[1];
+    dst[2] = h[2];
+    dst[3] = h[3];
+}
 // layer i (>= 1) from layer i-1: one thread per node
 __global__ void __launch_bounds__(HASH_CTA, HASH_MINB) k_merkle_level(TreeView t, uint32_t i) {
     const uint32_t sub_log = t.log_n - t.cap_height;
@@ -423,6 +446,23 @@ __global__ void k_tree_open(TreeView t, const u64* indices, u64* out_leaves, u64
         out_paths[(size_t)blockIdx.x * num_layers * 4 + k] = sub[4 * digest_pos(sib, i) + w];
     }
 }
+// k_tree_open on a tree hashed by k_leaf_hash_prefixed: the leaves it returns are `prefix || row`, W + 4 words
+__global__ void k_tree_open_prefixed(TreeView t, const u64* prefix, const u64* indices, u64* out_leaves,
+                                     u64* out_paths) {
+    const size_t idx = indices[blockIdx.x];
+    const uint32_t num_layers = t.log_n - t.cap_height;
+    const uint32_t lw = t.W + 4;
+    for (uint32_t k = threadIdx.x; k < lw; k += blockDim.x)
+        out_leaves[(size_t)blockIdx.x * lw + k] = k < 4 ? prefix[4 * idx + k] : t.leaves[idx * t.ls + (size_t)(k - 4) * t.es];
+    const size_t L = (size_t)1 << num_layers;
+    const size_t tree_index = idx >> num_layers;
+    const u64* sub = t.digests + 4 * (tree_index * 2 * (L - 1));
+    for (uint32_t k = threadIdx.x; k < num_layers * 4; k += blockDim.x) {
+        const uint32_t i = k >> 2, w = k & 3;
+        const size_t node = (idx & (L - 1)) >> i;
+        out_paths[(size_t)blockIdx.x * num_layers * 4 + k] = sub[4 * digest_pos(node ^ 1, i) + w];
+    }
+}
 
 struct Tree {
     u64* leaves = nullptr;  // device
@@ -430,6 +470,7 @@ struct Tree {
     bool own_leaves = false;
     u64* digests = nullptr;
     u64* cap = nullptr;
+    u64* prefix = nullptr;  // owned, N x 4 words, or null: leaf j is `prefix[j] || row j` (a batch tree's later stage)
     size_t N = 0;
     size_t ls = 0, es = 1;  // leaf / element strides (ls == 0: row-major, ls = W)
     uint32_t W = 0, log_n = 0, cap_height = 0;
@@ -459,7 +500,10 @@ static int tree_build(gl_ctx* ctx, Tree& t) {
         PhaseScope ps(ctx, GL_PHASE_LEAF_HASH);
         // big CTAs (barrier-synchronised rounds) for big trees; small CTAs to spread small trees over the SMs
         const int cta = HASH_CTA;
-        k_leaf_hash<<<(unsigned)((t.N + cta - 1) / cta), cta, 0, ctx->stream>>>(v);
+        if (t.prefix)
+            k_leaf_hash_prefixed<<<(unsigned)((t.N + cta - 1) / cta), cta, 0, ctx->stream>>>(v, t.prefix);
+        else
+            k_leaf_hash<<<(unsigned)((t.N + cta - 1) / cta), cta, 0, ctx->stream>>>(v);
         CKL(ctx);
     }
     PhaseScope ps2(ctx, GL_PHASE_MERKLE_LEVELS);
@@ -488,7 +532,8 @@ static void tree_free(gl_ctx* ctx, Tree& t) {
     if (t.own_leaves) dfree(ctx, t.base ? t.base : t.leaves);
     dfree(ctx, t.digests);
     dfree(ctx, t.cap);
-    t.leaves = t.digests = t.cap = nullptr;
+    dfree(ctx, t.prefix);
+    t.leaves = t.digests = t.cap = t.prefix = nullptr;
 }
 static int tree_open(gl_ctx* ctx, const Tree& t, const u64* leaf_indices, size_t count, u64* out_leaves,
                      u64* out_paths) {
@@ -497,14 +542,18 @@ static int tree_open(gl_ctx* ctx, const Tree& t, const u64* leaf_indices, size_t
         if (leaf_indices[i] >= t.N) return set_err(ctx, GL_ERR_BAD_ARG, "leaf index %llu out of range",
                                                    (unsigned long long)leaf_indices[i]);
     const uint32_t layers = t.log_n - t.cap_height;
-    const size_t lw = count * t.W, pw = count * layers * 4;
+    const size_t lw = count * (t.W + (t.prefix ? 4 : 0)), pw = count * layers * 4;
     TRY(ensure_dstage(ctx, count + lw + pw));
     TRY(ensure_pinned(ctx, count + lw + pw));
     CK(ctx, cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->pinned, leaf_indices, count * 8);
     TRY(h2d(ctx, ctx->dstage, ctx->pinned, count));
-    k_tree_open<<<(unsigned)count, 128, 0, ctx->stream>>>(t.view(), ctx->dstage, ctx->dstage + count,
-                                                         ctx->dstage + count + lw);
+    if (t.prefix)
+        k_tree_open_prefixed<<<(unsigned)count, 128, 0, ctx->stream>>>(t.view(), t.prefix, ctx->dstage,
+                                                                      ctx->dstage + count, ctx->dstage + count + lw);
+    else
+        k_tree_open<<<(unsigned)count, 128, 0, ctx->stream>>>(t.view(), ctx->dstage, ctx->dstage + count,
+                                                             ctx->dstage + count + lw);
     CKL(ctx);
     TRY(d2h(ctx, ctx->pinned, ctx->dstage + count, lw + pw));
     memcpy(out_leaves, ctx->pinned, lw * 8);
@@ -1843,6 +1892,19 @@ int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem) {
     CK(ctx, cudaSetDevice(ctx->device));
     return commit_finish(ctx, c, salt, mem);
 }
+int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix) {
+    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    gl_ctx* ctx = c->ctx;
+    if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
+    if (!prefix) return set_err(ctx, GL_ERR_BAD_ARG, "null prefix");
+    if (c->blinding) return set_err(ctx, GL_ERR_UNSUPPORTED, "a prefixed commitment cannot be blinded");
+    CK(ctx, cudaSetDevice(ctx->device));
+    Tree& t = c->tree;
+    // a copy: the previous stage (the prefix's owner) may be destroyed before this commitment
+    TRY(dmalloc(ctx, &t.prefix, 4 * t.N));
+    CK(ctx, cudaMemcpyAsync(t.prefix, prefix, 4 * t.N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    return commit_finish(ctx, c, nullptr, GL_MEM_DEVICE);
+}
 int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]) {
     if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
     gl_ctx* ctx = c->ctx;
@@ -1918,6 +1980,7 @@ int gl_commit_cap(gl_commit* c, uint64_t* out, int mem) {
     NEED_FINISHED(c);
     return copy_out(c->ctx, out, c->tree.cap, c->tree.cap_words(), mem);
 }
+const uint64_t* gl_commit_dev_cap(const gl_commit* c) { return c && c->finished ? c->tree.cap : nullptr; }
 int gl_commit_coeffs(gl_commit* c, uint64_t* out, int mem) {
     return copy_out(c->ctx, out, c->coeffs, (size_t)c->B << c->degree_log, mem);
 }

@@ -11,7 +11,8 @@ plonky2 circuit, on the ranks of a group with these shards: besides the caps, on
 shard of the quotient coset (Placement.quotient_from_shards), the partial sums of the openings over each rank's block
 of coefficients (Placement.openings_from_shards) and the FRI query openings (Placement.open_many) cross ranks. The
 provers take a Placement -- Placement() on one device -- and never ask themselves whether there is more than one rank.
-prove_openings_sharded is fri.prove_openings on the oracles' own shards, for a caller that commits the shards itself."""
+prove_openings_sharded is fri.prove_openings, and batch_prove_openings_sharded batch_fri.batch_prove_openings, on the
+oracles' own shards, for a caller that commits the shards itself."""
 from dataclasses import dataclass
 
 import numpy as np
@@ -98,10 +99,12 @@ class Placement:
         return gather_cap(commitment.merkle_tree.cap, self.group, device=_comm_device(self.group, commitment.ctx))
 
     def open_many(self, batch, leaf_indices):
-        """MerkleTree::get + prove (merkle_tree.rs:226-237) for GLOBAL leaf indices of `batch`. Returns (leaves (q, W),
-        paths (q, L, 4)). On one device the tree opens them itself. With several ranks every rank opens the indices it
-        owns on its own GPU (local index, local cap subtree -- the sibling path is the same as in the single-device tree)
-        and the ranks all-gather the results: every rank must call it with the same indices."""
+        """MerkleTree::get + prove (merkle_tree.rs:226-237) for GLOBAL leaf indices of `batch`, a PolynomialBatch or a
+        BatchFriOracle (whose leaves are those of its tallest group). Returns (leaves (q, W), paths (q, L, 4)). On one
+        device the tree opens them itself. With several ranks every rank opens the indices it owns on its own GPU (local
+        index, local cap subtree -- the sibling path is the same as in the single-device tree; a batch oracle's owner of
+        leaf i of the tallest group owns leaf i >> (h0 - hk) of every group, so one rank answers the whole query) and
+        the ranks all-gather the results: every rank must call it with the same indices."""
         if self.num_shards == 1:
             return batch.merkle_tree.open_many(leaf_indices)
         import torch.distributed as dist
@@ -117,7 +120,7 @@ class Placement:
         else:
             parts = [None] * dist.get_world_size(self.group)
             dist.all_gather_object(parts, part, group=self.group)
-        layers = batch.degree_log + batch.rate_bits - batch.cap_height
+        layers = batch.lde_size.bit_length() - 1 - batch.cap_height
         leaves = np.empty((len(idx), batch.leaf_width), dtype=np.uint64)
         paths = np.empty((len(idx), layers, 4), dtype=np.uint64)
         seen = 0
@@ -218,6 +221,33 @@ def prove_openings_sharded(instance, oracles, challenger, fri_params, group=None
     placement = Placement(oracles[0].shard_index, oracles[0].num_shards, group)
     return prove_openings(instance, oracles, challenger, fri_params, final_poly_coeff_len, max_num_query_steps,
                           placement=placement)
+
+
+def check_batch_prove_openings(oracles, fri_params, world):
+    """batch_prove_openings_sharded's refusals, raised identically on every rank before any device work or collective: a
+    world size that is not a power of two or exceeds 2^cap_height, oracles that are not row-block sharded over `world`
+    ranks, and a blinding (hiding) oracle, which batch FRI does not support."""
+    from . import _native as N
+
+    _check_world("batch_prove_openings", fri_params.config.cap_height, world)
+    if fri_params.hiding or any(o.blinding for o in oracles):
+        raise N.ShapeError("batch FRI does not support blinding oracles")
+    if any(o.num_shards != world for o in oracles):
+        raise N.ShapeError("the oracles must be row-block shards over the %d ranks" % world)
+
+
+def batch_prove_openings_sharded(degree_bits, instances, oracles, challenger, fri_params, group=None):
+    """batch_fri.batch_prove_openings when the BatchFriOracles are this rank's row-block shards of `group`
+    (BatchFriOracle.from_values(..., shard=(rank, world))): the Placement of the oracles' shard, whose open_many routes
+    the query openings between the ranks. Collective; the caller must already have observed the full caps
+    (Placement.cap) in `challenger`. Returns the same FriProof on every rank, byte-identical to the single-device proof.
+    Refusals: check_batch_prove_openings (ShapeError on every rank). Without an initialised process group, or with one
+    rank, this is batch_prove_openings."""
+    from .batch_fri import batch_prove_openings
+
+    check_batch_prove_openings(oracles, fri_params, _world_size(group))
+    placement = Placement(oracles[0].shard_index, oracles[0].num_shards, group)
+    return batch_prove_openings(degree_bits, instances, oracles, challenger, fri_params, placement=placement)
 
 
 def all_gather_tensor(t, group=None):

@@ -7,7 +7,7 @@ import numpy as np
 
 from . import _native as N
 from .field import log2_strict
-from .hash import MerkleCap, MerkleProof, _open_leaves, _read_digests
+from .hash import NUM_HASH_OUT_ELTS, MerkleCap, MerkleProof, _open_leaves, _read_digests
 from .proof import eval_commitments
 
 SALT_SIZE = 4  # oracle.rs:26
@@ -92,9 +92,12 @@ class _DeviceMerkleTree:
         return self.get_rows(i, 1)[0]
 
     def open_many(self, indices):
+        """(leaves (q, W), paths (q, L, 4)) for local leaf indices; a prefixed batch's leaves are `prefix || row`, W + 4
+        words."""
         b = self._b
         layers = b.degree_log + b.rate_bits - b.cap_height  # local rows and local cap shrink together
-        return _open_leaves(N.lib().gl_commit_open, b.h, b.ctx, indices, b.leaf_width, layers)
+        width = b.leaf_width + (NUM_HASH_OUT_ELTS if b.prefixed else 0)
+        return _open_leaves(N.lib().gl_commit_open, b.h, b.ctx, indices, width, layers)
 
     def prove(self, leaf_index):
         return MerkleProof(self.open_many([leaf_index])[1][0])
@@ -112,26 +115,28 @@ class PolynomialBatch(N.Handle):
         self.leaf_width = num_polys + (SALT_SIZE if blinding else 0)
         self.lde_size = 1 << (degree_log + rate_bits)
         self.local_rows = self.lde_size // self.num_shards  # leaf rows [shard*local_rows, (shard+1)*local_rows)
+        self.prefixed = False  # a later stage of a batch Merkle tree: leaf j is `prefix j || LDE row j` (_from_device)
         self.merkle_tree = _DeviceMerkleTree(self)
 
     @classmethod
-    def _create(cls, cols, rate_bits, blinding, cap_height, is_coeffs, salt, ctx, shard=(0, 1), salt_key=None):
+    def _create(cls, cols, rate_bits, blinding, cap_height, is_coeffs, salt, ctx, shard=(0, 1), salt_key=None,
+                prefix=None):
         ctx = ctx or N.default_context()
         cols = np.ascontiguousarray(cols, dtype=np.uint64)
         if cols.ndim != 2 or cols.shape[0] == 0:
             raise N.ShapeError("expected a non-empty (num_polys, degree) array")
         B, n = cols.shape
         log_n = log2_strict(n)
-        if salt_key is not None:
+        if salt_key is not None or prefix is not None:
             if salt is not None:
-                raise N.ShapeError("salt= and salt_key= are exclusive")
+                raise N.ShapeError("salt= is exclusive with salt_key= and prefix=")
             kind = N.COLS_COEFFS if is_coeffs else N.COLS_VALUES
 
             def add_columns(h):
                 N.check(N.lib().gl_commit_add_columns(h, 0, B, N.np_ptr(cols), n, kind, N.MEM_HOST), ctx.h)
 
             return cls._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, blinding=blinding,
-                                    salt_key=salt_key, shard=shard)
+                                    salt_key=salt_key, shard=shard, prefix=prefix)
         sp = None
         if blinding:
             if salt is None:
@@ -149,14 +154,22 @@ class PolynomialBatch(N.Handle):
 
     @classmethod
     def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns, *, blinding=False,
-                     salt_key=None, shard=(0, 1)):
+                     salt_key=None, shard=(0, 1), prefix=None):
         """A batch committed incrementally: gl_commit_begin, then add_columns(h) issues the gl_commit_add_columns calls
         on the unfinished handle h, then gl_commit_finish -- or, with blinding, gl_commit_finish_keyed: the salt is
         drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). shard=(g, G): only
-        leaf rows [g*N/G, (g+1)*N/G) on this device, as in from_values. The columns' device memory only has to live
+        leaf rows [g*N/G, (g+1)*N/G) on this device, as in from_values. prefix: a finished PolynomialBatch whose local
+        cap has one entry per local leaf of this one; the tree is then a later stage of a batch Merkle tree, over the
+        leaves `its cap entry j || LDE row j` (gl_commit_finish_prefixed). The columns' device memory only has to live
         until this returns."""
         if salt_key is not None and not blinding:
             raise N.ShapeError("salt_key= needs blinding=True")
+        if prefix is not None:
+            if blinding:
+                raise N.ShapeError("a prefixed commitment cannot be blinded")
+            entries, rows = (1 << prefix.cap_height) // prefix.num_shards, (1 << (degree_log + rate_bits)) // shard[1]
+            if entries != rows:
+                raise N.ShapeError("the prefix has %d cap entries for %d leaves" % (entries, rows))
         key = _salt_key(salt_key) if salt_key is not None else None
         h = N.vp()
         N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, int(bool(blinding)),
@@ -164,7 +177,10 @@ class PolynomialBatch(N.Handle):
         batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
         try:
             add_columns(h)
-            if blinding:
+            if prefix is not None:
+                N.check(N.lib().gl_commit_finish_prefixed(h, N.lib().gl_commit_dev_cap(prefix.h)), ctx.h)
+                batch.prefixed = True
+            elif blinding:
                 N.check(N.lib().gl_commit_finish_keyed(h, key), ctx.h)
             else:
                 N.check(N.lib().gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
