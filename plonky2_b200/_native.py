@@ -202,6 +202,7 @@ class Handle:
 class Context(Handle):
     """One gl_ctx per (device, stream) (SURVEY.md section 8b, threading row)."""
     destroyer = "gl_ctx_destroy"
+    _torch_stream = None
 
     def __init__(self, device=0, stream=None):
         h = vp()
@@ -211,6 +212,18 @@ class Context(Handle):
 
     def synchronize(self):
         check(lib().gl_ctx_synchronize(self.h), self.h)
+
+    def after_caller(self):
+        """Order this context's stream after everything queued so far on torch's current stream of its device: the
+        library's later reads of a caller's tensor see the values that stream is still producing, and its writes into
+        a tensor torch allocated land after the reads torch queued on the block's previous tenant. An event wait on the
+        device: the host does not block. Every function that hands a torch tensor to the library calls it before its
+        first library call."""
+        import torch
+
+        if self._torch_stream is None:
+            self._torch_stream = torch.cuda.ExternalStream(self.stream, device=torch.device("cuda", self.device))
+        self._torch_stream.wait_stream(torch.cuda.current_stream(self._torch_stream.device))
 
     @property
     def stream(self):

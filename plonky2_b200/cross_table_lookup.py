@@ -232,6 +232,7 @@ def compute_ctl_helper_columns(trace, groups, ctl_challenges, constraint_degree,
     if tuple(out.shape) != (num_helpers + len(zs_index), n) or not out.is_contiguous():
         raise N.ShapeError("the CTL output must be a contiguous (%d, %d) tensor" % (num_helpers + len(zs_index), n))
     ch = np.array([int(v) % F.ORDER for c in ctl_challenges for v in (c.beta, c.gamma)], dtype=np.uint64)
+    ctx.after_caller()
     N.check(N.lib().gl_stark_ctl_helpers(ctx.h, N.vp(trace.data_ptr()), n, cols, F.log2_strict(n), prog,
                                          offsets.ctypes.data_as(N.u32p), len(offsets) - 1,
                                          N.np_ptr(consts) if len(consts) else None, len(consts), N.np_ptr(ch),
@@ -393,7 +394,8 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     order, the CTL challenge set (get_ctl_data), every table's CTL helper and Z columns on the device
     (cross_table_lookup_data at the system's largest constraint degree), then table by table on the same challenger its
     public inputs, the config and prove_with_commitment with its CTL data -- the order the reference's verifier-side
-    replay accepts. traces: per table (COLUMNS, n) host columns or a torch CUDA tensor, read on the device once. Raises
+    replay accepts. traces: per table (COLUMNS, n) host columns or a torch CUDA tensor, read on the device once; a torch
+    trace may still be in production on the caller's current torch stream, the library's work is ordered after it. Raises
     ShapeError before any device work for every shape the reference cannot prove or verify (check_prove_shapes).
     Returns a MultiStarkProof. distributed.prove_with_ctls proves the same system across several GPUs."""
     from .distributed import Placement

@@ -145,6 +145,7 @@ class Placement:
         size = (1 << degree_bits) << (quotient_degree_factor - 1).bit_length()
         dev = "cuda:%d" % ctx.device
         local = torch.empty((n_alphas, size // self.num_shards), dtype=torch.int64, device=dev)
+        ctx.after_caller()
         failure = None
         try:
             run_shard(local)

@@ -1447,6 +1447,7 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
     qdf = common_data.quotient_degree_factor
     ctx = wires_commitment.ctx
     handles = (C.c_void_p * 3)(*[c.h for c in commits])
+    ctx.after_caller()
     if placement.num_shards > 1:
         def run_shard(local):
             N.check(N.lib().gl_plonk_quotient_shard(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts),
@@ -1572,7 +1573,7 @@ def sigma_polys(config, degree_bits, pairs, num_virtual_targets=0, ctx=None):
         n_pairs, mem = len(host), N.MEM_HOST
         ptr = N.np_ptr(host) if n_pairs else None
     out = torch.empty((nr, n), dtype=torch.int64, device="cuda:%d" % ctx.device)
-    torch.cuda.synchronize(out.device)
+    ctx.after_caller()
     N.check(N.lib().gl_sigma_polys(ctx.h, ptr, n_pairs, mem, config.num_wires, nr, degree_bits, int(num_virtual_targets),
                                    N.np_ptr(k_is), N.vp(out.data_ptr()), N.MEM_DEVICE), ctx.h)
     ctx.synchronize()  # the tensor goes to torch, whose stream is not the context's
@@ -1586,6 +1587,7 @@ def commit_constants_sigmas(common_data, constant_vecs, sigmas, ctx=None, shard=
     ctx = ctx or N.default_context()
     consts = np.ascontiguousarray(np.stack(constant_vecs), dtype=np.uint64)
     n = 1 << common_data.degree_bits
+    ctx.after_caller()
 
     def add_columns(h):
         N.check(N.lib().gl_commit_add_columns(h, 0, len(consts), N.np_ptr(consts), n, N.COLS_VALUES, N.MEM_HOST), ctx.h)

@@ -198,6 +198,7 @@ class PolynomialBatch(N.Handle):
         blinding / salt_key / shard: as in _from_device."""
         ctx = ctx or N.default_context()
         n = 1 << degree_log
+        ctx.after_caller()
 
         def add_columns(h):
             for j in range(polys.shape[0]):

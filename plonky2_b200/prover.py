@@ -35,7 +35,7 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
     device matrix the wires commitment was built from) and the sigma value columns (resident since circuit build).
     Each gl_partial_products_and_zs call writes its columns straight into a device staging matrix; each column group is
     then handed to the incremental commitment (gl_commit_add_columns, GL_MEM_DEVICE): no H2D, no D2H.
-    The caller's tensors must be complete (their producing stream synchronised or ordered before ctx's stream).
+    The caller's tensors may still be in production on its current torch stream: the library's work is ordered after it.
     With blinding the salt is drawn on the device from salt_key (PolynomialBatch._from_device). shard=(g, G): only row
     block g of G of the LDE and tree on this device (the columns are computed over all n rows either way).
     Returns the PolynomialBatch (num_challenges * (num_partial_products + 1) polynomials)."""
@@ -51,8 +51,9 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
     k_is = np.ascontiguousarray(k_is, dtype=np.uint64)
     nch = len(betas)
     M = (R + degree - 1) // degree          # columns per challenge: M - 1 partial products, then Z
-    L = N.lib()
     stage = torch.empty((M, n), dtype=torch.int64, device=wires_dev.device)  # must outlive _from_device's synchronise
+    ctx.after_caller()
+    L = N.lib()
 
     def add_columns(h):
         for i in range(nch):

@@ -271,6 +271,7 @@ def compute_quotient_polys(stark, trace_commitment, public_inputs, alphas, auxil
                                      ctl_vars)
     ctx = trace_commitment.ctx
     prog = b.program()
+    ctx.after_caller()
     if placement.num_shards > 1:
         aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
 
@@ -327,7 +328,8 @@ def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx, out=None
     """The lookup helper columns (prover.rs:177-195, lookup_helper_columns) on the device: for every lookup, for every
     challenge, the h_k columns and Z, from the trace values `trace` -- a (COLUMNS, n) int64 CUDA tensor, read in place.
     Returns a (num_lookup_helper_columns, n) int64 CUDA tensor of values: `out` if given (a contiguous view, e.g. the
-    first rows of a table's auxiliary buffer), else a new one."""
+    first rows of a table's auxiliary buffer), else a new one. `trace` may still be in production, and `out` still be
+    read, on the caller's current torch stream: the library's work is ordered after it."""
     import torch
 
     from .lookup import row_programs
@@ -341,6 +343,7 @@ def compute_lookup_helper_columns(stark, trace, lookup_challenges, ctx, out=None
         out = torch.empty(shape, dtype=torch.int64, device=trace.device)
     elif tuple(out.shape) != shape or not out.is_contiguous():
         raise N.ShapeError("the lookup helper output must be a contiguous %r tensor" % (shape,))
+    ctx.after_caller()
     N.check(N.lib().gl_stark_lookup_helpers(ctx.h, N.vp(trace.data_ptr()), n, cols, F.log2_strict(n), prog,
                                             offsets.ctypes.data_as(N.u32p), len(offsets) - 1,
                                             N.np_ptr(consts) if len(consts) else None, len(consts), N.np_ptr(ch), len(ch),
@@ -354,6 +357,7 @@ def commit_auxiliary_polys(helper_columns, rate_bits, cap_height, ctx, **on):
     committed straight from the device tensor compute_lookup_helper_columns returned. on: shard=(g, G) commits row
     block g of G only."""
     B, n = helper_columns.shape
+    ctx.after_caller()
 
     def add_columns(h):
         N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(helper_columns.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE),
@@ -606,6 +610,7 @@ def _commit_trace(trace, rate_bits, cap_height, ctx, **on):
         cols = trace.contiguous().view(torch.int64)
         B, n = cols.shape
         log_n = F.log2_strict(n)
+        ctx.after_caller()
 
         def add_columns(h):
             N.check(N.lib().gl_commit_add_columns(h, 0, B, N.vp(cols.data_ptr()), n, N.COLS_VALUES, N.MEM_DEVICE), ctx.h)
@@ -622,10 +627,11 @@ def _device_trace(trace, ctx):
     if hasattr(trace, "data_ptr"):
         if not trace.is_cuda or trace.dim() != 2 or trace.element_size() != 8:
             raise N.ShapeError("a torch trace must be a (COLUMNS, n) CUDA tensor of 64-bit words")
-        return trace.contiguous().view(torch.int64)
-    host = np.ascontiguousarray(trace, dtype=np.uint64).view(np.int64)
-    dev = torch.from_numpy(host).to("cuda:%d" % ctx.device)
-    torch.cuda.synchronize(dev.device)  # the copy is on torch's stream; the library reads it on the context's
+        dev = trace.contiguous().view(torch.int64)
+    else:
+        host = np.ascontiguousarray(trace, dtype=np.uint64).view(np.int64)
+        dev = torch.from_numpy(host).to("cuda:%d" % ctx.device)
+    ctx.after_caller()  # a copy above is on torch's stream; the library reads the tensor on the context's
     return dev
 
 
@@ -673,8 +679,9 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     StarkProofWithPublicInputs. The trace commitment, then a fresh challenger observing the public inputs, the config
     and the trace cap, then prove_with_commitment without CTLs. verifier_circuit_fri_params: the FRI parameters of a
     verifier circuit made for another degree (ConstantArityBits only); the transcript then observes the zero caps and
-    coefficients that verifier expects. Raises ShapeError / NativeError with the reference's messages; every commitment
-    is released on every exit path."""
+    coefficients that verifier expects. A torch trace may still be in production on the caller's current torch stream:
+    the library's work is ordered after it. Raises ShapeError / NativeError with the reference's messages; every
+    commitment is released on every exit path."""
     return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, D.Placement())
 
 

@@ -177,6 +177,7 @@ def main():
 
     import oracle_lib
     import stark_twin as T
+    import torch
 
     import plonky2_b200 as pb
     from plonky2_b200 import stark as S
@@ -185,7 +186,7 @@ def main():
     stark, config = FibonacciPairsStark(), S.StarkConfig.standard_fast_config()
     t0 = time.perf_counter()
     trace = fibonacci_pairs_trace(args.log_n)
-    ctx.synchronize()
+    torch.cuda.synchronize()     # the generator's kernels run on torch's stream, not the context's
     gen_ms = (time.perf_counter() - t0) * 1e3
     for _ in range(args.warmup):
         S.prove(stark, config, trace, [], ctx=ctx)

@@ -139,7 +139,7 @@ def per_shard_run(args):
     qdf = stark.quotient_degree_factor()
     size = (1 << args.log_n) << (qdf - 1).bit_length()
     values = torch.empty((G, len(al), size // G), dtype=torch.int64, device="cuda")
-    ctx.synchronize()
+    torch.cuda.synchronize()     # the trace generator's kernels run on torch's stream, not the context's
 
     def timed(fn):
         ctx.synchronize()
