@@ -57,6 +57,11 @@ int gl_ctx_create(int device, void* stream, gl_ctx** out);
 void gl_ctx_destroy(gl_ctx* ctx);
 const char* gl_last_error(const gl_ctx* ctx); /* ctx may be NULL: last error of the calling thread */
 int gl_ctx_synchronize(gl_ctx* ctx);
+/* Bytes of the device's default memory pool in use now (*in_use) and at most since the last reset (*high), after the
+ * context's queued work has run (synchronises); reset_high != 0 then resets the high-water mark to the current use.
+ * Every device buffer of the library comes from that pool (cudaMallocAsync), so this is the library's footprint on the
+ * device -- of every context on it. Memory from torch's caching allocator, or any other cudaMalloc, is not in it. */
+int gl_ctx_device_bytes(gl_ctx* ctx, uint64_t* in_use, uint64_t* high, int reset_high);
 /* the cudaStream_t every call on this context is ordered on (callers that mix their own stream work with the
  * library's -- torch tensors, NCCL -- must issue it on this stream or order it with events) */
 void* gl_ctx_stream(const gl_ctx* ctx);
@@ -147,6 +152,26 @@ int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]);
  * handle's LDE, hashed in place. The handle keeps its own copy of the prefix. gl_commit_open then returns the prefixed
  * leaves (W + 4 words); gl_commit_leaves, gl_commit_get_lde_values and gl_commit_dev_lde still return the LDE alone. */
 int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix);
+/* A NON-RESIDENT commitment, for LDEs larger than device memory: gl_commit_begin's unsharded, unblinded handle, which
+ * keeps its coefficients, its whole digest buffer and its cap but never its LDE. num_blocks = G = 2^s, 1 <= G <=
+ * 2^cap_height (else GL_ERR_BAD_SHAPE): the LDE's row block g, leaves [g*N/G, (g+1)*N/G), is the coset
+ * (g_shift * w_N^{bitrev_s(g)}) <w_{N/G}> and holds whole cap subtrees, as a shard of gl_commit_create_sharded does.
+ *   gl_commit_add_columns  fills the coefficients (iNTT / canonicalise) and does not extend;
+ *   gl_commit_finish       salt = NULL: for g = 0 .. G-1, the coset LDE of all B columns onto block g into one scratch of
+ *                          B x N/G words, hashed into the block's range of the digests and cap; the scratch is freed.
+ *                          gl_commit_finish_keyed / _prefixed: GL_ERR_BAD_ARG (its cap may still be another handle's
+ *                          prefix).
+ * Cap, digests, leaves, Merkle paths and LDE values equal the resident commitment's bit for bit.
+ * gl_commit_leaves, gl_commit_get_lde_values and gl_commit_open rebuild the blocks that hold the requested rows, one at
+ * a time, into one B x N/G scratch freed before they return; gl_commit_dev_lde returns NULL; gl_openings and gl_fri_begin
+ * read the coefficients as for any handle; gl_stark_quotient[_aux] evaluate the quotient coset in G parts (below);
+ * gl_fri_begin_values, gl_stark_quotient_shard and gl_plonk_quotient[_shard] return GL_ERR_BAD_ARG.
+ * Device footprint: B x n coefficients + 8 x (N - 2^cap_height) + 4 x 2^cap_height digest words, plus B x N/G words
+ * of scratch (and as much again for the fold when N/G < n) while a block is built. */
+int gl_commit_begin_blocked(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits, uint32_t cap_height,
+                            uint32_t num_blocks, uint64_t* coeff_storage, gl_commit** out);
+/* G of a non-resident commitment; 0 for a resident one */
+uint32_t gl_commit_lde_blocks(const gl_commit* c);
 int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_shards);
 void gl_commit_destroy(gl_commit* c);
 /* shape queries */
@@ -287,6 +312,12 @@ int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* progr
 int gl_stark_quotient_aux(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
                           const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
                           uint32_t quotient_degree_factor, uint64_t* out_coeffs);
+/* Both also take NON-RESIDENT trace and auxiliary handles (gl_commit_begin_blocked; both or neither, else GL_ERR_BAD_ARG):
+ * the quotient coset is then evaluated in the trace's G parts on this device, part g being the points bitrev_s(g) + G*k
+ * that a shard g of G evaluates (gl_stark_quotient_shard below), from the LDE of the coefficients onto the part's coset
+ * (and onto that coset times w_n when the next row leaves the part), each part's values written to its points of
+ * out_coeffs. The result and the errors are the resident call's. Scratch per part: (B_trace + B_aux) x size/G words,
+ * twice that when G > 2^log2_ceil(quotient_degree_factor), plus n_alphas x size/G. G larger than size: GL_ERR_BAD_SHAPE. */
 /* The quotient of a STARK whose commitments are row-block shards (gl_commit_create_sharded / gl_commit_begin with
  * num_shards = G), in two steps with an all-gather between them. With size = n << log2_ceil(quotient_degree_factor),
  * shard g owns the points i = r + G*k (k < M = size / G, r = the s-bit reversal of g, G = 2^s) of the quotient coset

@@ -31,7 +31,8 @@ EXPORTS = [
     "gl_merkle_cap", "gl_merkle_digests", "gl_merkle_open", "gl_fri_begin", "gl_fri_begin_values", "gl_fri_values_local", "gl_fri_begin_from_coeffs",
     "gl_fri_destroy", "gl_fri_coeffs", "gl_fri_commit_round", "gl_fri_commit_round_sharded", "gl_fri_mix", "gl_fri_fold", "gl_fri_final_poly",
     "gl_fri_open", "gl_fri_num_rounds", "gl_fri_pow", "gl_commit_finish_keyed", "gl_random_field_elements",
-    "gl_commit_finish_prefixed", "gl_commit_dev_cap",
+    "gl_commit_finish_prefixed", "gl_commit_dev_cap", "gl_commit_begin_blocked", "gl_commit_lde_blocks",
+    "gl_ctx_device_bytes",
 ]
 
 
@@ -66,6 +67,7 @@ def lib():
     L.gl_last_error.argtypes = [vp]
     L.gl_last_error.restype = C.c_char_p
     L.gl_ctx_synchronize.argtypes = [vp]
+    L.gl_ctx_device_bytes.argtypes = [vp, u64p, u64p, C.c_int]
     L.gl_ctx_launch_count.argtypes = [vp]
     L.gl_ctx_launch_count.restype = C.c_uint64
     L.gl_ctx_set_ntt_group.argtypes = [vp, C.c_uint32]
@@ -76,6 +78,8 @@ def lib():
     L.gl_bcast.argtypes = [vp, vp, C.c_size_t, C.POINTER(vp), C.c_uint32, C.c_uint32]
     L.gl_commit_begin.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32,
                                   vp, C.POINTER(vp)]
+    L.gl_commit_begin_blocked.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp,
+                                          C.POINTER(vp)]
     L.gl_commit_add_columns.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_size_t, C.c_int, C.c_int]
     L.gl_commit_finish.argtypes = [vp, vp, C.c_int]
     L.gl_commit_finish_keyed.argtypes = [vp, C.c_char_p]
@@ -92,7 +96,7 @@ def lib():
     L.gl_commit_destroy.argtypes = [vp]
     L.gl_commit_destroy.restype = None
     for n in ("gl_commit_num_polys", "gl_commit_leaf_width", "gl_commit_degree_log", "gl_commit_rate_bits",
-              "gl_commit_cap_height"):
+              "gl_commit_cap_height", "gl_commit_lde_blocks"):
         getattr(L, n).argtypes = [vp]
         getattr(L, n).restype = C.c_uint32
     L.gl_commit_cap.argtypes = [vp, vp, C.c_int]
@@ -229,6 +233,15 @@ class Context(Handle):
     def stream(self):
         """The cudaStream_t (as an int) every call on this context is ordered on."""
         return int(lib().gl_ctx_stream(self.h) or 0)
+
+    def device_bytes(self, reset_high=False):
+        """(in_use, high): bytes of the device's default memory pool in use now and at most since the last reset, after
+        this context's queued work has run; reset_high then resets the high-water mark to the current use. Every device
+        buffer of the library, on any context of this device, comes from that pool; torch's caching allocator does not
+        (gl_ctx_device_bytes)."""
+        in_use, high = C.c_uint64(), C.c_uint64()
+        check(lib().gl_ctx_device_bytes(self.h, C.byref(in_use), C.byref(high), int(bool(reset_high))), self.h)
+        return in_use.value, high.value
 
     @property
     def launch_count(self):

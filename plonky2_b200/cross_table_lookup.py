@@ -372,9 +372,9 @@ class MultiStarkProof:
         return dict(ctl_challenges=ctl_challenges, stark_challenges=out)
 
 
-def check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs):
+def check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs, lde_blocks=0):
     """prove_with_ctls's refusals, before any device work: trace and public-input counts, every table's
-    stark.prove checks, check_ctl_shapes and check_lookup_shapes. Returns (each table's ProveParams,
+    stark.prove checks (with lde_blocks), check_ctl_shapes and check_lookup_shapes. Returns (each table's ProveParams,
     max_constraint_degree)."""
     from . import stark as S
 
@@ -382,14 +382,15 @@ def check_prove_shapes(starks, config, traces, cross_table_lookups, public_input
         raise N.ShapeError("expected %d traces, got %d" % (len(starks), len(traces)))
     if len(public_inputs) != len(starks):
         raise N.ShapeError("expected %d public-input lists, got %d" % (len(starks), len(public_inputs)))
-    params = [S._check_prove_shapes(s, config, t, p) for s, t, p in zip(starks, traces, public_inputs)]
+    params = [S._check_prove_shapes(s, config, t, p, lde_blocks=lde_blocks)
+              for s, t, p in zip(starks, traces, public_inputs)]
     max_degree = check_ctl_shapes(starks, cross_table_lookups, config.num_challenges)
     for s in starks:
         S.check_lookup_shapes(s)
     return params, max_degree
 
 
-def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None):
+def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None, lde_blocks=None):
     """A multi-STARK proof with cross-table lookups: every table's trace commitment, every trace cap observed in table
     order, the CTL challenge set (get_ctl_data), every table's CTL helper and Z columns on the device
     (cross_table_lookup_data at the system's largest constraint degree), then table by table on the same challenger its
@@ -397,10 +398,12 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     replay accepts. traces: per table (COLUMNS, n) host columns or a torch CUDA tensor, read on the device once; a torch
     trace may still be in production on the caller's current torch stream, the library's work is ordered after it. Raises
     ShapeError before any device work for every shape the reference cannot prove or verify (check_prove_shapes).
-    Returns a MultiStarkProof. distributed.prove_with_ctls proves the same system across several GPUs."""
-    from .distributed import Placement
+    Returns a MultiStarkProof. distributed.prove_with_ctls proves the same system across several GPUs. lde_blocks=G:
+    every commitment is non-resident, as in stark.prove; G must also be at most every table's quotient coset size."""
+    from . import stark as S
 
-    return _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, Placement())
+    return _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx,
+                            S.lde_placement(config, lde_blocks))
 
 
 def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement):
@@ -411,8 +414,9 @@ def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs,
     from .lookup import get_grand_product_challenge_set
     from . import stark as S
 
+    params, max_degree = check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs,
+                                            placement.lde_blocks)
     ctx = ctx or N.default_context()
-    params, max_degree = check_prove_shapes(starks, config, traces, cross_table_lookups, public_inputs)
     public_inputs = [[int(v) % F.ORDER for v in p] for p in public_inputs]
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     dev_traces, commitments = [], []

@@ -487,6 +487,7 @@ static int log2_exact(size_t n, uint32_t* out) {
     return 0;
 }
 
+static int tree_hash(gl_ctx* ctx, const Tree& t);
 // MerkleTree::new over device leaves (merkle_tree.rs:193-224)
 static int tree_build(gl_ctx* ctx, Tree& t) {
     if (log2_exact(t.N, &t.log_n)) return set_err(ctx, GL_ERR_BAD_SHAPE, "Not a power of two: %zu", t.N);
@@ -495,6 +496,10 @@ static int tree_build(gl_ctx* ctx, Tree& t) {
                        t.log_n);
     TRY(dmalloc(ctx, &t.digests, t.digest_words()));
     TRY(dmalloc(ctx, &t.cap, t.cap_words()));
+    return tree_hash(ctx, t);
+}
+// The leaf hashes and Merkle levels of t into its (allocated) digests and cap
+static int tree_hash(gl_ctx* ctx, const Tree& t) {
     TreeView v = t.view();
     {
         PhaseScope ps(ctx, GL_PHASE_LEAF_HASH);
@@ -568,11 +573,13 @@ struct gl_commit {
     gl_ctx* ctx;
     uint32_t B, W, degree_log, rate_bits;
     uint32_t shard_index = 0, shard_log = 0;  // this handle holds leaf rows [g*N/G, (g+1)*N/G)
+    // Non-resident (gl_commit_begin_blocked): lde_blocks = 2^block_log row blocks of the LDE, each built from the
+    // coefficients where it is hashed or read and never kept; tree.leaves is NULL. 0: the LDE is resident in tree.leaves.
+    uint32_t lde_blocks = 0, block_log = 0;
     bool blinding;
     u64* coeffs = nullptr;  // B x n
     bool own_coeffs = true; // false: caller-owned storage handed to gl_commit_begin
     bool finished = false;  // tree built (handles from gl_commit_begin: after gl_commit_finish)
-    u64 sg = 0;             // coset shift of this shard's row block
     Tree tree;
 };
 
@@ -636,7 +643,8 @@ static int coset_lde_columns(gl_ctx* ctx, const u64* coeffs, uint32_t ncols, uin
     return lde_columns(ctx, folded.get(), M, ncols, (int)log_M, 0, shift, out, out_stride);
 }
 
-// Allocate the device state of a commitment: coefficients (or adopt the caller's matrix) and the column-major LDE.
+// Allocate the device state of a commitment: coefficients (or adopt the caller's matrix) and the column-major LDE
+// (none for a non-resident commitment).
 static int commit_alloc(gl_ctx* ctx, gl_commit* c, uint32_t cap_height, u64* ext_coeffs) {
     const size_t n = (size_t)1 << c->degree_log, N = n << c->rate_bits;
     if (ext_coeffs) {
@@ -645,30 +653,40 @@ static int commit_alloc(gl_ctx* ctx, gl_commit* c, uint32_t cap_height, u64* ext
     } else {
         TRY(dmalloc(ctx, &c->coeffs, (size_t)c->B * n));
     }
-    // Row-block sharding (SURVEY section 8e): shard g of G = 2^s owns leaves [g*N/G, (g+1)*N/G), i.e. the
-    // LDE points i = g' (mod G), g' = bitrev_s(g): the coset (g * w_N^{g'}) <w_{N/G}> in bit-reversed order.
     const uint32_t sl = c->shard_log;
     const size_t Nloc = N >> sl;
-    const uint32_t gprime = bitrev32(c->shard_index, sl);
-    c->sg = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(root_of_unity(c->degree_log + c->rate_bits), gprime));
     Tree& t = c->tree;
     t.N = Nloc;
     t.W = c->W;
+    t.log_n = c->degree_log + c->rate_bits - sl;
     t.cap_height = cap_height - sl;
-    t.own_leaves = true;
     t.ls = 1;       // column-major LDE: column k at leaves + k*Nloc, leaf order inside
     t.es = Nloc;
+    if (c->lde_blocks) return GL_OK;
+    t.own_leaves = true;
     TRY(dmalloc(ctx, &t.leaves, Nloc * (size_t)c->W));
     return GL_OK;
 }
+// Columns [g0, g0 + gc) of c's LDE on its row block g of G = 2^s, from the coefficients, column b at
+// out + (b - g0)*out_stride. Row-block sharding (SURVEY section 8e): block g owns leaves [g*N/G, (g+1)*N/G), i.e. the
+// LDE points i = g' (mod G), g' = bitrev_s(g): the coset (g * w_N^{g'}) <w_{N/G}> in bit-reversed order. A shard's
+// resident LDE is its block (shard_index, shard_log); a non-resident commitment builds its blocks (g, block_log) one at
+// a time.
+static int commit_extend(gl_ctx* ctx, const gl_commit* c, uint32_t g0, uint32_t gc, uint32_t g, uint32_t s, u64* out,
+                         size_t out_stride) {
+    PhaseScope ps(ctx, GL_PHASE_LDE);
+    const u64 shift =
+        mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(root_of_unity(c->degree_log + c->rate_bits), bitrev32(g, s)));
+    return coset_lde_columns(ctx, c->coeffs + ((size_t)g0 << c->degree_log), gc, c->degree_log,
+                             c->degree_log + c->rate_bits - s, shift, out, out_stride);
+}
 // Columns [g0, g0 + gc) sit in c->coeffs as values (kind 0), coefficients (1) or canonical coefficients (2):
 // iNTT ("IFFT", oracle.rs:65-69) / canonicalise, then the leaf-major coset LDE ("FFT + blinding" + "transpose LDEs" +
-// bit-reversal, fused) into this shard's rows.
+// bit-reversal, fused) into this shard's rows. A non-resident commitment stops at the coefficients: gl_commit_finish
+// extends them block by block.
 static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int kind) {
     const size_t n = (size_t)1 << c->degree_log;
-    const uint32_t sl = c->shard_log;
     Tree& t = c->tree;
-    const size_t Nloc = t.N;
     u64* cg = c->coeffs + (size_t)g0 * n;
     if (kind == 0) {
         PhaseScope ps(ctx, GL_PHASE_INTT);
@@ -678,9 +696,44 @@ static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int
         k_canon<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(cg, tot);
         CKL(ctx);
     }
-    PhaseScope ps(ctx, GL_PHASE_LDE);
-    return coset_lde_columns(ctx, cg, gc, c->degree_log, c->degree_log + c->rate_bits - sl, c->sg,
-                             t.leaves + (size_t)g0 * Nloc, Nloc);
+    if (c->lde_blocks) return GL_OK;
+    return commit_extend(ctx, c, g0, gc, c->shard_index, c->shard_log, t.leaves + (size_t)g0 * t.N, t.N);
+}
+// Row block g of a non-resident commitment's LDE into lde (W x N/G words, column-major, leaf order)
+static int block_lde(gl_ctx* ctx, const gl_commit* c, uint32_t g, u64* lde) {
+    const size_t Nb = c->tree.N >> c->block_log;
+    return commit_extend(ctx, c, 0, c->B, g, c->block_log, lde, Nb);
+}
+// The Merkle tree of row block g of a non-resident commitment, over the leaves in lde: its C/G cap subtrees, whose
+// digests and cap entries are one contiguous range of the whole tree's (DESIGN section 5)
+static Tree block_tree(const gl_commit* c, uint32_t g, u64* lde) {
+    const Tree& w = c->tree;
+    Tree t;
+    t.N = w.N >> c->block_log;
+    t.W = w.W;
+    t.log_n = w.log_n - c->block_log;
+    t.cap_height = w.cap_height - c->block_log;
+    t.ls = 1;
+    t.es = t.N;
+    t.leaves = lde;
+    t.digests = w.digests + (size_t)g * t.digest_words();
+    t.cap = w.cap + (size_t)g * t.cap_words();
+    return t;
+}
+// "build Merkle tree" of a non-resident commitment: every block's LDE, built into one scratch buffer, hashed into the
+// block's range of the whole digest buffer and cap
+static int commit_finish_blocked(gl_ctx* ctx, gl_commit* c) {
+    Tree& t = c->tree;
+    TRY(dmalloc(ctx, &t.digests, t.digest_words()));
+    TRY(dmalloc(ctx, &t.cap, t.cap_words()));
+    DevBuf lde(ctx);
+    TRY(lde.alloc((size_t)c->W * (t.N >> c->block_log)));
+    for (uint32_t g = 0; g < c->lde_blocks; g++) {
+        TRY(block_lde(ctx, c, g, lde.get()));
+        TRY(tree_hash(ctx, block_tree(c, g, lde.get())));
+    }
+    c->finished = true;
+    return GL_OK;
 }
 // salt columns (blinding) + "build Merkle tree"
 static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem) {
@@ -1385,6 +1438,14 @@ __global__ void k_stark_unshard(const u64* values, uint32_t log_M, uint32_t shar
     const size_t r = bitrev32(s, shard_log);
     out[((size_t)a << (log_M + shard_log)) + r + (k << shard_log)] = values[((size_t)s * n_alphas + a) * M + k];
 }
+// part r = bitrev(g) of G = 2^shard_log of the quotient coset, evaluated on one device: values[a][k] -> out[a][r + G*k]
+__global__ void k_stark_place(const u64* values, uint32_t log_M, uint32_t shard_log, size_t r, u64* out) {
+    const size_t M = (size_t)1 << log_M;
+    const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= M) return;
+    const uint32_t a = blockIdx.y;
+    out[((size_t)a << (log_M + shard_log)) + r + (k << shard_log)] = values[(size_t)a * M + k];
+}
 // ---- starky's logUp helper columns (lookup_helper_columns, starky/src/lookup.rs:579-652): one thread per row of one
 // Lookup, every challenge; the row's arithmetic is gl_logup.cuh. Z is the additive mscan of the `term` sequences.
 __global__ void __launch_bounds__(128) k_logup_rows(LogupParams p, unsigned int* flag) {
@@ -1713,6 +1774,23 @@ int gl_ctx_synchronize(gl_ctx* ctx) {
     CK(ctx, cudaStreamSynchronize(ctx->stream));
     return GL_OK;
 }
+int gl_ctx_device_bytes(gl_ctx* ctx, uint64_t* in_use, uint64_t* high, int reset_high) {
+    if (!ctx) return set_err(ctx, GL_ERR_BAD_ARG, "null context");
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, cudaStreamSynchronize(ctx->stream));  // the stream-ordered allocations and frees queued so far have run
+    cudaMemPool_t pool;
+    CK(ctx, cudaDeviceGetDefaultMemPool(&pool, ctx->device));
+    uint64_t v = 0;
+    CK(ctx, cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &v));
+    if (in_use) *in_use = v;
+    CK(ctx, cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &v));
+    if (high) *high = v;
+    if (reset_high) {
+        uint64_t zero = 0;  // resets the high-water mark to the current use
+        CK(ctx, cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));
+    }
+    return GL_OK;
+}
 uint64_t gl_ctx_launch_count(const gl_ctx* ctx) { return ctx->launches; }
 int gl_ctx_set_ntt_group(gl_ctx* ctx, uint32_t columns) {
     // bit 31 selects the kernel variant of the column pass (a measurement switch, see gl_ntt_host.cuh)
@@ -1867,6 +1945,24 @@ int gl_commit_begin(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits,
     *out = c.release();
     return GL_OK;
 }
+int gl_commit_begin_blocked(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t rate_bits, uint32_t cap_height,
+                            uint32_t num_blocks, uint64_t* coeff_storage, gl_commit** out) {
+    if (!ctx || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    uint32_t shard_log = 0, block_log = 0;
+    TRY(commit_check_shape(ctx, B, log_n, rate_bits, cap_height, 0, 1, &shard_log));
+    if (log2_exact(num_blocks, &block_log) || block_log > cap_height)
+        return set_err(ctx, GL_ERR_BAD_SHAPE,
+                       "num_blocks=%u: a power of two of at most the cap size 2^%u (blocks own whole cap subtrees)",
+                       num_blocks, cap_height);
+    CK(ctx, cudaSetDevice(ctx->device));
+    CommitPtr c = commit_new(ctx, B, log_n, rate_bits, false, 0, 0);
+    c->lde_blocks = num_blocks;
+    c->block_log = block_log;
+    TRY(commit_alloc(ctx, c.get(), cap_height, coeff_storage));
+    *out = c.release();
+    return GL_OK;
+}
 int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, const uint64_t* cols, size_t col_stride,
                           int kind, int mem) {
     if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
@@ -1890,6 +1986,7 @@ int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem) {
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (c->blinding != (salt != nullptr)) return set_err(ctx, GL_ERR_BAD_ARG, "salt must be given exactly when blinding was requested");
     CK(ctx, cudaSetDevice(ctx->device));
+    if (c->lde_blocks) return commit_finish_blocked(ctx, c);
     return commit_finish(ctx, c, salt, mem);
 }
 int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix) {
@@ -1898,6 +1995,7 @@ int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix) {
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (!prefix) return set_err(ctx, GL_ERR_BAD_ARG, "null prefix");
     if (c->blinding) return set_err(ctx, GL_ERR_UNSUPPORTED, "a prefixed commitment cannot be blinded");
+    if (c->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "a non-resident commitment cannot be a prefixed stage");
     CK(ctx, cudaSetDevice(ctx->device));
     Tree& t = c->tree;
     // a copy: the previous stage (the prefix's owner) may be destroyed before this commitment
@@ -1984,22 +2082,38 @@ const uint64_t* gl_commit_dev_cap(const gl_commit* c) { return c && c->finished 
 int gl_commit_coeffs(gl_commit* c, uint64_t* out, int mem) {
     return copy_out(c->ctx, out, c->coeffs, (size_t)c->B << c->degree_log, mem);
 }
+// Rows [row_begin, row_begin + row_count) of the W-column LDE `lde` (column k at lde + k*es) as row-major leaves
+static int rows_out(gl_ctx* ctx, const u64* lde, size_t es, uint32_t W, size_t row_begin, size_t row_count, u64* out,
+                    int mem) {
+    // the LDE is column-major on the device; the reference's row-major leaves are produced on demand, in slabs
+    const size_t slab = ((size_t)1 << 27) / W + 1;  // ~1 GiB of staging at most
+    DevBuf stage(ctx);
+    if (mem == GL_MEM_HOST) TRY(stage.alloc((row_count < slab ? row_count : slab) * W));
+    for (size_t r0 = 0; r0 < row_count; r0 += slab) {
+        const size_t rows = row_count - r0 < slab ? row_count - r0 : slab;
+        u64* dst = mem == GL_MEM_HOST ? stage.get() : out + r0 * W;
+        k_rows_from_columns<<<dim3((unsigned)((rows + 31) / 32), (W + 31) / 32), dim3(32, 8), 0, ctx->stream>>>(
+            lde, es, row_begin + r0, rows, W, dst);
+        CKL(ctx);
+        if (mem == GL_MEM_HOST) TRY(d2h(ctx, out + r0 * W, stage.get(), rows * W));
+    }
+    return GL_OK;
+}
 int gl_commit_leaves(gl_commit* c, size_t row_begin, size_t row_count, uint64_t* out, int mem) {
     gl_ctx* ctx = c->ctx;
     if (row_begin + row_count > c->tree.N) return set_err(ctx, GL_ERR_BAD_ARG, "row range out of bounds");
     if (row_count == 0) return GL_OK;
     CK(ctx, cudaSetDevice(ctx->device));
-    // the LDE is column-major on the device; the reference's row-major leaves are produced on demand, in slabs
-    const size_t slab = ((size_t)1 << 27) / c->W + 1;  // ~1 GiB of staging at most
-    DevBuf stage(ctx);
-    if (mem == GL_MEM_HOST) TRY(stage.alloc((row_count < slab ? row_count : slab) * c->W));
-    for (size_t r0 = 0; r0 < row_count; r0 += slab) {
-        const size_t rows = row_count - r0 < slab ? row_count - r0 : slab;
-        u64* dst = mem == GL_MEM_HOST ? stage.get() : out + r0 * c->W;
-        k_rows_from_columns<<<dim3((unsigned)((rows + 31) / 32), (c->W + 31) / 32), dim3(32, 8), 0, ctx->stream>>>(
-            c->tree.leaves, c->tree.es, row_begin + r0, rows, c->W, dst);
-        CKL(ctx);
-        if (mem == GL_MEM_HOST) TRY(d2h(ctx, out + r0 * c->W, stage.get(), rows * c->W));
+    if (!c->lde_blocks) return rows_out(ctx, c->tree.leaves, c->tree.es, c->W, row_begin, row_count, out, mem);
+    // non-resident: the blocks that hold the rows, one at a time
+    const size_t Nb = c->tree.N >> c->block_log, row_end = row_begin + row_count;
+    DevBuf lde(ctx);
+    TRY(lde.alloc((size_t)c->W * Nb));
+    for (size_t r = row_begin; r < row_end;) {
+        const size_t g = r / Nb, end = (g + 1) * Nb < row_end ? (g + 1) * Nb : row_end;
+        TRY(block_lde(ctx, c, (uint32_t)g, lde.get()));
+        TRY(rows_out(ctx, lde.get(), Nb, c->W, r - g * Nb, end - r, out + (r - row_begin) * c->W, mem));
+        r = end;
     }
     return GL_OK;
 }
@@ -2015,8 +2129,18 @@ int gl_commit_get_lde_values(gl_commit* c, size_t index, size_t step, uint64_t* 
     for (uint32_t i = 0; i < bits; i++) rev |= ((idx >> i) & 1) << (bits - 1 - i);
     const size_t row0 = (size_t)c->shard_index * c->tree.N;
     if (rev < row0 || rev >= row0 + c->tree.N) return set_err(c->ctx, GL_ERR_BAD_ARG, "LDE row held by another shard");
-    CK(c->ctx, cudaMemcpy2DAsync(out, 8, c->tree.leaves + (rev - row0), c->tree.es * 8, 8, c->B, cudaMemcpyDeviceToHost,
-                                 c->ctx->stream));
+    CK(c->ctx, cudaSetDevice(c->ctx->device));
+    const u64* lde = c->tree.leaves;
+    size_t row = rev - row0, es = c->tree.es;
+    DevBuf block(c->ctx);
+    if (c->lde_blocks) {  // non-resident: the block that holds the row
+        es = c->tree.N >> c->block_log;
+        TRY(block.alloc((size_t)c->W * es));
+        TRY(block_lde(c->ctx, c, (uint32_t)(row / es), block.get()));
+        lde = block.get();
+        row %= es;
+    }
+    CK(c->ctx, cudaMemcpy2DAsync(out, 8, lde + row, es * 8, 8, c->B, cudaMemcpyDeviceToHost, c->ctx->stream));
     CK(c->ctx, cudaStreamSynchronize(c->ctx->stream));
     return GL_OK;
 }
@@ -2025,9 +2149,40 @@ int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_sha
     if (num_shards) *num_shards = 1u << c->shard_log;
     return GL_OK;
 }
+uint32_t gl_commit_lde_blocks(const gl_commit* c) { return c->lde_blocks; }
 int gl_commit_open(gl_commit* c, const uint64_t* leaf_indices, size_t count, uint64_t* out_leaves, uint64_t* out_paths) {
     NEED_FINISHED(c);
-    return tree_open(c->ctx, c->tree, leaf_indices, count, out_leaves, out_paths);
+    if (!c->lde_blocks) return tree_open(c->ctx, c->tree, leaf_indices, count, out_leaves, out_paths);
+    // non-resident: each block that holds a requested leaf is built once and opened as its own tree, whose sibling
+    // paths are the whole tree's (its cap subtrees' digests are a range of the whole digest buffer)
+    gl_ctx* ctx = c->ctx;
+    const Tree& t = c->tree;
+    const size_t Nb = t.N >> c->block_log, layers = t.log_n - t.cap_height;
+    std::map<uint32_t, std::vector<size_t>> by_block;  // block -> positions in leaf_indices
+    for (size_t i = 0; i < count; i++) {
+        if (leaf_indices[i] >= t.N)
+            return set_err(ctx, GL_ERR_BAD_ARG, "leaf index %llu out of range", (unsigned long long)leaf_indices[i]);
+        by_block[(uint32_t)(leaf_indices[i] / Nb)].push_back(i);
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    DevBuf lde(ctx);
+    if (count) TRY(lde.alloc((size_t)c->W * Nb));
+    std::vector<u64> idx, lv, pv;
+    for (const auto& kv : by_block) {
+        const uint32_t g = kv.first;
+        const std::vector<size_t>& pos = kv.second;
+        idx.resize(pos.size());
+        for (size_t k = 0; k < pos.size(); k++) idx[k] = leaf_indices[pos[k]] - (size_t)g * Nb;
+        lv.resize(pos.size() * c->W);
+        pv.resize(pos.size() * layers * 4 + 1);
+        TRY(block_lde(ctx, c, g, lde.get()));
+        TRY(tree_open(ctx, block_tree(c, g, lde.get()), idx.data(), pos.size(), lv.data(), pv.data()));
+        for (size_t k = 0; k < pos.size(); k++) {
+            memcpy(out_leaves + pos[k] * c->W, lv.data() + k * c->W, c->W * 8);
+            if (layers) memcpy(out_paths + pos[k] * layers * 4, pv.data() + k * layers * 4, layers * 4 * 8);
+        }
+    }
+    return GL_OK;
 }
 int gl_commit_eval_ext(gl_commit* c, const uint64_t point[2], uint64_t* out) {
     const uint32_t point_index = 0;
@@ -2099,7 +2254,7 @@ int gl_openings_shard(gl_ctx* ctx, gl_commit* const* commits, const uint32_t* po
 }
 const uint64_t* gl_commit_dev_lde(const gl_commit* c, size_t* col_stride) {
     if (col_stride) *col_stride = c->tree.es;
-    return c->tree.leaves;
+    return c->tree.leaves;  // NULL for a non-resident commitment
 }
 const uint64_t* gl_commit_dev_coeffs(const gl_commit* c) { return c->coeffs; }
 
@@ -2315,11 +2470,14 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
     if (n_alphas == 0 || n_alphas > GL_STARK_MAX_ALPHAS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d challenges", GL_STARK_MAX_ALPHAS);
     if (quotient_degree_factor == 0) return set_err(ctx, GL_ERR_BAD_ARG, "quotient_degree_factor is 0: the STARK has no quotient");
     if (whole && trace->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
+    if (!whole && trace->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "a shard's quotient needs a resident trace commitment");
     // unfinished handles: the error goes to `ctx`, the context the caller reads it from
     if (!trace->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the trace commitment");
     if (aux) {
         if (aux->ctx->device != ctx->device) return set_err(ctx, GL_ERR_BAD_ARG, "the auxiliary commitment is on another device");
         if (whole && aux->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole auxiliary LDE on this device");
+        if ((aux->lde_blocks != 0) != (trace->lde_blocks != 0))
+            return set_err(ctx, GL_ERR_BAD_ARG, "the trace and auxiliary commitments must both be resident or both not");
         if (!whole && (aux->shard_index != trace->shard_index || aux->shard_log != trace->shard_log))
             return set_err(ctx, GL_ERR_BAD_ARG, "the auxiliary commitment is shard %u of %u, the trace shard %u of %u",
                            aux->shard_index, 1u << aux->shard_log, trace->shard_index, 1u << trace->shard_log);
@@ -2327,8 +2485,8 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
             return set_err(ctx, GL_ERR_BAD_SHAPE, "the auxiliary commitment's degree or rate differs from the trace's");
         if (!aux->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called on the auxiliary commitment");
     }
-    TRY(quotient_shape_check(ctx, trace->degree_log, trace->rate_bits, trace->shard_log, quotient_degree_factor,
-                             GL_STARK_MAX_QD, qd_bits_out));
+    TRY(quotient_shape_check(ctx, trace->degree_log, trace->rate_bits, trace->shard_log + trace->block_log,
+                             quotient_degree_factor, GL_STARK_MAX_QD, qd_bits_out));
     for (uint32_t k = 0; k < n_instr; k++) {  // validate once on the host: the kernel trusts the program
         const gl_stark_instr in = program[k];
         bool ok = true;
@@ -2344,9 +2502,9 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
     }
     return GL_OK;
 }
-// The part of the quotient coset g*<w_size> (size = 2^(degree_log + qd_bits)) that a commitment's shard evaluates: shard
-// g of G = 2^sl owns the M = size / G points g*w_size^r*<w_M>, r = the sl-bit reversal of g (the whole coset for an
-// unsharded commitment)
+// The part g of G = 2^sl of the quotient coset g*<w_size> (size = 2^(degree_log + qd_bits)) that one evaluation covers:
+// the M = size / G points g*w_size^r*<w_M>, r = the sl-bit reversal of g. A shard evaluates its own part (the whole coset
+// for an unsharded commitment); a non-resident commitment's quotient is evaluated part by part, one per LDE block.
 struct QuotientCoset {
     uint32_t size_log, log_M;
     size_t size, M, r;
@@ -2358,17 +2516,16 @@ struct QuotientCoset {
     // Else the values on the coset times w_n.
     bool next_in_shard;
 };
-static QuotientCoset quotient_coset(const gl_commit* c, uint32_t qd_bits) {
+static QuotientCoset quotient_coset(const gl_commit* c, uint32_t qd_bits, uint32_t g, uint32_t sl) {
     QuotientCoset q;
-    const uint32_t sl = c->shard_log;
     q.size_log = c->degree_log + qd_bits;
     q.log_M = q.size_log - sl;
     q.size = (size_t)1 << q.size_log;
     q.M = (size_t)1 << q.log_M;
-    q.r = bitrev32(c->shard_index, sl);
+    q.r = bitrev32(g, sl);
     q.w_size = root_of_unity(q.size_log);
     q.shift = mul(MULTIPLICATIVE_GROUP_GENERATOR, gl::pow(q.w_size, q.r));
-    q.local_in_place = sl == 0 || qd_bits == c->rate_bits;
+    q.local_in_place = !c->lde_blocks && (sl == 0 || qd_bits == c->rate_bits);
     q.next_in_shard = sl <= qd_bits;
     return q;
 }
@@ -2395,13 +2552,14 @@ static int quotient_views(gl_ctx* ctx, const QuotientCoset& q, const gl_commit* 
     else TRY(values_on(mul(q.shift, root_of_unity(c->degree_log)), nbuf, next));
     return GL_OK;
 }
-// C(x)/Z_H(x) on the trace handle's shard of the quotient coset (the whole coset for an unsharded handle): M values per
+// C(x)/Z_H(x) on part g of 2^sl of the quotient coset (quotient_coset; for a shard, its own part): M values per
 // challenge in local natural order, at out + a*M. Division by zero sets bit 1 of dflag.
 static int stark_quotient_values(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
                                  uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
-                                 uint32_t n_alphas, uint32_t qd_bits, uint64_t* out, const DevBuf& dflag) {
-    const uint32_t db = trace->degree_log, sl = trace->shard_log;
-    const QuotientCoset q = quotient_coset(trace, qd_bits);
+                                 uint32_t n_alphas, uint32_t qd_bits, uint32_t g, uint32_t sl, uint64_t* out,
+                                 const DevBuf& dflag) {
+    const uint32_t db = trace->degree_log;
+    const QuotientCoset q = quotient_coset(trace, qd_bits, g, sl);
     DevBuf dprog(ctx), dconst(ctx), xtab(ctx), tl(ctx), tn(ctx), al(ctx), an(ctx);
     ColumnsView trl, trn, axl, axn;
     TRY(quotient_views(ctx, q, trace, true, tl, tn, &trl, &trn));
@@ -2478,8 +2636,21 @@ static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
     TRY(stark_quotient_check(ctx, trace, aux, program, n_instr, n_consts, alphas, n_alphas, quotient_degree_factor, out,
                              whole, &qd_bits));
     return run_quotient(ctx, whole, out, trace->degree_log, n_alphas, quotient_degree_factor, [&](const DevBuf& dflag) {
-        return stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, out,
-                                     dflag);
+        if (!trace->lde_blocks)
+            return stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits,
+                                         trace->shard_index, trace->shard_log, out, dflag);
+        // non-resident: the coset in one part per LDE block, each part's values placed at its points of `out`
+        const uint32_t sl = trace->block_log, log_M = trace->degree_log + qd_bits - sl;
+        DevBuf part(ctx);
+        TRY(part.alloc((size_t)n_alphas << log_M));
+        for (uint32_t g = 0; g < trace->lde_blocks; g++) {
+            TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, g,
+                                      sl, part.get(), dflag));
+            k_stark_place<<<dim3((unsigned)((((size_t)1 << log_M) + 127) / 128), n_alphas), 128, 0, ctx->stream>>>(
+                part.get(), log_M, sl, bitrev32(g, sl), out);
+            CKL(ctx);
+        }
+        return GL_OK;
     });
 }
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
@@ -2708,6 +2879,7 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
         if (!commits[c]) return set_err(ctx, GL_ERR_BAD_ARG, "null commitment");
         if (commits[c]->ctx != ctx) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u belongs to another context", c);
         if (whole && commits[c]->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
+        if (commits[c]->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is not resident: the plonky2 quotient reads the LDE", c);
         if (!whole && (commits[c]->shard_index != commits[0]->shard_index || commits[c]->shard_log != commits[0]->shard_log))
             return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is shard %u of %u, commitment 0 shard %u of %u", c,
                            commits[c]->shard_index, 1u << commits[c]->shard_log, commits[0]->shard_index,
@@ -2719,7 +2891,7 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
     TRY(quotient_shape_check(ctx, commits[0]->degree_log, commits[0]->rate_bits, commits[0]->shard_log,
                              quotient_degree_factor, GL_VP_MAX_QD, qd_bits_out));
     // a shard whose quotient coset is not its LDE coset reads values computed from the coefficients: no salt columns
-    const bool in_place = quotient_coset(commits[0], *qd_bits_out).local_in_place;
+    const bool in_place = quotient_coset(commits[0], *qd_bits_out, commits[0]->shard_index, commits[0]->shard_log).local_in_place;
     uint32_t next_mask = 0;
     {  // validate once on the host: the kernel trusts the program (operands in range, no register read before it is written)
         bool written[GL_VP_MAX_REGS] = {false};
@@ -2754,7 +2926,7 @@ static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_
                                  const DevBuf& dflag) {
     const gl_commit* c0 = commits[0];
     const uint32_t db = c0->degree_log;
-    const QuotientCoset q = quotient_coset(c0, qd_bits);
+    const QuotientCoset q = quotient_coset(c0, qd_bits, c0->shard_index, c0->shard_log);
     VanishingParams p;
     std::vector<DevBuf> bufs;  // per commitment: its values on the coset, and at the next row
     for (uint32_t k = 0; k < 2 * n_commits; k++) bufs.emplace_back(ctx);
@@ -3050,6 +3222,7 @@ int gl_fri_begin_values(gl_ctx* ctx, gl_commit* const* oracles, size_t n_oracles
     for (size_t o = 0; o < n_oracles; o++) {
         const gl_commit* c = oracles[o];
         if (!c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called");
+        if (c->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "a non-resident commitment has no LDE to read");
         if (c->degree_log != c0->degree_log || c->rate_bits != c0->rate_bits)
             return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent");
         if (c->shard_index != c0->shard_index || c->shard_log != c0->shard_log)

@@ -70,10 +70,20 @@ class Placement:
     opens its queries with `open_many`); the two compute_quotient_polys and proof.eval_commitments pick their C entry
     point by num_shards and, with several ranks, gather the quotient with `quotient_from_shards` and the openings with
     `openings_from_shards`. Nothing else in the provers tests whether there is more than one rank. On one device both
-    keyword sets are empty, so every call a prover makes is the plain single-device call."""
+    keyword sets are empty, so every call a prover makes is the plain single-device call.
+    lde_blocks=G (one device only) makes every commitment non-resident, its LDE built in G row blocks where it is
+    hashed or read (PolynomialBatch.from_values); the C entry points take such commitments directly, so step_kwargs
+    stays empty."""
     shard_index: int = 0
     num_shards: int = 1
     group: object = None
+    lde_blocks: int = 0
+
+    def __post_init__(self):
+        from . import _native as N
+
+        if self.lde_blocks and self.num_shards > 1:
+            raise N.ShapeError("lde_blocks= proves on one device; it cannot be combined with %d shards" % self.num_shards)
 
     @property
     def shard(self):
@@ -82,9 +92,11 @@ class Placement:
 
     @property
     def commit_kwargs(self):
-        """The keyword arguments that build a commitment on this placement: shard=(g, G), or none on one device, whose
-        default is the unsharded commitment."""
-        return {} if self.num_shards == 1 else dict(shard=self.shard)
+        """The keyword arguments that build a commitment on this placement: shard=(g, G), lde_blocks=G on one device with
+        non-resident commitments, or none on one device, whose default is the unsharded resident commitment."""
+        if self.num_shards > 1:
+            return dict(shard=self.shard)
+        return dict(lde_blocks=self.lde_blocks) if self.lde_blocks else {}
 
     @property
     def step_kwargs(self):

@@ -57,6 +57,25 @@ def random_field_elements_keyed(key, column, first, count, ctx=None):
     return out
 
 
+def check_lde_blocks(lde_blocks, cap_height, *, blinding=False, salt=None, salt_key=None, shard=(0, 1), prefix=None):
+    """The refusals of lde_blocks=G (a non-resident batch), before any device work: G must be a power of two of at most
+    2^cap_height (each block holds whole cap subtrees), and the batch unblinded, unsharded and not a prefixed stage."""
+    if lde_blocks is None:
+        return
+    G = int(lde_blocks)
+    if G <= 0 or G & (G - 1):
+        raise N.ShapeError("lde_blocks=%d is not a positive power of two" % G)
+    if G > 1 << cap_height:
+        raise N.ShapeError("lde_blocks=%d exceeds the %d cap entries (cap_height %d): blocks own whole cap subtrees"
+                           % (G, 1 << cap_height, cap_height))
+    if blinding or salt is not None or salt_key is not None:
+        raise N.ShapeError("a non-resident batch (lde_blocks=) cannot be blinded or salted")
+    if tuple(shard) != (0, 1):
+        raise N.ShapeError("lde_blocks= cannot be combined with shard=")
+    if prefix is not None:
+        raise N.ShapeError("lde_blocks= cannot be combined with prefix=")
+
+
 class _DeviceMerkleTree:
     """View of PolynomialBatch.merkle_tree (merkle_tree.rs:46-62) living on the device."""
 
@@ -107,9 +126,10 @@ class PolynomialBatch(N.Handle):
     """PolynomialBatch<F, PoseidonGoldilocksConfig, 2> (oracle.rs:30-37)."""
     destroyer = "gl_commit_destroy"
 
-    def __init__(self, handle, ctx, num_polys, degree_log, rate_bits, cap_height, blinding, shard=(0, 1)):
+    def __init__(self, handle, ctx, num_polys, degree_log, rate_bits, cap_height, blinding, shard=(0, 1), lde_blocks=0):
         self.h, self.ctx = handle, ctx
         self.shard_index, self.num_shards = shard
+        self.lde_blocks = lde_blocks  # G of a non-resident batch (its LDE is rebuilt block by block where read), else 0
         self.num_polys, self.degree_log, self.rate_bits = num_polys, degree_log, rate_bits
         self.cap_height, self.blinding = cap_height, blinding
         self.leaf_width = num_polys + (SALT_SIZE if blinding else 0)
@@ -120,14 +140,16 @@ class PolynomialBatch(N.Handle):
 
     @classmethod
     def _create(cls, cols, rate_bits, blinding, cap_height, is_coeffs, salt, ctx, shard=(0, 1), salt_key=None,
-                prefix=None):
+                prefix=None, lde_blocks=None):
+        check_lde_blocks(lde_blocks, cap_height, blinding=blinding, salt=salt, salt_key=salt_key, shard=shard,
+                         prefix=prefix)
         ctx = ctx or N.default_context()
         cols = np.ascontiguousarray(cols, dtype=np.uint64)
         if cols.ndim != 2 or cols.shape[0] == 0:
             raise N.ShapeError("expected a non-empty (num_polys, degree) array")
         B, n = cols.shape
         log_n = log2_strict(n)
-        if salt_key is not None or prefix is not None:
+        if salt_key is not None or prefix is not None or lde_blocks is not None:
             if salt is not None:
                 raise N.ShapeError("salt= is exclusive with salt_key= and prefix=")
             kind = N.COLS_COEFFS if is_coeffs else N.COLS_VALUES
@@ -136,7 +158,7 @@ class PolynomialBatch(N.Handle):
                 N.check(N.lib().gl_commit_add_columns(h, 0, B, N.np_ptr(cols), n, kind, N.MEM_HOST), ctx.h)
 
             return cls._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, blinding=blinding,
-                                    salt_key=salt_key, shard=shard, prefix=prefix)
+                                    salt_key=salt_key, shard=shard, prefix=prefix, lde_blocks=lde_blocks)
         sp = None
         if blinding:
             if salt is None:
@@ -154,14 +176,15 @@ class PolynomialBatch(N.Handle):
 
     @classmethod
     def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns, *, blinding=False,
-                     salt_key=None, shard=(0, 1), prefix=None):
+                     salt_key=None, shard=(0, 1), prefix=None, lde_blocks=None):
         """A batch committed incrementally: gl_commit_begin, then add_columns(h) issues the gl_commit_add_columns calls
         on the unfinished handle h, then gl_commit_finish -- or, with blinding, gl_commit_finish_keyed: the salt is
         drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). shard=(g, G): only
         leaf rows [g*N/G, (g+1)*N/G) on this device, as in from_values. prefix: a finished PolynomialBatch whose local
         cap has one entry per local leaf of this one; the tree is then a later stage of a batch Merkle tree, over the
         leaves `its cap entry j || LDE row j` (gl_commit_finish_prefixed). The columns' device memory only has to live
-        until this returns."""
+        until this returns. lde_blocks=G: a non-resident batch (gl_commit_begin_blocked), as in from_values."""
+        check_lde_blocks(lde_blocks, cap_height, blinding=blinding, salt_key=salt_key, shard=shard, prefix=prefix)
         if salt_key is not None and not blinding:
             raise N.ShapeError("salt_key= needs blinding=True")
         if prefix is not None:
@@ -172,9 +195,14 @@ class PolynomialBatch(N.Handle):
                 raise N.ShapeError("the prefix has %d cap entries for %d leaves" % (entries, rows))
         key = _salt_key(salt_key) if salt_key is not None else None
         h = N.vp()
-        N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, int(bool(blinding)),
-                                        int(shard[0]), int(shard[1]), None, C.byref(h)), ctx.h)
-        batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
+        if lde_blocks is not None:
+            N.check(N.lib().gl_commit_begin_blocked(ctx.h, num_polys, degree_log, rate_bits, cap_height, int(lde_blocks),
+                                                    None, C.byref(h)), ctx.h)
+        else:
+            N.check(N.lib().gl_commit_begin(ctx.h, num_polys, degree_log, rate_bits, cap_height, int(bool(blinding)),
+                                            int(shard[0]), int(shard[1]), None, C.byref(h)), ctx.h)
+        batch = cls(h, ctx, num_polys, degree_log, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])),
+                    int(lde_blocks or 0))
         try:
             add_columns(h)
             if prefix is not None:
@@ -192,10 +220,11 @@ class PolynomialBatch(N.Handle):
 
     @classmethod
     def _from_coeff_chunks(cls, polys, chunks, degree_log, rate_bits, cap_height, ctx=None, *, blinding=False,
-                           salt_key=None, shard=(0, 1)):
+                           salt_key=None, shard=(0, 1), lde_blocks=None):
         """Every row of the device tensor `polys` cut into `chunks` coefficient polynomials of 2^degree_log, committed
         in row order: the quotient commitment of plonky2 and starky (plonk/prover.rs:319-352, starky/prover.rs:391-421).
-        blinding / salt_key / shard: as in _from_device."""
+        blinding / salt_key / shard / lde_blocks: as in _from_device."""
+        check_lde_blocks(lde_blocks, cap_height, blinding=blinding, salt_key=salt_key, shard=shard)
         ctx = ctx or N.default_context()
         n = 1 << degree_log
         ctx.after_caller()
@@ -206,23 +235,29 @@ class PolynomialBatch(N.Handle):
                                                       N.COLS_COEFFS, N.MEM_DEVICE), ctx.h)
 
         return cls._from_device(ctx, polys.shape[0] * chunks, degree_log, rate_bits, cap_height, add_columns,
-                                blinding=blinding, salt_key=salt_key, shard=shard)
+                                blinding=blinding, salt_key=salt_key, shard=shard, lde_blocks=lde_blocks)
 
     @classmethod
     def from_values(cls, values, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,
-                    salt=None, ctx=None, shard=(0, 1), salt_key=None):
+                    salt=None, ctx=None, shard=(0, 1), salt_key=None, lde_blocks=None):
         """from_values (oracle.rs:57-79). `timing`/`fft_root_table` are accepted for signature parity.
         shard=(g, G): build only leaf rows [g*N/G, (g+1)*N/G) on this device (multi-GPU row-block sharding).
         With blinding, the salt is `salt` (4 x N, by LDE row), else, with salt_key (32 bytes, or "fresh" for a key from
         the OS CSPRNG), drawn on the device: salt column s at LDE row i = random_field_elements_keyed(key, s, i, 1);
-        else drawn on the host from the OS CSPRNG."""
-        return cls._create(values, rate_bits, blinding, cap_height, False, salt, ctx, shard, salt_key)
+        else drawn on the host from the OS CSPRNG.
+        lde_blocks=G: a non-resident batch, for LDEs larger than device memory. It keeps its coefficients, digests and cap
+        but never its LDE: the LDE is built in G row blocks to be hashed, and the blocks a reader asks for are rebuilt
+        (merkle_tree.leaves / get_rows / open_many / prove, get_lde_values). Everything it returns equals the resident
+        batch's. check_lde_blocks lists its refusals."""
+        return cls._create(values, rate_bits, blinding, cap_height, False, salt, ctx, shard, salt_key,
+                           lde_blocks=lde_blocks)
 
     @classmethod
     def from_coeffs(cls, polynomials, rate_bits, blinding, cap_height, timing=None, fft_root_table=None, *,
-                    salt=None, ctx=None, shard=(0, 1), salt_key=None):
-        """from_coeffs (oracle.rs:82-112); salt / salt_key as in from_values."""
-        return cls._create(polynomials, rate_bits, blinding, cap_height, True, salt, ctx, shard, salt_key)
+                    salt=None, ctx=None, shard=(0, 1), salt_key=None, lde_blocks=None):
+        """from_coeffs (oracle.rs:82-112); salt / salt_key / lde_blocks as in from_values."""
+        return cls._create(polynomials, rate_bits, blinding, cap_height, True, salt, ctx, shard, salt_key,
+                           lde_blocks=lde_blocks)
 
     @property
     def polynomials(self):

@@ -17,7 +17,7 @@ from . import _native as N
 from . import distributed as D
 from . import field as F
 from .fri import starky_standard_fast_fri_config
-from .polynomial_batch import PolynomialBatch
+from .polynomial_batch import PolynomialBatch, check_lde_blocks
 from .proof import StarkOpeningSet
 
 OP_LOCAL, OP_NEXT, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_EMIT, OP_AUX_LOCAL, OP_AUX_NEXT = range(9)
@@ -635,8 +635,10 @@ def _device_trace(trace, ctx):
     return dev
 
 
-def _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params=None):
-    """prove's checks (prover.rs:53-81,153-162), before any device work. Returns the ProveParams of the trace."""
+def _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, lde_blocks=0):
+    """prove's checks (prover.rs:53-81,153-162), before any device work. Returns the ProveParams of the trace.
+    lde_blocks=G (non-resident commitments, lde_placement): G at most the quotient coset's size, since the quotient is
+    evaluated in one part of it per block."""
     shape = tuple(trace.shape)
     if len(shape) != 2 or shape[0] != stark.COLUMNS:
         raise N.ShapeError("the trace must be (COLUMNS = %d, n), got %r" % (stark.COLUMNS, shape))
@@ -662,6 +664,11 @@ def _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fr
             raise N.ShapeError("the verifier circuit's final polynomial has %d coefficients, expected %d"
                                % (final_poly_coeff_len, 1 << (1 + strategy[2])))
         max_num_query_steps = len(vp.reduction_arity_bits)
+    qdf = stark.quotient_degree_factor()
+    if lde_blocks and qdf:
+        size = (1 << degree_bits) << (qdf - 1).bit_length()
+        if lde_blocks > size:
+            raise N.ShapeError("lde_blocks=%d exceeds the %d points of the quotient coset" % (lde_blocks, size))
     return ProveParams(degree_bits, fri_params, final_poly_coeff_len, max_num_query_steps)
 
 
@@ -674,23 +681,36 @@ class ProveParams:
         self.final_poly_coeff_len, self.max_num_query_steps = final_poly_coeff_len, max_num_query_steps
 
 
-def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None):
+def lde_placement(config, lde_blocks):
+    """The one-device Placement of a prover's lde_blocks argument: Placement() for None (resident commitments), else
+    non-resident commitments of lde_blocks row blocks (refused as PolynomialBatch.check_lde_blocks refuses it, before
+    any device work)."""
+    if lde_blocks is None:
+        return D.Placement()
+    check_lde_blocks(lde_blocks, config.fri_config.cap_height)
+    return D.Placement(lde_blocks=int(lde_blocks))
+
+
+def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None, lde_blocks=None):
     """prove (starky/src/prover.rs:40-114) for one Stark: trace = (COLUMNS, n) host columns or torch CUDA tensor ->
     StarkProofWithPublicInputs. The trace commitment, then a fresh challenger observing the public inputs, the config
     and the trace cap, then prove_with_commitment without CTLs. verifier_circuit_fri_params: the FRI parameters of a
     verifier circuit made for another degree (ConstantArityBits only); the transcript then observes the zero caps and
     coefficients that verifier expects. A torch trace may still be in production on the caller's current torch stream:
     the library's work is ordered after it. Raises ShapeError / NativeError with the reference's messages; every
-    commitment is released on every exit path."""
-    return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, D.Placement())
+    commitment is released on every exit path. lde_blocks=G: every commitment is non-resident
+    (PolynomialBatch.from_values), for traces whose LDEs exceed device memory; the proof is the same. G must be a power
+    of two of at most 2^cap_height and of at most the quotient coset's size (ShapeError before any device work)."""
+    return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx,
+                  lde_placement(config, lde_blocks))
 
 
 def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement):
     """prove on a distributed.Placement (see prove_with_commitment)."""
     from .challenger import Challenger
 
+    params = _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params, placement.lde_blocks)
     ctx = ctx or N.default_context()
-    params = _check_prove_shapes(stark, config, trace, public_inputs, verifier_circuit_fri_params)
     public_inputs = [int(v) % F.ORDER for v in public_inputs]
     rate_bits, cap_height = config.fri_config.rate_bits, config.fri_config.cap_height
     if stark.uses_lookups():
