@@ -18,6 +18,7 @@
  *  - Every function returns an int status: GL_OK or a GL_ERR_* code; gl_last_error(ctx) gives text.
  *    Nothing unwinds or aborts across the ABI. Shape errors mirror the reference's panics
  *    (field/src/fft.rs:171-177, plonky2/src/hash/merkle_tree.rs:195-200, plonky2/src/fri/oracle.rs:128).
+ *    A gl_commit_* call that returns a status refuses a NULL handle with GL_ERR_BAD_ARG ("null handle").
  *  - One gl_ctx per (device, stream). Calls on one context are serialised by the caller; different
  *    contexts are independent (no global mutable state). The library owns all device memory behind
  *    opaque handles; the caller owns every host buffer.
@@ -111,7 +112,9 @@ int gl_bcast(gl_ctx* ctx, const uint64_t* src, size_t words, uint64_t* const* de
  * words (column s at salt + s*N) appended to every leaf -- the reference draws them from OsRng
  * (oracle.rs:133-137); here the caller supplies them so the result is deterministic.
  * The handle keeps coefficients (B x n), the LDE (W columns of N values in leaf order, leaf j = LDE row bitrev(j)),
- * digests (reference layout, merkle_tree.rs:50-58) and the cap on the device. */
+ * digests (reference layout, merkle_tree.rs:50-58) and the cap on the device.
+ * Defined as the incremental build below: gl_commit_begin (blinding iff salt != NULL), one gl_commit_add_columns of all
+ * B columns (GL_COLS_COEFFS if is_coeffs, else GL_COLS_VALUES) and gl_commit_finish(salt, mem). */
 int gl_commit_create(gl_ctx* ctx, const uint64_t* cols, size_t col_stride, uint32_t B, uint32_t log_n,
                      uint32_t rate_bits, uint32_t cap_height, const uint64_t* salt, int is_coeffs,
                      int mem, gl_commit** out);
@@ -130,7 +133,9 @@ int gl_commit_create_sharded(gl_ctx* ctx, const uint64_t* cols, size_t col_strid
  *                          outlive the handle; columns passed from inside it are not copied);
  *   gl_commit_add_columns  columns [first_col, first_col + count), each exactly once, in any order:
  *                          kind GL_COLS_VALUES (iNTT + LDE), GL_COLS_COEFFS (canonicalise + LDE) or
- *                          GL_COLS_COEFFS_CANONICAL (LDE only);
+ *                          GL_COLS_COEFFS_CANONICAL (LDE only). More than 32 host columns (GL_MEM_HOST) are copied
+ *                          in chunks of 8, then 32 columns on a second stream, each chunk transformed as soon as its
+ *                          copy lands, so the copies overlap the transforms;
  *   gl_commit_finish       salt columns (iff blinding) and the Merkle tree. Accessors are valid after it. */
 #define GL_COLS_VALUES 0
 #define GL_COLS_COEFFS 1

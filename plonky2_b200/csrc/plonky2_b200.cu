@@ -1,7 +1,7 @@
 // plonky2_b200.cu -- sm_90a kernels + host orchestration + the C ABI of include/plonky2_b200.h.
 //
 // Hot path implemented here (reference -> this file):
-//   PolynomialBatch::from_values/from_coeffs  plonky2/src/fri/oracle.rs:57-139   -> commit_build()
+//   PolynomialBatch::from_values/from_coeffs  plonky2/src/fri/oracle.rs:57-139   -> gl_commit_begin/add_columns/finish
 //   MerkleTree::new / prove                   plonky2/src/hash/merkle_tree.rs:86-237 -> tree_build(), tree_open()
 //   prove_openings (pre-FRI part)             plonky2/src/fri/oracle.rs:176-220   -> gl_fri_begin()
 //   fri_committed_trees / fri_proof_of_work   plonky2/src/fri/prover.rs:84-202    -> gl_fri_commit_round/fold/pow
@@ -574,7 +574,8 @@ struct gl_commit {
     uint32_t B, W, degree_log, rate_bits;
     uint32_t shard_index = 0, shard_log = 0;  // this handle holds leaf rows [g*N/G, (g+1)*N/G)
     // Non-resident (gl_commit_begin_blocked): lde_blocks = 2^block_log row blocks of the LDE, each built from the
-    // coefficients where it is hashed or read and never kept; tree.leaves is NULL. 0: the LDE is resident in tree.leaves.
+    // coefficients where it is hashed or read and never kept; tree.leaves is NULL. 0: the LDE is resident in tree.leaves,
+    // one block (block_log = 0).
     uint32_t lde_blocks = 0, block_log = 0;
     bool blinding;
     u64* coeffs = nullptr;  // B x n
@@ -699,70 +700,56 @@ static int commit_chunk(gl_ctx* ctx, gl_commit* c, uint32_t g0, uint32_t gc, int
     if (c->lde_blocks) return GL_OK;
     return commit_extend(ctx, c, g0, gc, c->shard_index, c->shard_log, t.leaves + (size_t)g0 * t.N, t.N);
 }
-// Row block g of a non-resident commitment's LDE into lde (W x N/G words, column-major, leaf order)
-static int block_lde(gl_ctx* ctx, const gl_commit* c, uint32_t g, u64* lde) {
-    const size_t Nb = c->tree.N >> c->block_log;
-    return commit_extend(ctx, c, 0, c->B, g, c->block_log, lde, Nb);
-}
-// The Merkle tree of row block g of a non-resident commitment, over the leaves in lde: its C/G cap subtrees, whose
-// digests and cap entries are one contiguous range of the whole tree's (DESIGN section 5)
-static Tree block_tree(const gl_commit* c, uint32_t g, u64* lde) {
-    const Tree& w = c->tree;
-    Tree t;
-    t.N = w.N >> c->block_log;
-    t.W = w.W;
-    t.log_n = w.log_n - c->block_log;
-    t.cap_height = w.cap_height - c->block_log;
-    t.ls = 1;
+// Row block g of the 2^block_log blocks of c's local rows, as the Merkle tree of its C/G cap subtrees, whose digests
+// and cap entries are one contiguous range of the whole tree's (DESIGN section 5). A resident commitment is one block,
+// its LDE in place. A non-resident commitment's block is rebuilt from the coefficients into `scratch` (W x N/G words,
+// column-major, leaf order; allocated on first use, so one buffer serves every block of a walk).
+static int commit_block(gl_ctx* ctx, const gl_commit* c, uint32_t g, DevBuf& scratch, Tree* out) {
+    Tree t = c->tree;
+    t.N >>= c->block_log;
+    t.log_n -= c->block_log;
+    t.cap_height -= c->block_log;
     t.es = t.N;
-    t.leaves = lde;
-    t.digests = w.digests + (size_t)g * t.digest_words();
-    t.cap = w.cap + (size_t)g * t.cap_words();
-    return t;
-}
-// "build Merkle tree" of a non-resident commitment: every block's LDE, built into one scratch buffer, hashed into the
-// block's range of the whole digest buffer and cap
-static int commit_finish_blocked(gl_ctx* ctx, gl_commit* c) {
-    Tree& t = c->tree;
-    TRY(dmalloc(ctx, &t.digests, t.digest_words()));
-    TRY(dmalloc(ctx, &t.cap, t.cap_words()));
-    DevBuf lde(ctx);
-    TRY(lde.alloc((size_t)c->W * (t.N >> c->block_log)));
-    for (uint32_t g = 0; g < c->lde_blocks; g++) {
-        TRY(block_lde(ctx, c, g, lde.get()));
-        TRY(tree_hash(ctx, block_tree(c, g, lde.get())));
+    if (t.cap) {  // hashed, or being hashed: commit_finish allocates the digests and cap first
+        t.digests += (size_t)g * t.digest_words();
+        t.cap += (size_t)g * t.cap_words();
     }
-    c->finished = true;
+    if (c->lde_blocks) {
+        if (!scratch.get()) TRY(scratch.alloc((size_t)c->W * t.N));
+        TRY(commit_extend(ctx, c, 0, c->B, g, c->block_log, scratch.get(), t.N));
+        t.leaves = scratch.get();
+    }
+    *out = t;
     return GL_OK;
 }
-// salt columns (blinding) + "build Merkle tree"
-static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem) {
-    const size_t n = (size_t)1 << c->degree_log, N = n << c->rate_bits;
-    Tree& t = c->tree;
-    const size_t Nloc = t.N;
-    if (salt) {
-        DevBuf dsalt(ctx);
-        u64* sp;
-        TRY(device_in(ctx, salt, GL_SALT_SIZE * N, mem, dsalt, &sp));
-        k_salt<<<(unsigned)((Nloc + 255) / 256), 256, 0, ctx->stream>>>(sp, N, c->degree_log + c->rate_bits,
-                                                                       (size_t)c->shard_index * Nloc, Nloc, t.leaves,
-                                                                       Nloc, c->B);
-        CKL(ctx);
-    }
-    TRY(tree_build(ctx, t));
-    c->finished = true;
-    return GL_OK;
-}
-// salt columns drawn on the device from a ChaCha20 key (gl_chacha.cuh), this shard's leaves only, + "build Merkle tree"
-static int commit_finish_keyed(gl_ctx* ctx, gl_commit* c, const ChaChaKey& key) {
+// salt columns (blinding: from `salt`, GL_SALT_SIZE x N by LDE row in `mem`, or drawn on the device from a ChaCha20
+// `key` (gl_chacha.cuh), this shard's rows only) + "build Merkle tree", one row block at a time
+static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem, const ChaChaKey* key) {
     Tree& t = c->tree;
     const size_t Nloc = t.N;
     const uint32_t log_N = c->degree_log + c->rate_bits;
-    const size_t items = salt_fill_items(log_N, Nloc);
-    k_chacha_salt<<<dim3((unsigned)((items + 255) / 256), GL_SALT_SIZE), 256, 0, ctx->stream>>>(
-        key, log_N, (u64)c->shard_index * Nloc, Nloc, t.leaves + (size_t)c->B * Nloc, Nloc);
-    CKL(ctx);
-    TRY(tree_build(ctx, t));
+    if (salt) {
+        DevBuf dsalt(ctx);
+        u64* sp;
+        TRY(device_in(ctx, salt, (size_t)GL_SALT_SIZE << log_N, mem, dsalt, &sp));
+        k_salt<<<(unsigned)((Nloc + 255) / 256), 256, 0, ctx->stream>>>(sp, (size_t)1 << log_N, log_N,
+                                                                       (size_t)c->shard_index * Nloc, Nloc, t.leaves,
+                                                                       Nloc, c->B);
+        CKL(ctx);
+    } else if (key) {
+        const size_t items = salt_fill_items(log_N, Nloc);
+        k_chacha_salt<<<dim3((unsigned)((items + 255) / 256), GL_SALT_SIZE), 256, 0, ctx->stream>>>(
+            *key, log_N, (u64)c->shard_index * Nloc, Nloc, t.leaves + (size_t)c->B * Nloc, Nloc);
+        CKL(ctx);
+    }
+    TRY(dmalloc(ctx, &t.digests, t.digest_words()));
+    TRY(dmalloc(ctx, &t.cap, t.cap_words()));
+    DevBuf scratch(ctx);
+    for (uint32_t g = 0; g < (1u << c->block_log); g++) {
+        Tree b;
+        TRY(commit_block(ctx, c, g, scratch, &b));
+        TRY(tree_hash(ctx, b));
+    }
     c->finished = true;
     return GL_OK;
 }
@@ -778,63 +765,6 @@ static int os_random_key(gl_ctx* ctx, uint8_t out[32]) {
         got += (size_t)r;
     }
     return GL_OK;
-}
-
-static int commit_build(gl_ctx* ctx, gl_commit* c, const u64* cols, size_t col_stride, const u64* salt, int is_coeffs,
-                        int mem, uint32_t cap_height) {
-    const size_t n = (size_t)1 << c->degree_log;
-    const uint32_t B = c->B;
-    TRY(commit_alloc(ctx, c, cap_height, nullptr));
-    // Column chunks flow through  H2D copy -> iNTT -> LDE; the copy of chunk k+1 (separate stream) overlaps the
-    // transforms of chunk k.
-    // 32-column chunks: launches big enough for full waves; the FIRST chunk is 8 columns so that only ~1.2 ms of H2D
-    // (n = 2^20) is exposed before the first transform starts instead of ~5 ms.
-    const uint32_t CH = 32, CH0 = 8;
-    const bool overlap = (mem == GL_MEM_HOST) && B > CH;
-    struct EventList {  // destroyed on every exit path
-        std::vector<cudaEvent_t> v;
-        ~EventList() {
-            for (auto e : v) cudaEventDestroy(e);
-        }
-    } evl;
-    std::vector<cudaEvent_t>& evs = evl.v;
-    std::vector<std::pair<uint32_t, uint32_t>> chunks;  // (first column, count)
-    if (overlap) {
-        for (uint32_t g0 = 0; g0 < B;) {
-            const uint32_t want = g0 == 0 ? CH0 : CH, gc = (B - g0 < want) ? B - g0 : want;
-            chunks.emplace_back(g0, gc);
-            g0 += gc;
-        }
-        if (!ctx->copy_stream) CK(ctx, cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        cudaEvent_t ready;
-        CK(ctx, cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-        CK(ctx, cudaEventRecord(ready, ctx->stream));  // the stream-ordered allocations above
-        CK(ctx, cudaStreamWaitEvent(ctx->copy_stream, ready, 0));
-        cudaEventDestroy(ready);
-        for (auto& ch : chunks) {
-            const uint32_t g0 = ch.first, gc = ch.second;
-            if (col_stride == n) {
-                CK(ctx, cudaMemcpyAsync(c->coeffs + (size_t)g0 * n, cols + (size_t)g0 * n, (size_t)gc * n * 8,
-                                        cudaMemcpyHostToDevice, ctx->copy_stream));
-            } else {
-                CK(ctx, cudaMemcpy2DAsync(c->coeffs + (size_t)g0 * n, n * 8, cols + (size_t)g0 * col_stride,
-                                          col_stride * 8, n * 8, gc, cudaMemcpyHostToDevice, ctx->copy_stream));
-            }
-            cudaEvent_t e;
-            CK(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            CK(ctx, cudaEventRecord(e, ctx->copy_stream));
-            evs.push_back(e);
-        }
-    } else {
-        chunks.emplace_back(0u, B);
-        CK(ctx, cudaMemcpy2DAsync(c->coeffs, n * 8, cols, col_stride * 8, n * 8, B,
-                                  mem == GL_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    for (size_t k = 0; k < chunks.size(); k++) {
-        if (overlap) CK(ctx, cudaStreamWaitEvent(ctx->stream, evs[k], 0));
-        TRY(commit_chunk(ctx, c, chunks[k].first, chunks[k].second, is_coeffs ? 1 : 0));
-    }
-    return commit_finish(ctx, c, salt, mem);
 }
 
 // =====================================================================================
@@ -1963,9 +1893,19 @@ int gl_commit_begin_blocked(gl_ctx* ctx, uint32_t B, uint32_t log_n, uint32_t ra
     *out = c.release();
     return GL_OK;
 }
+// Every entry point that takes a handle and returns a status starts with one of these
+#define NEED_HANDLE(c)                                                         \
+    do {                                                                       \
+        if (!(c)) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");       \
+    } while (0)
+#define NEED_FINISHED(c)                                                                                     \
+    do {                                                                                                     \
+        NEED_HANDLE(c);                                                                                      \
+        if (!(c)->finished) return set_err((c)->ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called"); \
+    } while (0)
 int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, const uint64_t* cols, size_t col_stride,
                           int kind, int mem) {
-    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    NEED_HANDLE(c);
     gl_ctx* ctx = c->ctx;
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (!cols || kind < 0 || kind > 2) return set_err(ctx, GL_ERR_BAD_ARG, "bad argument");
@@ -1975,22 +1915,66 @@ int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, cons
     if (count > 1 && col_stride < n) return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent (stride < n)");
     CK(ctx, cudaSetDevice(ctx->device));
     u64* dst = c->coeffs + (size_t)first_col * n;
-    if (!(mem == GL_MEM_DEVICE && cols == dst && (col_stride == n || count == 1)))
-        CK(ctx, cudaMemcpy2DAsync(dst, n * 8, cols, col_stride * 8, n * 8, count,
-                                  mem == GL_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, ctx->stream));
-    return commit_chunk(ctx, c, first_col, count, kind);
+    // Host column chunks flow through  H2D copy -> iNTT -> LDE; the copy of chunk k+1 (separate stream) overlaps the
+    // transforms of chunk k.
+    // 32-column chunks: launches big enough for full waves; the FIRST chunk is 8 columns so that only ~1.2 ms of H2D
+    // (n = 2^20) is exposed before the first transform starts instead of ~5 ms.
+    const uint32_t CH = 32, CH0 = 8;
+    if (mem != GL_MEM_HOST || count <= CH) {
+        if (!(mem == GL_MEM_DEVICE && cols == dst && (col_stride == n || count == 1)))
+            CK(ctx, cudaMemcpy2DAsync(dst, n * 8, cols, col_stride * 8, n * 8, count,
+                                      mem == GL_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
+                                      ctx->stream));
+        return commit_chunk(ctx, c, first_col, count, kind);
+    }
+    struct EventList {  // destroyed on every exit path
+        std::vector<cudaEvent_t> v;
+        ~EventList() {
+            for (auto e : v) cudaEventDestroy(e);
+        }
+    } evs;
+    std::vector<std::pair<uint32_t, uint32_t>> chunks;  // (first column, count), relative to first_col
+    for (uint32_t k0 = 0; k0 < count;) {
+        const uint32_t want = k0 == 0 ? CH0 : CH, kc = (count - k0 < want) ? count - k0 : want;
+        chunks.emplace_back(k0, kc);
+        k0 += kc;
+    }
+    if (!ctx->copy_stream) CK(ctx, cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+    cudaEvent_t ready;
+    CK(ctx, cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+    CK(ctx, cudaEventRecord(ready, ctx->stream));  // the stream-ordered allocation of the coefficients
+    CK(ctx, cudaStreamWaitEvent(ctx->copy_stream, ready, 0));
+    cudaEventDestroy(ready);
+    for (auto& ch : chunks) {
+        const uint32_t k0 = ch.first, kc = ch.second;
+        if (col_stride == n) {
+            CK(ctx, cudaMemcpyAsync(dst + (size_t)k0 * n, cols + (size_t)k0 * n, (size_t)kc * n * 8,
+                                    cudaMemcpyHostToDevice, ctx->copy_stream));
+        } else {
+            CK(ctx, cudaMemcpy2DAsync(dst + (size_t)k0 * n, n * 8, cols + (size_t)k0 * col_stride, col_stride * 8, n * 8,
+                                      kc, cudaMemcpyHostToDevice, ctx->copy_stream));
+        }
+        cudaEvent_t e;
+        CK(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        CK(ctx, cudaEventRecord(e, ctx->copy_stream));
+        evs.v.push_back(e);
+    }
+    for (size_t k = 0; k < chunks.size(); k++) {
+        CK(ctx, cudaStreamWaitEvent(ctx->stream, evs.v[k], 0));
+        TRY(commit_chunk(ctx, c, first_col + chunks[k].first, chunks[k].second, kind));
+    }
+    return GL_OK;
 }
 int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem) {
-    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    NEED_HANDLE(c);
     gl_ctx* ctx = c->ctx;
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (c->blinding != (salt != nullptr)) return set_err(ctx, GL_ERR_BAD_ARG, "salt must be given exactly when blinding was requested");
     CK(ctx, cudaSetDevice(ctx->device));
-    if (c->lde_blocks) return commit_finish_blocked(ctx, c);
-    return commit_finish(ctx, c, salt, mem);
+    return commit_finish(ctx, c, salt, mem, nullptr);
 }
 int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix) {
-    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    NEED_HANDLE(c);
     gl_ctx* ctx = c->ctx;
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (!prefix) return set_err(ctx, GL_ERR_BAD_ARG, "null prefix");
@@ -2001,10 +1985,10 @@ int gl_commit_finish_prefixed(gl_commit* c, const uint64_t* prefix) {
     // a copy: the previous stage (the prefix's owner) may be destroyed before this commitment
     TRY(dmalloc(ctx, &t.prefix, 4 * t.N));
     CK(ctx, cudaMemcpyAsync(t.prefix, prefix, 4 * t.N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
-    return commit_finish(ctx, c, nullptr, GL_MEM_DEVICE);
+    return commit_finish(ctx, c, nullptr, GL_MEM_DEVICE, nullptr);
 }
 int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]) {
-    if (!c) return set_err(nullptr, GL_ERR_BAD_ARG, "null handle");
+    NEED_HANDLE(c);
     gl_ctx* ctx = c->ctx;
     if (c->finished) return set_err(ctx, GL_ERR_BAD_ARG, "commitment already finished");
     if (!c->blinding) return set_err(ctx, GL_ERR_BAD_ARG, "a salt key was given for a commitment begun without blinding");
@@ -2016,7 +2000,7 @@ int gl_commit_finish_keyed(gl_commit* c, const uint8_t key[32]) {
     const ChaChaKey k = chacha_key_from_bytes(key);
     memset(fresh, 0, sizeof(fresh));
     CK(ctx, cudaSetDevice(ctx->device));
-    return commit_finish_keyed(ctx, c, k);
+    return commit_finish(ctx, c, nullptr, GL_MEM_DEVICE, &k);
 }
 int gl_random_field_elements(gl_ctx* ctx, const uint8_t key[32], uint32_t column, uint64_t first, size_t count,
                              uint64_t* out, int mem) {
@@ -2048,13 +2032,11 @@ int gl_commit_create_sharded(gl_ctx* ctx, const uint64_t* cols, size_t col_strid
                              uint32_t shard_index, uint32_t num_shards, gl_commit** out) {
     if (!ctx || !cols || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     *out = nullptr;
-    uint32_t shard_log = 0;
-    TRY(commit_check_shape(ctx, B, log_n, rate_bits, cap_height, shard_index, num_shards, &shard_log));
-    CK(ctx, cudaSetDevice(ctx->device));
-    if (B > 1 && col_stride < ((size_t)1 << log_n))
-        return set_err(ctx, GL_ERR_BAD_SHAPE, "Polynomial degrees inconsistent (stride < n)");
-    CommitPtr c = commit_new(ctx, B, log_n, rate_bits, salt != nullptr, shard_index, shard_log);
-    TRY(commit_build(ctx, c.get(), cols, col_stride, salt, is_coeffs, mem, cap_height));
+    gl_commit* h;
+    TRY(gl_commit_begin(ctx, B, log_n, rate_bits, cap_height, salt != nullptr, shard_index, num_shards, nullptr, &h));
+    CommitPtr c(h, gl_commit_destroy);
+    TRY(gl_commit_add_columns(h, 0, B, cols, col_stride, is_coeffs ? GL_COLS_COEFFS : GL_COLS_VALUES, mem));
+    TRY(gl_commit_finish(h, salt, mem));
     *out = c.release();
     return GL_OK;
 }
@@ -2070,16 +2052,13 @@ uint32_t gl_commit_leaf_width(const gl_commit* c) { return c->W; }
 uint32_t gl_commit_degree_log(const gl_commit* c) { return c->degree_log; }
 uint32_t gl_commit_rate_bits(const gl_commit* c) { return c->rate_bits; }
 uint32_t gl_commit_cap_height(const gl_commit* c) { return c->tree.cap_height + c->shard_log; }
-#define NEED_FINISHED(c)                                                                                     \
-    do {                                                                                                     \
-        if (!(c)->finished) return set_err((c)->ctx, GL_ERR_BAD_ARG, "gl_commit_finish has not been called"); \
-    } while (0)
 int gl_commit_cap(gl_commit* c, uint64_t* out, int mem) {
     NEED_FINISHED(c);
     return copy_out(c->ctx, out, c->tree.cap, c->tree.cap_words(), mem);
 }
 const uint64_t* gl_commit_dev_cap(const gl_commit* c) { return c && c->finished ? c->tree.cap : nullptr; }
 int gl_commit_coeffs(gl_commit* c, uint64_t* out, int mem) {
+    NEED_HANDLE(c);
     return copy_out(c->ctx, out, c->coeffs, (size_t)c->B << c->degree_log, mem);
 }
 // Rows [row_begin, row_begin + row_count) of the W-column LDE `lde` (column k at lde + k*es) as row-major leaves
@@ -2100,19 +2079,19 @@ static int rows_out(gl_ctx* ctx, const u64* lde, size_t es, uint32_t W, size_t r
     return GL_OK;
 }
 int gl_commit_leaves(gl_commit* c, size_t row_begin, size_t row_count, uint64_t* out, int mem) {
+    NEED_HANDLE(c);
     gl_ctx* ctx = c->ctx;
     if (row_begin + row_count > c->tree.N) return set_err(ctx, GL_ERR_BAD_ARG, "row range out of bounds");
     if (row_count == 0) return GL_OK;
     CK(ctx, cudaSetDevice(ctx->device));
-    if (!c->lde_blocks) return rows_out(ctx, c->tree.leaves, c->tree.es, c->W, row_begin, row_count, out, mem);
-    // non-resident: the blocks that hold the rows, one at a time
+    // the blocks that hold the rows, one at a time
     const size_t Nb = c->tree.N >> c->block_log, row_end = row_begin + row_count;
-    DevBuf lde(ctx);
-    TRY(lde.alloc((size_t)c->W * Nb));
+    DevBuf scratch(ctx);
     for (size_t r = row_begin; r < row_end;) {
         const size_t g = r / Nb, end = (g + 1) * Nb < row_end ? (g + 1) * Nb : row_end;
-        TRY(block_lde(ctx, c, (uint32_t)g, lde.get()));
-        TRY(rows_out(ctx, lde.get(), Nb, c->W, r - g * Nb, end - r, out + (r - row_begin) * c->W, mem));
+        Tree b;
+        TRY(commit_block(ctx, c, (uint32_t)g, scratch, &b));
+        TRY(rows_out(ctx, b.leaves, b.es, c->W, r - g * Nb, end - r, out + (r - row_begin) * c->W, mem));
         r = end;
     }
     return GL_OK;
@@ -2122,6 +2101,7 @@ int gl_commit_digests(gl_commit* c, uint64_t* out, int mem) {
     return copy_out(c->ctx, out, c->tree.digests, c->tree.digest_words(), mem);
 }
 int gl_commit_get_lde_values(gl_commit* c, size_t index, size_t step, uint64_t* out) {
+    NEED_HANDLE(c);
     const uint32_t bits = c->degree_log + c->rate_bits;
     size_t idx = index * step;
     if (idx >= ((size_t)1 << bits)) return set_err(c->ctx, GL_ERR_BAD_ARG, "index out of range");
@@ -2130,21 +2110,17 @@ int gl_commit_get_lde_values(gl_commit* c, size_t index, size_t step, uint64_t* 
     const size_t row0 = (size_t)c->shard_index * c->tree.N;
     if (rev < row0 || rev >= row0 + c->tree.N) return set_err(c->ctx, GL_ERR_BAD_ARG, "LDE row held by another shard");
     CK(c->ctx, cudaSetDevice(c->ctx->device));
-    const u64* lde = c->tree.leaves;
-    size_t row = rev - row0, es = c->tree.es;
-    DevBuf block(c->ctx);
-    if (c->lde_blocks) {  // non-resident: the block that holds the row
-        es = c->tree.N >> c->block_log;
-        TRY(block.alloc((size_t)c->W * es));
-        TRY(block_lde(c->ctx, c, (uint32_t)(row / es), block.get()));
-        lde = block.get();
-        row %= es;
-    }
-    CK(c->ctx, cudaMemcpy2DAsync(out, 8, lde + row, es * 8, 8, c->B, cudaMemcpyDeviceToHost, c->ctx->stream));
+    const size_t row = rev - row0, Nb = c->tree.N >> c->block_log;
+    DevBuf scratch(c->ctx);
+    Tree b;
+    TRY(commit_block(c->ctx, c, (uint32_t)(row / Nb), scratch, &b));
+    CK(c->ctx, cudaMemcpy2DAsync(out, 8, b.leaves + row % Nb, b.es * 8, 8, c->B, cudaMemcpyDeviceToHost,
+                                 c->ctx->stream));
     CK(c->ctx, cudaStreamSynchronize(c->ctx->stream));
     return GL_OK;
 }
 int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_shards) {
+    NEED_HANDLE(c);
     if (shard_index) *shard_index = c->shard_index;
     if (num_shards) *num_shards = 1u << c->shard_log;
     return GL_OK;
@@ -2152,12 +2128,11 @@ int gl_commit_shard(const gl_commit* c, uint32_t* shard_index, uint32_t* num_sha
 uint32_t gl_commit_lde_blocks(const gl_commit* c) { return c->lde_blocks; }
 int gl_commit_open(gl_commit* c, const uint64_t* leaf_indices, size_t count, uint64_t* out_leaves, uint64_t* out_paths) {
     NEED_FINISHED(c);
-    if (!c->lde_blocks) return tree_open(c->ctx, c->tree, leaf_indices, count, out_leaves, out_paths);
-    // non-resident: each block that holds a requested leaf is built once and opened as its own tree, whose sibling
-    // paths are the whole tree's (its cap subtrees' digests are a range of the whole digest buffer)
+    // each block that holds a requested leaf is built once and opened as its own tree, whose sibling paths are the
+    // whole tree's (its cap subtrees' digests are a range of the whole digest buffer)
     gl_ctx* ctx = c->ctx;
     const Tree& t = c->tree;
-    const size_t Nb = t.N >> c->block_log, layers = t.log_n - t.cap_height;
+    const size_t Nb = t.N >> c->block_log, layers = t.log_n - t.cap_height, lw = t.W + (t.prefix ? 4 : 0);
     std::map<uint32_t, std::vector<size_t>> by_block;  // block -> positions in leaf_indices
     for (size_t i = 0; i < count; i++) {
         if (leaf_indices[i] >= t.N)
@@ -2165,26 +2140,29 @@ int gl_commit_open(gl_commit* c, const uint64_t* leaf_indices, size_t count, uin
         by_block[(uint32_t)(leaf_indices[i] / Nb)].push_back(i);
     }
     CK(ctx, cudaSetDevice(ctx->device));
-    DevBuf lde(ctx);
-    if (count) TRY(lde.alloc((size_t)c->W * Nb));
+    DevBuf scratch(ctx);
     std::vector<u64> idx, lv, pv;
     for (const auto& kv : by_block) {
         const uint32_t g = kv.first;
         const std::vector<size_t>& pos = kv.second;
+        Tree b;
+        TRY(commit_block(ctx, c, g, scratch, &b));
+        if (g == 0 && pos.size() == count)  // block 0 holds the whole request (a resident LDE always): no staging
+            return tree_open(ctx, b, leaf_indices, count, out_leaves, out_paths);
         idx.resize(pos.size());
         for (size_t k = 0; k < pos.size(); k++) idx[k] = leaf_indices[pos[k]] - (size_t)g * Nb;
-        lv.resize(pos.size() * c->W);
+        lv.resize(pos.size() * lw);
         pv.resize(pos.size() * layers * 4 + 1);
-        TRY(block_lde(ctx, c, g, lde.get()));
-        TRY(tree_open(ctx, block_tree(c, g, lde.get()), idx.data(), pos.size(), lv.data(), pv.data()));
+        TRY(tree_open(ctx, b, idx.data(), pos.size(), lv.data(), pv.data()));
         for (size_t k = 0; k < pos.size(); k++) {
-            memcpy(out_leaves + pos[k] * c->W, lv.data() + k * c->W, c->W * 8);
+            memcpy(out_leaves + pos[k] * lw, lv.data() + k * lw, lw * 8);
             if (layers) memcpy(out_paths + pos[k] * layers * 4, pv.data() + k * layers * 4, layers * 4 * 8);
         }
     }
     return GL_OK;
 }
 int gl_commit_eval_ext(gl_commit* c, const uint64_t point[2], uint64_t* out) {
+    NEED_HANDLE(c);
     const uint32_t point_index = 0;
     return gl_openings(c->ctx, &c, &point_index, 1, point, 1, out, GL_MEM_HOST);
 }

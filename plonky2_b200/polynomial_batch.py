@@ -149,41 +149,37 @@ class PolynomialBatch(N.Handle):
             raise N.ShapeError("expected a non-empty (num_polys, degree) array")
         B, n = cols.shape
         log_n = log2_strict(n)
-        if salt_key is not None or prefix is not None or lde_blocks is not None:
-            if salt is not None:
-                raise N.ShapeError("salt= is exclusive with salt_key= and prefix=")
-            kind = N.COLS_COEFFS if is_coeffs else N.COLS_VALUES
-
-            def add_columns(h):
-                N.check(N.lib().gl_commit_add_columns(h, 0, B, N.np_ptr(cols), n, kind, N.MEM_HOST), ctx.h)
-
-            return cls._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, blinding=blinding,
-                                    salt_key=salt_key, shard=shard, prefix=prefix, lde_blocks=lde_blocks)
-        sp = None
-        if blinding:
+        if salt is not None and (salt_key is not None or prefix is not None or lde_blocks is not None):
+            raise N.ShapeError("salt= is exclusive with salt_key= and prefix=")
+        if blinding and salt_key is None and prefix is None:
             if salt is None:
                 # the reference draws the salt from OsRng (oracle.rs:133-137); same source here
                 salt = random_field_elements(SALT_SIZE * (n << rate_bits)).reshape(SALT_SIZE, -1)
             salt = np.ascontiguousarray(salt, dtype=np.uint64)
             if salt.shape != (SALT_SIZE, n << rate_bits):
                 raise N.ShapeError("salt must be (4, n << rate_bits)")
-            sp = N.np_ptr(salt)
-        h = N.vp()
-        N.check(N.lib().gl_commit_create_sharded(ctx.h, N.np_ptr(cols), n, B, log_n, rate_bits, cap_height, sp,
-                                                 int(is_coeffs), N.MEM_HOST, int(shard[0]), int(shard[1]),
-                                                 C.byref(h)), ctx.h)
-        return cls(h, ctx, B, log_n, rate_bits, cap_height, bool(blinding), (int(shard[0]), int(shard[1])))
+        else:
+            salt = None  # without blinding, a salt argument is ignored
+        kind = N.COLS_COEFFS if is_coeffs else N.COLS_VALUES
+
+        def add_columns(h):
+            N.check(N.lib().gl_commit_add_columns(h, 0, B, N.np_ptr(cols), n, kind, N.MEM_HOST), ctx.h)
+
+        return cls._from_device(ctx, B, log_n, rate_bits, cap_height, add_columns, blinding=blinding, salt=salt,
+                                salt_key=salt_key, shard=shard, prefix=prefix, lde_blocks=lde_blocks, wait=False)
 
     @classmethod
     def _from_device(cls, ctx, num_polys, degree_log, rate_bits, cap_height, add_columns, *, blinding=False,
-                     salt_key=None, shard=(0, 1), prefix=None, lde_blocks=None):
+                     salt=None, salt_key=None, shard=(0, 1), prefix=None, lde_blocks=None, wait=True):
         """A batch committed incrementally: gl_commit_begin, then add_columns(h) issues the gl_commit_add_columns calls
-        on the unfinished handle h, then gl_commit_finish -- or, with blinding, gl_commit_finish_keyed: the salt is
-        drawn on the device from salt_key (32 bytes; None or "fresh": a key from the OS CSPRNG). shard=(g, G): only
-        leaf rows [g*N/G, (g+1)*N/G) on this device, as in from_values. prefix: a finished PolynomialBatch whose local
-        cap has one entry per local leaf of this one; the tree is then a later stage of a batch Merkle tree, over the
-        leaves `its cap entry j || LDE row j` (gl_commit_finish_prefixed). The columns' device memory only has to live
-        until this returns. lde_blocks=G: a non-resident batch (gl_commit_begin_blocked), as in from_values."""
+        on the unfinished handle h, then gl_commit_finish -- with blinding, over the host salt array `salt` (4 x N, by
+        LDE row) if given, else through gl_commit_finish_keyed: the salt is drawn on the device from salt_key (32 bytes;
+        None or "fresh": a key from the OS CSPRNG). shard=(g, G): only leaf rows [g*N/G, (g+1)*N/G) on this device, as
+        in from_values. prefix: a finished PolynomialBatch whose local cap has one entry per local leaf of this one; the
+        tree is then a later stage of a batch Merkle tree, over the leaves `its cap entry j || LDE row j`
+        (gl_commit_finish_prefixed). lde_blocks=G: a non-resident batch (gl_commit_begin_blocked), as in from_values.
+        The columns' device memory only has to live until this returns; wait=False skips that wait on the library's
+        stream, for pageable host columns, which the copies have read when gl_commit_add_columns returns."""
         check_lde_blocks(lde_blocks, cap_height, blinding=blinding, salt_key=salt_key, shard=shard, prefix=prefix)
         if salt_key is not None and not blinding:
             raise N.ShapeError("salt_key= needs blinding=True")
@@ -208,11 +204,14 @@ class PolynomialBatch(N.Handle):
             if prefix is not None:
                 N.check(N.lib().gl_commit_finish_prefixed(h, N.lib().gl_commit_dev_cap(prefix.h)), ctx.h)
                 batch.prefixed = True
+            elif salt is not None:
+                N.check(N.lib().gl_commit_finish(h, N.np_ptr(salt), N.MEM_HOST), ctx.h)
             elif blinding:
                 N.check(N.lib().gl_commit_finish_keyed(h, key), ctx.h)
             else:
                 N.check(N.lib().gl_commit_finish(h, None, N.MEM_DEVICE), ctx.h)
-            ctx.synchronize()  # the library's stream-ordered reads of the caller's (torch) columns are done
+            if wait:
+                ctx.synchronize()  # the library's stream-ordered reads of the caller's (torch) columns are done
         except Exception:
             batch.close()
             raise

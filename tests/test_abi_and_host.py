@@ -49,6 +49,32 @@ def test_no_cpu_fallback_without_gpu(native):
         pb.PolynomialBatch.from_values(np.zeros((2, 8), dtype=np.uint64), 1, False, 0)
 
 
+def test_null_commitment_handle_is_refused(native):
+    """Every entry point that takes a commitment handle and returns a status refuses NULL with GL_ERR_BAD_ARG before
+    it reads anything (no context or device needed)."""
+    L = native.lib()
+    buf = np.zeros(64, dtype=np.uint64)
+    p, host = native.np_ptr(buf), native.MEM_HOST
+    u = np.zeros(1, dtype=np.uint32).ctypes.data_as(native.u32p)
+    calls = {
+        "gl_commit_cap": (p, host),
+        "gl_commit_coeffs": (p, host),
+        "gl_commit_leaves": (0, 1, p, host),
+        "gl_commit_digests": (p, host),
+        "gl_commit_get_lde_values": (0, 1, p),
+        "gl_commit_open": (p, 1, p, p),
+        "gl_commit_eval_ext": (p, p),
+        "gl_commit_shard": (u, u),
+        "gl_commit_add_columns": (0, 1, p, 8, native.COLS_VALUES, host),
+        "gl_commit_finish": (None, host),
+        "gl_commit_finish_prefixed": (p,),
+        "gl_commit_finish_keyed": (bytes(32),),
+    }
+    for name, args in calls.items():
+        assert getattr(L, name)(None, *args) == native.GL_ERR_BAD_ARG, name
+        assert L.gl_last_error(None) == b"null handle", name
+
+
 def test_product_does_not_import_oracle():
     pkg = os.path.join(ROOT, "plonky2_b200")
     for dirpath, _, files in os.walk(pkg):
