@@ -14,7 +14,9 @@
  *  - F_{p^2} element = 2 consecutive words (c0, c1), X^2 = 7 (field/src/goldilocks_extensions.rs:14-27).
  *  - Hash = 4 words (plonky2/src/hash/hash_types.rs:20-27).
  *  - `mem` arguments: GL_MEM_HOST (pageable or pinned host memory; the call does the copies) or
- *    GL_MEM_DEVICE (device pointers on the context's device; no copies, stream-ordered).
+ *    GL_MEM_DEVICE (device pointers on the context's device; no copies, stream-ordered). A GL_MEM_HOST
+ *    input, pageable or pinned, has been read when the call returns: the caller may overwrite or free
+ *    it at once, while the device work queued behind the copy may still be running.
  *  - Every function returns an int status: GL_OK or a GL_ERR_* code; gl_last_error(ctx) gives text.
  *    Nothing unwinds or aborts across the ABI. Shape errors mirror the reference's panics
  *    (field/src/fft.rs:171-177, plonky2/src/hash/merkle_tree.rs:195-200, plonky2/src/fri/oracle.rs:128).

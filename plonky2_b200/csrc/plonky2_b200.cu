@@ -224,6 +224,42 @@ static int device_in(gl_ctx* ctx, const u64* in, size_t words, int mem, DevBuf& 
     *view = stage.get();
     return GL_OK;
 }
+// A copy from a caller's page-locked host buffer reads it when its stream reaches the copy, which can be after
+// cudaMemcpyAsync has returned (a pageable source is staged before it returns). An entry point that copies from a
+// caller's host buffer and does not end in a synchronising read-back marks the stream after its last such copy and,
+// once the work that depends on the copies is queued, waits for the mark: the caller's buffers have been read when the
+// call returns, while the transforms and hashes queued behind the copies keep running. Every exit path waits.
+class HostReads {
+  public:
+    explicit HostReads(gl_ctx* ctx) : ctx_(ctx) {}
+    HostReads(const HostReads&) = delete;
+    HostReads& operator=(const HostReads&) = delete;
+    ~HostReads() {
+        if (!ev_) return;
+        cudaEventSynchronize(ev_);
+        cudaEventDestroy(ev_);
+    }
+    // after a copy from the caller's `mem` buffer on `s`; a no-op for GL_MEM_DEVICE, which is stream-ordered
+    int mark(cudaStream_t s, int mem) {
+        if (mem != GL_MEM_HOST) return GL_OK;
+        if (!ev_) CK(ctx_, cudaEventCreateWithFlags(&ev_, cudaEventDisableTiming));
+        CK(ctx_, cudaEventRecord(ev_, s));
+        return GL_OK;
+    }
+    int wait() {
+        if (!ev_) return GL_OK;
+        const cudaError_t e = cudaEventSynchronize(ev_);
+        cudaEventDestroy(ev_);
+        ev_ = nullptr;
+        if (e != cudaSuccess)
+            return set_err(ctx_, GL_ERR_CUDA, "waiting for the host input copies: %s", cudaGetErrorString(e));
+        return GL_OK;
+    }
+
+  private:
+    gl_ctx* ctx_;
+    cudaEvent_t ev_ = nullptr;
+};
 // Where a `words`-word result is written on the device: the caller's `out` unless mem == GL_MEM_HOST, else `stage`,
 // which the entry point copies to `out` at the end
 static int device_out(u64* out, size_t words, int mem, DevBuf& stage, u64** view) {
@@ -728,10 +764,12 @@ static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem, co
     Tree& t = c->tree;
     const size_t Nloc = t.N;
     const uint32_t log_N = c->degree_log + c->rate_bits;
+    HostReads reads(ctx);
     if (salt) {
         DevBuf dsalt(ctx);
         u64* sp;
         TRY(device_in(ctx, salt, (size_t)GL_SALT_SIZE << log_N, mem, dsalt, &sp));
+        TRY(reads.mark(ctx->stream, mem));
         k_salt<<<(unsigned)((Nloc + 255) / 256), 256, 0, ctx->stream>>>(sp, (size_t)1 << log_N, log_N,
                                                                        (size_t)c->shard_index * Nloc, Nloc, t.leaves,
                                                                        Nloc, c->B);
@@ -750,6 +788,7 @@ static int commit_finish(gl_ctx* ctx, gl_commit* c, const u64* salt, int mem, co
         TRY(commit_block(ctx, c, g, scratch, &b));
         TRY(tree_hash(ctx, b));
     }
+    TRY(reads.wait());
     c->finished = true;
     return GL_OK;
 }
@@ -1921,11 +1960,14 @@ int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, cons
     // (n = 2^20) is exposed before the first transform starts instead of ~5 ms.
     const uint32_t CH = 32, CH0 = 8;
     if (mem != GL_MEM_HOST || count <= CH) {
+        HostReads reads(ctx);
         if (!(mem == GL_MEM_DEVICE && cols == dst && (col_stride == n || count == 1)))
             CK(ctx, cudaMemcpy2DAsync(dst, n * 8, cols, col_stride * 8, n * 8, count,
                                       mem == GL_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
                                       ctx->stream));
-        return commit_chunk(ctx, c, first_col, count, kind);
+        TRY(reads.mark(ctx->stream, mem));
+        TRY(commit_chunk(ctx, c, first_col, count, kind));
+        return reads.wait();
     }
     struct EventList {  // destroyed on every exit path
         std::vector<cudaEvent_t> v;
@@ -1959,11 +2001,13 @@ int gl_commit_add_columns(gl_commit* c, uint32_t first_col, uint32_t count, cons
         CK(ctx, cudaEventRecord(e, ctx->copy_stream));
         evs.v.push_back(e);
     }
+    HostReads reads(ctx);  // after the last chunk's copy
+    TRY(reads.mark(ctx->copy_stream, mem));
     for (size_t k = 0; k < chunks.size(); k++) {
         CK(ctx, cudaStreamWaitEvent(ctx->stream, evs.v[k], 0));
         TRY(commit_chunk(ctx, c, first_col + chunks[k].first, chunks[k].second, kind));
     }
-    return GL_OK;
+    return reads.wait();
 }
 int gl_commit_finish(gl_commit* c, const uint64_t* salt, int mem) {
     NEED_HANDLE(c);
@@ -2410,13 +2454,15 @@ int gl_sigma_polys(gl_ctx* ctx, const uint64_t* pairs, size_t n_pairs, int pairs
     k_sigma_heads<<<sigma_blocks(count), 256, 0, ctx->stream>>>(kout, count, L);
     CKL(ctx);
     TRY(dk.alloc(num_routed_wires));
+    HostReads reads(ctx);
     TRY(h2d(ctx, dk.get(), k_is, num_routed_wires));
+    TRY(reads.mark(ctx->stream, GL_MEM_HOST));
     TRY(x_pow_tables(ctx, root_of_unity(degree_bits), n, xtab));
     const SigmaFill f{kout, vout, L, count, s, dk.get(), xtab.get(), xtab.get() + x_pow_table_len(n), dout};
     k_sigma_fill<<<sigma_blocks(count), 256, 0, ctx->stream>>>(f);
     CKL(ctx);
     if (out_mem == GL_MEM_HOST) TRY(d2h(ctx, out, dout, count));
-    return GL_OK;
+    return reads.wait();
 }
 
 // log2_ceil(quotient_degree_factor)
@@ -3046,8 +3092,11 @@ int gl_merkle_build(gl_ctx* ctx, const uint64_t* leaves, size_t N, uint32_t W, u
     m->tree.W = W;
     m->tree.cap_height = cap_height;
     DevBuf dleaves(ctx);  // GL_MEM_DEVICE: the caller keeps its buffer alive for the life of the tree
+    HostReads reads(ctx);
     TRY(device_in(ctx, leaves, N * (size_t)W, mem, dleaves, &m->tree.leaves));
+    TRY(reads.mark(ctx->stream, mem));
     TRY(tree_build(ctx, m->tree));
+    TRY(reads.wait());
     m->tree.own_leaves = mem == GL_MEM_HOST;
     dleaves.release();
     *out = m.release();
@@ -3289,10 +3338,13 @@ int gl_fri_begin_from_coeffs(gl_ctx* ctx, const uint64_t* coeffs_ext, uint32_t l
     DevBuf tmp(ctx);
     TRY(dmalloc(ctx, &f->coeff_cols, 2 * n));
     TRY(tmp.alloc(2 * n));
+    HostReads reads(ctx);
     TRY(h2d(ctx, tmp.get(), coeffs_ext, 2 * n));
+    TRY(reads.mark(ctx->stream, GL_MEM_HOST));
     k_split_ext<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(tmp.get(), n, f->coeff_cols);
     CKL(ctx);
     TRY(fri_finish_begin(ctx, f.get()));
+    TRY(reads.wait());
     *out = f.release();
     return GL_OK;
 }

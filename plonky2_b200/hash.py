@@ -186,7 +186,9 @@ class MerkleTree(N.Handle):
 
     def __init__(self, leaves, cap_height, ctx=None):
         self.ctx = ctx or N.default_context()
-        leaves = np.ascontiguousarray(leaves, dtype=np.uint64)
+        # a copy of its own, as the reference's tree owns its Vec: `leaves` and get() stay the leaves the tree was
+        # built from when the caller refills its array
+        leaves = np.array(leaves, dtype=np.uint64, order="C")
         if leaves.ndim != 2:
             raise N.ShapeError("leaves must be (N, W)")
         self.N, self.W = leaves.shape

@@ -179,7 +179,8 @@ class PolynomialBatch(N.Handle):
         tree is then a later stage of a batch Merkle tree, over the leaves `its cap entry j || LDE row j`
         (gl_commit_finish_prefixed). lde_blocks=G: a non-resident batch (gl_commit_begin_blocked), as in from_values.
         The columns' device memory only has to live until this returns; wait=False skips that wait on the library's
-        stream, for pageable host columns, which the copies have read when gl_commit_add_columns returns."""
+        stream, for host columns (pageable or pinned) and a host salt, which the library has read when
+        gl_commit_add_columns and gl_commit_finish return."""
         check_lde_blocks(lde_blocks, cap_height, blinding=blinding, salt_key=salt_key, shard=shard, prefix=prefix)
         if salt_key is not None and not blinding:
             raise N.ShapeError("salt_key= needs blinding=True")
