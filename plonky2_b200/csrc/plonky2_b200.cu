@@ -466,12 +466,13 @@ __global__ void __launch_bounds__(128) k_two_to_one_many(const u64* in, size_t n
     two_to_one(l, r, h);
     for (int k = 0; k < 4; k++) out[4 * j + k] = h[k];
 }
-// Openings: one CTA per queried leaf; copies the leaf and its sibling path (merkle_tree.rs:151-190).
+// Openings: one CTA per queried leaf; copies the leaf (canonicalised: a gl_merkle_build caller's leaves may not be) and
+// its sibling path (merkle_tree.rs:151-190).
 __global__ void k_tree_open(TreeView t, const u64* indices, u64* out_leaves, u64* out_paths) {
     const size_t idx = indices[blockIdx.x];
     const uint32_t num_layers = t.log_n - t.cap_height;
     for (uint32_t k = threadIdx.x; k < t.W; k += blockDim.x)
-        out_leaves[(size_t)blockIdx.x * t.W + k] = t.leaves[idx * t.ls + (size_t)k * t.es];
+        out_leaves[(size_t)blockIdx.x * t.W + k] = canon(t.leaves[idx * t.ls + (size_t)k * t.es]);
     const size_t L = (size_t)1 << num_layers;
     const size_t tree_index = idx >> num_layers;
     const u64* sub = t.digests + 4 * (tree_index * 2 * (L - 1));
@@ -482,14 +483,16 @@ __global__ void k_tree_open(TreeView t, const u64* indices, u64* out_leaves, u64
         out_paths[(size_t)blockIdx.x * num_layers * 4 + k] = sub[4 * digest_pos(sib, i) + w];
     }
 }
-// k_tree_open on a tree hashed by k_leaf_hash_prefixed: the leaves it returns are `prefix || row`, W + 4 words
+// k_tree_open on a tree hashed by k_leaf_hash_prefixed: the leaves it returns are `prefix || row`, W + 4 words (the
+// prefix is the caller's device array: canonicalised)
 __global__ void k_tree_open_prefixed(TreeView t, const u64* prefix, const u64* indices, u64* out_leaves,
                                      u64* out_paths) {
     const size_t idx = indices[blockIdx.x];
     const uint32_t num_layers = t.log_n - t.cap_height;
     const uint32_t lw = t.W + 4;
     for (uint32_t k = threadIdx.x; k < lw; k += blockDim.x)
-        out_leaves[(size_t)blockIdx.x * lw + k] = k < 4 ? prefix[4 * idx + k] : t.leaves[idx * t.ls + (size_t)(k - 4) * t.es];
+        out_leaves[(size_t)blockIdx.x * lw + k] =
+            canon(k < 4 ? prefix[4 * idx + k] : t.leaves[idx * t.ls + (size_t)(k - 4) * t.es]);
     const size_t L = (size_t)1 << num_layers;
     const size_t tree_index = idx >> num_layers;
     const u64* sub = t.digests + 4 * (tree_index * 2 * (L - 1));
