@@ -70,7 +70,9 @@ int gl_ctx_device_bytes(gl_ctx* ctx, uint64_t* in_use, uint64_t* high, int reset
 void* gl_ctx_stream(const gl_ctx* ctx);
 /* number of kernels this context has launched so far (for bench.py's gpu_launches) */
 uint64_t gl_ctx_launch_count(const gl_ctx* ctx);
-/* tuning: columns per multi-pass NTT group (scratch = group * n * 8 bytes; default: as many as fit 1 GiB) */
+/* tuning: columns per multi-pass NTT group (scratch = group * n * 8 bytes; default: as many as fit 1 GiB). A coset LDE
+ * that batches its cosets takes group / 2^min(rate_bits, 3) columns at a time, so its scratch is the same. Measurement
+ * switches: bit 31 selects the two-copy pass kernels, bit 30 one LDE transform per coset instead of batched cosets. */
 int gl_ctx_set_ntt_group(gl_ctx* ctx, uint32_t columns);
 /* Optional CUDA-event phase timing on the context's stream (the analogue of the reference's TimingTree
  * scopes "IFFT" / "FFT + blinding" / "build Merkle tree", plonky2/src/fri/oracle.rs:65-103). */

@@ -11,7 +11,8 @@
 //   j1; writes Y[p][j2] * w_n^{k1*j2} with p = bitrev(k1) (the in-place DIF order).
 // * row pass ("B", contiguous): TPT threads own one row of C = 2^LOG contiguous elements and store either
 //     - bit-reversed   out[row_base + bitrev(k2)]  -- the LDE: with column-major leaves this IS the reference's
-//                       leaf order (transpose + reverse_index_bits, oracle.rs:97-98), written with 128-bit stores, or
+//                       leaf order (transpose + reverse_index_bits, oracle.rs:97-98), for even LOG transposed per line through
+//                       shared memory so that each store instruction writes adjacent words, or
 //     - natural order  out[k1 + R*k2] (NTT / iNTT API), gathered through shared memory so that a CTA writes
 //                       segments of adjacent k1 (optional index reversal for the inverse, fft.rs:80-90).
 //   Three passes (n > 2^20) run the column pass twice (the second time inside every row of the first).
@@ -148,16 +149,50 @@ GL_HD void col_unit(const ColPass& cp, int blk, size_t& in_off, size_t& out_off,
 }
 // phase 1a: global loads (tid < COL_THREADS); phase 1b: step 1 + write the exchange tile
 template <int LOG>
-GL_HD void col_load(const ColPass& cp, int blk, int tid, uint64_t* x) {
+GL_HD void col_load_at(const ColPass& cp, size_t in_off, int tile, int tid, uint64_t* x) {
     using Cf = PassCfg<LOG>;
     const int tt = tid % Cf::T, t = tid / Cf::T;
-    size_t in_off, out_off;
-    int tile;
-    col_unit<LOG>(cp, blk, in_off, out_off, tile);
     const size_t C = (size_t)1 << cp.log_c;
     const uint64_t* src = cp.in + in_off + (size_t)tile * Cf::T + tt;
 #pragma unroll
     for (int q = 0; q < Cf::E; q++) x[q] = src[(size_t)(t + Cf::TPT * q) * C];
+}
+template <int LOG>
+GL_HD void col_load(const ColPass& cp, int blk, int tid, uint64_t* x) {
+    size_t in_off, out_off;
+    int tile;
+    col_unit<LOG>(cp, blk, in_off, out_off, tile);
+    col_load_at<LOG>(cp, in_off, tile, tid, x);
+}
+
+// ---------------------------------------------------------------- column pass over several cosets at once
+// The first column pass of a coset LDE for 2^log_cos cosets of the same coefficient columns in one launch. Only the
+// coset's pre-weights and its two tables differ between cosets; `cp` holds everything else (cp.tw, cp.twa and cp.uq
+// unused). Coset c of matrix column col goes to out + (col * 2^log_cos + c) * out_stride.
+constexpr int COL_LOG_MAX_COSETS = 3;  // 8 cosets: the parameter block stays under 4 KiB
+struct ColCosets {
+    ColPass cp;
+    int log_cos;
+    int ncols;
+    const uint64_t* tw[1 << COL_LOG_MAX_COSETS];
+    const uint64_t* twa[1 << COL_LOG_MAX_COSETS];
+    uint64_t uq[1 << COL_LOG_MAX_COSETS][32];
+};
+// CTA blk -> (coset c, matrix column col, tile), cosets fastest, then columns: the CTAs that read one coefficient tile
+// run side by side, so that tile can come from HBM once and from L2 for the other cosets, and the CTAs that read one
+// tile's rows of a coset's post table run within a few waves of each other.
+template <int LOG>
+GL_HD void col_cosets_unit(const ColCosets& cc, int blk, int& c, size_t& in_off, size_t& out_off, int& tile) {
+    c = blk & ((1 << cc.log_cos) - 1);
+    const int rest = blk >> cc.log_cos;
+    const size_t col = (size_t)(rest % cc.ncols);
+    tile = rest / cc.ncols;
+    in_off = col * cc.cp.in_stride;
+    out_off = ((col << cc.log_cos) + c) * cc.cp.out_stride;
+}
+template <int LOG>
+GL_HD int col_cosets_blocks(const ColCosets& cc) {
+    return (cc.ncols << cc.log_cos) * (int)(((size_t)1 << cc.cp.log_c) / PassCfg<LOG>::T);
 }
 template <int LOG>
 GL_HD void col_phase1(const ColPass& cp, uint64_t* S, int blk, int tid, uint64_t* x) {
@@ -259,7 +294,9 @@ struct RowPass {
     int has_uq;
     int reverse;           // RM_NATURAL: write to (n - k) mod n   (ifft index reversal, fft.rs:80-90)
     size_t row0;           // RM_BITREV: offset added to the output position (first row of this coset block)
-    int n_peer;            // RM_NATURAL: additional destinations with the same addressing as `out` (peer GPUs'
+    int log_cos;           // RM_BITREV: input column v is coset (v mod 2^log_cos) of output column v >> log_cos,
+    size_t cos_step;       //   which starts cos_step words after the previous coset's
+    int n_peer;           // RM_NATURAL: additional destinations with the same addressing as `out` (peer GPUs'
     uint64_t* out_peer[7]; // coefficient buffers mapped over NVLink: the store IS the all-gather)
     uint64_t uq[32];
 };
@@ -326,13 +363,19 @@ GL_HD void row_phase2_load(const uint64_t* S, int tid, int m, uint64_t* z) {
 #pragma unroll
     for (int j = 0; j < Cf::TPT; j++) z[j] = Sl[q * Cf::ROW_PITCH + j];
 }
+// first output word of row prow of input column col (RM_BITREV)
+template <int LOG>
+GL_HD uint64_t* row_bitrev_dst(const RowPass& rp, size_t col, size_t prow) {
+    const size_t cos = col & (((size_t)1 << rp.log_cos) - 1);
+    return rp.out + (col >> rp.log_cos) * rp.out_stride + rp.row0 + cos * rp.cos_step + (prow << LOG);
+}
 template <int LOG>
 GL_HD void row_store_bitrev(const RowPass& rp, int blk, int tid, int m, const uint64_t* z) {
     using Cf = PassCfg<LOG>;
     const int l = tid / Cf::TPT, t = tid % Cf::TPT;
     size_t col, prow, kbase;
     if (!row_line<LOG, RM_BITREV>(rp, blk, l, col, prow, kbase)) return;
-    uint64_t* dst = rp.out + col * rp.out_stride + rp.row0 + (prow << LOG);
+    uint64_t* dst = row_bitrev_dst<LOG>(rp, col, prow);
     if constexpr (Cf::R2 == 0) {  // z = x[q]: position q, this thread holds the whole line
 #pragma unroll
         for (int q = 0; q < Cf::E; q++) dst[q] = canon(z[q]);
@@ -351,6 +394,30 @@ GL_HD void row_store_bitrev(const RowPass& rp, int blk, int tid, int m, const ui
         for (int j = 0; j < Cf::TPT; j++) d[j] = canon(z[j]);
 #endif
     }
+}
+// RM_BITREV of a single-step-2 line (E == TPT) through the line's exchange buffer, in two parts with a warp barrier
+// between them: thread t holds positions t*TPT + j (row_stage_bitrev writes them to row t of the buffer), then stores
+// positions k*TPT + t (column t), so that every store instruction of a line writes TPT adjacent words. Stored from the
+// registers, each 128-bit store instruction of a warp writes 16 bytes at 32 places 256 bytes apart.
+template <int LOG>
+GL_HD void row_stage_bitrev(uint64_t* S, int tid, const uint64_t* z) {
+    using Cf = PassCfg<LOG>;
+    static_assert(Cf::E == Cf::TPT, "one step-2 transform per thread");
+    const int l = tid / Cf::TPT, t = tid % Cf::TPT;
+    uint64_t* Sl = S + (size_t)l * Cf::ROW_S_WORDS;
+#pragma unroll
+    for (int j = 0; j < Cf::TPT; j++) Sl[t * Cf::ROW_PITCH + j] = canon(z[j]);
+}
+template <int LOG>
+GL_HD void row_store_bitrev_staged(const RowPass& rp, const uint64_t* S, int blk, int tid) {
+    using Cf = PassCfg<LOG>;
+    const int l = tid / Cf::TPT, t = tid % Cf::TPT;
+    size_t col, prow, kbase;
+    if (!row_line<LOG, RM_BITREV>(rp, blk, l, col, prow, kbase)) return;
+    uint64_t* dst = row_bitrev_dst<LOG>(rp, col, prow) + t;
+    const uint64_t* Sl = S + (size_t)l * Cf::ROW_S_WORDS + t;
+#pragma unroll
+    for (int k = 0; k < Cf::E; k++) dst[(size_t)k * Cf::TPT] = Sl[k * Cf::ROW_PITCH];
 }
 template <int LOG>
 GL_HD void row_gather_write(uint64_t* G, int tid, int m, const uint64_t* z) {
@@ -463,6 +530,28 @@ inline void ntt_make_job(int log_n, NttPlan pl, uint64_t scale, uint64_t shift, 
     }
     job.row_step = TableReq{pl.b, 0, scale, one};
     rp.tw_full = canon(scale) != 1 ? 1 : 0;
+}
+// Cosets c0 .. c0 + 2^log_kc - 1 of the coset LDE of size-2^log_n columns on base_shift * <w_N>, N = 2^(log_n +
+// rate_bits), coset c on base_shift * w_N^bitrev(c) <w_n> (lde_columns in gl_ntt_host.cuh), as ONE job of a multi-pass
+// plan: cc is the first column pass over all of them, steps[c] / posts[c] its tables; the a2 pass and the row pass do
+// not depend on the coset and run over all 2^log_kc cosets of every column as job.c2 and job.rp.
+inline void lde_make_cosets_job(int log_n, NttPlan pl, int rate_bits, uint64_t base_shift, int c0, int log_kc,
+                                NttJob& job, ColCosets& cc, TableReq* steps, TableReq* posts) {
+    const uint64_t wN = root_of_unity((uint32_t)(log_n + rate_bits));
+    cc = ColCosets{};
+    for (int c = 0; c < (1 << log_kc); c++) {
+        const uint64_t s = mul(base_shift, pow(wN, bitrev32((uint32_t)(c0 + c), (uint32_t)rate_bits)));
+        NttJob jc;
+        ntt_make_job(log_n, pl, 1, s, jc);
+        if (c == 0) job = jc;
+        steps[c] = jc.c1_step;
+        posts[c] = jc.c1_post;
+        for (int q = 0; q < 32; q++) cc.uq[c][q] = jc.c1.has_uq ? jc.c1.uq[q] : 1;  // s = 1: no coset, weights 1
+    }
+    cc.cp = job.c1;
+    cc.cp.has_uq = cc.cp.tw_full = 1;  // one pair of flags for every coset: s = 1 multiplies by ones
+    cc.log_cos = log_kc;
+    job.rp.log_cos = log_kc;
 }
 template <int LOG>
 GL_HD int col_blocks(const ColPass& cp, size_t ncols) {

@@ -1,5 +1,6 @@
 // gl_ntt_host.cuh -- kernels and host orchestration of the multi-pass NTT (included by plonky2_b200.cu).
 //   k_ntt_col<LOG>        strided ("column") pass: T adjacent columns-of-the-matrix x 2^LOG strided points per CTA
+//   k_ntt_col_cosets<LOG> the LDE's first column pass for up to 8 cosets of a column group in one launch
 //   k_ntt_row<LOG, MODE>  contiguous ("row") pass: rows of 2^LOG points, bit-reversed (LDE) or natural-order stores
 // The step twiddle table of a pass (<= 8 KiB) is staged into shared memory by a TMA bulk copy (cp.async.bulk +
 // mbarrier) that overlaps the global loads of the data; the exchange tile lives next to it.
@@ -50,27 +51,26 @@ __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_M
 // Even LOG (E == TPT): both steps of the pass are "radix-E lazy DFT, normalise, multiply by a twiddle", so ONE copy of
 // that body serves both (a rolled 2-trip loop; only the I/O around it differs). The two-copy kernel above is ~90 KiB of
 // SASS, large enough for instruction fetch to stall it; this one is about half that.
+// The body of one CTA: tile `tile` of the unit at in_off / out_off, step table tw, post table twa, pre-weights uq.
 template <int LOG, bool ASYNC_TW>
-__global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_MIN_BLOCKS) k_ntt_col_shared(ColPass cp) {
+__device__ __forceinline__ void col_shared_body(const ColPass& cp, const u64* tw, const u64* twa, const u64 (&uq)[32],
+                                                size_t in_off, size_t out_off, int tile) {
     using Cf = PassCfg<LOG>;
     static_assert(Cf::E == Cf::TPT, "shared-body column pass needs an even LOG");
     extern __shared__ __align__(16) u64 smem[];
     u64* tw_s = smem;                    // 2^LOG words
     u64* S = smem + (1 << LOG);          // exchange tile
     u64* mbar = S + Cf::COL_S_WORDS;
-    tma_table_issue(tw_s, cp.tw, (uint32_t)((1 << LOG) * 8), mbar);
+    tma_table_issue(tw_s, tw, (uint32_t)((1 << LOG) * 8), mbar);
     u64 x[Cf::E];
-    col_load<LOG>(cp, blockIdx.x, threadIdx.x, x);
+    col_load_at<LOG>(cp, in_off, tile, threadIdx.x, x);
     __syncthreads();
     tma_table_wait(mbar);
     const int tt = threadIdx.x % Cf::T, t = threadIdx.x / Cf::T;
-    size_t in_off, out_off;
-    int tile;
-    col_unit<LOG>(cp, blockIdx.x, in_off, out_off, tile);
     const size_t C = (size_t)1 << cp.log_c;
     if (cp.has_uq) {
 #pragma unroll
-        for (int q = 1; q < Cf::E; q++) x[q] = mul(x[q], cp.uq[q]);
+        for (int q = 1; q < Cf::E; q++) x[q] = mul(x[q], uq[q]);
     }
     const u64* twp = tw_s + t;           // step 1: tw[q*TPT + t]
     size_t tws = Cf::TPT;
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_M
 #pragma unroll
             for (int j = 0; j < Cf::TPT; j++) x[j] = S[t * Cf::COL_QPITCH + j * Cf::T + tt];  // step 2 works on row q = t
             skip0 = false;
-            const u64* tw2 = cp.twa + (((size_t)t * Cf::TPT) << cp.log_c) + (size_t)tile * Cf::T + tt;  // output p = t*TPT + j
+            const u64* tw2 = twa + (((size_t)t * Cf::TPT) << cp.log_c) + (size_t)tile * Cf::T + tt;  // output p = t*TPT + j
             if (ASYNC_TW) {
                 __syncthreads();         // every thread holds its part of the tile: S is free
 #pragma unroll
@@ -115,6 +115,22 @@ __global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_M
     u64* dst = cp.out + out_off + (size_t)tile * Cf::T + tt;
 #pragma unroll
     for (int j = 0; j < Cf::TPT; j++) dst[((size_t)t * Cf::TPT + j) * C] = x[j];
+}
+template <int LOG, bool ASYNC_TW>
+__global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_MIN_BLOCKS) k_ntt_col_shared(ColPass cp) {
+    size_t in_off, out_off;
+    int tile;
+    col_unit<LOG>(cp, blockIdx.x, in_off, out_off, tile);
+    col_shared_body<LOG, ASYNC_TW>(cp, cp.tw, cp.twa, cp.uq, in_off, out_off, tile);
+}
+// The first column pass of up to 8 cosets of an LDE in one launch (ColCosets, gl_ntt.cuh): the same body per CTA, with
+// the tables and pre-weights of the CTA's coset.
+template <int LOG>
+__global__ void __launch_bounds__(PassCfg<LOG>::COL_THREADS, PassCfg<LOG>::COL_MIN_BLOCKS) k_ntt_col_cosets(ColCosets cc) {
+    size_t in_off, out_off;
+    int c, tile;
+    col_cosets_unit<LOG>(cc, blockIdx.x, c, in_off, out_off, tile);
+    col_shared_body<LOG, true>(cc.cp, cc.tw[c], cc.twa[c], cc.uq[c], in_off, out_off, tile);
 }
 
 template <int LOG, int MODE>
@@ -216,7 +232,10 @@ __global__ void __launch_bounds__(PassCfg<LOG>::ROW_THREADS, PassCfg<LOG>::ROW_M
         }
     }
     if (MODE == RM_BITREV) {
-        row_store_bitrev<LOG>(rp, blockIdx.x, threadIdx.x, 0, x);
+        __syncwarp();  // the line's step-2 loads from the exchange buffer are done
+        row_stage_bitrev<LOG>(S, threadIdx.x, x);
+        __syncwarp();
+        row_store_bitrev_staged<LOG>(rp, S, blockIdx.x, threadIdx.x);
     } else {
         __syncthreads();  // the gather tile aliases the exchange buffers
         row_gather_write<LOG>(S, threadIdx.x, 0, x);
@@ -299,6 +318,30 @@ static int dispatch_col(gl_ctx* ctx, int a, const ColPass& cp, size_t ncols) {
     }
     return set_err(ctx, GL_ERR_UNSUPPORTED, "column pass log %d", a);
 }
+template <int LOG>
+static int launch_col_cosets(gl_ctx* ctx, const ColCosets& cc) {
+    const size_t smem = ((size_t)(1 << LOG) + PassCfg<LOG>::COL_S_WORDS) * 8 + 16;
+    auto kern = k_ntt_col_cosets<LOG>;
+    const void* fn = (const void*)kern;
+    if (!ctx->smem_attr_done.count(fn)) {
+        CK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        ctx->smem_attr_done.insert(fn);
+    }
+    kern<<<col_cosets_blocks<LOG>(cc), PassCfg<LOG>::COL_THREADS, smem, ctx->stream>>>(cc);
+    CKL(ctx);
+    return GL_OK;
+}
+// the coset-batched first column pass exists for the shared-body (even) pass sizes only
+static bool col_cosets_supported(int a) { return a == 6 || a == 8 || a == 10; }
+static int dispatch_col_cosets(gl_ctx* ctx, int a, const ColCosets& cc) {
+    switch (a) {
+        case 6: return launch_col_cosets<6>(ctx, cc);
+        case 8: return launch_col_cosets<8>(ctx, cc);
+        case 10: return launch_col_cosets<10>(ctx, cc);
+    }
+    return set_err(ctx, GL_ERR_UNSUPPORTED, "coset column pass log %d", a);
+}
 static int dispatch_row(gl_ctx* ctx, int b, int mode, const RowPass& rp) {
 #define ROW_CASE(L)                                                     \
     case L:                                                             \
@@ -352,7 +395,9 @@ static int get_post(gl_ctx* ctx, int a, int b, u64 base, const u64** out) {
 }
 // Columns per multi-pass group (scratch = group * n * 8 bytes). The passes are instruction-bound, so large launches
 // (full waves) beat keeping the intermediate L2-resident (tools/ntt_sweep.py, round 1): as many columns as fit 1 GiB.
-static uint32_t group_cols(const gl_ctx* ctx, int log_n, uint32_t ncols) {
+// A group of the coset-batched LDE holds `cosets` transforms per column: it is 1/cosets as many columns, so that the
+// scratch and the size of a launch stay the same.
+static uint32_t group_cols(const gl_ctx* ctx, int log_n, uint32_t ncols, uint32_t cosets = 1) {
     uint32_t g = ctx->ntt_group;
     if (g == 0) {
         size_t col_bytes = (size_t)8 << log_n;
@@ -361,6 +406,10 @@ static uint32_t group_cols(const gl_ctx* ctx, int log_n, uint32_t ncols) {
         if (g < 8) g = 8;
     }
     g = (g + 7) & ~7u;
+    if (cosets > 1) {
+        g = g / cosets ? g / cosets : 1;
+        return g < ncols ? g : ncols;
+    }
     if (g > ((ncols + 7) & ~7u)) g = (ncols + 7) & ~7u;
     return g;
 }
@@ -493,6 +542,11 @@ __global__ void k_lde_const(const u64* coeffs, size_t stride, uint32_t ncols, in
 //   lde[col*lde_stride + c*n + j] = P_col( g * w_N^{bitrev_r(c)} * w_n^{bitrev(j)} ),  g = base_shift,
 // i.e. leaf row (c*n + j) of the reference's transposed + bit-reversed matrix (oracle.rs:97-98) is the vector of
 // these entries over all columns: block c is the size-n NTT (bit-reversed stores) on the coset g*w_N^{bitrev(c)}<w_n>.
+//
+// Multi-pass plans with an even first column pass run every pass once per column group for up to 8 cosets at a time
+// (lde_make_cosets_job): a group is G/8 columns x 8 cosets, the same G transforms per launch and the same scratch as
+// one coset of G columns, but the coefficients are read from HBM once per group instead of once per coset. Single-pass
+// sizes, odd first passes and ctx->lde_per_coset run one transform per coset and group.
 static int lde_columns(gl_ctx* ctx, const u64* coeffs, size_t coeff_stride, uint32_t ncols, int log_n, int rate_bits,
                        u64 base_shift, u64* lde, size_t lde_stride) {
     if (ncols == 0) return GL_OK;
@@ -503,8 +557,53 @@ static int lde_columns(gl_ctx* ctx, const u64* coeffs, size_t coeff_stride, uint
         CKL(ctx);
         return GL_OK;
     }
+    const NttPlan pl = ntt_plan(log_n);
+    if (ncos > 1 && pl.a1 && col_cosets_supported(pl.a1) && ctx->ntt_variant == 0 && !ctx->lde_per_coset) {
+        const int log_kc = rate_bits < COL_LOG_MAX_COSETS ? rate_bits : COL_LOG_MAX_COSETS, kc = 1 << log_kc;
+        const uint32_t G = group_cols(ctx, log_n, ncols, kc);
+        TRY(ensure_scratch(ctx, (size_t)G * kc * n));
+        for (uint32_t g0 = 0; g0 < ncols; g0 += G) {
+            const uint32_t gc = (ncols - g0 < G) ? ncols - g0 : G;
+            for (int c0 = 0; c0 < ncos; c0 += kc) {
+                table_cache_trim(ctx, (size_t)(kc + 1) * (n * 8 + (1 << 16)));  // before any table of this job is fetched
+                NttJob job;
+                ColCosets cc;
+                TableReq steps[1 << COL_LOG_MAX_COSETS], posts[1 << COL_LOG_MAX_COSETS];
+                lde_make_cosets_job(log_n, pl, rate_bits, base_shift, c0, log_kc, job, cc, steps, posts);
+                for (int c = 0; c < kc; c++) {
+                    TRY(get_step(ctx, steps[c].a, steps[c].scale, steps[c].base, &cc.tw[c]));
+                    TRY(get_post(ctx, posts[c].a, posts[c].b, posts[c].base, &cc.twa[c]));
+                }
+                cc.cp.in = coeffs + (size_t)g0 * coeff_stride;
+                cc.cp.in_stride = coeff_stride;
+                cc.cp.out = ctx->scratch;
+                cc.cp.out_stride = n;
+                cc.ncols = (int)gc;
+                TRY(dispatch_col_cosets(ctx, pl.a1, cc));
+                if (pl.a2) {
+                    ColPass& c2 = job.c2;
+                    c2.in = c2.out = ctx->scratch;
+                    c2.in_stride = c2.out_stride = n;
+                    TRY(get_step(ctx, job.c2_step.a, job.c2_step.scale, job.c2_step.base, &c2.tw));
+                    TRY(get_post(ctx, job.c2_post.a, job.c2_post.b, job.c2_post.base, &c2.twa));
+                    TRY(dispatch_col(ctx, pl.a2, c2, (size_t)gc * kc));
+                }
+                RowPass& rp = job.rp;
+                TRY(get_step(ctx, job.row_step.a, job.row_step.scale, job.row_step.base, &rp.tw));
+                rp.in = ctx->scratch;
+                rp.in_stride = n;
+                rp.out = lde + (size_t)g0 * lde_stride;
+                rp.out_stride = lde_stride;
+                rp.row0 = (size_t)c0 * n;
+                rp.cos_step = n;
+                rp.ncols = (int)(gc * kc);
+                TRY(dispatch_row(ctx, pl.b, RM_BITREV, rp));
+            }
+        }
+        return GL_OK;
+    }
     const u64 wN = root_of_unity((uint32_t)(log_n + rate_bits));
-    // group-outer / coset-inner: the coefficients of a group are read by every coset while they are warm in L2
+    // group-outer / coset-inner
     const uint32_t G = log_n > NTT_MAX_LOG_PASS ? group_cols(ctx, log_n, ncols) : ncols;
     for (uint32_t g0 = 0; g0 < ncols; g0 += G) {
         const uint32_t gc = (ncols - g0 < G) ? ncols - g0 : G;

@@ -64,6 +64,7 @@ struct gl_ctx {
     size_t dstage_words = 0;
     uint32_t ntt_group = 0;                     // 0 = auto
     int ntt_variant = 0;                        // 0 = shared-body column pass for even LOG, 1 = two-copy kernels (A/B switch)
+    bool lde_per_coset = false;                 // coset LDE: one transform per coset instead of batched cosets (A/B switch)
     int sm_count = 0;                           // queried once for ctx->device in gl_ctx_create
     int coop_ok = 0;                            // cooperative launch supported on this device
     int coop_blocks_per_sm = 0;                 // resident CTAs/SM of k_merkle_upper on this device
@@ -1765,9 +1766,11 @@ int gl_ctx_device_bytes(gl_ctx* ctx, uint64_t* in_use, uint64_t* high, int reset
 }
 uint64_t gl_ctx_launch_count(const gl_ctx* ctx) { return ctx->launches; }
 int gl_ctx_set_ntt_group(gl_ctx* ctx, uint32_t columns) {
-    // bit 31 selects the kernel variant of the column pass (a measurement switch, see gl_ntt_host.cuh)
+    // bit 31 selects the kernel variant of the column pass, bit 30 the per-coset LDE loop (measurement switches, see
+    // gl_ntt_host.cuh)
     ctx->ntt_variant = (columns >> 31) & 1;
-    ctx->ntt_group = columns & 0x7FFFFFFFu;
+    ctx->lde_per_coset = (columns >> 30) & 1;
+    ctx->ntt_group = columns & 0x3FFFFFFFu;
     return GL_OK;
 }
 int gl_ctx_set_profiling(gl_ctx* ctx, int on) {

@@ -1,5 +1,6 @@
 """Sweep the column-group size of the 2^20 NTT and of the cfg2-shaped LDE (run on the H100): small groups keep the
-intermediate of the two passes in the 50 MB L2, large groups give full waves."""
+intermediate of the two passes in the 50 MB L2, large groups give full waves. The group counts transforms per launch:
+the rate-1/8 LDE runs a group of g as g/8 columns x 8 cosets."""
 import ctypes as C, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
