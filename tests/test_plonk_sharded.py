@@ -328,6 +328,18 @@ def test_entry_point_errors(pb):
     L.gl_commit_destroy(h)
     five = (program[0], program[1], np.arange(1, 6, dtype=np.uint64))
     assert _shard_call(ctx, base, five, qdf, nt, out) == N.GL_ERR_UNSUPPORTED
+    # one past each register-program limit, refused before any launch: 5 commitments, 65 537 terms, register 256, a
+    # CONST index (a | b << 16) equal to n_consts through its high half
+    consts = np.arange(65537, dtype=np.uint64)
+    cases = [(base + base[:2], program, nt, b"1..4 commitments", N.GL_ERR_UNSUPPORTED),
+             (base, program, 65537, b"1..65536 vanishing terms", N.GL_ERR_BAD_ARG)]
+    for instrs in ([(plonk.OP_X, 256, 0, 0)], [(plonk.OP_X, 0, 0, 0), (plonk.OP_CONST, 1, 1, 1)]):
+        prog = (plonk.VpInstr * len(instrs))(*[plonk.VpInstr(*i) for i in instrs])
+        cases.append((base, (prog, consts, program[2]), nt, b"bad instruction %d" % (len(instrs) - 1), N.GL_ERR_BAD_ARG))
+    for commits, prog, terms, msg, status in cases:
+        before = ctx.launch_count
+        assert _shard_call(ctx, commits, prog, qdf, terms, out) == status, msg
+        assert msg in L.gl_last_error(ctx.h) and ctx.launch_count == before
     for x in made:
         x.close()
 

@@ -644,6 +644,14 @@ def test_entry_point_errors(pb):
     assert call([(3, 4)], program=wide[0], offs=wide[1], zs=np.zeros(1, dtype=np.uint32)) == N.GL_ERR_UNSUPPORTED
     ngroups = X.ctl_row_programs([(0, [TableWithColumns(0, [Column.single(0)], Filter.default())])] * 17, 8)
     assert call([(3, 4)], program=ngroups[0], offs=ngroups[1], zs=np.arange(17, dtype=np.uint32)) == N.GL_ERR_UNSUPPORTED
+    long = np.zeros((257, 4), dtype=np.uint16)                        # LOCAL 0 ..., then one value and its filter
+    long[-2:, 0], long[-2:, 2] = S.OP_EMIT, [X.CTL_VALUE, X.CTL_FILTER]
+    one = np.zeros(1, dtype=np.uint32)
+    assert call([(3, 4)], program=long[1:].ctypes.data, offs=np.array([0, 256], dtype=np.uint32), zs=one) == N.GL_OK
+    before = ctx.launch_count
+    assert call([(3, 4)], program=long.ctypes.data, offs=np.array([0, 257], dtype=np.uint32),
+                zs=one) == N.GL_ERR_UNSUPPORTED
+    assert b"CTL group 0: row program of 1..256 instructions" in L.gl_last_error(ctx.h) and ctx.launch_count == before
     assert call([(3, 4)], cols=2) == N.GL_ERR_BAD_ARG                 # a program reads column 7 of a 2-column trace
     assert call([(3, 4)], zs=np.zeros(3, dtype=np.uint32)) == N.GL_ERR_BAD_ARG
     assert b"permutation" in L.gl_last_error(ctx.h)

@@ -580,6 +580,18 @@ def test_entry_point_errors(pb):
     wprog, woffs, _ = row_programs([wide], 3)
     assert call([5], offs=woffs, program=wprog) == N.GL_ERR_UNSUPPORTED
     assert call([5], cols=2) == N.GL_ERR_BAD_ARG                      # the program reads column 2 of a 2-column trace
+
+    def long_lookup(n_instr):                                         # LOCAL 0 ..., then one emit of each role
+        p = np.zeros((n_instr, 4), dtype=np.uint16)
+        p[-4:, 0], p[-4:, 2] = S.OP_EMIT, [0, 1, 2, 3]
+        return p
+
+    lp = long_lookup(256)
+    assert call([5], offs=np.array([0, 256], dtype=np.uint32), program=lp.ctypes.data) == N.GL_OK
+    lp = long_lookup(257)
+    before = ctx.launch_count
+    assert call([5], offs=np.array([0, 257], dtype=np.uint32), program=lp.ctypes.data) == N.GL_ERR_UNSUPPORTED
+    assert b"lookup 0: row program of 1..256 instructions" in L.gl_last_error(ctx.h) and ctx.launch_count == before
     cfg = S.StarkConfig.standard_fast_config().fri_config
     rs, rtrace, _ = RangeCheckStark(), RangeCheckStark.generate_trace(5), None
     tc = pb.PolynomialBatch.from_values(rtrace, cfg.rate_bits, False, cfg.cap_height)
@@ -614,6 +626,22 @@ def test_entry_point_errors(pb):
     rc = L.gl_stark_quotient(ctx.h, tc.h, b.program(), len(b.instrs), N.np_ptr(cs), len(cs), N.np_ptr(al), 2, 2,
                              N.vp(q.data_ptr()))
     assert rc == N.GL_ERR_BAD_ARG                                      # auxiliary reads without an auxiliary commitment
+    # 513 instructions; a quotient degree factor of 9 at rate_bits 4 (2^4 points per row, more than 8): refused before
+    # any launch
+    long = np.zeros((513, 4), dtype=np.uint16)
+    long[-1, 0] = S.OP_EMIT
+    before = ctx.launch_count
+    rc = L.gl_stark_quotient(ctx.h, tc.h, long.ctypes.data, 513, N.np_ptr(cs), len(cs), N.np_ptr(al), 2, 2,
+                             N.vp(q.data_ptr()))
+    assert rc == N.GL_ERR_UNSUPPORTED and ctx.launch_count == before
+    assert b"program of 513 instructions (max 512)" in L.gl_last_error(ctx.h)
+    tc4 = pb.PolynomialBatch.from_values(rtrace, 4, False, cfg.cap_height)
+    before = ctx.launch_count
+    rc = L.gl_stark_quotient(ctx.h, tc4.h, b.program(), len(b.instrs), N.np_ptr(cs), len(cs), N.np_ptr(al), 2, 9,
+                             N.vp(q.data_ptr()))
+    assert rc == N.GL_ERR_UNSUPPORTED and ctx.launch_count == before
+    assert b"quotient degree factor too large" in L.gl_last_error(ctx.h)
+    tc4.close()
     tc.close()
     other.close()
 
