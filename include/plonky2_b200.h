@@ -459,6 +459,9 @@ int gl_plonk_quotient_shard(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_c
                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                             uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_values);
 
+/* check_constraints (starky/src/prover.rs:670-820) and its plonky2 counterpart, every constraint of the programs above
+ * checked on every row of the trace subgroup: include/plonky2_b200_check.h. */
+
 /* ---- Hasher / MerkleTree  (plonky2/src/plonk/config.rs:36-77, plonky2/src/hash/merkle_tree.rs:193-237) */
 /* PoseidonPermutation::permute on the HOST for the sequential Fiat-Shamir transcript
  * (plonky2/src/iop/challenger.rs:129-144); the same source as the device permutation. */

@@ -1,0 +1,48 @@
+/*
+ * plonky2_b200_check.h -- constraint checks of the H100-native plonky2 / starky prover (sm_90a CUDA), for debug builds:
+ * the counterpart of starky's check_constraints (starky/src/prover.rs:241-256,670-820), which the reference runs under
+ * #[cfg(debug_assertions)] only. The conventions of plonky2_b200.h hold (status codes, gl_last_error, field elements
+ * as uint64_t, non-canonical inputs accepted); the programs and handles are the ones its quotient entry points take.
+ * Host inputs (the program and its constants) have been read when a call returns: every call ends in a synchronising
+ * read-back of its outputs.
+ */
+#ifndef PLONKY2_B200_CHECK_H
+#define PLONKY2_B200_CHECK_H
+#include "plonky2_b200.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* check_constraints (starky/src/prover.rs:670-820) on the device, and its plonky2 counterpart: the program the matching
+ * quotient entry point runs, checked on every row i of the trace subgroup H = <w_n> at x = w_n^i (no coset shift), each
+ * constraint on its own. The values on H are the NTT of each commitment's coefficients, so every kind of handle is
+ * checked alike: resident, non-resident (gl_commit_begin_blocked), a row-block shard (its coefficients are replicated)
+ * and salted (GL_VP_LOCAL / GL_VP_NEXT operands are bounded by B, never W: salt columns are not polynomials).
+ * A LOCAL operand reads row i, a NEXT operand row (i + 1) mod n. Nothing about the quotient degree is required: a STARK
+ * of constraint degree 0 is checked like any other.
+ *   gl_stark_check_rows  GL_STARK_EMIT number e (its ordinal among the program's EMITs) of value v fails at row i when
+ *                        v is nonzero and its filter is on: GL_STARK_CONSTRAINT always, GL_STARK_TRANSITION at every
+ *                        row but n - 1 (z_last = x - w_n^-1), GL_STARK_FIRST_ROW at row 0, GL_STARK_LAST_ROW at row
+ *                        n - 1 -- the reference's filter values on H. aux = NULL: the program may not read auxiliary
+ *                        columns. consts as for gl_stark_quotient; no alphas.
+ *   gl_plonk_check_rows  GL_VP_TERM b fails at row i when its value is nonzero. GL_VP_X is w_n^i, GL_VP_L0 the indicator
+ *                        [i = 0]; there is no Z_H and no alpha. On H only the row's own gate has a nonzero selector
+ *                        filter, so a failing gate-constraint term at row i is a constraint of the gate at row i.
+ * Outputs (HOST memory): *out_failures = the number of failing (row, index) pairs; out_pairs = the first max_report of
+ * them in (row, index) order, row then index, 2 x max_report words (may be NULL when max_report is 0);
+ * *out_reported = how many were written, min(*out_failures, max_report). GL_OK means the check ran, whether or not
+ * anything failed. Refused before any launch: a NULL argument, an unfinished handle, commitments of different degree
+ * or of another context, max_report > 65536 (GL_ERR_BAD_ARG / GL_ERR_BAD_SHAPE), and the quotient entry points' program
+ * errors with their messages. Scratch: B x n words per commitment read, plus 8 (n + 1) bytes. */
+int gl_stark_check_rows(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
+                        const uint64_t* consts, uint32_t n_consts, uint32_t max_report, uint64_t* out_failures,
+                        uint32_t* out_pairs, uint32_t* out_reported);
+int gl_plonk_check_rows(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                        uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, uint32_t n_terms,
+                        uint32_t max_report, uint64_t* out_failures, uint32_t* out_pairs, uint32_t* out_reported);
+
+#ifdef __cplusplus
+}
+#endif
+#endif

@@ -3,7 +3,8 @@ Goldilocks NTT / coset-LDE, Poseidon Merkle commitment and the FRI commit phase,
 include/plonky2_b200.h. This package is the host-side mirror of the reference's interface for that
 path (same names, argument meaning and error behaviour); see DESIGN.md and INTEGRATION.md."""
 from . import field  # noqa: F401
-from ._native import Context, NativeError, ShapeError, default_context  # noqa: F401
+from ._native import (ConstraintError, ConstraintReport, Context, NativeError, ShapeError,  # noqa: F401
+                      default_context)
 from .challenger import Challenger  # noqa: F401
 from .fft import (coset_fft, coset_fft_with_options, coset_ifft, fft, fft_with_options, ifft,  # noqa: F401
                   ifft_with_options, lde, lde_onto_coset)

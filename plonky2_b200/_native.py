@@ -34,6 +34,8 @@ EXPORTS = [
     "gl_commit_finish_prefixed", "gl_commit_dev_cap", "gl_commit_begin_blocked", "gl_commit_lde_blocks",
     "gl_ctx_device_bytes",
 ]
+# the constraint checks of include/plonky2_b200_check.h
+CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows"]
 
 
 class FriBatch(C.Structure):
@@ -47,6 +49,45 @@ class ShapeError(ValueError):
 
 class NativeError(RuntimeError):
     pass
+
+
+class ConstraintError(ValueError):
+    """A trace or witness that breaks a constraint, found by a prover's check_constraints=True (the reference's
+    "Constraint failed in {Stark} at row {row}", starky/src/prover.rs:812). `report` is the ConstraintReport."""
+
+    def __init__(self, message, report):
+        super().__init__(message)
+        self.report = report
+
+
+class ConstraintReport:
+    """What gl_stark_check_rows / gl_plonk_check_rows found: `failures`, the number of failing (row, index) pairs, and
+    `entries`, the first of them in (row, index) order as (row, index, label)."""
+
+    def __init__(self, failures, entries):
+        self.failures, self.entries = int(failures), list(entries)
+
+    def __bool__(self):
+        """True when nothing failed."""
+        return self.failures == 0
+
+    def __repr__(self):
+        return "ConstraintReport(failures=%d, entries=%r)" % (self.failures, self.entries)
+
+
+MAX_REPORT = 65536
+
+
+def check_rows(fn, ctx, args, max_report):
+    """Run the check entry point `fn` (gl_stark_check_rows or gl_plonk_check_rows) with `args` between the context and
+    max_report. Returns (failures, [(row, index)])."""
+    max_report = int(max_report)
+    if not 0 <= max_report <= MAX_REPORT:
+        raise ValueError("max_report must be in 0..%d" % MAX_REPORT)
+    failures, reported = C.c_uint64(), C.c_uint32()
+    pairs = np.zeros(2 * max(max_report, 1), dtype=np.uint32)
+    check(fn(ctx.h, *args, max_report, C.byref(failures), pairs.ctypes.data_as(u32p), C.byref(reported)), ctx.h)
+    return failures.value, [(int(r), int(i)) for r, i in pairs[:2 * reported.value].reshape(-1, 2)]
 
 
 _lib = None
@@ -121,6 +162,9 @@ def lib():
                                     C.c_uint32, vp]
     L.gl_plonk_quotient_shard.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32,
                                           C.c_uint32, C.c_uint32, vp]
+    L.gl_stark_check_rows.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, u64p, u32p, u32p]
+    L.gl_plonk_check_rows.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32, u64p,
+                                      u32p, u32p]
     L.gl_lookup_polys.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p, C.c_uint32, vp, C.c_int]
     L.gl_sigma_polys.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, vp, vp,
                                  C.c_int]

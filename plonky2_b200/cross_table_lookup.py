@@ -138,6 +138,7 @@ def eval_cross_table_lookup_checks(vars, ctl_vars, consumer, constraint_degree, 
     total = sum(len(v.helper_columns) for v in ctl_vars)
     start = num_lookup_columns
     for i, v in enumerate(ctl_vars):
+        consumer.begin_scope("CTL Z %d" % i)
         beta, gamma = vars.ctl_challenge(i)
         comb = lambda values: combine(vars, values, beta, gamma)  # noqa: E731
         evals = [[c.eval_with_next(vars) for c in cols] for cols in v.columns]
@@ -390,7 +391,8 @@ def check_prove_shapes(starks, config, traces, cross_table_lookups, public_input
     return params, max_degree
 
 
-def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None, lde_blocks=None):
+def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx=None, lde_blocks=None,
+                    check_constraints=False):
     """A multi-STARK proof with cross-table lookups: every table's trace commitment, every trace cap observed in table
     order, the CTL challenge set (get_ctl_data), every table's CTL helper and Z columns on the device
     (cross_table_lookup_data at the system's largest constraint degree), then table by table on the same challenger its
@@ -399,14 +401,16 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     trace may still be in production on the caller's current torch stream, the library's work is ordered after it. Raises
     ShapeError before any device work for every shape the reference cannot prove or verify (check_prove_shapes).
     Returns a MultiStarkProof. distributed.prove_with_ctls proves the same system across several GPUs. lde_blocks=G:
-    every commitment is non-resident, as in stark.prove; G must also be at most every table's quotient coset size."""
+    every commitment is non-resident, as in stark.prove; G must also be at most every table's quotient coset size.
+    check_constraints=True checks every table's constraints (its own, lookups and CTLs) as stark.prove does."""
     from . import stark as S
 
     return _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx,
-                            S.lde_placement(config, lde_blocks))
+                            S.lde_placement(config, lde_blocks), check_constraints)
 
 
-def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement):
+def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement,
+                     check_constraints=False):
     """prove_with_ctls on a distributed.Placement: every trace is committed with placement.commit_kwargs and observed
     as placement.cap, and each table runs prove_with_commitment on the placement. The CTL helper and Z columns are
     computed from the full traces on every rank."""
@@ -439,7 +443,7 @@ def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs,
             config.observe(challenger)
             proofs.append(S.prove_with_commitment(s, config, dev_traces[i], commitments[i], caps[i], ctl_data[i],
                                                   ctl_challenges, challenger, public_inputs[i], params[i], ctx=ctx,
-                                                  placement=placement))
+                                                  placement=placement, check_constraints=check_constraints))
             ctl_data[i] = None
         return MultiStarkProof(proofs)
     finally:

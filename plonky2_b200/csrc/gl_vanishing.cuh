@@ -8,7 +8,8 @@
 // The instruction stream is uniform across the warp (one broadcast load per instruction); the registers are a
 // per-thread array the compiler keeps in local memory, so gates of any size fit without a new kernel.
 //
-// The same source runs on the host in tests/emu/vanishing_emu.cpp (threads as a loop) against the oracle.
+// The same source runs on the host in tests/emu/vanishing_emu.cpp (threads as a loop) against the oracle, and the
+// row check below in tests/emu/check_rows_emu.cpp.
 #pragma once
 #include "../../include/plonky2_b200.h"
 #include "gl_field.cuh"
@@ -106,6 +107,54 @@ GL_HD bool vp_eval_point(const VanishingParams& p, size_t j, uint64_t* regs) {
     const uint32_t log_M = size_log - p.shard_log;  // i = bitrev(g) + G*k: local point k = i >> shard_log
     for (uint32_t a = 0; a < p.n_alphas; a++) p.out[((size_t)a << log_M) + (i >> p.shard_log)] = canon(mul(acc[a], zi));
     return ok;
+}
+
+// The same program checked on one row i of the trace subgroup H = <w_n>, at x = w_n^i with no coset shift
+// (gl_plonk_check_rows): every GL_VP_TERM on its own, without alphas or Z_H. On H, L_0 is the indicator [i = 0] (its
+// closed form above divides by zero at x = 1), and only the row's own gate has a nonzero selector filter, so a failing
+// gate-constraint term at row i is a constraint of the gate placed at row i.
+struct VpRowsParams {
+    const uint64_t* val[GL_VP_MAX_COMMITS];  // commitment c's values on H, column k at val[c] + k*n, natural order
+    uint32_t log_n;
+    const gl_vp_instr* prog;          // validated by the caller
+    uint32_t n_instr;
+    const uint64_t* consts;
+    const uint64_t *xhi, *xlo;        // w_n^i = xhi[i >> 12] * xlo[i & 4095]
+};
+
+// The number of GL_VP_TERMs whose value is nonzero at row i. With pairs != NULL, failure m is also written as the pair
+// (row i, the term number b) at pairs[2m], pairs[2m + 1], in program order. regs: GL_VP_MAX_REGS words of scratch.
+GL_HD uint32_t vp_check_row(const VpRowsParams& p, size_t i, uint64_t* regs, uint32_t* pairs) {
+    const size_t n = (size_t)1 << p.log_n;
+    const size_t in = (i + 1) & (n - 1);
+    uint32_t fails = 0;
+    for (uint32_t k = 0; k < p.n_instr; k++) {
+        const gl_vp_instr ins = p.prog[k];
+        uint64_t r;
+        switch (ins.op) {
+            case GL_VP_LOCAL: r = p.val[ins.a][((size_t)ins.b << p.log_n) + i]; break;
+            case GL_VP_NEXT: r = p.val[ins.a][((size_t)ins.b << p.log_n) + in]; break;
+            case GL_VP_CONST: r = p.consts[(uint32_t)ins.a | ((uint32_t)ins.b << 16)]; break;
+            case GL_VP_X: r = mul(p.xhi[i >> 12], p.xlo[i & 4095]); break;
+            case GL_VP_L0: r = i == 0; break;
+            case GL_VP_ADD: r = add(regs[ins.a], regs[ins.b]); break;
+            case GL_VP_SUB: r = sub(regs[ins.a], regs[ins.b]); break;
+            case GL_VP_MUL: r = mul(regs[ins.a], regs[ins.b]); break;
+            case GL_VP_ADDC: r = add(regs[ins.a], p.consts[ins.b]); break;
+            case GL_VP_MULC: r = mul(regs[ins.a], p.consts[ins.b]); break;
+            default:  // GL_VP_TERM
+                if (canon(regs[ins.a]) != 0) {
+                    if (pairs) {
+                        pairs[2 * fails] = (uint32_t)i;
+                        pairs[2 * fails + 1] = ins.b;
+                    }
+                    fails++;
+                }
+                continue;
+        }
+        regs[ins.dst] = r;
+    }
+    return fails;
 }
 
 }  // namespace gl

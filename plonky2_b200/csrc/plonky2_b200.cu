@@ -8,8 +8,10 @@
 // There is no CPU fallback anywhere in this file: every compute entry point launches kernels.
 #include <cooperative_groups.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -34,6 +36,7 @@
 #include "gl_ntt.cuh"
 #include "gl_poseidon.cuh"
 #include "gl_sigma.cuh"
+#include "gl_stark_rows.cuh"
 #include "gl_vanishing.cuh"
 
 using namespace gl;
@@ -2490,6 +2493,28 @@ static int quotient_shape_check(gl_ctx* ctx, uint32_t db, uint32_t rate_bits, ui
     *qd_bits_out = qd_bits;
     return GL_OK;
 }
+// A STARK constraint program, validated once on the host (the kernels trust it): column operands below the trace's
+// and the auxiliary commitment's B (no auxiliary operand without `aux`), constants below n_consts, values read after
+// they are made. Sets *n_emit (if given) to the number of GL_STARK_EMITs.
+static int stark_program_check(gl_ctx* ctx, const gl_stark_instr* program, uint32_t n_instr, const gl_commit* trace,
+                               const gl_commit* aux, uint32_t n_consts, uint32_t* n_emit) {
+    uint32_t emits = 0;
+    for (uint32_t k = 0; k < n_instr; k++) {
+        const gl_stark_instr in = program[k];
+        bool ok = true;
+        switch (in.op) {
+            case GL_STARK_LOCAL: case GL_STARK_NEXT: ok = in.a < trace->B; break;
+            case GL_STARK_AUX_LOCAL: case GL_STARK_AUX_NEXT: ok = aux && in.a < aux->B; break;
+            case GL_STARK_CONST: ok = in.a < n_consts; break;
+            case GL_STARK_ADD: case GL_STARK_SUB: case GL_STARK_MUL: ok = in.a < k && in.b < k; break;
+            case GL_STARK_EMIT: ok = in.a < k && in.b <= GL_STARK_LAST_ROW; emits++; break;
+            default: ok = false;
+        }
+        if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "constraint program: bad instruction %u", k);
+    }
+    if (n_emit) *n_emit = emits;
+    return GL_OK;
+}
 // The checks of gl_stark_quotient[_aux] (whole = true: both LDEs whole on this device) and gl_stark_quotient_shard
 // (whole = false: the trace and the auxiliary commitment are shards of the same index and count). Sets *qd_bits.
 static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
@@ -2517,20 +2542,7 @@ static int stark_quotient_check(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, c
     }
     TRY(quotient_shape_check(ctx, trace->degree_log, trace->rate_bits, trace->shard_log + trace->block_log,
                              quotient_degree_factor, GL_STARK_MAX_QD, qd_bits_out));
-    for (uint32_t k = 0; k < n_instr; k++) {  // validate once on the host: the kernel trusts the program
-        const gl_stark_instr in = program[k];
-        bool ok = true;
-        switch (in.op) {
-            case GL_STARK_LOCAL: case GL_STARK_NEXT: ok = in.a < trace->B; break;
-            case GL_STARK_AUX_LOCAL: case GL_STARK_AUX_NEXT: ok = aux && in.a < aux->B; break;
-            case GL_STARK_CONST: ok = in.a < n_consts; break;
-            case GL_STARK_ADD: case GL_STARK_SUB: case GL_STARK_MUL: ok = in.a < k && in.b < k; break;
-            case GL_STARK_EMIT: ok = in.a < k && in.b <= GL_STARK_LAST_ROW; break;
-            default: ok = false;
-        }
-        if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "constraint program: bad instruction %u", k);
-    }
-    return GL_OK;
+    return stark_program_check(ctx, program, n_instr, trace, aux, n_consts, nullptr);
 }
 // The part g of G = 2^sl of the quotient coset g*<w_size> (size = 2^(degree_log + qd_bits)) that one evaluation covers:
 // the M = size / G points g*w_size^r*<w_M>, r = the sl-bit reversal of g. A shard evaluates its own part (the whole coset
@@ -2892,6 +2904,37 @@ int gl_stark_ctl_helpers(gl_ctx* ctx, const uint64_t* trace, size_t col_stride, 
     return flag_status(ctx, dflag, {INVERT_ZERO});
 }
 
+// A vanishing program, validated once on the host (the kernels trust it): operands in range -- column operands below
+// each commitment's W with salt_readable, else its B -- and no register read before it is written. Sets *next_mask_out
+// (bit c: the program reads commitment c's next row) and *n_term (if given) to the number of GL_VP_TERMs.
+static int vp_program_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                            uint32_t n_instr, uint32_t n_consts, uint32_t n_terms, bool salt_readable,
+                            uint32_t* next_mask_out, uint32_t* n_term) {
+    uint32_t next_mask = 0, terms = 0;
+    bool written[GL_VP_MAX_REGS] = {false};
+    auto readable = [&](uint16_t r) { return r < GL_VP_MAX_REGS && written[r]; };
+    for (uint32_t k = 0; k < n_instr; k++) {
+        const gl_vp_instr in = program[k];
+        bool ok = in.dst < GL_VP_MAX_REGS;
+        switch (in.op) {
+            case GL_VP_LOCAL: case GL_VP_NEXT:
+                ok = ok && in.a < n_commits && in.b < (salt_readable ? commits[in.a]->W : commits[in.a]->B);
+                if (ok && in.op == GL_VP_NEXT) next_mask |= 1u << in.a;
+                break;
+            case GL_VP_CONST: ok = ok && ((uint32_t)in.a | ((uint32_t)in.b << 16)) < n_consts; break;
+            case GL_VP_X: case GL_VP_L0: break;
+            case GL_VP_ADD: case GL_VP_SUB: case GL_VP_MUL: ok = ok && readable(in.a) && readable(in.b); break;
+            case GL_VP_ADDC: case GL_VP_MULC: ok = ok && readable(in.a) && in.b < n_consts; break;
+            case GL_VP_TERM: ok = readable(in.a) && in.b < n_terms; terms++; break;
+            default: ok = false;
+        }
+        if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "vanishing program: bad instruction %u", k);
+        if (in.op != GL_VP_TERM) written[in.dst] = true;
+    }
+    *next_mask_out = next_mask;
+    if (n_term) *n_term = terms;
+    return GL_OK;
+}
 // The checks of gl_plonk_quotient (whole = true: every LDE whole on this device) and gl_plonk_quotient_shard
 // (whole = false: the commitments are shards of the same index and count). Sets *qd_bits_out and *next_mask_out (bit c:
 // the program reads commitment c's next row).
@@ -2922,31 +2965,8 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
                              quotient_degree_factor, GL_VP_MAX_QD, qd_bits_out));
     // a shard whose quotient coset is not its LDE coset reads values computed from the coefficients: no salt columns
     const bool in_place = quotient_coset(commits[0], *qd_bits_out, commits[0]->shard_index, commits[0]->shard_log).local_in_place;
-    uint32_t next_mask = 0;
-    {  // validate once on the host: the kernel trusts the program (operands in range, no register read before it is written)
-        bool written[GL_VP_MAX_REGS] = {false};
-        auto readable = [&](uint16_t r) { return r < GL_VP_MAX_REGS && written[r]; };
-        for (uint32_t k = 0; k < n_instr; k++) {
-            const gl_vp_instr in = program[k];
-            bool ok = in.dst < GL_VP_MAX_REGS;
-            switch (in.op) {
-                case GL_VP_LOCAL: case GL_VP_NEXT:
-                    ok = ok && in.a < n_commits && in.b < (in_place ? commits[in.a]->W : commits[in.a]->B);
-                    if (ok && in.op == GL_VP_NEXT) next_mask |= 1u << in.a;
-                    break;
-                case GL_VP_CONST: ok = ok && ((uint32_t)in.a | ((uint32_t)in.b << 16)) < n_consts; break;
-                case GL_VP_X: case GL_VP_L0: break;
-                case GL_VP_ADD: case GL_VP_SUB: case GL_VP_MUL: ok = ok && readable(in.a) && readable(in.b); break;
-                case GL_VP_ADDC: case GL_VP_MULC: ok = ok && readable(in.a) && in.b < n_consts; break;
-                case GL_VP_TERM: ok = readable(in.a) && in.b < n_terms; break;
-                default: ok = false;
-            }
-            if (!ok) return set_err(ctx, GL_ERR_BAD_ARG, "vanishing program: bad instruction %u", k);
-            if (in.op != GL_VP_TERM) written[in.dst] = true;
-        }
-    }
-    *next_mask_out = next_mask;
-    return GL_OK;
+    return vp_program_check(ctx, commits, n_commits, program, n_instr, n_consts, n_terms, in_place, next_mask_out,
+                            nullptr);
 }
 // The vanishing polynomial over Z_H on the commitments' shard of the quotient coset (the whole coset for unsharded
 // handles): M values per challenge in local natural order, at out + a*M. L_0 asked for at x = 1 sets bit 0 of dflag.
@@ -3558,3 +3578,6 @@ int gl_fri_pow(gl_ctx* ctx, const uint64_t state[12], uint32_t pos, uint32_t min
 }
 
 }  // extern "C"
+
+// gl_stark_check_rows and gl_plonk_check_rows (include/plonky2_b200_check.h), on the helpers above
+#include "gl_check_rows_host.cuh"

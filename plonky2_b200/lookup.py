@@ -220,9 +220,10 @@ def eval_packed_lookups_generic(stark, lookups, vars, num_lookup_challenges, yie
     challenges with lookup_challenge (bound at evaluation time like the public inputs)."""
     degree = stark.constraint_degree()
     start = 0
-    for lookup in lookups:
+    for li, lookup in enumerate(lookups):
         nh = lookup.num_helper_columns(degree)
         for c in range(num_lookup_challenges):
+            yield_constr.begin_scope("lookup %d, challenge %d" % (li, c))
             challenge = vars.lookup_challenge(c)
             lookup_columns = [col.eval_with_next(vars) for col in lookup.columns]
             helpers = [vars.aux_local(start + k) for k in range(nh - 1)]

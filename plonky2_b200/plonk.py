@@ -1486,6 +1486,71 @@ def quotient_program(common_data, commits, public_inputs_hash, betas, gammas, al
     return prog, consts, np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
 
 
+def check_constraints(common_data, constants_sigmas_commitment, public_inputs_hash, wires_commitment,
+                      zs_partial_products_commitment, betas, gammas, deltas=(), max_report=64):
+    """The vanishing polynomial's terms checked on every row of the trace subgroup H, each on its own
+    (gl_plonk_check_rows): the program compute_quotient_polys runs, at x = w_n^i without alphas or Z_H. Takes what
+    compute_quotient_polys takes but the alphas. Returns a ConstraintReport whose entries are (row, term number, label)
+    for the first max_report (0..65536) failing (row, term) pairs in (row, term) order; the labels follow
+    vanishing_program's term layout, and a gate constraint's label names the gate placed at that row."""
+    commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
+    # no alphas: the betas stand in for quotient_program's count check, and its alpha array is not used
+    prog, consts, _ = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, betas, deltas)
+    ctx = wires_commitment.ctx
+    handles = (C.c_void_p * 3)(*[c.h for c in commits])
+    failures, pairs = N.check_rows(N.lib().gl_plonk_check_rows, ctx, (handles, 3, prog, len(prog), N.np_ptr(consts),
+                                                                      len(consts), common_data.num_vanishing_terms()),
+                                   max_report)
+    return N.ConstraintReport(failures, _term_labels(common_data, constants_sigmas_commitment, pairs))
+
+
+def _raise_on_failure(common_data, *commitments_and_challenges):
+    """prove_with_witness's check_constraints=True: ConstraintError with the first failure's row and label and the
+    total."""
+    report = check_constraints(common_data, *commitments_and_challenges)
+    if report.failures:
+        row, _, label = report.entries[0]
+        raise N.ConstraintError("Constraint failed in the circuit at row %d: %s; %d failing (row, term) pairs in all"
+                                % (row, label, report.failures), report)
+
+
+def _term_labels(cd, constants_sigmas_commitment, pairs):
+    """(row, term, label) for check_constraints' (row, term) pairs, by vanishing_program's term layout. The gate at a
+    gate constraint's row is read from the selector polynomials evaluated at w_n^row."""
+    nc, num_prods = cd.config.num_challenges, cd.num_partial_products
+    n_lookup = cd.num_lookup_terms()
+    lookup_base = nc + nc * (num_prods + 1)
+    base = lookup_base + nc * n_lookup
+    gate_rows = sorted({row for row, t in pairs if t >= base})
+    gates = {}
+    if gate_rows:
+        from .proof import eval_commitments
+
+        w = F.primitive_root_of_unity(cd.degree_bits)
+        num_selectors = cd.selectors_info.num_selectors()
+        evals = eval_commitments([(constants_sigmas_commitment, (pow(w, row, F.ORDER), 0)) for row in gate_rows])
+        for row, ev in zip(gate_rows, evals):
+            sel = [int(v) for v in ev[:num_selectors, 0]]
+            used = [v for v in sel if v != UNUSED_SELECTOR]
+            gates[row] = cd.gates[used[0]].id() if used and used[0] < len(cd.gates) else "no gate"
+    out = []
+    for row, t in pairs:
+        if t < nc:
+            label = "Z(1) = 1 of challenge %d" % t
+        elif t < lookup_base:
+            i, k = (t - nc) // (num_prods + 1), (t - nc) % (num_prods + 1)
+            label = "partial-product check %d of challenge %d" % (k, i)
+            if k == num_prods and row == (1 << cd.degree_bits) - 1:
+                label += " (the permutation does not close: a copy constraint is violated)"
+        elif t < base:
+            i, k = (t - lookup_base) // n_lookup, (t - lookup_base) % n_lookup
+            label = "lookup term %d of challenge %d" % (k, i)
+        else:
+            label = "gate constraint %d of %s" % (t - base, gates[row])
+        out.append((row, t, label))
+    return out
+
+
 def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None, shard=(0, 1)):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients (trim_to_len(quotient_degree) was checked by the kernel call), all
@@ -1818,7 +1883,8 @@ def _to_device(columns, ctx):
     return t
 
 
-def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None, *, salt_keys=None):
+def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None, *, salt_keys=None,
+                       check_constraints=False):
     """prove_with_partition_witness (plonk/prover.rs:132-360) from the full witness matrix `wires` (num_wires, n) -- the
     generators' output -- to ProofWithPublicInputs, every array-sized step on the device: wires commitment, Z / partial
     products (+ lookup) commitment, quotient polynomials from the LDEs in place and their commitment, the openings at
@@ -1828,11 +1894,16 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
     prover.rs:179,249,297 do (the constants / sigmas commitment never is), and prover_data.fri_params.hiding must be set.
     The salt is drawn on the device: salt_keys = three 32-byte keys (wires, Z's, quotient) give a reproducible proof;
     None draws a fresh key from the OS CSPRNG per commitment. The blinding rows of the circuit (blinding_counts) are part
-    of the witness, which the caller generates."""
-    return _prove(prover_data, common_data, wires, public_inputs, ctx, distributed.Placement(), salt_keys)
+    of the witness, which the caller generates.
+
+    check_constraints=True: after the Z / partial-product commitment, before the quotient, every term of the vanishing
+    polynomial is checked on every row of H with the proof's own challenges (check_constraints), and a failure raises
+    ConstraintError naming the row and the term; the proof is unchanged."""
+    return _prove(prover_data, common_data, wires, public_inputs, ctx, distributed.Placement(), salt_keys,
+                  check_constraints)
 
 
-def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys=None):
+def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys=None, check_constraints=False):
     """prove_with_witness on a distributed.Placement. With G > 1 ranks this one holds row block g of the wires,
     Z / partial-product (+ lookup) and quotient commitments, and prover_data.constants_sigmas_commitment is that shard
     too: the caps are all-gathered before they are observed, the quotient is evaluated shard by shard and all-gathered,
@@ -1898,6 +1969,8 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
         challenger.observe_cap(zs_cap)
         alphas = challenger.get_n_challenges(nc)
         cs = prover_data.constants_sigmas_commitment
+        if check_constraints:
+            _raise_on_failure(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas, gammas, deltas)
         quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas,
                                                 gammas, alphas, deltas, **placement.step_kwargs)
         quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx,

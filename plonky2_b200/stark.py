@@ -22,6 +22,7 @@ from .proof import StarkOpeningSet
 
 OP_LOCAL, OP_NEXT, OP_CONST, OP_ADD, OP_SUB, OP_MUL, OP_EMIT, OP_AUX_LOCAL, OP_AUX_NEXT = range(9)
 KIND_CONSTRAINT, KIND_TRANSITION, KIND_FIRST_ROW, KIND_LAST_ROW = range(4)
+KIND_NAMES = ("every row", "transition", "first row", "last row")
 
 
 class StarkInstr(C.Structure):
@@ -61,6 +62,9 @@ class ConstraintBuilder:
         self.instrs, self.consts = [], [None] * self.num_bound
         self.num_columns, self.num_pi, self.num_aux = num_columns, num_public_inputs, num_aux
         self._cache = {}
+        # what check_constraints names each EMIT by: the Stark's own constraints are numbered in emission order, the
+        # lookup and CTL recorders open a scope of their own (begin_scope) whose checks are numbered from 0
+        self.labels, self._scope, self._scope_count = [], "constraint", 0
 
     def _push(self, op, a=0, b=0):
         key = (op, a, b)
@@ -110,18 +114,27 @@ class ConstraintBuilder:
             self.consts.append(v)
         return self._push(OP_CONST, self.num_bound + self.consts[self.num_bound:].index(v))
 
+    def begin_scope(self, name):
+        """Label the EMITs that follow as checks 0, 1, ... of `name` (a lookup's challenge, a CTL Z)."""
+        self._scope, self._scope_count = name + ", check", 0
+
     # ConstraintConsumer
+    def _emit(self, e, kind):
+        self._push(OP_EMIT, e.idx, kind)
+        self.labels.append("%s %d (%s)" % (self._scope, self._scope_count, KIND_NAMES[kind]))
+        self._scope_count += 1
+
     def constraint(self, e):
-        self._push(OP_EMIT, e.idx, KIND_CONSTRAINT)
+        self._emit(e, KIND_CONSTRAINT)
 
     def constraint_transition(self, e):
-        self._push(OP_EMIT, e.idx, KIND_TRANSITION)
+        self._emit(e, KIND_TRANSITION)
 
     def constraint_first_row(self, e):
-        self._push(OP_EMIT, e.idx, KIND_FIRST_ROW)
+        self._emit(e, KIND_FIRST_ROW)
 
     def constraint_last_row(self, e):
-        self._push(OP_EMIT, e.idx, KIND_LAST_ROW)
+        self._emit(e, KIND_LAST_ROW)
 
     def program(self):
         arr = (StarkInstr * len(self.instrs))()
@@ -310,6 +323,34 @@ def quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment=No
     if len(public_inputs) != stark.PUBLIC_INPUTS:
         raise N.ShapeError("expected %d public inputs" % stark.PUBLIC_INPUTS)
     return b, consts, np.array([int(a) % F.ORDER for a in alphas], dtype=np.uint64)
+
+
+def check_constraints(stark, trace_commitment, public_inputs, auxiliary_polys_commitment=None, lookup_challenges=None,
+                      ctl_vars=None, max_report=64):
+    """check_constraints (starky/src/prover.rs:670-820) on the device: every constraint of the Stark -- its own, then its
+    lookups', then its CTLs' -- on every row of the trace subgroup H, each constraint on its own (gl_stark_check_rows).
+    Takes what compute_quotient_polys takes but the alphas, on any kind of commitment (resident, non-resident, a
+    row-block shard: its coefficients are replicated); a Stark of constraint degree 0 is checked too. Returns a
+    ConstraintReport: the number of failing (row, constraint) pairs and the first max_report (0..65536) of them in
+    (row, constraint) order as (row, EMIT ordinal, label), the label naming the Stark's own constraint by its number in
+    eval_packed_generic's order, a lookup's check by lookup and challenge, or a CTL check by its Z."""
+    b, consts, _ = quotient_program(stark, public_inputs, [], auxiliary_polys_commitment, lookup_challenges, ctl_vars)
+    ctx = trace_commitment.ctx
+    aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
+    failures, pairs = N.check_rows(N.lib().gl_stark_check_rows, ctx, (trace_commitment.h, aux_h, b.program(),
+                                                                      len(b.instrs), N.np_ptr(consts), len(consts)),
+                                   max_report)
+    return N.ConstraintReport(failures, [(row, e, b.labels[e]) for row, e in pairs])
+
+
+def _raise_on_failure(stark, trace_commitment, public_inputs, **quotient_args):
+    """check_constraints=True of the provers: ConstraintError with the reference's wording, the first failure's label
+    and the total."""
+    report = check_constraints(stark, trace_commitment, public_inputs, **quotient_args)
+    if report.failures:
+        row, _, label = report.entries[0]
+        raise N.ConstraintError("Constraint failed in %s at row %d: %s; %d failing (row, constraint) pairs in all"
+                                % (type(stark).__name__, row, label, report.failures), report)
 
 
 def _ctl_bound(ctl_vars):
@@ -691,7 +732,8 @@ def lde_placement(config, lde_blocks):
     return D.Placement(lde_blocks=int(lde_blocks))
 
 
-def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None, lde_blocks=None):
+def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None, ctx=None, lde_blocks=None,
+          check_constraints=False):
     """prove (starky/src/prover.rs:40-114) for one Stark: trace = (COLUMNS, n) host columns or torch CUDA tensor ->
     StarkProofWithPublicInputs. The trace commitment, then a fresh challenger observing the public inputs, the config
     and the trace cap, then prove_with_commitment without CTLs. verifier_circuit_fri_params: the FRI parameters of a
@@ -700,12 +742,15 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     the library's work is ordered after it. Raises ShapeError / NativeError with the reference's messages; every
     commitment is released on every exit path. lde_blocks=G: every commitment is non-resident
     (PolynomialBatch.from_values), for traces whose LDEs exceed device memory; the proof is the same. G must be a power
-    of two of at most 2^cap_height and of at most the quotient coset's size (ShapeError before any device work)."""
+    of two of at most 2^cap_height and of at most the quotient coset's size (ShapeError before any device work).
+    check_constraints=True: every constraint is checked on every row of H before the quotient, where the reference's
+    debug builds check them (prover.rs:241-256), and a failure raises ConstraintError naming the row and the constraint;
+    the proof is unchanged."""
     return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx,
-                  lde_placement(config, lde_blocks))
+                  lde_placement(config, lde_blocks), check_constraints)
 
 
-def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement):
+def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement, check_constraints=False):
     """prove on a distributed.Placement (see prove_with_commitment)."""
     from .challenger import Challenger
 
@@ -724,13 +769,14 @@ def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx
         trace_cap = placement.cap(trace_commitment)
         challenger.observe_cap(trace_cap)
         return prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, None, None, challenger,
-                                     public_inputs, params, ctx=ctx, placement=placement)
+                                     public_inputs, params, ctx=ctx, placement=placement,
+                                     check_constraints=check_constraints)
     finally:
         trace_commitment.close()
 
 
 def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl_data, ctl_challenges, challenger,
-                          public_inputs, params, ctx=None, placement=D.Placement()):
+                          public_inputs, params, ctx=None, placement=D.Placement(), check_constraints=False):
     """prove_with_commitment (starky/src/prover.rs:125-484): one table's proof from its committed trace, on a challenger
     that has already observed what precedes it (the config and trace_cap, the trace's full cap, among them). Every
     array-sized step runs on the device (lookup helper columns and the auxiliary commitment, quotient from the LDEs in
@@ -743,7 +789,8 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
     the quotient is evaluated shard by shard and all-gathered, the openings are summed over each rank's block of the
     coefficients and added up, and FRI routes the query openings between the ranks.
     Everything else runs redundantly on every rank, so every rank returns the same proof. Every commitment made here is
-    released on every exit path; the trace commitment stays the caller's."""
+    released on every exit path; the trace commitment stays the caller's. check_constraints=True (one device): after
+    the auxiliary commitment, check_constraints with the proof's own challenges; ConstraintError if anything fails."""
     from .fri import prove_openings
     from .lookup import get_grand_product_challenge_set
 
@@ -782,6 +829,8 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
             aux_cap = placement.cap(aux_commitment)
             challenger.observe_cap(aux_cap)
             quotient_args["auxiliary_polys_commitment"] = aux_commitment
+        if check_constraints:                                            # prover.rs:241-256
+            _raise_on_failure(stark, trace_commitment, public_inputs, **quotient_args)
         num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
         num_ctl_helpers, num_ctl_zs = sum(num_ctl_polys), len(num_ctl_polys)
         alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
