@@ -36,6 +36,8 @@ EXPORTS = [
 ]
 # the constraint checks of include/plonky2_b200_check.h
 CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows"]
+# the plonky2 quotient on non-resident commitments of include/plonky2_b200_blocked.h
+BLOCKED_EXPORTS = ["gl_plonk_quotient_blocked"]
 
 
 class FriBatch(C.Structure):
@@ -162,6 +164,8 @@ def lib():
                                     C.c_uint32, vp]
     L.gl_plonk_quotient_shard.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32,
                                           C.c_uint32, C.c_uint32, vp]
+    L.gl_plonk_quotient_blocked.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32,
+                                            C.c_uint32, C.c_uint32, vp]
     L.gl_stark_check_rows.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, u64p, u32p, u32p]
     L.gl_plonk_check_rows.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32, u64p,
                                       u32p, u32p]

@@ -406,7 +406,7 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     from . import stark as S
 
     return _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx,
-                            S.lde_placement(config, lde_blocks), check_constraints)
+                            S.lde_placement(config.fri_config.cap_height, lde_blocks), check_constraints)
 
 
 def _prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement,

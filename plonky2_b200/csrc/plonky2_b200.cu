@@ -2657,6 +2657,23 @@ static int quotient_coeffs(gl_ctx* ctx, uint64_t* coeffs, uint32_t degree_bits, 
     }
     return flag_status(ctx, dflag, {INVERT_ZERO, QUOTIENT_FAILED});
 }
+// The quotient coset of 2^size_log points evaluated in its 2^sl parts (quotient_coset), one after another on this
+// device, as a non-resident commitment's quotient is, one part per LDE block: values(g, part) writes part g's M values
+// per challenge to `part` (at part + a*M, local natural order), and each part's values go to their points of `out`.
+// Both quotients number a part's local points alike (k_stark_place).
+static int quotient_in_parts(gl_ctx* ctx, uint32_t size_log, uint32_t sl, uint32_t n_alphas, uint64_t* out,
+                             const std::function<int(uint32_t, u64*)>& values) {
+    const uint32_t log_M = size_log - sl;
+    DevBuf part(ctx);
+    TRY(part.alloc((size_t)n_alphas << log_M));
+    for (uint32_t g = 0; g < (1u << sl); g++) {
+        TRY(values(g, part.get()));
+        k_stark_place<<<dim3((unsigned)((((size_t)1 << log_M) + 127) / 128), n_alphas), 128, 0, ctx->stream>>>(
+            part.get(), log_M, sl, bitrev32(g, sl), out);
+        CKL(ctx);
+    }
+    return GL_OK;
+}
 // What every quotient entry point runs after its checks, on its context's device: values(dflag) writes the values on
 // this device's shard of the quotient coset to `out`; then, for the whole coset, the coefficients in place
 // (quotient_coeffs), else the flags alone
@@ -2681,18 +2698,11 @@ static int stark_quotient(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const g
         if (!trace->lde_blocks)
             return stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits,
                                          trace->shard_index, trace->shard_log, out, dflag);
-        // non-resident: the coset in one part per LDE block, each part's values placed at its points of `out`
-        const uint32_t sl = trace->block_log, log_M = trace->degree_log + qd_bits - sl;
-        DevBuf part(ctx);
-        TRY(part.alloc((size_t)n_alphas << log_M));
-        for (uint32_t g = 0; g < trace->lde_blocks; g++) {
-            TRY(stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits, g,
-                                      sl, part.get(), dflag));
-            k_stark_place<<<dim3((unsigned)((((size_t)1 << log_M) + 127) / 128), n_alphas), 128, 0, ctx->stream>>>(
-                part.get(), log_M, sl, bitrev32(g, sl), out);
-            CKL(ctx);
-        }
-        return GL_OK;
+        const uint32_t sl = trace->block_log;
+        return quotient_in_parts(ctx, trace->degree_log + qd_bits, sl, n_alphas, out, [&](uint32_t g, u64* part) {
+            return stark_quotient_values(ctx, trace, aux, program, n_instr, consts, n_consts, alphas, n_alphas, qd_bits,
+                                         g, sl, part, dflag);
+        });
     });
 }
 int gl_stark_quotient(gl_ctx* ctx, gl_commit* trace, const gl_stark_instr* program, uint32_t n_instr,
@@ -2935,13 +2945,17 @@ static int vp_program_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_c
     if (n_term) *n_term = terms;
     return GL_OK;
 }
-// The checks of gl_plonk_quotient (whole = true: every LDE whole on this device) and gl_plonk_quotient_shard
-// (whole = false: the commitments are shards of the same index and count). Sets *qd_bits_out and *next_mask_out (bit c:
-// the program reads commitment c's next row).
+// How a plonky2 quotient entry point holds its commitments: every LDE whole on this device (gl_plonk_quotient), row-block
+// shards of one index and count (gl_plonk_quotient_shard), or non-resident handles of one G (gl_plonk_quotient_blocked,
+// plonky2_b200_blocked.h)
+enum class PlonkHandles { WHOLE, SHARD, BLOCKED };
+// The checks of the three plonky2 quotient entry points. Sets *qd_bits_out and *next_mask_out (bit c: the program reads
+// commitment c's next row).
 static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                                 uint32_t n_instr, uint32_t n_consts, const uint64_t* alphas, uint32_t n_alphas,
-                                uint32_t n_terms, uint32_t quotient_degree_factor, const uint64_t* out, bool whole,
-                                uint32_t* qd_bits_out, uint32_t* next_mask_out) {
+                                uint32_t n_terms, uint32_t quotient_degree_factor, const uint64_t* out,
+                                PlonkHandles kind, uint32_t* qd_bits_out, uint32_t* next_mask_out) {
+    const bool whole = kind != PlonkHandles::SHARD;
     if (!ctx || !commits || !program || !alphas || !out) return set_err(ctx, GL_ERR_BAD_ARG, "null argument");
     if (n_commits == 0 || n_commits > GL_VP_MAX_COMMITS) return set_err(ctx, GL_ERR_UNSUPPORTED, "1..%d commitments", GL_VP_MAX_COMMITS);
     if (n_instr == 0) return set_err(ctx, GL_ERR_BAD_ARG, "empty program");
@@ -2951,8 +2965,19 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
     for (uint32_t c = 0; c < n_commits; c++) {
         if (!commits[c]) return set_err(ctx, GL_ERR_BAD_ARG, "null commitment");
         if (commits[c]->ctx != ctx) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u belongs to another context", c);
+        if (kind == PlonkHandles::BLOCKED) {
+            if (commits[c]->shard_log)
+                return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is row-block shard %u of %u: the blocked quotient takes "
+                               "non-resident handles", c, commits[c]->shard_index, 1u << commits[c]->shard_log);
+            if (!commits[c]->lde_blocks)
+                return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is resident: the blocked quotient takes non-resident "
+                               "handles (gl_plonk_quotient reads a resident LDE)", c);
+            if (commits[c]->lde_blocks != commits[0]->lde_blocks)
+                return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is in %u LDE blocks, commitment 0 in %u", c,
+                               commits[c]->lde_blocks, commits[0]->lde_blocks);
+        }
         if (whole && commits[c]->shard_log) return set_err(ctx, GL_ERR_UNSUPPORTED, "quotient evaluation needs the whole LDE on this device");
-        if (commits[c]->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is not resident: the plonky2 quotient reads the LDE", c);
+        if (kind != PlonkHandles::BLOCKED && commits[c]->lde_blocks) return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is not resident: the plonky2 quotient reads the LDE", c);
         if (!whole && (commits[c]->shard_index != commits[0]->shard_index || commits[c]->shard_log != commits[0]->shard_log))
             return set_err(ctx, GL_ERR_BAD_ARG, "commitment %u is shard %u of %u, commitment 0 shard %u of %u", c,
                            commits[c]->shard_index, 1u << commits[c]->shard_log, commits[0]->shard_index,
@@ -2963,20 +2988,24 @@ static int plonk_quotient_check(gl_ctx* ctx, gl_commit* const* commits, uint32_t
     }
     TRY(quotient_shape_check(ctx, commits[0]->degree_log, commits[0]->rate_bits, commits[0]->shard_log,
                              quotient_degree_factor, GL_VP_MAX_QD, qd_bits_out));
+    // one part of the quotient coset per LDE block
+    if (commits[0]->block_log > commits[0]->degree_log + *qd_bits_out)
+        return set_err(ctx, GL_ERR_BAD_ARG, "%u LDE blocks of a quotient coset of 2^%u points", commits[0]->lde_blocks,
+                       commits[0]->degree_log + *qd_bits_out);
     // a shard whose quotient coset is not its LDE coset reads values computed from the coefficients: no salt columns
     const bool in_place = quotient_coset(commits[0], *qd_bits_out, commits[0]->shard_index, commits[0]->shard_log).local_in_place;
     return vp_program_check(ctx, commits, n_commits, program, n_instr, n_consts, n_terms, in_place, next_mask_out,
                             nullptr);
 }
-// The vanishing polynomial over Z_H on the commitments' shard of the quotient coset (the whole coset for unsharded
-// handles): M values per challenge in local natural order, at out + a*M. L_0 asked for at x = 1 sets bit 0 of dflag.
+// The vanishing polynomial over Z_H on part g of 2^sl of the quotient coset (quotient_coset; for a shard, its own part):
+// M values per challenge in local natural order, at out + a*M. L_0 asked for at x = 1 sets bit 0 of dflag.
 static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                                  uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
-                                 uint32_t n_alphas, uint32_t n_terms, uint32_t qd_bits, uint32_t next_mask, uint64_t* out,
-                                 const DevBuf& dflag) {
+                                 uint32_t n_alphas, uint32_t n_terms, uint32_t qd_bits, uint32_t next_mask, uint32_t g,
+                                 uint32_t sl, uint64_t* out, const DevBuf& dflag) {
     const gl_commit* c0 = commits[0];
     const uint32_t db = c0->degree_log;
-    const QuotientCoset q = quotient_coset(c0, qd_bits, c0->shard_index, c0->shard_log);
+    const QuotientCoset q = quotient_coset(c0, qd_bits, g, sl);
     VanishingParams p;
     std::vector<DevBuf> bufs;  // per commitment: its values on the coset, and at the next row
     for (uint32_t k = 0; k < 2 * n_commits; k++) bufs.emplace_back(ctx);
@@ -3016,36 +3045,45 @@ static int plonk_quotient_values(gl_ctx* ctx, gl_commit* const* commits, uint32_
     zero_poly_coset(db, qd_bits, p.zh, p.zh_inv);
     p.out = out;
     p.flag = (unsigned int*)dflag.get();
-    p.row0 = (size_t)c0->shard_index << q.log_M;
-    p.shard_log = c0->shard_log;
+    p.row0 = (size_t)g << q.log_M;
+    p.shard_log = sl;
     p.next_in_shard = q.next_in_shard;
     k_plonk_quotient<<<(unsigned)((q.M + 127) / 128), 128, 0, ctx->stream>>>(p);
     CKL(ctx);
     return GL_OK;
 }
-// gl_plonk_quotient (whole) and gl_plonk_quotient_shard (!whole: the values on the shard's part of the coset)
+// gl_plonk_quotient (WHOLE), gl_plonk_quotient_shard (SHARD: the values on the shard's part of the coset) and
+// gl_plonk_quotient_blocked (BLOCKED: the whole coset, one part per LDE block)
 static int plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                           uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
-                          uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out, bool whole) {
+                          uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out,
+                          PlonkHandles kind) {
     uint32_t qd_bits = 0, next_mask = 0;
     TRY(plonk_quotient_check(ctx, commits, n_commits, program, n_instr, n_consts, alphas, n_alphas, n_terms,
-                             quotient_degree_factor, out, whole, &qd_bits, &next_mask));
-    return run_quotient(ctx, whole, out, commits[0]->degree_log, n_alphas, quotient_degree_factor, [&](const DevBuf& dflag) {
+                             quotient_degree_factor, out, kind, &qd_bits, &next_mask));
+    const gl_commit* c0 = commits[0];
+    auto values = [&](uint32_t g, uint32_t sl, u64* dst, const DevBuf& dflag) {
         return plonk_quotient_values(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas,
-                                     n_terms, qd_bits, next_mask, out, dflag);
+                                     n_terms, qd_bits, next_mask, g, sl, dst, dflag);
+    };
+    return run_quotient(ctx, kind != PlonkHandles::SHARD, out, c0->degree_log, n_alphas, quotient_degree_factor,
+                        [&](const DevBuf& dflag) {
+        if (kind != PlonkHandles::BLOCKED) return values(c0->shard_index, c0->shard_log, out, dflag);
+        return quotient_in_parts(ctx, c0->degree_log + qd_bits, c0->block_log, n_alphas, out,
+                                 [&](uint32_t g, u64* part) { return values(g, c0->block_log, part, dflag); });
     });
 }
 int gl_plonk_quotient(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                       uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                       uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_coeffs) {
     return plonk_quotient(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
-                          quotient_degree_factor, out_coeffs, true);
+                          quotient_degree_factor, out_coeffs, PlonkHandles::WHOLE);
 }
 int gl_plonk_quotient_shard(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, const uint64_t* alphas,
                             uint32_t n_alphas, uint32_t n_terms, uint32_t quotient_degree_factor, uint64_t* out_values) {
     return plonk_quotient(ctx, commits, n_commits, program, n_instr, consts, n_consts, alphas, n_alphas, n_terms,
-                          quotient_degree_factor, out_values, false);
+                          quotient_degree_factor, out_values, PlonkHandles::SHARD);
 }
 
 void gl_poseidon_permute_host(uint64_t state[12]) {
@@ -3581,3 +3619,5 @@ int gl_fri_pow(gl_ctx* ctx, const uint64_t state[12], uint32_t pos, uint32_t min
 
 // gl_stark_check_rows and gl_plonk_check_rows (include/plonky2_b200_check.h), on the helpers above
 #include "gl_check_rows_host.cuh"
+// gl_plonk_quotient_blocked (include/plonky2_b200_blocked.h), on plonk_quotient above
+#include "gl_plonk_blocked_host.cuh"

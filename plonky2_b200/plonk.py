@@ -1438,10 +1438,16 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
     stay where they are; nothing but the program and the challenges crosses PCIe. On a placement of several ranks the
     commitments are this rank's row-block shards: each rank evaluates the vanishing polynomial over Z_H on its shard of
     the quotient coset (gl_plonk_quotient_shard), and every rank gets the same quotient
-    (Placement.quotient_from_shards; collective, a failure on any rank raises on every rank)."""
+    (Placement.quotient_from_shards; collective, a failure on any rank raises on every rank). On non-resident
+    commitments (lde_blocks=G, all of one G) the quotient coset is evaluated in G parts, one per LDE block
+    (gl_plonk_quotient_blocked), to the same result; resident and non-resident commitments together are a ShapeError."""
     import torch
 
     commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
+    blocks = sorted({c.lde_blocks for c in commits})
+    if len(blocks) > 1:
+        raise N.ShapeError("the quotient's commitments must be all resident or all non-resident with one lde_blocks, "
+                           "got lde_blocks %s (0: resident)" % [c.lde_blocks for c in commits])
     prog, consts, al = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, alphas, deltas)
     nc = common_data.config.num_challenges
     qdf = common_data.quotient_degree_factor
@@ -1457,8 +1463,9 @@ def compute_quotient_polys(common_data, constants_sigmas_commitment, public_inpu
         return placement.quotient_from_shards(ctx, run_shard, nc, common_data.degree_bits, qdf)
     size = (1 << common_data.degree_bits) << (qdf - 1).bit_length()
     out = torch.empty((nc, size), dtype=torch.int64, device="cuda:%d" % ctx.device)
-    N.check(N.lib().gl_plonk_quotient(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts), N.np_ptr(al), nc,
-                                      common_data.num_vanishing_terms(), qdf, N.vp(out.data_ptr())), ctx.h)
+    quotient = N.lib().gl_plonk_quotient_blocked if blocks[0] else N.lib().gl_plonk_quotient
+    N.check(quotient(ctx.h, handles, 3, prog, len(prog), N.np_ptr(consts), len(consts), N.np_ptr(al), nc,
+                     common_data.num_vanishing_terms(), qdf, N.vp(out.data_ptr())), ctx.h)
     ctx.synchronize()
     return out
 
@@ -1551,15 +1558,17 @@ def _term_labels(cd, constants_sigmas_commitment, pairs):
     return out
 
 
-def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None, shard=(0, 1)):
+def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None, shard=(0, 1),
+                          lde_blocks=None):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
     quotient_degree_factor chunks of n coefficients (trim_to_len(quotient_degree) was checked by the kernel call), all
     chunks committed with from_coeffs -- straight from the device tensor compute_quotient_polys returned. With blinding
-    the salt is drawn on the device from salt_key (PolynomialBatch._from_device). shard=(g, G): row block g of G only."""
+    the salt is drawn on the device from salt_key (PolynomialBatch._from_device). shard=(g, G): row block g of G only.
+    lde_blocks=G: a non-resident batch."""
     cfg = common_data.config
     return PolynomialBatch._from_coeff_chunks(quotient_polys, common_data.quotient_degree_factor,
                                               common_data.degree_bits, cfg.rate_bits, cfg.cap_height, ctx,
-                                              blinding=blinding, salt_key=salt_key, shard=shard)
+                                              blinding=blinding, salt_key=salt_key, shard=shard, lde_blocks=lde_blocks)
 
 
 # ------------------------------------------------------------------ prove (plonk/prover.rs:113-360)
@@ -1645,9 +1654,10 @@ def sigma_polys(config, degree_bits, pairs, num_virtual_targets=0, ctx=None):
     return out
 
 
-def commit_constants_sigmas(common_data, constant_vecs, sigmas, ctx=None, shard=(0, 1)):
+def commit_constants_sigmas(common_data, constant_vecs, sigmas, ctx=None, shard=(0, 1), lde_blocks=None):
     """The constants/sigmas commitment (circuit_builder.rs:1177-1188, never blinded): the constant columns (host), then
-    the sigma columns read in place from the device tensor sigma_polys returned. shard=(g, G): row block g of G."""
+    the sigma columns read in place from the device tensor sigma_polys returned. shard=(g, G): row block g of G.
+    lde_blocks=G: a non-resident batch."""
     cfg = common_data.config
     ctx = ctx or N.default_context()
     consts = np.ascontiguousarray(np.stack(constant_vecs), dtype=np.uint64)
@@ -1660,7 +1670,7 @@ def commit_constants_sigmas(common_data, constant_vecs, sigmas, ctx=None, shard=
                                               N.COLS_VALUES, N.MEM_DEVICE), ctx.h)
 
     return PolynomialBatch._from_device(ctx, len(consts) + cfg.num_routed_wires, common_data.degree_bits, cfg.rate_bits,
-                                        cfg.cap_height, add_columns, shard=shard)
+                                        cfg.cap_height, add_columns, shard=shard, lde_blocks=lde_blocks)
 
 
 def circuit_digest(constants_sigmas_cap, domain_separator, degree_bits):
@@ -1675,15 +1685,19 @@ def circuit_digest(constants_sigmas_cap, domain_separator, degree_bits):
 
 
 def build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets=0, luts=(), lookup_rows=(),
-                       domain_separator=(), ctx=None):
+                       domain_separator=(), ctx=None, lde_blocks=None):
     """CircuitBuilder::build_with_options(true) (plonk/circuit_builder.rs:1061-1321) from the placed circuit on one
     device: `instances` already through blind_and_pad, the copy constraints as an (E, 2) array in target_indices'
     encoding, num_virtual_targets virtual targets. Returns CircuitData(common, prover_only, verifier_only), equal to the
     reference's: the sigma polynomials and the constants/sigmas commitment are computed on the device, the digest
     from the cap. prover_only.sigmas is the host (num_routed_wires, n) array prove_with_witness reads.
-    distributed.build_circuit_data builds the same data with the commitment sharded over ranks."""
+    distributed.build_circuit_data builds the same data with the commitment sharded over ranks. lde_blocks=G: the
+    constants/sigmas commitment is non-resident (PolynomialBatch.from_values), as prove_with_witness(lde_blocks=G)
+    needs it; its digest and cap are the resident commitment's."""
+    from .stark import lde_placement
+
     return _build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets, luts, lookup_rows,
-                               domain_separator, ctx, distributed.Placement())
+                               domain_separator, ctx, lde_placement(config.cap_height, lde_blocks))
 
 
 def _build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets, luts, lookup_rows,
@@ -1884,7 +1898,7 @@ def _to_device(columns, ctx):
 
 
 def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None, *, salt_keys=None,
-                       check_constraints=False):
+                       check_constraints=False, lde_blocks=None):
     """prove_with_partition_witness (plonk/prover.rs:132-360) from the full witness matrix `wires` (num_wires, n) -- the
     generators' output -- to ProofWithPublicInputs, every array-sized step on the device: wires commitment, Z / partial
     products (+ lookup) commitment, quotient polynomials from the LDEs in place and their commitment, the openings at
@@ -1898,9 +1912,34 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
 
     check_constraints=True: after the Z / partial-product commitment, before the quotient, every term of the vanishing
     polynomial is checked on every row of H with the proof's own challenges (check_constraints), and a failure raises
-    ConstraintError naming the row and the term; the proof is unchanged."""
-    return _prove(prover_data, common_data, wires, public_inputs, ctx, distributed.Placement(), salt_keys,
-                  check_constraints)
+    ConstraintError naming the row and the term; the proof is unchanged.
+
+    lde_blocks=G: the wires, Z / partial-product (+ lookup) and quotient commitments are non-resident
+    (PolynomialBatch.from_values), for circuits whose LDEs exceed device memory; prover_data must come from
+    build_circuit_data(..., lde_blocks=G). The quotient is evaluated in G parts of its coset and every LDE block is
+    rebuilt from the coefficients where it is hashed or read; the proof is the same. Refused with ShapeError before any
+    device work: check_lde_blocks' refusals, G above the quotient coset's points, a constants/sigmas commitment that is
+    resident or of another G, and a zero-knowledge config (a non-resident batch cannot be blinded)."""
+    from .stark import lde_placement
+
+    placement = lde_placement(common_data.config.cap_height, lde_blocks)
+    if lde_blocks is not None:
+        _check_lde_blocks(prover_data, common_data, placement.lde_blocks)
+    return _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys, check_constraints)
+
+
+def _check_lde_blocks(prover_data, common_data, G):
+    """prove_with_witness's refusals of lde_blocks=G beyond check_lde_blocks'."""
+    if common_data.config.zero_knowledge:
+        raise N.ShapeError("lde_blocks= cannot prove with zero knowledge: a non-resident batch cannot be blinded")
+    size = (1 << common_data.degree_bits) << (common_data.quotient_degree_factor - 1).bit_length()
+    if G > size:
+        raise N.ShapeError("lde_blocks=%d exceeds the %d points of the quotient coset" % (G, size))
+    cs_blocks = prover_data.constants_sigmas_commitment.lde_blocks
+    if cs_blocks != G:
+        raise N.ShapeError("lde_blocks=%d, but the constants/sigmas commitment is %s: build it with "
+                           "build_circuit_data(..., lde_blocks=%d)"
+                           % (G, "non-resident in %d blocks" % cs_blocks if cs_blocks else "resident", G))
 
 
 def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys=None, check_constraints=False):

@@ -26,7 +26,7 @@ def wires_permutation_partial_products_and_zs(wires, sigmas, k_is, beta, gamma, 
 
 
 def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degree, rate_bits, cap_height, ctx=None, *,
-                               blinding=False, salt_key=None, shard=(0, 1)):
+                               blinding=False, salt_key=None, shard=(0, 1), lde_blocks=None):
     """The second commitment of prove() without leaving the device (prover.rs:220-254):
     all_wires_permutation_partial_products for every challenge pair (beta_i, gamma_i) -> Z's moved to the front
     (`[plonk_z_vecs, partial_products.concat()].concat()`) -> PolynomialBatch::from_values.
@@ -38,6 +38,7 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
     The caller's tensors may still be in production on its current torch stream: the library's work is ordered after it.
     With blinding the salt is drawn on the device from salt_key (PolynomialBatch._from_device). shard=(g, G): only row
     block g of G of the LDE and tree on this device (the columns are computed over all n rows either way).
+    lde_blocks=G: a non-resident batch, its LDE built in G row blocks where it is hashed or read.
     Returns the PolynomialBatch (num_challenges * (num_partial_products + 1) polynomials)."""
     import torch
 
@@ -67,7 +68,7 @@ def commit_zs_partial_products(wires_dev, sigmas_dev, k_is, betas, gammas, degre
                                                 N.MEM_DEVICE), ctx.h)
 
     return PolynomialBatch._from_device(ctx, nch * M, log_n, rate_bits, cap_height, add_columns, blinding=blinding,
-                                        salt_key=salt_key, shard=shard)
+                                        salt_key=salt_key, shard=shard, lde_blocks=lde_blocks)
 
 
 def compute_lookup_polys(wires, num_routed_wires, max_quotient_degree_factor, deltas, lookup_rows, ctx=None):

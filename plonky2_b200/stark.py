@@ -722,13 +722,13 @@ class ProveParams:
         self.final_poly_coeff_len, self.max_num_query_steps = final_poly_coeff_len, max_num_query_steps
 
 
-def lde_placement(config, lde_blocks):
+def lde_placement(cap_height, lde_blocks):
     """The one-device Placement of a prover's lde_blocks argument: Placement() for None (resident commitments), else
-    non-resident commitments of lde_blocks row blocks (refused as PolynomialBatch.check_lde_blocks refuses it, before
-    any device work)."""
+    non-resident commitments of lde_blocks row blocks under a cap of 2^cap_height entries (refused as
+    PolynomialBatch.check_lde_blocks refuses it, before any device work). The starky and plonky2 provers share it."""
     if lde_blocks is None:
         return D.Placement()
-    check_lde_blocks(lde_blocks, config.fri_config.cap_height)
+    check_lde_blocks(lde_blocks, cap_height)
     return D.Placement(lde_blocks=int(lde_blocks))
 
 
@@ -747,7 +747,7 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     debug builds check them (prover.rs:241-256), and a failure raises ConstraintError naming the row and the constraint;
     the proof is unchanged."""
     return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx,
-                  lde_placement(config, lde_blocks), check_constraints)
+                  lde_placement(config.fri_config.cap_height, lde_blocks), check_constraints)
 
 
 def _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement, check_constraints=False):
