@@ -531,7 +531,9 @@ int gl_fri_commit_round_sharded(gl_fri* f, uint32_t arity_bits, uint32_t shard_i
 /*   fold:   with beta from the transcript, values' = fold(values, beta) on the coset shift^arity. */
 int gl_fri_fold(gl_fri* f, const uint64_t beta[2]);
 /* batch-FRI mixing step (plonky2/src/batch_fri/prover.rs:118-132): when `f`'s codeword has been folded down to the
- * length of `other`'s (the next, lower-degree instance from its own gl_fri_begin), values <- values * beta + other's. */
+ * length of `other`'s (the next, lower-degree instance from its own gl_fri_begin), values <- values * beta + other's.
+ * Row-block sharded states (gl_fri_begin_values) mix their local blocks; both must hold the same shard of the same
+ * number of shards (else GL_ERR_BAD_ARG). */
 int gl_fri_mix(gl_fri* f, const gl_fri* other, const uint64_t beta[2]);
 /* Final polynomial after the last fold, truncated by 2^rate_bits (prover.rs:134-139):
  * *len_out coefficients (2 words each) written to out (capacity `cap_words` words). */

@@ -3547,7 +3547,10 @@ int gl_fri_mix(gl_fri* f, const gl_fri* other, const uint64_t beta[2]) {
     if (f->committed || other->committed || !f->values || !other->values)
         return set_err(ctx, GL_ERR_BAD_ARG, "both codewords must be between rounds (folded, not committed)");
     if (f->log_cur != other->log_cur) return set_err(ctx, GL_ERR_BAD_SHAPE, "codeword lengths differ: 2^%u vs 2^%u", f->log_cur, other->log_cur);
-    const size_t count = (size_t)1 << f->log_cur;
+    if (f->vshard_index != other->vshard_index || f->vshard_log != other->vshard_log)
+        return set_err(ctx, GL_ERR_BAD_ARG, "this FRI state is row-block sharded %u of %u, the other %u of %u", f->vshard_index,
+                       1u << f->vshard_log, other->vshard_index, 1u << other->vshard_log);
+    const size_t count = (size_t)1 << (f->log_cur - f->vshard_log);  // the local block of a row-block sharded codeword
     k_fri_mix<<<(unsigned)((count + 255) / 256), 256, 0, ctx->stream>>>(f->values, other->values, count,
                                                                          E2{canon(beta[0]), canon(beta[1])});
     CKL(ctx);
