@@ -34,13 +34,33 @@ extern "C" {
  * *out_reported = how many were written, min(*out_failures, max_report). GL_OK means the check ran, whether or not
  * anything failed. Refused before any launch: a NULL argument, an unfinished handle, commitments of different degree
  * or of another context, max_report > 65536 (GL_ERR_BAD_ARG / GL_ERR_BAD_SHAPE), and the quotient entry points' program
- * errors with their messages. Scratch: B x n words per commitment read, plus 8 (n + 1) bytes. */
+ * errors with their messages. Scratch: B x n words per commitment read, plus 8 (n + 1) bytes.
+ *
+ * The _part entry points check one part of H, for checks whose scratch must shrink (a non-resident proof checks its
+ * parts one after another) or be split between devices (each rank of a distributed proof checks its own part). Part g
+ * of parts = G = 2^s is the rows i = g (mod G), the coset w_n^g <w_M> with M = n / G; its values are a size-M NTT of the
+ * coefficients folded mod X^M - w_G^g, and a commitment the program reads with NEXT also gets its values on the next
+ * rows, w_n^(g+1) <w_M>. Every row-dependent quantity (the filters, GL_VP_X, GL_VP_L0) is the global row's, and rows
+ * are reported as global indices in (row, index) order. (part, parts) = (0, 1) is exactly gl_*_check_rows.
+ * Refused before any launch, after the refusals above: parts not a power of two or above n (GL_ERR_BAD_SHAPE), part >=
+ * parts (GL_ERR_BAD_ARG). Scratch: B x M words per commitment read, plus B x M more per commitment read with NEXT when
+ * G > 1, plus 8 (M + 1) bytes.
+ * Merging the G parts' reports gives the whole check's: the failures add up, and the first max_report pairs of the
+ * sorted union of the parts' pairs are the whole check's pairs. Each part's pairs are a subsequence of the global (row,
+ * index) order, so the global first max_report pairs all lie within their parts' first max_report. */
 int gl_stark_check_rows(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program, uint32_t n_instr,
                         const uint64_t* consts, uint32_t n_consts, uint32_t max_report, uint64_t* out_failures,
                         uint32_t* out_pairs, uint32_t* out_reported);
 int gl_plonk_check_rows(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
                         uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, uint32_t n_terms,
                         uint32_t max_report, uint64_t* out_failures, uint32_t* out_pairs, uint32_t* out_reported);
+int gl_stark_check_rows_part(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const gl_stark_instr* program,
+                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, uint32_t part, uint32_t parts,
+                             uint32_t max_report, uint64_t* out_failures, uint32_t* out_pairs, uint32_t* out_reported);
+int gl_plonk_check_rows_part(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_commits, const gl_vp_instr* program,
+                             uint32_t n_instr, const uint64_t* consts, uint32_t n_consts, uint32_t n_terms,
+                             uint32_t part, uint32_t parts, uint32_t max_report, uint64_t* out_failures,
+                             uint32_t* out_pairs, uint32_t* out_reported);
 
 #ifdef __cplusplus
 }

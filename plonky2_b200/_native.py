@@ -35,7 +35,7 @@ EXPORTS = [
     "gl_ctx_device_bytes",
 ]
 # the constraint checks of include/plonky2_b200_check.h
-CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows"]
+CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows", "gl_stark_check_rows_part", "gl_plonk_check_rows_part"]
 # the plonky2 quotient on non-resident commitments of include/plonky2_b200_blocked.h
 BLOCKED_EXPORTS = ["gl_plonk_quotient_blocked"]
 
@@ -81,8 +81,8 @@ MAX_REPORT = 65536
 
 
 def check_rows(fn, ctx, args, max_report):
-    """Run the check entry point `fn` (gl_stark_check_rows or gl_plonk_check_rows) with `args` between the context and
-    max_report. Returns (failures, [(row, index)])."""
+    """Run the check entry point `fn` (gl_stark_check_rows, gl_plonk_check_rows or their _part counterparts) with `args`
+    between the context and max_report. Returns (failures, [(row, index)])."""
     max_report = int(max_report)
     if not 0 <= max_report <= MAX_REPORT:
         raise ValueError("max_report must be in 0..%d" % MAX_REPORT)
@@ -90,6 +90,45 @@ def check_rows(fn, ctx, args, max_report):
     pairs = np.zeros(2 * max(max_report, 1), dtype=np.uint32)
     check(fn(ctx.h, *args, max_report, C.byref(failures), pairs.ctypes.data_as(u32p), C.byref(reported)), ctx.h)
     return failures.value, [(int(r), int(i)) for r, i in pairs[:2 * reported.value].reshape(-1, 2)]
+
+
+def check_parts(parts):
+    """parts=G of check_constraints: a positive power of two (ShapeError otherwise, before any device work)."""
+    if not isinstance(parts, (int, np.integer)) or parts < 1 or parts & (parts - 1):
+        raise ShapeError("parts=%r is not a positive power of two" % (parts,))
+    return int(parts)
+
+
+def check_rows_in_parts(fn, fn_part, ctx, args, max_report, log_n, parts=1, placement=None):
+    """The whole check of H by the entry point `fn` (gl_stark_check_rows / gl_plonk_check_rows), or by its _part
+    counterpart `fn_part` in parts of H, with `args` between the context and (part, parts) or max_report. Returns
+    (failures, [(row, index)]), the same in every case:
+    - placement of G > 1 ranks (distributed.Placement): this rank checks part shard_index of min(G, n) (a rank >= n has
+      no rows) and the ranks merge their reports (Placement.report_from_shards). Collective.
+    - parts=G on one device: the min(G, n) parts one after another, merged (merge_reports); each part's scratch is 1/G
+      of the whole check's.
+    - otherwise the whole check, one call of `fn`."""
+    parts = check_parts(parts)
+    n = 1 << int(log_n)
+    if placement is not None and placement.num_shards > 1:
+        g, G = placement.shard_index, min(placement.num_shards, n)
+
+        def run_part():
+            return check_rows(fn_part, ctx, args + (g, G), max_report) if g < G else (0, [])
+        return placement.report_from_shards(ctx, run_part, max_report)
+    if parts == 1:
+        return check_rows(fn, ctx, args, max_report)
+    G = min(parts, n)
+    return merge_reports([check_rows(fn_part, ctx, args + (g, G), max_report) for g in range(G)], max_report)
+
+
+def merge_reports(parts, max_report):
+    """The whole check's (failures, [(row, index)]) from its parts' reports, each (failures, pairs) as check_rows returns
+    it for one part of H with the same max_report: the failures add up, and the pairs are the first max_report of the
+    sorted union of the parts' pairs. This is exact: a part's pairs are a subsequence of the global (row, index) order,
+    so the global first max_report pairs all lie within their parts' first max_report."""
+    parts = list(parts)
+    return sum(int(f) for f, _ in parts), sorted(p for _, pairs in parts for p in pairs)[:int(max_report)]
 
 
 _lib = None
@@ -169,6 +208,10 @@ def lib():
     L.gl_stark_check_rows.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, u64p, u32p, u32p]
     L.gl_plonk_check_rows.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32, u64p,
                                       u32p, u32p]
+    L.gl_stark_check_rows_part.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32,
+                                           C.c_uint32, u64p, u32p, u32p]
+    L.gl_plonk_check_rows_part.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32,
+                                           C.c_uint32, C.c_uint32, u64p, u32p, u32p]
     L.gl_lookup_polys.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p, C.c_uint32, vp, C.c_int]
     L.gl_sigma_polys.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, vp, vp,
                                  C.c_int]

@@ -9,7 +9,7 @@
 // per-thread array the compiler keeps in local memory, so gates of any size fit without a new kernel.
 //
 // The same source runs on the host in tests/emu/vanishing_emu.cpp (threads as a loop) against the oracle, and the
-// row check below in tests/emu/check_rows_emu.cpp.
+// row check below in tests/emu/check_rows_emu.cpp and tests/emu/check_rows_parts_emu.cpp.
 #pragma once
 #include "../../include/plonky2_b200.h"
 #include "gl_field.cuh"
@@ -113,27 +113,38 @@ GL_HD bool vp_eval_point(const VanishingParams& p, size_t j, uint64_t* regs) {
 // (gl_plonk_check_rows): every GL_VP_TERM on its own, without alphas or Z_H. On H, L_0 is the indicator [i = 0] (its
 // closed form above divides by zero at x = 1), and only the row's own gate has a nonzero selector filter, so a failing
 // gate-constraint term at row i is a constraint of the gate placed at row i.
+// Part g of G = 2^part_log of H is the rows i = g + G*j (gl_stark_rows.cuh); the whole of H is part 0 of 1.
 struct VpRowsParams {
-    const uint64_t* val[GL_VP_MAX_COMMITS];  // commitment c's values on H, column k at val[c] + k*n, natural order
+    const uint64_t* val[GL_VP_MAX_COMMITS];  // commitment c's values on the part, column k at val[c] + k*M, local row j
     uint32_t log_n;
     const gl_vp_instr* prog;          // validated by the caller
     uint32_t n_instr;
     const uint64_t* consts;
     const uint64_t *xhi, *xlo;        // w_n^i = xhi[i >> 12] * xlo[i & 4095]
+    // Part addressing; the defaults are the whole of H, part 0 of 1. Local row j is global row i = part + (j << part_log).
+    uint32_t part_log = 0;
+    size_t part = 0;
+    // commitment c's values at the next rows i + 1, same layout (NULL: read at local row (j + 1) mod M of val[c])
+    const uint64_t* val_next[GL_VP_MAX_COMMITS] = {};
 };
 
-// The number of GL_VP_TERMs whose value is nonzero at row i. With pairs != NULL, failure m is also written as the pair
-// (row i, the term number b) at pairs[2m], pairs[2m + 1], in program order. regs: GL_VP_MAX_REGS words of scratch.
-GL_HD uint32_t vp_check_row(const VpRowsParams& p, size_t i, uint64_t* regs, uint32_t* pairs) {
-    const size_t n = (size_t)1 << p.log_n;
-    const size_t in = (i + 1) & (n - 1);
+// The number of GL_VP_TERMs whose value is nonzero at local row j of the part, global row i. With pairs != NULL,
+// failure m is also written as the pair (row i, the term number b) at pairs[2m], pairs[2m + 1], in program order.
+// regs: GL_VP_MAX_REGS words of scratch.
+GL_HD uint32_t vp_check_row(const VpRowsParams& p, size_t j, uint64_t* regs, uint32_t* pairs) {
+    const uint32_t log_M = p.log_n - p.part_log;
+    const size_t i = p.part + (j << p.part_log);
+    const size_t jn = (j + 1) & (((size_t)1 << log_M) - 1);
     uint32_t fails = 0;
     for (uint32_t k = 0; k < p.n_instr; k++) {
         const gl_vp_instr ins = p.prog[k];
         uint64_t r;
         switch (ins.op) {
-            case GL_VP_LOCAL: r = p.val[ins.a][((size_t)ins.b << p.log_n) + i]; break;
-            case GL_VP_NEXT: r = p.val[ins.a][((size_t)ins.b << p.log_n) + in]; break;
+            case GL_VP_LOCAL: r = p.val[ins.a][((size_t)ins.b << log_M) + j]; break;
+            case GL_VP_NEXT:
+                r = p.val_next[ins.a] ? p.val_next[ins.a][((size_t)ins.b << log_M) + j]
+                                      : p.val[ins.a][((size_t)ins.b << log_M) + jn];
+                break;
             case GL_VP_CONST: r = p.consts[(uint32_t)ins.a | ((uint32_t)ins.b << 16)]; break;
             case GL_VP_X: r = mul(p.xhi[i >> 12], p.xlo[i & 4095]); break;
             case GL_VP_L0: r = i == 0; break;

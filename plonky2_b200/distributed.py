@@ -70,10 +70,11 @@ class Placement:
     opens its queries with `open_many`); the two compute_quotient_polys and proof.eval_commitments pick their C entry
     point by num_shards and, with several ranks, gather the quotient with `quotient_from_shards` and the openings with
     `openings_from_shards`. Nothing else in the provers tests whether there is more than one rank. On one device both
-    keyword sets are empty, so every call a prover makes is the plain single-device call.
+    keyword sets are empty, so every call a prover makes is the plain single-device call. check_constraints runs with
+    `check_kwargs`: each rank checks its own part of H and the ranks merge their reports (`report_from_shards`).
     lde_blocks=G (one device only) makes every commitment non-resident, its LDE built in G row blocks where it is
     hashed or read (PolynomialBatch.from_values); the C entry points take such commitments directly, so step_kwargs
-    stays empty."""
+    stays empty, and check_kwargs checks H in G parts one after another."""
     shard_index: int = 0
     num_shards: int = 1
     group: object = None
@@ -103,6 +104,15 @@ class Placement:
         """The keyword arguments that run compute_quotient_polys, OpeningSet.new / StarkOpeningSet.new or
         fri.prove_openings on this placement: placement=self, or none on one device, their default."""
         return {} if self.num_shards == 1 else dict(placement=self)
+
+    @property
+    def check_kwargs(self):
+        """The keyword arguments that run stark.check_constraints / plonk.check_constraints on this placement: parts=G
+        for non-resident commitments (H checked in G parts one after another, so that the check's scratch shrinks with
+        the LDE's), placement=self with several ranks (each rank checks its own part), or none on one device."""
+        if self.num_shards > 1:
+            return dict(placement=self)
+        return dict(parts=self.lde_blocks) if self.lde_blocks else {}
 
     def cap(self, commitment):
         """The commitment's full Merkle cap: its own on one device, every rank's cap entries all-gathered otherwise."""
@@ -195,6 +205,33 @@ class Placement:
         for p in parts[1:]:
             out = _add_mod_p(out, p)
         return out
+
+    def report_from_shards(self, ctx, run_part, max_report):
+        """The whole constraint check's (failures, [(row, index)]) from the ranks' parts of H. run_part() checks this
+        rank's part through gl_*_check_rows_part and returns its (failures, pairs), at most max_report pairs. Then the
+        ranks all-gather one fixed-size record each (failures, the number of pairs, max_report packed pairs) and every
+        rank merges them in rank order (_native.merge_reports). Collective. Returns the same report on every rank. A
+        failure on one rank raises on every rank: its own exception there, NativeError elsewhere."""
+        import torch
+
+        from . import _native as N
+
+        result, failure = (0, []), None
+        try:
+            result = run_part()
+        except Exception as e:  # raised below on every rank, so that no rank waits in the all-gather for this one
+            failure = e
+        self._agree_on_failure(failure, ctx, N.NativeError, "the constraint check failed on rank %d")
+        failures, pairs = result
+        record = np.zeros(2 + max_report, dtype=np.uint64)
+        record[0], record[1] = failures, len(pairs)
+        for k, (row, index) in enumerate(pairs):
+            record[2 + k] = (int(row) << 32) | int(index)
+        t = torch.from_numpy(record.view(np.int64))
+        dev = _comm_device(self.group, ctx)
+        records = all_gather_tensor(t.to(dev) if dev else t, self.group).cpu().numpy().view(np.uint64)
+        return N.merge_reports([(int(r[0]), [(int(w) >> 32, int(w) & 0xFFFFFFFF) for w in r[2:2 + int(r[1])]])
+                                for r in records], max_report)
 
     def _agree_on_failure(self, failure, ctx, error, message):
         """Every rank learns whether any rank failed. `failure` (an exception, or None) is raised on its own rank, and
@@ -327,7 +364,8 @@ def check_prove_stark(stark, config, world):
                            "cross_table_lookup.prove_with_ctls")
 
 
-def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circuit_fri_params=None, ctx=None):
+def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circuit_fri_params=None, ctx=None,
+                check_constraints=False):
     """stark.prove on the ranks of a torch.distributed group (the default group if None): rank g commits row block g
     of the trace, auxiliary and quotient LDEs, evaluates the quotient on its shard of the quotient coset, sums block g
     of the coefficients into the openings and answers the FRI queries that land in its rows; the coefficients and the
@@ -336,12 +374,15 @@ def prove_stark(stark, config, trace, public_inputs, group=None, verifier_circui
     StarkProofWithPublicInputs, equal to what stark.prove returns on one device. The world size must be a power of two
     of at most 2^cap_height, and the Stark must not take part in cross-table lookups (ShapeError otherwise, on every
     rank). Without an initialised process group, or with one rank, this is stark.prove. ctx: this rank's context
-    (default: the current CUDA device's)."""
+    (default: the current CUDA device's).
+    check_constraints=True (equal on every rank, like every other argument): before the quotient, each rank checks
+    every constraint on its own part of H, the rows i = rank (mod world), and the ranks merge their reports; a failure
+    raises the same ConstraintError on every rank, with stark.prove's message and report."""
     from . import stark as S
 
     check_prove_stark(stark, config, _world_size(group))
     placement, ctx = _placement(group, ctx)
-    return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement)
+    return S._prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx, placement, check_constraints)
 
 
 def check_prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, world):
@@ -361,7 +402,8 @@ def check_prove_with_ctls(starks, config, traces, cross_table_lookups, public_in
             raise N.ShapeError("table %d's quotient coset has %d points, fewer than the %d ranks" % (i, size, world))
 
 
-def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, group=None, ctx=None):
+def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, group=None, ctx=None,
+                    check_constraints=False):
     """cross_table_lookup.prove_with_ctls on the ranks of a torch.distributed group (the default group if None): rank g
     commits row block g of every table's trace, auxiliary and quotient LDEs, evaluates each quotient on its shard of
     the quotient coset, sums block g of the coefficients into the openings and answers the FRI queries that land in its
@@ -369,12 +411,16 @@ def prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, 
     chained through the tables run on every rank. Collective: every rank passes the same full traces (host columns or
     torch CUDA tensors) and returns the same MultiStarkProof, field for field prove_with_ctls's on one device.
     Refusals: check_prove_with_ctls (ShapeError on every rank). Without an initialised process group, or with one rank,
-    this is prove_with_ctls. ctx: this rank's context (default: the current CUDA device's)."""
+    this is prove_with_ctls. ctx: this rank's context (default: the current CUDA device's).
+    check_constraints=True (equal on every rank): every table is checked as prove_stark checks its Stark, each rank on
+    its own part of H; a failure raises the same ConstraintError on every rank, with prove_with_ctls's message and
+    report."""
     from . import cross_table_lookup as X
 
     check_prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, _world_size(group))
     placement, ctx = _placement(group, ctx)
-    return X._prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement)
+    return X._prove_with_ctls(starks, config, traces, cross_table_lookups, public_inputs, ctx, placement,
+                              check_constraints)
 
 
 def _check_constants_sigmas_shard(prover_data, rank, world):
@@ -395,7 +441,8 @@ def check_prove_plonk(prover_data, common_data, world, rank=0):
     _check_constants_sigmas_shard(prover_data, rank, world)
 
 
-def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=None, *, salt_keys=None):
+def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=None, *, salt_keys=None,
+                check_constraints=False):
     """plonk.prove_with_witness on the ranks of a torch.distributed group (the default group if None): rank g commits
     row block g of the wires, Z / partial-product (+ lookup) and quotient LDEs, evaluates the quotient on its shard of
     the quotient coset, sums block g of the replicated coefficients into the openings and answers the FRI queries that
@@ -414,7 +461,11 @@ def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=
     prove_with_witness(..., salt_keys=salt_keys), since a keyed shard holds the unsharded commitment's salted leaves. With
     None ("fresh" keys) each rank draws its own key for its own rows, without a collective: a leaf's salt is only ever
     read by the rank that owns the leaf (Placement.open_many), so the proof is valid and hiding, but no single-device run
-    reproduces it."""
+    reproduces it.
+
+    check_constraints=True (equal on every rank): before the quotient, each rank checks every term of the vanishing
+    polynomial on its own part of H, the rows i = rank (mod world), and the ranks merge their reports; a failure raises
+    the same ConstraintError on every rank, with prove_with_witness's message and report."""
     import torch.distributed as dist
 
     from . import _native as N
@@ -434,7 +485,7 @@ def prove_plonk(prover_data, common_data, wires, public_inputs, group=None, ctx=
     # the shard check may fail on some ranks only: every rank learns the outcome before a collective could wait
     placement._agree_on_failure(refusal, ctx, N.ShapeError,
                                 "rank %d's constants/sigmas commitment is not its row-block shard")
-    return P._prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys)
+    return P._prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_keys, check_constraints)
 
 
 def build_circuit_data(config, fri_config, instances, copy_constraints, num_virtual_targets=0, luts=(), lookup_rows=(),

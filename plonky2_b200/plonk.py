@@ -1494,27 +1494,35 @@ def quotient_program(common_data, commits, public_inputs_hash, betas, gammas, al
 
 
 def check_constraints(common_data, constants_sigmas_commitment, public_inputs_hash, wires_commitment,
-                      zs_partial_products_commitment, betas, gammas, deltas=(), max_report=64):
+                      zs_partial_products_commitment, betas, gammas, deltas=(), max_report=64, parts=1, placement=None):
     """The vanishing polynomial's terms checked on every row of the trace subgroup H, each on its own
     (gl_plonk_check_rows): the program compute_quotient_polys runs, at x = w_n^i without alphas or Z_H. Takes what
     compute_quotient_polys takes but the alphas. Returns a ConstraintReport whose entries are (row, term number, label)
     for the first max_report (0..65536) failing (row, term) pairs in (row, term) order; the labels follow
-    vanishing_program's term layout, and a gate constraint's label names the gate placed at that row."""
+    vanishing_program's term layout, and a gate constraint's label names the gate placed at that row.
+    parts=G (a power of two): H is checked in min(G, n) parts one after another (gl_plonk_check_rows_part), each with
+    1/G of the whole check's scratch; the report is the same. placement: a distributed.Placement of several ranks, whose
+    commitments these are: each rank checks its own part and the ranks merge their reports (collective; every rank
+    returns the same report). The labels are attached after the merge, from local evaluations of the constants/sigmas
+    commitment, so every rank labels the same pairs alike."""
+    parts = N.check_parts(parts)
     commits = [constants_sigmas_commitment, wires_commitment, zs_partial_products_commitment]
     # no alphas: the betas stand in for quotient_program's count check, and its alpha array is not used
     prog, consts, _ = quotient_program(common_data, commits, public_inputs_hash, betas, gammas, betas, deltas)
     ctx = wires_commitment.ctx
     handles = (C.c_void_p * 3)(*[c.h for c in commits])
-    failures, pairs = N.check_rows(N.lib().gl_plonk_check_rows, ctx, (handles, 3, prog, len(prog), N.np_ptr(consts),
-                                                                      len(consts), common_data.num_vanishing_terms()),
-                                   max_report)
+    L = N.lib()
+    failures, pairs = N.check_rows_in_parts(L.gl_plonk_check_rows, L.gl_plonk_check_rows_part, ctx,
+                                            (handles, 3, prog, len(prog), N.np_ptr(consts), len(consts),
+                                             common_data.num_vanishing_terms()), max_report, common_data.degree_bits,
+                                            parts, placement)
     return N.ConstraintReport(failures, _term_labels(common_data, constants_sigmas_commitment, pairs))
 
 
-def _raise_on_failure(common_data, *commitments_and_challenges):
+def _raise_on_failure(common_data, *commitments_and_challenges, **check_kwargs):
     """prove_with_witness's check_constraints=True: ConstraintError with the first failure's row and label and the
-    total."""
-    report = check_constraints(common_data, *commitments_and_challenges)
+    total. check_kwargs: the placement's (Placement.check_kwargs)."""
+    report = check_constraints(common_data, *commitments_and_challenges, **check_kwargs)
     if report.failures:
         row, _, label = report.entries[0]
         raise N.ConstraintError("Constraint failed in the circuit at row %d: %s; %d failing (row, term) pairs in all"
@@ -1912,7 +1920,8 @@ def prove_with_witness(prover_data, common_data, wires, public_inputs, ctx=None,
 
     check_constraints=True: after the Z / partial-product commitment, before the quotient, every term of the vanishing
     polynomial is checked on every row of H with the proof's own challenges (check_constraints), and a failure raises
-    ConstraintError naming the row and the term; the proof is unchanged.
+    ConstraintError naming the row and the term; the proof is unchanged. With lde_blocks=G the check runs in G parts
+    of H, one after another, with the same message and report.
 
     lde_blocks=G: the wires, Z / partial-product (+ lookup) and quotient commitments are non-resident
     (PolynomialBatch.from_values), for circuits whose LDEs exceed device memory; prover_data must come from
@@ -1948,7 +1957,8 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
     too: the caps are all-gathered before they are observed, the quotient is evaluated shard by shard and all-gathered,
     each rank sums its block of the coefficients into the openings and the ranks add up the partial sums, and FRI routes
     the query openings between the ranks. The Z's, partial products and lookup columns and the transcript run on every
-    rank, so every rank returns the same proof."""
+    rank, so every rank returns the same proof. check_constraints runs with placement.check_kwargs: each rank checks its
+    own part of H and every rank raises the same ConstraintError."""
     from .challenger import Challenger
     from .fri import prove_openings
     from .hash import PoseidonHash
@@ -2009,7 +2019,8 @@ def _prove(prover_data, common_data, wires, public_inputs, ctx, placement, salt_
         alphas = challenger.get_n_challenges(nc)
         cs = prover_data.constants_sigmas_commitment
         if check_constraints:
-            _raise_on_failure(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas, gammas, deltas)
+            _raise_on_failure(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas, gammas, deltas,
+                              **placement.check_kwargs)
         quotient_polys = compute_quotient_polys(cd, cs, public_inputs_hash, wires_commitment, zs_commitment, betas,
                                                 gammas, alphas, deltas, **placement.step_kwargs)
         quotient_commitment = commit_quotient_polys(cd, quotient_polys, ctx,

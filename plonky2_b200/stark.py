@@ -326,20 +326,26 @@ def quotient_program(stark, public_inputs, alphas, auxiliary_polys_commitment=No
 
 
 def check_constraints(stark, trace_commitment, public_inputs, auxiliary_polys_commitment=None, lookup_challenges=None,
-                      ctl_vars=None, max_report=64):
+                      ctl_vars=None, max_report=64, parts=1, placement=None):
     """check_constraints (starky/src/prover.rs:670-820) on the device: every constraint of the Stark -- its own, then its
     lookups', then its CTLs' -- on every row of the trace subgroup H, each constraint on its own (gl_stark_check_rows).
     Takes what compute_quotient_polys takes but the alphas, on any kind of commitment (resident, non-resident, a
     row-block shard: its coefficients are replicated); a Stark of constraint degree 0 is checked too. Returns a
     ConstraintReport: the number of failing (row, constraint) pairs and the first max_report (0..65536) of them in
     (row, constraint) order as (row, EMIT ordinal, label), the label naming the Stark's own constraint by its number in
-    eval_packed_generic's order, a lookup's check by lookup and challenge, or a CTL check by its Z."""
+    eval_packed_generic's order, a lookup's check by lookup and challenge, or a CTL check by its Z.
+    parts=G (a power of two): H is checked in min(G, n) parts one after another (gl_stark_check_rows_part), each with
+    1/G of the whole check's scratch; the report is the same. placement: a distributed.Placement of several ranks, whose
+    commitments these are: each rank checks its own part and the ranks merge their reports (collective; every rank
+    returns the same report)."""
+    parts = N.check_parts(parts)
     b, consts, _ = quotient_program(stark, public_inputs, [], auxiliary_polys_commitment, lookup_challenges, ctl_vars)
     ctx = trace_commitment.ctx
     aux_h = auxiliary_polys_commitment.h if auxiliary_polys_commitment is not None else None
-    failures, pairs = N.check_rows(N.lib().gl_stark_check_rows, ctx, (trace_commitment.h, aux_h, b.program(),
-                                                                      len(b.instrs), N.np_ptr(consts), len(consts)),
-                                   max_report)
+    L = N.lib()
+    failures, pairs = N.check_rows_in_parts(L.gl_stark_check_rows, L.gl_stark_check_rows_part, ctx,
+                                            (trace_commitment.h, aux_h, b.program(), len(b.instrs), N.np_ptr(consts),
+                                             len(consts)), max_report, trace_commitment.degree_log, parts, placement)
     return N.ConstraintReport(failures, [(row, e, b.labels[e]) for row, e in pairs])
 
 
@@ -745,7 +751,8 @@ def prove(stark, config, trace, public_inputs, verifier_circuit_fri_params=None,
     of two of at most 2^cap_height and of at most the quotient coset's size (ShapeError before any device work).
     check_constraints=True: every constraint is checked on every row of H before the quotient, where the reference's
     debug builds check them (prover.rs:241-256), and a failure raises ConstraintError naming the row and the constraint;
-    the proof is unchanged."""
+    the proof is unchanged. With lde_blocks=G the check runs in G parts of H, one after another, with the same message
+    and report."""
     return _prove(stark, config, trace, public_inputs, verifier_circuit_fri_params, ctx,
                   lde_placement(config.fri_config.cap_height, lde_blocks), check_constraints)
 
@@ -789,8 +796,10 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
     the quotient is evaluated shard by shard and all-gathered, the openings are summed over each rank's block of the
     coefficients and added up, and FRI routes the query openings between the ranks.
     Everything else runs redundantly on every rank, so every rank returns the same proof. Every commitment made here is
-    released on every exit path; the trace commitment stays the caller's. check_constraints=True (one device): after
-    the auxiliary commitment, check_constraints with the proof's own challenges; ConstraintError if anything fails."""
+    released on every exit path; the trace commitment stays the caller's. check_constraints=True: after the auxiliary
+    commitment, check_constraints with the proof's own challenges, on the placement (placement.check_kwargs: part by
+    part for non-resident commitments, each rank its own part with several ranks); ConstraintError if anything fails,
+    with the same message and report on every rank."""
     from .fri import prove_openings
     from .lookup import get_grand_product_challenge_set
 
@@ -830,7 +839,7 @@ def prove_with_commitment(stark, config, trace, trace_commitment, trace_cap, ctl
             challenger.observe_cap(aux_cap)
             quotient_args["auxiliary_polys_commitment"] = aux_commitment
         if check_constraints:                                            # prover.rs:241-256
-            _raise_on_failure(stark, trace_commitment, public_inputs, **quotient_args)
+            _raise_on_failure(stark, trace_commitment, public_inputs, **quotient_args, **placement.check_kwargs)
         num_ctl_polys = ctl_data.num_ctl_helper_polys() if ctl_data is not None else []
         num_ctl_helpers, num_ctl_zs = sum(num_ctl_polys), len(num_ctl_polys)
         alphas = _bind_constraints(stark, challenger, public_inputs, config.num_challenges, degree_bits,
