@@ -9,13 +9,14 @@
 // constants runs on the FP64 pipe instead, exactly (integers < 2^53 in doubles):
 //  * full rounds: x^7 = two squarings + two multiplies per lane on the integer pipes; the last 128-bit product is
 //    handed to the FP64 pipe unreduced (sbox7_f64: 2^64 = 2^32 - 1, 2^96 = -1 turn its four words into a signed
-//    limb pair with three FP64 adds), the circulant MDS runs on two 32-bit-limb vectors through x^12 - 1 =
-//    (x^6 - 1)(x^6 + 1) (circ12_f64: 96 FP64 operations per vector) with the NEXT round's constants as seeds, and one 96-bit reduction per lane brings the state back;
+//    limb pair, built as 2^52-offset bit patterns by integer adds, one FP64 add each), the circulant MDS runs on two
+//    32-bit-limb vectors through x^12 - 1 = (x^6 - 1)(x^6 + 1) (circ12_f64: 96 FP64 operations per vector) with the
+//    NEXT round's constants as seeds, and a short 2^64 = 2^32 - 1 fold per lane brings the state back
+//    (f64_pair_to_u64);
 //  * partial rounds: lanes 1..11 never leave the FP64 pipe for all 22 rounds and two rounds are one linear step
 //    (poseidon_partial_rounds_f64) -- the reference's "fast" w_hat / v factorisation (23 64x64 products per
 //    round) is only used on the host and under -DGL_PARTIAL_FAST;
-//  * f64 -> u64 conversions are F2I on the XU pipe; the S-box's u32 words enter the FP64 pipe as 2^52-offset doubles
-//    built by register moves (sbox7_f64), the squarings are three 32x32 products each (sqr_3w).
+//  * f64 -> u64 conversions are F2I on the XU pipe; the squarings are three 32x32 products each (sqr_3w).
 // The rounds are rolled loops (one copy of each round body) so the permutation fits the instruction cache.
 // Each of these steps (single 128-bit product, FP64-resident partial rounds, two rounds per step, split circulant
 // MDS) was kept because it raised the leaf-hash permutation rate over the integer fast form; tools/variants/
@@ -30,8 +31,9 @@
 // Other measured alternatives kept as switches: GL_PARTIAL_FAST (integer rounds everywhere),
 // GL_CVT_MAGIC (2^52 magic-number conversions on the FP64 pipe everywhere), GL_SBOX_I2F (I2F in the S-box),
 // GL_SBOX_SQR4 (four-product squarings in the S-box), GL_PAIR_RENORM_F64 (the partial-round pair's former form:
-// two separate rank-one updates, renormalisation on the FP64 pipe); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT,
-// GL_REDUCE_V1. tools/variants/ ranks them with one GPU call.
+// two separate rank-one updates, renormalisation on the FP64 pipe), GL_SBOX_MOVE_HANDOVER (the S-box's FP64 limbs
+// from four register-built 2^52 + w doubles and five DADDs), GL_RET_REDUCE96 (f64_pair_to_u64 through a full 96-bit
+// reduction); gl_field.cuh: GL_SQR_3WIDE, GL_MUL_EXPLICIT, GL_REDUCE_V1. tools/variants/ ranks them with one GPU call.
 #if !defined(GL_MDS_INT) && !defined(GL_MDS_FP64)
 #define GL_MDS_FP64 1
 #endif
@@ -315,7 +317,37 @@ GL_HD double f64_from_bits(uint64_t b) {
 }
 // al + 2^32 * ah (mod p) for NON-NEGATIVE integers al, ah < 2^52 held in doubles.
 GL_HD uint64_t f64_pair_to_u64(double al, double ah) {
-#if defined(__CUDA_ARCH__) && !defined(GL_CVT_MAGIC)
+#if (defined(__CUDA_ARCH__) || defined(GL_FORCE_32BIT_PATH)) && !defined(GL_CVT_MAGIC) && !defined(GL_RET_REDUCE96)
+    // ul = al, uh = ah < 2^52 as integers (F2I.U64.F64 on the XU pipe). With uh = uh0 + 2^32*uh1 and 2^64 = 2^32 - 1:
+    //   ul + 2^32*uh = ul + uh1*(2^32 - 1) + 2^32*uh0  (mod p).
+    // b = ul + uh1*(2^32 - 1) < 2^52 + 2^52 cannot wrap (one IADD3 + IADD3.X); adding uh0 to its high word wraps at
+    // most once (carry c), and then that word is below 2^21, so the fix-up c*(2^32 - 1) cannot wrap: 8 instructions
+    // in one PTX carry chain instead of the 96-bit reduction's 10 plus the assembly of its input (written in C, ptxas
+    // turns b into an extra IMAD.WIDE and the carry test into compares and selects). The result is some u64
+    // congruent to the value, not necessarily the one reduce96 gives; the host build computes the same u64.
+#if defined(__CUDA_ARCH__)
+    const uint64_t ul = __double2ull_rz(al), uh = __double2ull_rz(ah);
+    uint32_t r0, r1;
+    asm("{\n\t.reg .u32 t, m;\n\t"
+        "add.u32 t, %3, %5;\n\t"         // ul1 + uh1 < 2^21
+        "sub.cc.u32 %0, %2, %5;\n\t"     // b = ul + uh1*(2^32 - 1): a borrow implies uh1 > 0, so t > 0
+        "subc.u32 %1, t, 0;\n\t"
+        "add.cc.u32 %1, %1, %4;\n\t"     // + 2^32*uh0, carry c
+        "addc.u32 m, 0, 0;\n\t"
+        "neg.s32 m, m;\n\t"              // m = -c: c*(2^32 - 1) = c*2^32 - c, the 2^32 part is the carry itself
+        "add.cc.u32 %0, %0, m;\n\t"
+        "addc.u32 %1, %1, 0;\n\t}"
+        : "=&r"(r0), "=&r"(r1)
+        : "r"(lo32(ul)), "r"(hi32(ul)), "r"(lo32(uh)), "r"(hi32(uh)));
+    return pack64(r0, r1);
+#else
+    const uint64_t ul = (uint64_t)al, uh = (uint64_t)ah;
+    const uint32_t uh1 = (uint32_t)(uh >> 32);
+    const uint64_t b = ul + (((uint64_t)uh1 << 32) - uh1);
+    const uint64_t s = b + (uh << 32);
+    return s < b ? s + EPS : s;
+#endif
+#elif defined(__CUDA_ARCH__) && !defined(GL_CVT_MAGIC)
     // F2I.U64.F64 (XU pipe, exact on integers) instead of the 2^52 magic add (FP64 pipe) + mask: fewer instructions
     const uint64_t ul = __double2ull_rz(al), uh = __double2ull_rz(ah);
     uint32_t r1, r2;
@@ -372,11 +404,11 @@ GL_HD uint64_t sbox7(uint64_t x) {  // sbox_monomial, poseidon.rs:689-696
 // words, 2^64 = 2^32 - 1 and 2^96 = -1 give  x^7 = (p0 - p2 - p3) + 2^32 * (p1 + p2)  (mod p), i.e. exactly a
 // (signed) limb pair (L, H), |L| < 2^33.6, 0 <= H < 2^33: three FP64 adds replace the 11-instruction integer
 // reduce128, and the MDS constants carry a bias = 0 (mod p) that makes its outputs positive again.
-// The squarings are the three-product form (sqr_3w; -DGL_SBOX_SQR4 restores mul_wide's four), and the four words
-// enter the FP64 pipe as 2^52 + w (bits 0x43300000:w, a register move each) instead of through four I2F.F64, which
-// cost about 6 issue clocks each when mixed with IMAD.WIDE (tools/pipe_mix2.cu); -DGL_SBOX_I2F restores them. The
-// 2^52 offsets cancel inside the same adds: H = (m1 - 2^53) + m2, L = (m0 - m2) - (m3 - 2^52); every intermediate
-// is an integer below 2^53 in magnitude, so all five adds are exact.
+// The squarings are the three-product form (sqr_3w; -DGL_SBOX_SQR4 restores mul_wide's four). The limbs enter the
+// FP64 pipe as bit patterns built on the integer pipes (2 IADD3-class instructions and one DADD per limb), not through
+// I2F.F64, which costs about 6 issue clocks when mixed with IMAD.WIDE (tools/pipe_mix2.cu; -DGL_SBOX_I2F), nor as four
+// 2^52 + w doubles (bits 0x43300000:w, a register move each) combined by five DADDs (-DGL_SBOX_MOVE_HANDOVER):
+// H = (m1 - 2^53) + m2, L = (m0 - m2) - (m3 - 2^52). All three forms give the same integers L and H.
 GL_HD void sbox7_f64(uint64_t x, double& L, double& H) {
 #if defined(GL_SBOX_SQR4)
     const uint64_t x2 = sqr(x);
@@ -388,7 +420,16 @@ GL_HD void sbox7_f64(uint64_t x, double& L, double& H) {
     const uint64_t x3 = mul(x, x2);
     uint64_t lo, hi;
     mul_wide(x3, x4, lo, hi);
-#if !defined(GL_SBOX_I2F)
+#if !defined(GL_SBOX_I2F) && !defined(GL_SBOX_MOVE_HANDOVER)
+    // The limbs built as bit patterns on the integer pipes: 2^52 + H and 1.5 * 2^52 + L, each a 64-bit add of
+    // 32-bit words to the pattern's constant (IADD3 + IADD3.X), then one DADD removes the offset. H = w1 + w2 < 2^33
+    // and -2^33 < L = w0 - w2 - w3 < 2^32 are the same integers as below, so the patterns hold them exactly
+    // (2^52 <= 2^52 + H < 2^53 and 2^52 <= 1.5 * 2^52 + L < 2^53: one unit in the last place is 1).
+    const uint64_t hb = 0x4330000000000000ULL + (lo >> 32) + (uint32_t)hi;
+    const uint64_t lb = 0x4338000000000000ULL + (uint32_t)lo - (uint64_t)(uint32_t)hi - (hi >> 32);
+    H = f64_from_bits(hb) - 4503599627370496.0;  // 2^52
+    L = f64_from_bits(lb) - 6755399441055744.0;  // 1.5 * 2^52
+#elif !defined(GL_SBOX_I2F)
     const double m0 = u32_magic_f64((uint32_t)lo), m1 = u32_magic_f64((uint32_t)(lo >> 32));
     const double m2 = u32_magic_f64((uint32_t)hi), m3 = u32_magic_f64((uint32_t)(hi >> 32));
     H = (m1 - 9007199254740992.0) + m2;

@@ -14,6 +14,9 @@ v mulx -DGL_MUL_EXPLICIT
 v sqr3 -DGL_SQR_3WIDE
 v sboxsqr4 -DGL_SBOX_SQR4
 v sboxi2f -DGL_SBOX_I2F
+v movehand -DGL_SBOX_MOVE_HANDOVER                     # the S-box limbs from register-built doubles and 5 DADDs
+v retr96 -DGL_RET_REDUCE96                             # the FP64 -> u64 return through a 96-bit reduction
+v prevbase -DGL_SBOX_MOVE_HANDOVER -DGL_RET_REDUCE96   # both: the full round before the integer hand-overs
 v pairf64 -DGL_PAIR_RENORM_F64                          # the partial-round pair before the ALU renormalisation
 v parent -DGL_SBOX_SQR4 -DGL_SBOX_I2F -DVB_MINB=5      # the S-box and budget before the spill-free change
 v parentb4 -DGL_SBOX_SQR4 -DGL_SBOX_I2F                # that S-box at the shipped budget
