@@ -16,13 +16,12 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.distributed as dist  # noqa: E402
 
 import plonky2_b200 as pb  # noqa: E402
 from plonky2_b200 import _native as N  # noqa: E402
 from plonky2_b200 import distributed as D  # noqa: E402
 from plonky2_b200.fri import FriProof  # noqa: E402
+from ranks import finish_rank, init_rank  # noqa: E402
 
 # (degree bits per group, polynomials per group, rate bits, cap height, arities, queries, PoW bits, two points)
 CASES = {
@@ -56,15 +55,7 @@ def _instances(lens, counts, zeta, two_points):
 def main():
     import oracle_lib
 
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
+    rank, world, _, ctx = init_rank()
     placement = D.Placement(rank, world, None)
     failures, verified = [], []
 
@@ -127,15 +118,7 @@ def main():
             if not oracle_lib.verify_batch_fri_proof([oo.cap], [counts], lens, oinsts, opened, vch.clone(), oparams,
                                                      tampered):
                 failures.append("%s: the verifier accepts a flipped initial-tree leaf" % name)
-    everyone = [None] * world
-    dist.all_gather_object(everyone, failures)
-    ok = not any(everyone)
-    if rank == 0:
-        print("MGPU_BATCH_FRI_CHECK", "OK" if ok else "FAILED", "world", world, "backend", dist.get_backend(),
-              [f for r in everyone for f in r], flush=True)
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+    finish_rank("MGPU_BATCH_FRI_CHECK", failures)
 
 
 if __name__ == "__main__":

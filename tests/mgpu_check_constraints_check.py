@@ -18,13 +18,12 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np
-import torch
-import torch.distributed as dist
 
 import plonky2_b200 as pb
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 from plonky2_b200 import stark as S
+from ranks import finish_rank, init_rank
 
 P = 0xFFFFFFFF00000001
 DIGEST = [11, 22, 33, 44]
@@ -42,7 +41,7 @@ def error_of(fn):
 
 
 def main():
-    from mgpu_stark_check import same_proof
+    import stark_twin as T
     from plonky2_b200 import cross_table_lookup as X
     from plonky2_b200 import plonk
     from plonky2_b200.fri import standard_recursion_fri_config
@@ -50,15 +49,7 @@ def main():
     from test_stark_ctl import system, system_traces
     from test_stark_lookups import RangeCheckStark
 
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
+    rank, world, _, ctx = init_rank()
     config = S.StarkConfig.standard_fast_config()
     failures = []
 
@@ -68,8 +59,8 @@ def main():
     fib_pis = [0, 1, int(fib_trace[1, -1])]
     for name, stark, trace, pis in (("fibonacci", fib, fib_trace, fib_pis),
                                     ("range_check", RangeCheckStark(), RangeCheckStark.generate_trace(10), [0])):
-        bad = same_proof(D.prove_stark(stark, config, trace, pis, ctx=ctx, check_constraints=True),
-                         D.prove_stark(stark, config, trace, pis, ctx=ctx))
+        bad = T.proof_diff(D.prove_stark(stark, config, trace, pis, ctx=ctx, check_constraints=True),
+                           D.prove_stark(stark, config, trace, pis, ctx=ctx))
         if bad:
             failures.append("prove_stark %s: %s differ with the flag" % (name, bad))
     broken = fib_trace.copy()
@@ -103,10 +94,9 @@ def main():
     traces, pis = system_traces()
     got = D.prove_with_ctls(starks, ctl_config, traces, ctls, pis, ctx=ctx, check_constraints=True)
     plain = D.prove_with_ctls(starks, ctl_config, traces, ctls, pis, ctx=ctx)
-    for k, (p, q) in enumerate(zip(got.stark_proofs, plain.stark_proofs)):
-        bad = same_proof(p, q)
-        if bad:
-            failures.append("prove_with_ctls table %d: %s differ with the flag" % (k, bad))
+    bad = T.proof_diff(got, plain)
+    if bad:
+        failures.append("prove_with_ctls: %s differ with the flag" % bad)
     real_ctl = X.cross_table_lookup_data
 
     def broken_ctl(*a, **k):                          # the looked table's last CTL Z, one value changed at row 5
@@ -150,15 +140,7 @@ def main():
         whole.close()
         mine.close()
 
-    everyone = [None] * world
-    dist.all_gather_object(everyone, failures)
-    ok = not any(everyone)
-    if rank == 0:
-        print("MGPU_CHECK_CONSTRAINTS", "OK" if ok else "FAILED", "world", world, "backend", dist.get_backend(),
-              [f for fs in everyone for f in fs])
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+    finish_rank("MGPU_CHECK_CONSTRAINTS", failures)
 
 
 if __name__ == "__main__":

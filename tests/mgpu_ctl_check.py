@@ -1,11 +1,10 @@
 """distributed.prove_with_ctls across ranks (run under torchrun, one rank per GPU): for the three-table CTL system of
 tests/test_stark_ctl.py (its CPU table also has a logUp lookup) from host columns and from torch device traces, and for
 a variant whose memory table has a logUp lookup of its own, every rank's MultiStarkProof equals
-cross_table_lookup.prove_with_ctls's on its own device, table by table -- caps, openings, ctl_zs_first, FRI bytes and
-proof-of-work witness -- and rank 0 has the restated verifier (tests/stark_twin.py) accept it. Too many ranks for
-the cap and a wrong trace count are refused on every rank. With fewer GPUs than ranks all ranks share GPU 0 and
-exchange through gloo, since NCCL refuses two ranks on one device. Launched by tests/test_stark_ctl_sharded.py, or by
-hand:
+cross_table_lookup.prove_with_ctls's on its own device, table count and every table field for field (proof_diff), and
+rank 0 has the restated verifier (tests/stark_twin.py) accept it. Too many ranks for the cap and a wrong trace count
+are refused on every rank. With fewer GPUs than ranks all ranks share GPU 0 and exchange through gloo, since NCCL
+refuses two ranks on one device. Launched by tests/test_stark_ctl_sharded.py, or by hand:
   python -m torch.distributed.run --standalone --nproc-per-node 2 tests/mgpu_ctl_check.py
 """
 import os
@@ -16,16 +15,6 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np
-
-from mgpu_stark_check import same_proof
-
-
-def same_multi_proof(a, b):
-    """Field-for-field equality of two MultiStarkProofs: the names of the fields that differ, per table."""
-    if len(a.stark_proofs) != len(b.stark_proofs):
-        return ["number of tables"]
-    return ["table %d: %s" % (i, bad) for i, (x, y) in enumerate(zip(a.stark_proofs, b.stark_proofs))
-            for bad in [same_proof(x, y)] if bad]
 
 
 def lookup_system():
@@ -55,23 +44,16 @@ def lookup_system():
 
 def main():
     import torch
-    import torch.distributed as dist
 
     import plonky2_b200 as pb
+    import stark_twin as T
     from plonky2_b200 import _native as N
     from plonky2_b200 import cross_table_lookup as X
     from plonky2_b200 import distributed as D
+    from ranks import finish_rank, init_rank
     from test_stark_ctl import system, system_traces
 
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
+    rank, _, dev, ctx = init_rank()
     failures = []
 
     starks, config, ctls = system()
@@ -85,7 +67,7 @@ def main():
     for name, st, cfg, cl, arg, pi in cases:
         got = D.prove_with_ctls(st, cfg, arg, cl, pi, ctx=ctx)
         want = X.prove_with_ctls(st, cfg, arg, cl, pi, ctx=ctx)
-        bad = same_multi_proof(got, want)
+        bad = T.proof_diff(got, want)
         if bad:
             failures.append("%s: %s differ" % (name, bad))
         proofs.append((name, st, cfg, cl, got))
@@ -100,21 +82,12 @@ def main():
             pass
     if rank == 0:
         import oracle_lib
-        import stark_twin as T
 
         for name, st, cfg, cl, proof in proofs:
             verdict = T.verify_with_ctls(oracle_lib, st, cfg, cl, proof)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
-    everyone = [None] * world
-    dist.all_gather_object(everyone, failures)
-    ok = not any(everyone)
-    if rank == 0:
-        print("MGPU_CTL_CHECK", "OK" if ok else "FAILED", "world", world, "backend", dist.get_backend(),
-              [f for r in everyone for f in r], flush=True)
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+    finish_rank("MGPU_CTL_CHECK", failures)
 
 
 if __name__ == "__main__":

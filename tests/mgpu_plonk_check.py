@@ -15,13 +15,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-import torch  # noqa: E402
-import torch.distributed as dist  # noqa: E402
 
 import plonky2_b200 as pb  # noqa: E402
 from plonky2_b200 import _native as N  # noqa: E402
 from plonky2_b200 import distributed as D  # noqa: E402
 from plonky2_b200 import plonk  # noqa: E402
+from ranks import finish_rank, init_rank  # noqa: E402
 
 DIGEST = [11, 22, 33, 44]
 
@@ -34,15 +33,7 @@ def main():
 
     from plonky2_b200.fri import standard_recursion_fri_config
 
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
+    rank, world, _, ctx = init_rank()
     failures = []
 
     zk_cfg = plonk.standard_recursion_zk_config()
@@ -104,15 +95,7 @@ def main():
             verdict = PC.oracle_verify(oracle_lib, plonk, c, DIGEST, fri_cfg, parts)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
-    everyone = [None] * world
-    dist.all_gather_object(everyone, failures)
-    ok = not any(everyone)
-    if rank == 0:
-        print("MGPU_PLONK_CHECK", "OK" if ok else "FAILED", "world", world, "backend", dist.get_backend(),
-              [f for r in everyone for f in r], flush=True)
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+    finish_rank("MGPU_PLONK_CHECK", failures)
 
 
 if __name__ == "__main__":

@@ -14,23 +14,16 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 import plonky2_b200 as pb
 from conftest import synth
 from plonky2_b200 import distributed as D
+from ranks import finish_rank, init_rank
 
 
 def main():
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+    rank, world, dev, ctx = init_rank()
     shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
     log_n, r, h = 10, 3, 4
     Bs = [7, 5, 3]
     vals = [synth(0x60 + i, (B, 1 << log_n)) for i, B in enumerate(Bs)]
@@ -46,7 +39,7 @@ def main():
                               [pb.FriBatchInfo(zeta, allp), pb.FriBatchInfo(gz, [pb.FriPolynomialInfo(2, 0)])])
     params = pb.FriParams(pb.FriConfig(r, h, 8, ("Fixed", [4, 2]), 12), False, log_n, [4, 2])
     proof = D.prove_openings_sharded(inst, commits, ch, params)
-    ok = True
+    failures = []
     # column-sharded iNTT whose stores are the coefficient all-gather + row-block sharded LDE/Merkle (PipelinedCommitter)
     import ctypes as C
     from plonky2_b200 import _native as N_
@@ -78,22 +71,23 @@ def main():
         import oracle_lib
 
         ocommits = [oracle_lib.Commit(v, r, h) for v in vals]
-        for cap, o in zip(caps, ocommits):
-            ok &= bool(np.array_equal(cap.hashes, o.cap))
+        for k, (cap, o) in enumerate(zip(caps, ocommits)):
+            if not np.array_equal(cap.hashes, o.cap):
+                failures.append("commitment %d: the gathered cap differs from the oracle's" % k)
         och = oracle_lib.Challenger()
         for o in ocommits:
             och.observe_cap(o.cap)
         obatches = [(b.point, [(p.oracle_index, p.polynomial_index) for p in b.polynomials]) for b in inst.batches]
         oproof = oracle_lib.prove_openings(ocommits, obatches, och, oracle_lib.make_params(r, h, 8, 12, [4, 2]))
-        ok &= proof.to_bytes() == oproof
+        if proof.to_bytes() != oproof:
+            failures.append("prove_openings_sharded: the proof bytes differ from the oracle's")
         want = oracle_lib.Commit(vals_c, 2, 3).cap
-        ok &= len(full_caps_c) > 0  # at least one coefficient transport must have run
-        for fc in full_caps_c:
-            ok &= bool(np.array_equal(fc.hashes, want))
-        print("MGPU_PROVE_CHECK", "OK" if ok else "FAILED", "world", world, "transports", transports, flush=True)
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+        if not full_caps_c:
+            failures.append("PipelinedCommitter: no coefficient transport ran")
+        for k, fc in enumerate(full_caps_c):
+            if not np.array_equal(fc.hashes, want):
+                failures.append("PipelinedCommitter commitment %d: the gathered cap differs from the oracle's" % k)
+    finish_rank("MGPU_PROVE_CHECK", failures, transports=transports)
 
 
 if __name__ == "__main__":

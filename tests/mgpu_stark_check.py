@@ -1,9 +1,9 @@
 """distributed.prove_stark across ranks (run under torchrun, one rank per GPU): for FibonacciStark and the lookup
 RangeCheckStark of tests/test_stark_lookups.py at 2^12 - 2^14 rows in standard_fast_config, from host columns and from
-a torch device trace, every rank's proof equals stark.prove's on its own device -- caps, openings, FRI bytes and
-proof-of-work witness -- and rank 0 has the restated verifier (tests/stark_twin.py) accept it; a verifier circuit's
-FRI shape passes through; too many ranks for the cap and a Stark with CTLs are refused on every rank. With fewer GPUs
-than ranks all ranks share GPU 0 and exchange through gloo, since NCCL refuses two ranks on one device. Launched by
+a torch device trace, every rank's proof equals stark.prove's on its own device field for field (proof_diff) and
+rank 0 has the restated verifier (tests/stark_twin.py) accept it; a verifier circuit's FRI shape passes through; too
+many ranks for the cap and a Stark with CTLs are refused on every rank. With fewer GPUs than ranks all ranks share
+GPU 0 and exchange through gloo, since NCCL refuses two ranks on one device. Launched by
 tests/test_gpu_stark_sharded.py, or by hand:
   python -m torch.distributed.run --standalone --nproc-per-node 2 tests/mgpu_stark_check.py
 """
@@ -16,32 +16,13 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 import plonky2_b200 as pb
+import stark_twin as T
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 from plonky2_b200 import stark as S
-
-
-def same_proof(a, b):
-    """Field-for-field equality of two StarkProofWithPublicInputs; the names of the fields that differ."""
-    pa, pb_ = a.proof, b.proof
-    bad = [] if a.public_inputs == b.public_inputs else ["public_inputs"]
-    for name in ("trace_cap", "quotient_polys_cap", "auxiliary_polys_cap"):
-        x, y = getattr(pa, name), getattr(pb_, name)
-        if (x is None) != (y is None) or (x is not None and not np.array_equal(x.hashes, y.hashes)):
-            bad.append(name)
-    for name in ("local_values", "next_values", "auxiliary_polys", "auxiliary_polys_next", "quotient_polys",
-                 "ctl_zs_first"):
-        x, y = getattr(pa.openings, name), getattr(pb_.openings, name)
-        if (x is None) != (y is None) or (x is not None and not np.array_equal(x, y)):
-            bad.append(name)
-    if pa.opening_proof.to_bytes() != pb_.opening_proof.to_bytes():
-        bad.append("fri_bytes")
-    if pa.opening_proof.pow_witness != pb_.opening_proof.pow_witness:
-        bad.append("pow_witness")
-    return bad
+from ranks import finish_rank, init_rank
 
 
 class _CtlStark(S.FibonacciStark):
@@ -52,15 +33,7 @@ class _CtlStark(S.FibonacciStark):
 def main():
     from test_stark_lookups import RangeCheckStark
 
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    shared = torch.cuda.device_count() < world
-    dev = torch.device("cuda", 0 if shared else local)
-    torch.cuda.set_device(dev)
-    if shared:
-        dist.init_process_group("gloo")
-    else:
-        dist.init_process_group("nccl", device_id=dev)
-    ctx = pb.default_context(dev.index)
+    rank, _, dev, ctx = init_rank()
     config = S.StarkConfig.standard_fast_config()
     failures = []
 
@@ -81,15 +54,15 @@ def main():
             torch.cuda.synchronize(dev)
         got = D.prove_stark(stark, config, arg, pi, ctx=ctx)
         want = S.prove(stark, config, arg, pi, ctx=ctx)
-        bad = same_proof(got, want)
+        bad = T.proof_diff(got, want)
         if bad:
             failures.append("%s: %s differ" % (name, bad))
         proofs.append((name, stark, got))
     # a verifier circuit's FRI shape (zero caps and coefficients observed): the same transcript on every path
     stark, trace, pi = fib(12)
     vp = config.fri_params(14)
-    bad = same_proof(D.prove_stark(stark, config, trace, pi, verifier_circuit_fri_params=vp, ctx=ctx),
-                     S.prove(stark, config, trace, pi, verifier_circuit_fri_params=vp, ctx=ctx))
+    bad = T.proof_diff(D.prove_stark(stark, config, trace, pi, verifier_circuit_fri_params=vp, ctx=ctx),
+                       S.prove(stark, config, trace, pi, verifier_circuit_fri_params=vp, ctx=ctx))
     if bad:
         failures.append("verifier_circuit_fri_params: %s differ" % bad)
     # refusals, on every rank, before any collective
@@ -102,21 +75,12 @@ def main():
             pass
     if rank == 0:
         import oracle_lib
-        import stark_twin as T
 
         for name, stark, proof in proofs:
             verdict = T.verify(oracle_lib, stark, config, proof)
             if verdict is not None:
                 failures.append("%s: the restated verifier rejects the proof: %s" % (name, verdict))
-    everyone = [None] * world
-    dist.all_gather_object(everyone, failures)
-    ok = not any(everyone)
-    if rank == 0:
-        print("MGPU_STARK_CHECK", "OK" if ok else "FAILED", "world", world, "backend", dist.get_backend(),
-              [f for r in everyone for f in r], flush=True)
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(0 if ok else 1)
+    finish_rank("MGPU_STARK_CHECK", failures)
 
 
 if __name__ == "__main__":

@@ -384,9 +384,9 @@ def fri_batches(stark, config, zeta, g, num_aux=0, ctl_first=None):
 def prove_table(oracle, stark, config, trace, trace_commit, ch, public_inputs, lookup_challenge_set=None, ctl_zs=()):
     """prove_with_commitment (prover.rs:125-484) with the oracle's pieces, on a challenger that has observed what
     precedes the table. lookup_challenge_set: the (beta, gamma) pairs whose betas the lookups use (None without lookups
-    or CTLs); ctl_zs: the table's CtlZData from cross_table_lookup_data (empty without CTLs). Returns a dict: trace_cap,
-    aux_cap, quotient_cap, local_values, next_values, auxiliary_polys, auxiliary_polys_next, ctl_zs_first,
-    quotient_polys, fri_bytes, alphas, zeta; what the table does not have is None."""
+    or CTLs); ctl_zs: the table's CtlZData from cross_table_lookup_data (empty without CTLs). Returns a dict:
+    public_inputs, trace_cap, aux_cap, quotient_cap, local_values, next_values, auxiliary_polys, auxiliary_polys_next,
+    ctl_zs_first, quotient_polys, fri_bytes, alphas, zeta; what the table does not have is None."""
     f = config.fri_config
     n = trace.shape[1]
     degree_bits = n.bit_length() - 1
@@ -421,10 +421,10 @@ def prove_table(oracle, stark, config, trace, trace_commit, ch, public_inputs, l
     arity_bits = f.fri_params(degree_bits, False).reduction_arity_bits
     params = oracle.make_params(f.rate_bits, f.cap_height, f.proof_of_work_bits, f.num_query_rounds, arity_bits)
     fri_bytes = oracle.prove_openings(commits, batches, ch, params)
-    return dict(trace_cap=trace_commit.cap, aux_cap=ac.cap if ac is not None else None,
-                quotient_cap=qc.cap if qc is not None else None, local_values=local, next_values=nxt,
-                auxiliary_polys=al, auxiliary_polys_next=an, ctl_zs_first=first, quotient_polys=quot,
-                fri_bytes=fri_bytes, alphas=alphas, zeta=zeta)
+    return dict(public_inputs=list(public_inputs), trace_cap=trace_commit.cap,
+                aux_cap=ac.cap if ac is not None else None, quotient_cap=qc.cap if qc is not None else None,
+                local_values=local, next_values=nxt, auxiliary_polys=al, auxiliary_polys_next=an, ctl_zs_first=first,
+                quotient_polys=quot, fri_bytes=fri_bytes, alphas=alphas, zeta=zeta)
 
 
 def twin_prove(oracle, stark, config, trace, public_inputs):
@@ -615,3 +615,52 @@ def verify_with_ctls(oracle, starks, config, ctls, multi_proof, extra_looking_su
             return "table %d: %s" % (i, reason)
     return verify_cross_table_lookups(ctls, [p.proof.openings.ctl_zs_first for p in proofs], config.num_challenges,
                                       extra_looking_sums)
+
+
+# ------------------------------------------------------------------------------------------- comparing proofs
+def proof_diff(a, b, path=""):
+    """Where two proof objects differ, [] when they are equal. The walk compares arrays (shape and words), integers,
+    lists, dicts and the attributes of every object, and also to_bytes() where an object has one; a list of another
+    length is reported by its two lengths and not walked."""
+    if isinstance(a, (list, tuple)) and isinstance(b, (list, tuple)):
+        if len(a) != len(b):
+            return ["%s: %d entries against %d" % (path, len(a), len(b))]
+        return [d for k, (x, y) in enumerate(zip(a, b)) for d in proof_diff(x, y, "%s[%d]" % (path, k))]
+    if isinstance(a, dict) and isinstance(b, dict):
+        if sorted(a) != sorted(b):
+            return ["%s: keys %s against %s" % (path, sorted(a), sorted(b))]
+        return [d for k in sorted(a) for d in proof_diff(a[k], b[k], "%s.%s" % (path, k))]
+    if isinstance(a, np.ndarray) or isinstance(b, np.ndarray):
+        same = isinstance(a, np.ndarray) and isinstance(b, np.ndarray) and a.shape == b.shape and np.array_equal(a, b)
+        return [] if same else [path]
+    if isinstance(a, (int, np.integer)) and isinstance(b, (int, np.integer)):
+        return [] if int(a) == int(b) else [path]
+    if hasattr(a, "__dict__") and type(a) is type(b):
+        diff = proof_diff(vars(a), vars(b), path)
+        if hasattr(a, "to_bytes") and a.to_bytes() != b.to_bytes():
+            diff.append(path + ".to_bytes()")
+        return diff
+    return [] if type(a) is type(b) and a == b else [path]
+
+
+def assert_matches_twin(proof, twin):
+    """The product's proof equals the twin's: a StarkProofWithPublicInputs against twin_prove's dict, a MultiStarkProof
+    against twin_prove_with_ctls' (the table count first, then table by table). Public inputs, the trace, auxiliary and
+    quotient caps, every opening including ctl_zs_first, and the FRI bytes (which end with the proof-of-work witness);
+    what the twin does not have (None) the proof must not have either."""
+    if "tables" in twin:
+        assert len(proof.stark_proofs) == len(twin["tables"]), "number of tables"
+        for p, t in zip(proof.stark_proofs, twin["tables"]):
+            assert_matches_twin(p, t)
+        return
+    p, o = proof.proof, proof.proof.openings
+    assert proof.public_inputs == twin["public_inputs"], "public_inputs"
+    for key, got in (("trace_cap", p.trace_cap), ("aux_cap", p.auxiliary_polys_cap),
+                     ("quotient_cap", p.quotient_polys_cap)):
+        want = twin[key]
+        assert (got is None) == (want is None) and (want is None or np.array_equal(got.hashes, want)), key
+    for key in ("local_values", "next_values", "auxiliary_polys", "auxiliary_polys_next", "quotient_polys",
+                "ctl_zs_first"):
+        got, want = getattr(o, key), twin[key]
+        assert (got is None) == (want is None) and (want is None or np.array_equal(got, want)), key
+    assert p.opening_proof.to_bytes() == twin["fri_bytes"], "fri_bytes"

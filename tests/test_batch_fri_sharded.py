@@ -14,9 +14,6 @@ oracle. batch_prove_openings_sharded without a process group gives batch_prove_o
 GPUs) torchrun ranks (tests/mgpu_batch_fri_check.py) every rank's bytes equal the single-device proof's and the oracle's,
 and the restated batch verifier accepts them."""
 import os
-import signal
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -25,8 +22,8 @@ from conftest import synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 from plonky2_b200.fri import FriConfig, FriParams
+from ranks import run_ranks
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GS = [1, 2, 4, 8]
 
 # (degree bits per group, polynomials per group, rate bits, cap height, from_coeffs)
@@ -215,16 +212,4 @@ def test_batch_prove_openings_sharded_on_one_rank_is_batch_prove_openings(pb):
 def test_batch_prove_openings_across_ranks(pb):
     """torchrun, one rank per GPU (2, or 4 with four GPUs; the ranks share GPU 0 over gloo on a single-GPU machine):
     every rank's bytes equal the single-device proof's and the oracle's, and the restated verifier accepts them."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_batch_fri_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)   # torchrun and every rank it started
-        out, err = p.communicate()
-        pytest.fail("mgpu_batch_fri_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_BATCH_FRI_CHECK OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_batch_fri_check.py", "MGPU_BATCH_FRI_CHECK OK", timeout=900)

@@ -25,6 +25,7 @@ import numpy as np
 import pytest
 
 import gl_numpy as G
+import stark_twin as T
 from conftest import P, synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import field as E
@@ -453,16 +454,6 @@ def _assert_log(log):
         assert [(r, e) for r, e, _ in report.entries] == want, name
 
 
-def _same_stark_proof(p, q):
-    for x, y in ((p.proof.trace_cap, q.proof.trace_cap), (p.proof.quotient_polys_cap, q.proof.quotient_polys_cap),
-                 (p.proof.auxiliary_polys_cap, q.proof.auxiliary_polys_cap)):
-        assert (x is None) == (y is None) and (x is None or np.array_equal(x.hashes, y.hashes))
-    for a, b in zip(p.proof.openings.to_fri_openings(), q.proof.openings.to_fri_openings()):
-        assert np.array_equal(a, b)
-    assert p.proof.opening_proof.to_bytes() == q.proof.opening_proof.to_bytes()
-    assert p.public_inputs == q.public_inputs
-
-
 def _stark_cases():
     from test_stark_lookups import PermutationStark, RangeCheckStark, RangeCheckStark4
 
@@ -490,7 +481,7 @@ def test_holding_starks_report_nothing_and_prove_the_same(pb, oracle, monkeypatc
     checked = S.prove(stark, config, trace, pis, check_constraints=True)
     assert len(log) == 1 and log[0][1].failures == 0
     _assert_log(log)
-    _same_stark_proof(checked, S.prove(stark, config, trace, pis))
+    assert not T.proof_diff(checked, S.prove(stark, config, trace, pis))
     assert len(log) == 1
 
 
@@ -549,8 +540,7 @@ def test_ctl_system_holds_and_a_broken_value_is_named(pb, oracle, monkeypatch):
     assert all(r.failures == 0 for _, r, _ in log)
     _assert_log(log)
     plain = X.prove_with_ctls(starks, config, traces, ctls, pis)
-    for p, q in zip(checked.stark_proofs, plain.stark_proofs):
-        _same_stark_proof(p, q)
+    assert not T.proof_diff(checked, plain)
     log.clear()
     real = X.cross_table_lookup_data
 

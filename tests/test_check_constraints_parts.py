@@ -14,18 +14,18 @@ page-locked and non-canonical host inputs, the scratch high-water mark, and the 
 (tests/mgpu_check_constraints_check.py): the three distributed provers with check_constraints=True."""
 import ctypes as C
 import os
-import signal
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 import gl_numpy as G
+import stark_twin as T
 from conftest import P, synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import field as E
 from plonky2_b200 import stark as S
+from ranks import run_ranks
 from test_check_constraints import _sparse, _stark_cases, _twin, stark_expected, vp_expected
 from test_gpu_programs import STARK_MAX_INSTR, VP_CONSTS, VP_MAX_COMMITS, stark_program, vp_program
 
@@ -431,14 +431,12 @@ def _record_parts(monkeypatch, module):
 def test_blocked_starks_hold_and_prove_the_same(pb, monkeypatch, name):
     """FibonacciStark, RangeCheckStark (lookups) and PermutationStark (degree 0): with lde_blocks=4 and 16 the check
     runs in that many parts, finds nothing, and the proof equals the proof without the flag."""
-    from test_check_constraints import _same_stark_proof
-
     stark, trace, pis = _stark_cases()[name]
     config = S.StarkConfig.standard_fast_config()
     seen = _record_parts(monkeypatch, S)
     for G_ in (4, 16):
         checked = S.prove(stark, config, trace, pis, lde_blocks=G_, check_constraints=True)
-        _same_stark_proof(checked, S.prove(stark, config, trace, pis, lde_blocks=G_))
+        assert not T.proof_diff(checked, S.prove(stark, config, trace, pis, lde_blocks=G_))
     assert seen == [4, 16]
 
 
@@ -474,7 +472,6 @@ def test_blocked_ctl_system_holds_and_a_broken_value_raises_the_resident_error(p
     """The CTL system of test_stark_ctl.py with lde_blocks=4: every table checked in 4 parts, the proofs equal those
     without the flag; one CTL Z value changed raises the resident run's ConstraintError."""
     from plonky2_b200 import cross_table_lookup as X
-    from test_check_constraints import _same_stark_proof
     from test_stark_ctl import system, system_traces
 
     starks, config, ctls = system()
@@ -482,8 +479,7 @@ def test_blocked_ctl_system_holds_and_a_broken_value_raises_the_resident_error(p
     seen = _record_parts(monkeypatch, S)
     checked = X.prove_with_ctls(starks, config, traces, ctls, pis, lde_blocks=4, check_constraints=True)
     assert seen == [4, 4, 4]
-    for p, q in zip(checked.stark_proofs, X.prove_with_ctls(starks, config, traces, ctls, pis, lde_blocks=4).stark_proofs):
-        _same_stark_proof(p, q)
+    assert not T.proof_diff(checked, X.prove_with_ctls(starks, config, traces, ctls, pis, lde_blocks=4))
     real = X.cross_table_lookup_data
 
     def broken(*a, **k):                              # the looked table's last CTL Z, one value changed at row 5
@@ -555,16 +551,4 @@ def test_distributed_provers_check_constraints(pb):
     """torchrun, one rank per GPU (2, or 4 with four GPUs; the ranks share GPU 0 over gloo on a single-GPU machine):
     distributed.prove_stark, prove_with_ctls and prove_plonk with check_constraints=True (tests/mgpu_check_constraints_
     check.py)."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_check_constraints_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)   # torchrun and every rank it started
-        out, err = p.communicate()
-        pytest.fail("mgpu_check_constraints_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_CHECK_CONSTRAINTS OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_check_constraints_check.py", "MGPU_CHECK_CONSTRAINTS OK", timeout=900)

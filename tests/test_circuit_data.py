@@ -15,9 +15,7 @@ zero knowledge) only under the built digest; distributed.build_circuit_data + pr
 (tests/mgpu_circuit_data_check.py)."""
 import ctypes as C
 import os
-import signal
 import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -28,6 +26,7 @@ import plonk_circuits as PC
 from conftest import synth
 from plonk_circuits import instances_of, pairs_from_sigmas
 from plonky2_b200 import _native as N
+from ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -473,16 +472,4 @@ def test_zero_knowledge_build_then_prove_is_accepted(pb):
 def test_build_across_ranks(pb):
     """torchrun: distributed.build_circuit_data + prove_plonk give every rank the bytes of the single-device build +
     prove_with_witness (tests/mgpu_circuit_data_check.py)."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_circuit_data_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=1200)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)
-        out, err = p.communicate()
-        pytest.fail("mgpu_circuit_data_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_CIRCUIT_DATA_CHECK OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_circuit_data_check.py", "MGPU_CIRCUIT_DATA_CHECK OK", timeout=1200)

@@ -1,68 +1,35 @@
 """world_size-2 gloo test of the multi-GPU host logic (plonky2_b200/distributed.py) on CPU: each rank
 owns one row block of the commitment (its leaves/cap come from the oracle here, since there is no GPU),
 the ranks all-gather their cap entries, and every rank must end with the single-device cap."""
-import os
-import socket
-import sys
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from ranks import spawn_ranks
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch.distributed as dist
-
+def _worker(rank, world):
     import oracle_lib
     from conftest import synth
     from plonky2_b200 import distributed as D
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        B, log_n, r, h = 5, 6, 2, 3
-        N = 1 << (log_n + r)
-        vals = synth(0x55, (B, 1 << log_n))
-        full = oracle_lib.Commit(vals, r, h, nthreads=1)
-        lo, hi = D.shard_row_range(N, rank, world)
-        clo, chi = D.shard_cap_range(h, rank, world)
-        # this rank's shard: its own leaves reduced to its own cap entries
-        _, local_cap = oracle_lib.merkle_build(full.leaves[lo:hi], h - int(np.log2(world)), nthreads=1)
-        assert np.array_equal(local_cap, full.cap[clo:chi])
-        cap = D.gather_cap(local_cap)
-        ok = np.array_equal(cap.hashes, full.cap)
-        owner = D.owner_of_leaf(N - 1, N, world)
-        q.put((rank, bool(ok), owner))
-    finally:
-        dist.destroy_process_group()
+    B, log_n, r, h = 5, 6, 2, 3
+    N = 1 << (log_n + r)
+    vals = synth(0x55, (B, 1 << log_n))
+    full = oracle_lib.Commit(vals, r, h, nthreads=1)
+    lo, hi = D.shard_row_range(N, rank, world)
+    clo, chi = D.shard_cap_range(h, rank, world)
+    # this rank's shard: its own leaves reduced to its own cap entries
+    _, local_cap = oracle_lib.merkle_build(full.leaves[lo:hi], h - int(np.log2(world)), nthreads=1)
+    assert np.array_equal(local_cap, full.cap[clo:chi])
+    cap = D.gather_cap(local_cap)
+    ok = np.array_equal(cap.hashes, full.cap)
+    owner = D.owner_of_leaf(N - 1, N, world)
+    return rank, bool(ok), owner
 
 
 def test_cap_all_gather_two_ranks():
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=180) for _ in procs]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    assert sorted(r[0] for r in res) == [0, 1]
+    res = spawn_ranks(_worker, 2, timeout=180)
+    assert [r[0] for r in res] == [0, 1]
     assert all(r[1] for r in res)
     assert all(r[2] == (1, 127) for r in res)
 
@@ -111,40 +78,22 @@ def test_placement_open_many_routing_single_process():
     assert one.cap(FakeBatch()) is FakeBatch.merkle_tree.cap
 
 
-def _failure_worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    import torch.distributed as dist
-
+def _failure_worker(rank, world):
     from plonky2_b200 import distributed as D
 
-    dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%d" % port, rank=rank, world_size=world)
+    placement = D.Placement(rank, world, None)
     try:
-        placement = D.Placement(rank, world, None)
-        try:
-            placement._agree_on_failure(ValueError("rank 1's own failure") if rank == 1 else None, None, RuntimeError,
-                                        "rank %d failed")
-            q.put((rank, None))
-        except Exception as e:
-            q.put((rank, "%s: %s" % (type(e).__name__, e)))
-    finally:
-        dist.destroy_process_group()
+        placement._agree_on_failure(ValueError("rank 1's own failure") if rank == 1 else None, None, RuntimeError,
+                                    "rank %d failed")
+        return rank, None
+    except Exception as e:
+        return rank, "%s: %s" % (type(e).__name__, e)
 
 
 def test_failure_on_one_rank_raises_on_every_rank():
     """Placement._agree_on_failure over two gloo ranks, rank 1 failing: rank 1 raises its own exception, rank 0 the
     agreed error naming rank 1, and neither waits for the other."""
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_failure_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted(q.get(timeout=180) for _ in procs)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = spawn_ranks(_failure_worker, 2, timeout=180)
     assert res == [(0, "RuntimeError: rank 1 failed"), (1, "ValueError: rank 1's own failure")]
 
 
@@ -167,7 +116,7 @@ def test_chunk_layout_tiles_the_coefficient_matrix(num_polys, world):
     assert covered == list(range(num_polys))
 
 
-def _pipeline_worker(rank, world, port, num_polys, n, out):
+def _pipeline_worker(rank, world, num_polys, n):
     """The committer's data movement with gloo standing in for NCCL: per chunk every rank contributes its (pc, n)
     block and the all-gather lands in rows [c*Wc, (c+1)*Wc) of the matrix."""
     import torch
@@ -175,32 +124,18 @@ def _pipeline_worker(rank, world, port, num_polys, n, out):
 
     from plonky2_b200 import distributed as D
 
-    dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%d" % port, rank=rank, world_size=world)
-    try:
-        pc, wc, K = D.chunk_layout(num_polys, world)
-        full = torch.arange(num_polys * n, dtype=torch.int64).reshape(num_polys, n) * 3 + 1  # "coefficients" of column b
-        coeffs = torch.zeros((K * wc, n), dtype=torch.int64)
-        for c in range(K):
-            b0, cnt = D.chunk_columns(num_polys, rank, world, c)
-            stage = torch.full((pc, n), -1, dtype=torch.int64)
-            stage[:cnt] = full[b0:b0 + cnt]
-            dist.all_gather_into_tensor(coeffs[c * wc:(c + 1) * wc], stage)
-        out.put((rank, bool(torch.equal(coeffs[:num_polys], full))))
-    finally:
-        dist.destroy_process_group()
+    pc, wc, K = D.chunk_layout(num_polys, world)
+    full = torch.arange(num_polys * n, dtype=torch.int64).reshape(num_polys, n) * 3 + 1  # "coefficients" of column b
+    coeffs = torch.zeros((K * wc, n), dtype=torch.int64)
+    for c in range(K):
+        b0, cnt = D.chunk_columns(num_polys, rank, world, c)
+        stage = torch.full((pc, n), -1, dtype=torch.int64)
+        stage[:cnt] = full[b0:b0 + cnt]
+        dist.all_gather_into_tensor(coeffs[c * wc:(c + 1) * wc], stage)
+    return rank, bool(torch.equal(coeffs[:num_polys], full))
 
 
 @pytest.mark.parametrize("num_polys", [11, 70])
 def test_pipelined_gather_layout_two_ranks_gloo(num_polys):
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    port = 29500 + (os.getpid() % 1000) + num_polys
-    procs = [ctx.Process(target=_pipeline_worker, args=(r, 2, port, num_polys, 8, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted(out.get(timeout=120) for _ in procs)
-    for p in procs:
-        p.join(timeout=60)
+    res = spawn_ranks(_pipeline_worker, 2, (num_polys, 8), timeout=120)
     assert res == [(0, True), (1, True)]

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from conftest import EDGE, P, synth
+from ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -460,16 +461,7 @@ def test_cfg5_shape_reduced_starky_commit_and_fri(pb, oracle):
 def test_multi_gpu_sharded_prove(pb):
     """torchrun, one rank per GPU (two ranks sharing GPU 0 over gloo on a single-GPU machine): cap all-gather,
     routed openings, pipelined column-sharded commitments; rank 0 checks caps and proof bytes against the CPU oracle."""
-    import subprocess
-    import sys
-    import torch
-
-    n = torch.cuda.device_count()
-    world = 2 if n < 4 else 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_prove_check.py")]  # --standalone: a free local port per run
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "MGPU_PROVE_CHECK OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    run_ranks("mgpu_prove_check.py", "MGPU_PROVE_CHECK OK", timeout=600)
 
 
 @pytest.mark.parametrize("B,log_n", [(3, 0), (5, 1), (7, 9), (20, 13), (4, 16)])

@@ -14,9 +14,6 @@ torchrun ranks (tests/mgpu_stark_check.py) every rank's proof equals stark.prove
 it."""
 import ctypes as C
 import os
-import signal
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -25,8 +22,8 @@ from conftest import synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 from plonky2_b200 import stark as S
+from ranks import run_ranks
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CAP_HEIGHT = 4
 
 
@@ -261,33 +258,15 @@ def test_entry_point_errors(pb):
 @pytest.mark.gpu
 def test_prove_stark_on_one_rank_is_prove(pb):
     """Without a process group prove_stark is stark.prove: the same proof, field for field."""
+    import stark_twin as T
     from test_stark_prove import _fib_case
-    from test_stark_prove import _same_as_twin as same_lookup_free
 
     stark, config, trace, pi = _fib_case(10)
-    want = S.prove(stark, config, trace, pi)
-    got = D.prove_stark(stark, config, trace, pi)
-    twin = {"trace_cap": want.proof.trace_cap.hashes, "quotient_cap": want.proof.quotient_polys_cap.hashes,
-            "quotient_polys": want.proof.openings.quotient_polys, "local_values": want.proof.openings.local_values,
-            "next_values": want.proof.openings.next_values, "fri_bytes": want.proof.opening_proof.to_bytes()}
-    same_lookup_free(got, twin)
-    assert got.proof.opening_proof.pow_witness == want.proof.opening_proof.pow_witness
+    assert not T.proof_diff(D.prove_stark(stark, config, trace, pi), S.prove(stark, config, trace, pi))
 
 
 @pytest.mark.gpu
 def test_prove_stark_across_ranks(pb):
     """torchrun, one rank per GPU (2, or 4 with four GPUs; the ranks share GPU 0 over gloo on a single-GPU machine):
     every rank's proof equals stark.prove's and the restated verifiers accept it; refusals on every rank."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_stark_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)   # torchrun and every rank it started
-        out, err = p.communicate()
-        pytest.fail("mgpu_stark_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_STARK_CHECK OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_stark_check.py", "MGPU_STARK_CHECK OK", timeout=900)

@@ -173,8 +173,6 @@ def test_prove_reads_a_trace_still_in_production(pb, oracle, layout):
     call run under `with torch.cuda.stream(s)`, so ordering after the default stream would not be enough."""
     import torch
 
-    from test_stark_prove import _same_as_twin
-
     from plonky2_b200 import stark as S
 
     stark, config, _, _ = _fib()
@@ -198,7 +196,7 @@ def test_prove_reads_a_trace_still_in_production(pb, oracle, layout):
         _delayed((buf, src))
         del decoy
         proof = S.prove(stark, config, arg, pi)
-    _same_as_twin(proof, T.twin_prove(oracle, stark, config, trace, pi))
+    T.assert_matches_twin(proof, T.twin_prove(oracle, stark, config, trace, pi))
     assert T.verify(oracle, stark, config, proof) is None
 
 
@@ -206,7 +204,7 @@ def test_prove_reads_a_trace_still_in_production(pb, oracle, layout):
 def test_prove_with_lookups_reads_a_trace_still_in_production(pb, oracle):
     """stark.prove for the logUp range-check STARK from a torch trace still being copied: _device_trace, the lookup
     helper columns and the auxiliary commitment all read it; equal to the CPU twin and accepted."""
-    from test_stark_lookups import RangeCheckStark, _range_case, _same_as_twin
+    from test_stark_lookups import RangeCheckStark, _range_case
 
     from plonky2_b200 import stark as S
 
@@ -214,7 +212,7 @@ def test_prove_with_lookups_reads_a_trace_still_in_production(pb, oracle):
     src, buf = _dev(trace), _dev(RangeCheckStark.generate_trace(10, seed=8))
     _delayed((buf, src))
     proof = S.prove(stark, config, buf, pi)
-    _same_as_twin(proof, T.twin_prove(oracle, stark, config, trace, pi))
+    T.assert_matches_twin(proof, T.twin_prove(oracle, stark, config, trace, pi))
     assert T.verify(oracle, stark, config, proof) is None
 
 
@@ -222,7 +220,7 @@ def test_prove_with_lookups_reads_a_trace_still_in_production(pb, oracle):
 def test_prove_with_ctls_reads_traces_still_in_production(pb, oracle):
     """prove_with_ctls with every table's trace a torch tensor still being copied: equal to the multi-STARK twin and
     accepted by the restated verifier."""
-    from test_stark_ctl import _same_as_twin, system, system_traces
+    from test_stark_ctl import system, system_traces
 
     from plonky2_b200 import cross_table_lookup as X
 
@@ -232,7 +230,7 @@ def test_prove_with_ctls_reads_traces_still_in_production(pb, oracle):
     srcs, bufs = [_dev(t) for t in traces], [_dev(t) for t in stale]
     _delayed(*zip(bufs, srcs))
     mp = X.prove_with_ctls(starks, config, bufs, ctls, pis)
-    _same_as_twin(mp, T.twin_prove_with_ctls(oracle, starks, config, traces, ctls, pis))
+    T.assert_matches_twin(mp, T.twin_prove_with_ctls(oracle, starks, config, traces, ctls, pis))
     assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
 
 

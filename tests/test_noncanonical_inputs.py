@@ -1096,31 +1096,27 @@ def test_narrow_leaves(pb, oracle, W):
 
 
 # ------------------------------------------------------------------------------------------------ GPU: whole proofs
-def _fields(obj, path="", seen=None):
-    """[(path, value)] of every field of a proof object, arrays and caps as tuples of ints, recursively."""
+def _proof_arrays(obj, path=""):
+    """[(path, array)] of every array in a proof object, recursively."""
     if isinstance(obj, np.ndarray):
-        return [(path, tuple(int(v) for v in obj.reshape(-1)) + obj.shape)]
-    if isinstance(obj, (int, np.integer)):
-        return [(path, int(obj))]
-    if obj is None or isinstance(obj, (str, bytes, float, bool)):
         return [(path, obj)]
     if isinstance(obj, (list, tuple)):
-        return [f for k, v in enumerate(obj) for f in _fields(v, "%s[%d]" % (path, k))]
+        return [f for k, v in enumerate(obj) for f in _proof_arrays(v, "%s[%d]" % (path, k))]
     if isinstance(obj, dict):
-        return [f for k in sorted(obj) for f in _fields(obj[k], "%s.%s" % (path, k))]
+        return [f for k in sorted(obj) for f in _proof_arrays(obj[k], "%s.%s" % (path, k))]
     if hasattr(obj, "__dict__"):
-        return [f for k in sorted(vars(obj)) for f in _fields(vars(obj)[k], "%s.%s" % (path, k))]
-    return [(path, repr(obj))]
+        return _proof_arrays(vars(obj), path)
+    return []
 
 
 def same_proofs(what, a, b):
-    fa, fb = _fields(a), _fields(b)
-    assert [p for p, _ in fa] == [p for p, _ in fb], what
-    for (p, x), (_, y) in zip(fa, fb):
-        assert x == y, "%s: the proof from non-canonical inputs differs at %s" % (what, p)
-    for p, x in fa:
-        if isinstance(x, tuple):
-            assert all(v < P for v in x), "%s: %s holds a non-canonical word" % (what, p)
+    """a and b equal field for field, and every word of them canonical."""
+    import stark_twin as T
+
+    diff = T.proof_diff(a, b)
+    assert not diff, "%s: the proof from non-canonical inputs differs at %s" % (what, diff)
+    for p, x in _proof_arrays(a):
+        assert all(int(v) < P for v in x.reshape(-1)), "%s: %s holds a non-canonical word" % (what, p)
 
 
 @pytest.mark.gpu

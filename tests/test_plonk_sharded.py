@@ -18,9 +18,7 @@ rank gives prove_with_witness's bytes, with and without zero knowledge; on 2 (4 
 (tests/mgpu_plonk_check.py) every rank's bytes equal prove_with_witness's and the restated verifiers accept them."""
 import ctypes as C
 import os
-import signal
 import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -31,6 +29,7 @@ from conftest import synth
 from plonk_circuits import LOOKUP_64, RECURSION_5
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
+from ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COSET_SHIFT = 14293326489335486720   # F::coset_shift()
@@ -394,16 +393,4 @@ def test_prove_plonk_on_one_rank_is_prove_with_witness(pb, zk):
 def test_prove_plonk_across_ranks(pb):
     """torchrun, one rank per GPU (2, or 4 with four GPUs; the ranks share GPU 0 over gloo on a single-GPU machine):
     every rank's bytes equal prove_with_witness's and the restated verifiers accept them; refusals on every rank."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_plonk_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=1200)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)   # torchrun and every rank it started
-        out, err = p.communicate()
-        pytest.fail("mgpu_plonk_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_PLONK_CHECK OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_plonk_check.py", "MGPU_PLONK_CHECK OK", timeout=1200)

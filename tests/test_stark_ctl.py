@@ -391,18 +391,6 @@ def _restated_table_aux(trace, groups, pairs, degree):
     return np.stack(helpers + zs)
 
 
-def _same_as_twin(mp, twin):
-    for p, t in zip(mp.stark_proofs, twin["tables"]):
-        o = p.proof.openings
-        assert np.array_equal(p.proof.trace_cap.hashes, t["trace_cap"])
-        assert np.array_equal(p.proof.auxiliary_polys_cap.hashes, t["aux_cap"])
-        assert np.array_equal(p.proof.quotient_polys_cap.hashes, t["quotient_cap"])
-        for k in ("local_values", "next_values", "auxiliary_polys", "auxiliary_polys_next", "quotient_polys",
-                  "ctl_zs_first"):
-            assert np.array_equal(getattr(o, k), t[k]), k
-        assert p.proof.opening_proof.to_bytes() == t["fri_bytes"]
-
-
 def _tampered(mp, what):
     bad = copy.deepcopy(mp)
     if what == "ctl_zs_first":
@@ -421,7 +409,7 @@ def test_prove_with_ctls_host_logic_with_cpu_backends(oracle, monkeypatch):
     calls = []
     logs, ctx = _cpu_ctl_backends(monkeypatch, oracle, calls)
     mp = X.prove_with_ctls(starks, config, traces, ctls, pis, ctx=ctx)
-    _same_as_twin(mp, twin)
+    T.assert_matches_twin(mp, twin)
     assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
     betas = [b for b, _ in twin["ctl_challenges"]]
     assert [c for c in calls if isinstance(c, tuple) and c[0] == "helpers"] == [("helpers", betas)]
@@ -569,7 +557,7 @@ def test_prove_with_ctls_on_device_equals_cpu_twin(pb, oracle, source):
     torch.cuda.synchronize()
     mp = X.prove_with_ctls(starks, config, arg, ctls, pis)
     twin = T.twin_prove_with_ctls(oracle, starks, config, traces, ctls, pis)
-    _same_as_twin(mp, twin)
+    T.assert_matches_twin(mp, twin)
     assert T.verify_with_ctls(oracle, starks, config, ctls, mp) is None
     ch = mp.get_challenges(starks, config, ctls)
     assert [(c.beta, c.gamma) for c in ch["ctl_challenges"]] == twin["ctl_challenges"]

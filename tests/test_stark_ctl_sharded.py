@@ -11,10 +11,6 @@ GL_ERR_BAD_ARG. prove_with_ctls on one rank is cross_table_lookup.prove_with_ctl
 ranks (tests/mgpu_ctl_check.py) every rank's proof equals it and the restated verifier accepts it."""
 import ctypes as C
 import os
-import signal
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -23,8 +19,7 @@ from conftest import P, synth
 from plonky2_b200 import _native as N
 from plonky2_b200 import distributed as D
 from plonky2_b200 import stark as S
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from ranks import run_ranks, spawn_ranks
 
 
 def block(n, g, G):
@@ -61,14 +56,6 @@ def test_add_mod_p_wraps_like_the_field():
     assert [int(v) for v in got] == [(int(x) + int(y)) % P for x, y in zip(a, b)]
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _partials(rank, total):
     """Rank `rank`'s stand-in partial sums: canonical values, with p - 1 in places so that the sum wraps."""
     v = synth(0x0C20 + rank, (total, 2))
@@ -87,11 +74,7 @@ class _Ctx:
     h, device = None, 0
 
 
-def _openings_worker(rank, world, port, fail_rank, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch.distributed as dist
-
+def _openings_worker(rank, world, fail_rank):
     from plonky2_b200 import _native as N_
     from plonky2_b200 import distributed as D_
     from plonky2_b200 import proof as proof_mod
@@ -111,36 +94,20 @@ def _openings_worker(rank, world, port, fail_rank, q):
             return b"stub failure"
 
     N_._lib = Stub()
-    dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%d" % port, rank=rank, world_size=world)
+    batches = [_Batch(3), _Batch(4)]
+    for b in batches:
+        b.ctx = _Ctx()
+    placement = D_.Placement(rank, world, None)
     try:
-        batches = [_Batch(3), _Batch(4)]
-        for b in batches:
-            b.ctx = _Ctx()
-        placement = D_.Placement(rank, world, None)
-        try:
-            res = proof_mod.eval_commitments([(batches[0], (5, 7)), (batches[1], (5, 7)), (batches[1], (1, 0))],
-                                             placement=placement)
-            q.put((rank, "ok", [r.tolist() for r in res]))
-        except Exception as e:
-            q.put((rank, "%s: %s" % (type(e).__name__, e), None))
-    finally:
-        dist.destroy_process_group()
+        res = proof_mod.eval_commitments([(batches[0], (5, 7)), (batches[1], (5, 7)), (batches[1], (1, 0))],
+                                         placement=placement)
+        return rank, "ok", [r.tolist() for r in res]
+    except Exception as e:
+        return rank, "%s: %s" % (type(e).__name__, e), None
 
 
 def _run_two_ranks(fail_rank):
-    import torch.multiprocessing as mp
-
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_openings_worker, args=(r, 2, port, fail_rank, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted(q.get(timeout=180) for _ in procs)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    return res
+    return spawn_ranks(_openings_worker, 2, (fail_rank,), timeout=180)
 
 
 def test_openings_gathered_and_summed_on_two_ranks():
@@ -313,14 +280,14 @@ def test_bad_shard_arguments(pb):
 def test_prove_with_ctls_on_one_rank_is_prove_with_ctls(pb):
     """Without a process group distributed.prove_with_ctls is cross_table_lookup.prove_with_ctls: the same proof, table
     by table, field for field."""
-    from mgpu_ctl_check import same_multi_proof
+    import stark_twin as T
     from plonky2_b200 import cross_table_lookup as X
     from test_stark_ctl import system, system_traces
 
     starks, config, ctls = system()
     traces, pis = system_traces()
-    assert same_multi_proof(D.prove_with_ctls(starks, config, traces, ctls, pis),
-                            X.prove_with_ctls(starks, config, traces, ctls, pis)) == []
+    assert not T.proof_diff(D.prove_with_ctls(starks, config, traces, ctls, pis),
+                            X.prove_with_ctls(starks, config, traces, ctls, pis))
 
 
 @pytest.mark.gpu
@@ -328,16 +295,4 @@ def test_prove_with_ctls_across_ranks(pb):
     """torchrun, one rank per GPU (2, or 4 with four GPUs; the ranks share GPU 0 over gloo on a single-GPU machine):
     every rank's MultiStarkProof equals prove_with_ctls's and the restated verifier accepts it; refusals on every
     rank."""
-    import torch
-
-    world = 4 if torch.cuda.device_count() >= 4 else 2
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--standalone", "--nproc-per-node", str(world),
-           os.path.join(ROOT, "tests", "mgpu_ctl_check.py")]
-    p = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
-    try:
-        out, err = p.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(p.pid, signal.SIGKILL)   # torchrun and every rank it started
-        out, err = p.communicate()
-        pytest.fail("mgpu_ctl_check.py timed out: " + out[-2000:] + err[-2000:])
-    assert p.returncode == 0 and "MGPU_CTL_CHECK OK" in out, out[-3000:] + err[-3000:]
+    run_ranks("mgpu_ctl_check.py", "MGPU_CTL_CHECK OK", timeout=900)

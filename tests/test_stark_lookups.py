@@ -370,22 +370,6 @@ def _cpu_lookup_backends(monkeypatch, oracle, stark, calls):
     return logs, ctx
 
 
-def _same_as_twin(proof, twin):
-    p, o = proof.proof, proof.proof.openings
-    assert np.array_equal(p.trace_cap.hashes, twin["trace_cap"])
-    assert np.array_equal(p.auxiliary_polys_cap.hashes, twin["aux_cap"])
-    assert (p.quotient_polys_cap is None) == (twin["quotient_cap"] is None)
-    if twin["quotient_cap"] is not None:
-        assert np.array_equal(p.quotient_polys_cap.hashes, twin["quotient_cap"])
-        assert np.array_equal(o.quotient_polys, twin["quotient_polys"])
-    else:
-        assert o.quotient_polys is None
-    assert np.array_equal(o.local_values, twin["local_values"]) and np.array_equal(o.next_values, twin["next_values"])
-    assert np.array_equal(o.auxiliary_polys, twin["auxiliary_polys"])
-    assert np.array_equal(o.auxiliary_polys_next, twin["auxiliary_polys_next"])
-    assert p.opening_proof.to_bytes() == twin["fri_bytes"]
-
-
 def _tampered(proof, what):
     bad = copy.deepcopy(proof)
     if what == "aux_opening":
@@ -407,7 +391,7 @@ def test_prove_host_logic_with_cpu_backends(oracle, monkeypatch, case):
     logs, ctx = _cpu_lookup_backends(monkeypatch, oracle, stark, calls)
     proof = S.prove(stark, config, trace, pi, ctx=ctx)
     assert calls.count("close") == (2 if case == "permutation" else 3)
-    _same_as_twin(proof, twin)
+    T.assert_matches_twin(proof, twin)
     assert T.verify(oracle, stark, config, proof) is None
     nq = stark.num_quotient_polys(config)
     assert len(proof.proof.opening_proof.query_round_proofs[0].initial_trees_proof.evals_proofs) == (3 if nq else 2)
@@ -525,7 +509,7 @@ def test_prove_on_device_equals_cpu_twin(pb, oracle, name, source):
         torch.cuda.synchronize()
     proof = S.prove(stark, config, arg, pi)
     twin = T.twin_prove(oracle, stark, config, trace, pi)
-    _same_as_twin(proof, twin)
+    T.assert_matches_twin(proof, twin)
     assert T.verify(oracle, stark, config, proof) is None
     ch = proof.get_challenges(stark, config)
     assert [(c.beta, c.gamma) for c in ch["lookup_challenge_set"]] == twin["lookup_challenge_set"]
@@ -651,11 +635,10 @@ def test_lookup_free_proof_through_the_same_prove(pb, oracle):
     """FibonacciStark through the prove that now also handles lookups: the proof test_stark_prove.py checks, no
     auxiliary cap or openings."""
     from test_stark_prove import _fib_case
-    from test_stark_prove import _same_as_twin as same_lookup_free
 
     stark, config, trace, pi = _fib_case(10)
     proof = S.prove(stark, config, trace, pi)
-    same_lookup_free(proof, T.twin_prove(oracle, stark, config, trace, pi))
+    T.assert_matches_twin(proof, T.twin_prove(oracle, stark, config, trace, pi))
     assert proof.proof.auxiliary_polys_cap is None
     assert proof.proof.openings.auxiliary_polys is None and proof.proof.openings.auxiliary_polys_next is None
     assert T.verify(oracle, stark, config, proof) is None

@@ -205,19 +205,6 @@ def _cpu_backends(monkeypatch, oracle, stark, calls):
     return logs, Ctx()
 
 
-def _same_as_twin(proof, twin):
-    p, o = proof.proof, proof.proof.openings
-    assert np.array_equal(p.trace_cap.hashes, twin["trace_cap"])
-    assert (p.quotient_polys_cap is None) == (twin["quotient_cap"] is None)
-    if twin["quotient_cap"] is not None:
-        assert np.array_equal(p.quotient_polys_cap.hashes, twin["quotient_cap"])
-        assert np.array_equal(o.quotient_polys, twin["quotient_polys"])
-    else:
-        assert o.quotient_polys is None
-    assert np.array_equal(o.local_values, twin["local_values"]) and np.array_equal(o.next_values, twin["next_values"])
-    assert p.opening_proof.to_bytes() == twin["fri_bytes"]
-
-
 def _tampered(proof, what):
     import copy
 
@@ -256,7 +243,7 @@ def test_prove_host_logic_with_cpu_backends(oracle, monkeypatch, case):
     proof = S.prove(stark, config, trace, pi, ctx=ctx)
     assert calls.count("close") == (2 if case == "fibonacci" else 1)
     assert [c for c in calls if isinstance(c, tuple) and c[0] == "prove_openings"] == [("prove_openings", None, None)]
-    _same_as_twin(proof, twin)
+    T.assert_matches_twin(proof, twin)
     assert T.verify(oracle, stark, config, proof) is None
     assert len(proof.proof.opening_proof.query_round_proofs[0].initial_trees_proof.evals_proofs) == (
         2 if case == "fibonacci" else 1)
@@ -380,7 +367,7 @@ def test_prove_on_device_equals_cpu_twin(pb, oracle, name):
     host_trace = trace.cpu().numpy().view(np.uint64) if hasattr(trace, "data_ptr") else trace
     proof = S.prove(stark, config, trace, pi)
     twin = T.twin_prove(oracle, stark, config, host_trace, pi)
-    _same_as_twin(proof, twin)
+    T.assert_matches_twin(proof, twin)
     fp = proof.proof.opening_proof
     degree_bits = host_trace.shape[1].bit_length() - 1
     widths = [stark.COLUMNS] + ([stark.num_quotient_polys(config)] if stark.constraint_degree() else [])
