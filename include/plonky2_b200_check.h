@@ -62,6 +62,51 @@ int gl_plonk_check_rows_part(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_
                              uint32_t part, uint32_t parts, uint32_t max_report, uint64_t* out_failures,
                              uint32_t* out_pairs, uint32_t* out_reported);
 
+/* plonky2's two global arguments checked on a witness, before any commitment: what the reference's witness generation
+ * stops at (iop/witness.rs:358, "Partition containing {target} was set twice with different values"; gates/lookup.rs:
+ * 208-220, "Incorrect input value provided") and what set_lookup_wires (plonk/prover.rs:50-108) writes. They read the
+ * witness, the sigma columns and the circuit's shape only: no commitment, no challenge. Witness column c (and sigma
+ * column c) is at wires + c * stride, on the host or the device (GL_MEM_HOST / GL_MEM_DEVICE); non-canonical values
+ * compare canonically. Outputs (HOST memory) as for gl_plonk_check_rows: *out_failures, the first max_report pairs in
+ * (first word, second word) order in out_pairs, *out_reported. Refused before any launch: a NULL argument, max_report >
+ * 65536 (GL_ERR_BAD_ARG), a stride below n (GL_ERR_BAD_SHAPE).
+ *   gl_plonk_check_copies   routed wire i = row * num_routed_wires + col (row < n = 2^log_n) has the identity value
+ *                           k_is[col] * w_n^row and the sigma value sigmas[col][row]; sigma(i) is the routed wire whose
+ *                           identity value is i's sigma value. The pair (i, sigma(i)) fails when the two wires' values
+ *                           differ. Sigmas that are not a permutation of the identity values are GL_ERR_BAD_ARG (corrupt
+ *                           prover data), found on the device; n * num_routed_wires must be below 2^31 - 1
+ *                           (GL_ERR_BAD_SHAPE). Both (u64 value, u32 index) lists are radix-sorted: scratch 36 bytes
+ *                           per routed wire at the peak (the sorted identity list and both buffers of the sigma list's
+ *                           sort), 32 while host sigmas are staged, 20 in the end (sigma, host wires, the report).
+ *   gl_plonk_check_lookups  table k of n_luts has the entries luts[2e], luts[2e + 1] (input, output) for e in
+ *                           [lut_offsets[k], lut_offsets[k + 1]) and the rows lookup_rows[3k .. 3k + 2] = (last_lu,
+ *                           last_lut, first_lut): LookupGate rows [last_lu, last_lut), num_routed_wires / 2 slots of
+ *                           (input, output) in wires (2s, 2s + 1); LookupTableGate rows [last_lut, first_lut],
+ *                           num_routed_wires / 3 slots of (input, output, multiplicity) in wires (3s, 3s + 1, 3s + 2).
+ *                           Entry e is placed at row first_lut - e / (num_routed_wires / 3), slot e % that; slots past
+ *                           the LUT hold entry 0 with multiplicity 0. A looking slot counts for the entry the reference's
+ *                           input -> index map gives its input (a later entry of one input wins); the run of slots at
+ *                           the end of row last_lut - 1 that all hold entry 0 is the reference's padding and counts for
+ *                           entry 0. The witness alone cannot tell that padding from real lookups of entry 0 which end
+ *                           the row; the two differ only when entry 0's input appears again later in the LUT (the
+ *                           reference counts a real lookup for the later entry), and then an honest witness gets two L3
+ *                           failures, for entry 0 and that later entry: a known false positive of a witness-only
+ *                           check. A failure is the pair (row, 4 * slot + kind): kind 1 (L1) a looking pair that is
+ *                           not an entry of the table; 2 (L2) a table slot that does not hold the entry placed there;
+ *                           3 (L3) a table slot whose multiplicity is not its entry's count. out_counts (may be NULL):
+ *                           every entry's count, laid out as luts. Refused: an empty LUT, rows out of order or past n,
+ *                           two tables' rows overlapping (GL_ERR_BAD_ARG), a LUT longer than its table rows hold
+ *                           (GL_ERR_BAD_SHAPE). Scratch: the wire columns read (host input), 256 KiB per table, 8 (n + 1)
+ *                           bytes. */
+int gl_plonk_check_copies(gl_ctx* ctx, const uint64_t* wires, size_t wires_stride, int wires_mem,
+                          const uint64_t* sigmas, size_t sigmas_stride, int sigmas_mem, const uint64_t* k_is,
+                          uint32_t log_n, uint32_t num_routed_wires, uint32_t max_report, uint64_t* out_failures,
+                          uint32_t* out_pairs, uint32_t* out_reported);
+int gl_plonk_check_lookups(gl_ctx* ctx, const uint64_t* wires, size_t col_stride, int mem, uint32_t log_n,
+                           uint32_t num_routed_wires, const uint16_t* luts, const uint32_t* lut_offsets,
+                           const uint32_t* lookup_rows, uint32_t n_luts, uint32_t* out_counts, uint32_t max_report,
+                           uint64_t* out_failures, uint32_t* out_pairs, uint32_t* out_reported);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,7 +35,8 @@ EXPORTS = [
     "gl_ctx_device_bytes",
 ]
 # the constraint checks of include/plonky2_b200_check.h
-CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows", "gl_stark_check_rows_part", "gl_plonk_check_rows_part"]
+CHECK_EXPORTS = ["gl_stark_check_rows", "gl_plonk_check_rows", "gl_stark_check_rows_part", "gl_plonk_check_rows_part",
+                 "gl_plonk_check_copies", "gl_plonk_check_lookups"]
 # the plonky2 quotient on non-resident commitments of include/plonky2_b200_blocked.h
 BLOCKED_EXPORTS = ["gl_plonk_quotient_blocked"]
 
@@ -212,6 +213,10 @@ def lib():
                                            C.c_uint32, u64p, u32p, u32p]
     L.gl_plonk_check_rows_part.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32,
                                            C.c_uint32, C.c_uint32, u64p, u32p, u32p]
+    L.gl_plonk_check_copies.argtypes = [vp, vp, C.c_size_t, C.c_int, vp, C.c_size_t, C.c_int, vp, C.c_uint32,
+                                        C.c_uint32, C.c_uint32, u64p, u32p, u32p]
+    L.gl_plonk_check_lookups.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, vp, u32p, u32p,
+                                         C.c_uint32, u32p, C.c_uint32, u64p, u32p, u32p]
     L.gl_lookup_polys.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p, C.c_uint32, vp, C.c_int]
     L.gl_sigma_polys.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, vp, vp,
                                  C.c_int]

@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libplonky2_b200.so")
 SOURCES = ["plonky2_b200.cu"]
 DEPS = ["plonky2_b200.cu", "gl_chacha.cuh", "gl_ctl.cuh", "gl_field.cuh", "gl_lazy.cuh", "gl_logup.cuh", "gl_ntt.cuh", "gl_ntt_host.cuh", "gl_poseidon.cuh", "gl_poseidon_constants.h",
-        "gl_sigma.cuh", "gl_stark_rows.cuh", "gl_vanishing.cuh", "gl_check_rows_host.cuh", "gl_plonk_blocked_host.cuh",
+        "gl_sigma.cuh", "gl_stark_rows.cuh", "gl_vanishing.cuh", "gl_check_rows_host.cuh", "gl_check_args.cuh", "gl_check_args_host.cuh", "gl_plonk_blocked_host.cuh",
         os.path.join("..", "..", "include", "plonky2_b200.h"), os.path.join("..", "..", "include", "plonky2_b200_check.h"),
         os.path.join("..", "..", "include", "plonky2_b200_blocked.h"),
         os.path.abspath(__file__)]  # this file holds NVCC_FLAGS (the target architecture among them)

@@ -88,15 +88,16 @@ static int part_views(gl_ctx* ctx, const gl_commit* c, uint32_t g, uint32_t s, b
     *next = nbuf.get();
     return GL_OK;
 }
-// The two passes of a row kernel over the 2^log_rows rows of a part, and the report: the total number of failing (row,
-// index) pairs and the first max_report of them in (row, index) order. launch(off, pairs) queues one pass (check_rows
-// kernels). Every row whose offset is below max_report writes all of its failures (at most max_per_row, in program
-// order), so after sorting the slots the one row that straddles max_report is complete; unwritten slots are all ones
-// and sort last. The rows of a part are in global order, so its pairs are too.
-static int check_rows_report(gl_ctx* ctx, uint32_t log_rows, uint32_t max_per_row, uint32_t max_report,
+// The two passes of a row kernel over the `rows` rows of a part (or the routed wires of gl_plonk_check_copies, one per
+// row), and the report: the total number of failing (row, index) pairs and the first max_report of them in (row, index)
+// order. launch(off, pairs) queues one pass (check_rows kernels). Every row whose offset is below max_report writes
+// all of its failures (at most max_per_row, in program order), so after sorting the slots the one row that straddles
+// max_report is complete; unwritten slots are all ones and sort last. The rows of a part are in global order, so its
+// pairs are too.
+static int check_rows_report(gl_ctx* ctx, size_t rows, uint32_t max_per_row, uint32_t max_report,
                              const std::function<int(u64*, uint32_t*)>& launch, uint64_t* out_failures,
                              uint32_t* out_pairs, uint32_t* out_reported) {
-    const size_t n = (size_t)1 << log_rows;
+    const size_t n = rows;
     DevBuf off(ctx), temp(ctx), dpairs(ctx);
     TRY(off.alloc(n + 1));  // per-row counts, then their exclusive scan; off[n] = the total
     CK(ctx, cudaMemsetAsync(off.get() + n, 0, 8, ctx->stream));
@@ -160,7 +161,7 @@ static int stark_check_rows(gl_ctx* ctx, gl_commit* trace, gl_commit* aux, const
     p.part_log = s;
     p.part = part;
     const size_t M = (size_t)1 << (log_n - s);
-    return check_rows_report(ctx, log_n - s, n_emit, max_report, [&](u64* off, uint32_t* pairs) {
+    return check_rows_report(ctx, M, n_emit, max_report, [&](u64* off, uint32_t* pairs) {
         k_stark_check_rows<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p, off, pairs, max_report);
         CKL(ctx);
         return GL_OK;
@@ -224,7 +225,7 @@ static int plonk_check_rows(gl_ctx* ctx, gl_commit* const* commits, uint32_t n_c
     p.part_log = s;
     p.part = part;
     const size_t M = n >> s;
-    return check_rows_report(ctx, log_n - s, n_term, max_report, [&](u64* off, uint32_t* pairs) {
+    return check_rows_report(ctx, M, n_term, max_report, [&](u64* off, uint32_t* pairs) {
         k_plonk_check_rows<<<(unsigned)((M + 127) / 128), 128, 0, ctx->stream>>>(p, off, pairs, max_report);
         CKL(ctx);
         return GL_OK;

@@ -3622,5 +3622,7 @@ int gl_fri_pow(gl_ctx* ctx, const uint64_t state[12], uint32_t pos, uint32_t min
 
 // gl_stark_check_rows and gl_plonk_check_rows (include/plonky2_b200_check.h), on the helpers above
 #include "gl_check_rows_host.cuh"
+// gl_plonk_check_copies and gl_plonk_check_lookups (include/plonky2_b200_check.h), on check_rows_report
+#include "gl_check_args_host.cuh"
 // gl_plonk_quotient_blocked (include/plonky2_b200_blocked.h), on plonk_quotient above
 #include "gl_plonk_blocked_host.cuh"

@@ -1566,6 +1566,154 @@ def _term_labels(cd, constants_sigmas_commitment, pairs):
     return out
 
 
+def _witness_columns(a, rows, n, what):
+    """(the array read, its column stride, memory kind, CUDA device or None) of a (rows, n) array whose column c is row c: a
+    host array (read in place when it is already C-contiguous uint64, page-locked or not) or a CUDA tensor of 8-byte
+    words with unit stride along n. ShapeError for any other shape."""
+    try:
+        import torch
+    except ImportError:  # pragma: no cover
+        torch = None
+    if torch is not None and isinstance(a, torch.Tensor) and a.is_cuda:
+        if tuple(a.shape) != (rows, n) or a.element_size() != 8 or (n > 1 and a.stride(1) != 1):
+            raise N.ShapeError("%s must be a (%d, %d) tensor of 8-byte words, unit stride along the rows"
+                               % (what, rows, n))
+        return a, a.stride(0), N.MEM_DEVICE, a.device.index or 0
+    h = np.ascontiguousarray(a, dtype=np.uint64)
+    if h.shape != (rows, n):
+        raise N.ShapeError("%s must be (%d, %d), got %s" % (what, rows, n, h.shape))
+    return h, n, N.MEM_HOST, None
+
+
+def _witness_values(w, rows, cols):
+    """Canonical values of the witness entries (rows[i], cols[i]) of a host array or CUDA tensor, as ints."""
+    rows, cols = np.asarray(rows, dtype=np.int64), np.asarray(cols, dtype=np.int64)
+    if isinstance(w, np.ndarray):
+        v = w[rows, cols] if len(rows) else np.zeros(0, dtype=np.uint64)
+    else:
+        import torch
+
+        idx = torch.from_numpy(rows).to(w.device), torch.from_numpy(cols).to(w.device)
+        v = w[idx].cpu().numpy().view(np.uint64) if len(rows) else np.zeros(0, dtype=np.uint64)
+    return [int(x) % F.ORDER for x in v.tolist()]
+
+
+def _check_max_report(max_report):
+    if not isinstance(max_report, (int, np.integer)) or not 0 <= max_report <= N.MAX_REPORT:
+        raise N.ShapeError("max_report=%r must be in 0..%d" % (max_report, N.MAX_REPORT))
+    return int(max_report)
+
+
+def check_copy_constraints(prover_data, common_data, wires, max_report=64, ctx=None):
+    """The copy constraints checked on a witness (gl_plonk_check_copies), before any commitment: routed wire (row, col)
+    must carry the value of wire sigma(row, col), the routed wire whose identity value k_is[col'] * w_n^row' is its
+    sigma value prover_data.sigmas[col][row]; the cycles of sigma include the joins through virtual targets. This is
+    what the reference's witness generation stops at ("Partition containing {target} was set twice with different
+    values"). wires: the (num_wires, n) witness, a host array or a CUDA tensor (the library's stream is ordered after
+    torch's current stream first). Returns a ConstraintReport of every failing wire and the first max_report of them in
+    (row, col) order, as (row, col, "wire (row, col) = v is copied to wire (row', col') = v'"). ShapeError before any
+    device work for a witness or sigmas of the wrong shape or max_report outside 0..65536; NativeError for sigmas that
+    are not a permutation of the identity values."""
+    cd, cfg = common_data, common_data.config
+    n, nr = 1 << cd.degree_bits, cfg.num_routed_wires
+    max_report = _check_max_report(max_report)
+    w, ws, wmem, wdev = _witness_columns(wires, cfg.num_wires, n, "the witness")
+    sg, ss, smem, sdev = _witness_columns(prover_data.sigmas, nr, n, "prover_data.sigmas")
+    k_is = np.array(cd.k_is, dtype=np.uint64)
+    if len(k_is) != nr:
+        raise N.ShapeError("common_data.k_is has %d shifts for %d routed wires" % (len(k_is), nr))
+    ctx = ctx or N.default_context(wdev if wdev is not None else sdev or 0)
+    if N.MEM_DEVICE in (wmem, smem):
+        ctx.after_caller()
+    wp, sp = [N.vp(a.data_ptr()) if m == N.MEM_DEVICE else N.np_ptr(a) for a, m in ((w, wmem), (sg, smem))]
+    failures, reported = C.c_uint64(), C.c_uint32()
+    pairs = np.zeros(2 * max(max_report, 1), dtype=np.uint32)
+    N.check(N.lib().gl_plonk_check_copies(ctx.h, wp, ws, wmem, sp, ss, smem, N.np_ptr(k_is), cd.degree_bits, nr,
+                                          max_report, C.byref(failures), pairs.ctypes.data_as(N.u32p),
+                                          C.byref(reported)), ctx.h)
+    pairs = pairs[:2 * reported.value].reshape(-1, 2).astype(np.int64)
+    i, j = pairs[:, 0], pairs[:, 1]
+    vi = _witness_values(w, i % nr, i // nr)
+    vj = _witness_values(w, j % nr, j // nr)
+    entries = [(int(a // nr), int(a % nr), "wire (%d, %d) = %d is copied to wire (%d, %d) = %d"
+                % (a // nr, a % nr, va, b // nr, b % nr, vb)) for a, b, va, vb in zip(i, j, vi, vj)]
+    return N.ConstraintReport(failures.value, entries)
+
+
+LOOKUP_KINDS = {1: "L1", 2: "L2", 3: "L3"}
+
+
+def check_lookups(common_data, wires, max_report=64, ctx=None):
+    """The lookup argument checked on a witness (gl_plonk_check_lookups), before any commitment, table by table of
+    common_data.luts, laid out by common_data.lookup_rows as set_lookup_wires (plonk/prover.rs:50-108) lays them out.
+    Three kinds of failure, each named by (row, slot):
+    - L1: a looking slot of a LookupGate row whose (input, output) is not an entry of its table (the reference's
+      witness generation stops at it: "Incorrect input value provided");
+    - L2: a slot of a LookupTableGate row whose (input, output) is not the table entry placed there;
+    - L3: a slot of a LookupTableGate row whose multiplicity is not the number of looking slots that count for its
+      entry, as the reference counts them (by input, a later entry of one input winning; the padding of the last
+      LookupGate row for entry 0). The padding is the run of entry-0 pairs that ends that row: when entry 0's input
+      appears again later in a LUT and real lookups of entry 0 end the row, an honest witness gets two L3 entries
+      (a known false positive of a check that sees the witness only).
+    wires: the (num_wires, n) witness, a host array or a CUDA tensor. Returns a ConstraintReport of every failure and
+    the first max_report of them in (row, slot, kind) order, as (row, slot, label); the label names the table, the kind
+    and the values. ShapeError before any device work for a witness of the wrong shape or max_report outside
+    0..65536."""
+    cd, cfg = common_data, common_data.config
+    n, nr = 1 << cd.degree_bits, cfg.num_routed_wires
+    max_report = _check_max_report(max_report)
+    w, ws, wmem, wdev = _witness_columns(wires, cfg.num_wires, n, "the witness")
+    luts = [np.asarray(t, dtype=np.int64).reshape(-1, 2) for t in cd.luts]
+    if len(cd.lookup_rows) != len(luts):
+        raise N.ShapeError("%d lookup tables but %d lookup_rows triples" % (len(luts), len(cd.lookup_rows)))
+    if any(len(t) == 0 or (t < 0).any() or (t >> 16).any() for t in luts):
+        raise N.ShapeError("lookup tables must be non-empty lists of u16 (input, output) pairs")
+    flat = np.ascontiguousarray(np.concatenate(luts) if luts else np.zeros((1, 2)), dtype=np.uint16)
+    offsets = np.concatenate([[0], np.cumsum([len(t) for t in luts])]).astype(np.uint32)
+    rows = np.ascontiguousarray(np.array(cd.lookup_rows, dtype=np.uint32).reshape(-1))
+    counts = np.zeros(max(int(offsets[-1]), 1), dtype=np.uint32)
+    ctx = ctx or N.default_context(wdev or 0)
+    if wmem == N.MEM_DEVICE:
+        ctx.after_caller()
+    wp = N.vp(w.data_ptr()) if wmem == N.MEM_DEVICE else N.np_ptr(w)
+    failures, reported = C.c_uint64(), C.c_uint32()
+    pairs = np.zeros(2 * max(max_report, 1), dtype=np.uint32)
+    N.check(N.lib().gl_plonk_check_lookups(ctx.h, wp, ws, wmem, cd.degree_bits, nr, flat.ctypes.data_as(N.vp),
+                                           offsets.ctypes.data_as(N.u32p), rows.ctypes.data_as(N.u32p), len(luts),
+                                           counts.ctypes.data_as(N.u32p), max_report, C.byref(failures),
+                                           pairs.ctypes.data_as(N.u32p), C.byref(reported)), ctx.h)
+    pairs = pairs[:2 * reported.value].reshape(-1, 2).astype(np.int64)
+    row, slot, kind = pairs[:, 0], pairs[:, 1] >> 2, pairs[:, 1] & 3
+    # the values each label names: a looking slot's pair, or a table slot's pair and multiplicity
+    looking = kind == 1
+    c0 = np.where(looking, 2 * slot, 3 * slot)
+    v_in, v_out = _witness_values(w, c0, row), _witness_values(w, c0 + 1, row)
+    # a multiplicity exists in table slots only: a looking slot's 3 * slot + 2 can lie past the witness's columns
+    table = ~looking
+    v_mul = [None] * len(row)
+    for t, m in zip(np.flatnonzero(table).tolist(), _witness_values(w, 3 * slot[table] + 2, row[table])):
+        v_mul[t] = m
+    nts = nr // 3
+    entries = []
+    for r, s, k, a, b, m in zip(row.tolist(), slot.tolist(), kind.tolist(), v_in, v_out, v_mul):
+        t = next(q for q, (lu, _, fl) in enumerate(cd.lookup_rows) if lu <= r <= fl)
+        head = "lookup table %d, %s: " % (t, LOOKUP_KINDS[k])
+        if k == 1:
+            label = head + "looking slot (%d, %d) holds (%d, %d), which is not an entry of the table" % (r, s, a, b)
+        else:
+            e = (cd.lookup_rows[t][2] - r) * nts + s
+            exp = tuple(int(x) for x in luts[t][e if e < len(luts[t]) else 0])
+            if k == 2:
+                label = head + "table slot (%d, %d) holds (%d, %d), but entry %d%s is (%d, %d)" % (
+                    r, s, a, b, e, "" if e < len(luts[t]) else " (padding, entry 0)", *exp)
+            else:
+                cnt = int(counts[offsets[t] + e]) if e < len(luts[t]) else 0
+                label = head + "table slot (%d, %d) of entry %d records multiplicity %d, but it is looked up %d times" % (
+                    r, s, e, m, cnt)
+        entries.append((r, s, label))
+    return N.ConstraintReport(failures.value, entries)
+
+
 def commit_quotient_polys(common_data, quotient_polys, ctx=None, *, blinding=False, salt_key=None, shard=(0, 1),
                           lde_blocks=None):
     """'split up quotient polys' + 'commit to quotient polys' (plonk/prover.rs:319-352): every polynomial is cut into
